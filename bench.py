@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — frames/s of the WVN hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py — frames/s of the WVN hot path (BASELINE.json metric) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...        (the reference algorithm on the host CPU cores)
     python bench.py --config c5 ...             (BASELINE.json config 5: ViT-B/8, 64x64 tokens, B = 128 per GPU)
+    python bench.py --dump-outputs DIR ...      (the last timed step's outputs as DIR/<name>.npy)
 
 One "step" = ``HotPathStep.step`` (wild_visual_navigation_b200/hot_path.py — the object tests/test_bench_path_gpu.py
 holds to the oracle) over one batch of synthetic frames per GPU:
@@ -46,16 +47,31 @@ IMG, BATCH = CONFIGS["c3"]["img"], CONFIGS["c3"]["batch"]   # the headline workl
 K_IMAGE_CLUSTERS, KMEANS_ITERS = 20, 10
 
 
-def read_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 6650.0, "fallback"
+# NVIDIA's data sheet for the H100 SXM at its 700 W limit: dense BF16 TFLOP/s.  A ceiling, not a rate this code has
+# reached.
+PEAK_BF16_TFLOPS = 989.0
+DUMP_MAX_ELEMS = 1 << 20   # --dump-outputs: larger arrays are sampled down to this many elements (4-8 MB each)
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes every array as <out_dir>/<name>.npy (floating point -> float32, integer / bool -> float64).  An array
+    with more than DUMP_MAX_ELEMS elements is reduced to a fixed, seeded sample of its flattened elements, the same
+    from run to run, so that the whole dump stays far below 64 MB."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        t = t.float() if t.is_floating_point() else t.double()
+        if t.numel() > DUMP_MAX_ELEMS:
+            g = torch.Generator().manual_seed(1234)
+            idx = torch.randint(0, t.numel(), (DUMP_MAX_ELEMS,), generator=g).sort().values
+            t = t.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), t.numpy())
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region (queries only)."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -178,11 +194,11 @@ def workload_config(args, frames_per_step):
             "frames_per_gpu_per_step": frames_per_step, "image": f"{c['img']}x{c['img']}",
             "backbone": f"DINO {c['backbone']}/8 (random-init, seeded)", "stego_flip_tta": False, "run_clustering": True,
             "parallelism": f"dp{args.gpus} (independent frames; in-library NCCL all-reduce of MLP stats + grads)",
-            "l2": "inputs rotate over 3 image batches (3 x 77 MB > 126 MB L2); activations >> L2"}
+            "l2": "inputs rotate over 3 image batches (3 x 77 MB > 50 MB L2); activations >> L2"}
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# CUDA arm
 # ------------------------------------------------------------------------------------------------
 def run_b200(args):
     import ctypes
@@ -301,7 +317,7 @@ def run_b200(args):
 
     for k in range(args.warmup):
         step(dev_imgs[k % 3])
-    if args.profile_only:  # short, launch-list friendly run for ncu (no CPU leg, no e2e leg)
+    if args.profile_only:  # short, launch-list friendly run for a profiler (no CPU leg, no e2e leg)
         for k in range(args.steps):
             step(dev_imgs[k % 3])
         torch.cuda.synchronize()
@@ -316,8 +332,27 @@ def run_b200(args):
         sampler.start()
     lib.wvn_profile_enable(3 if args.profile_gemm else 1)   # CUDA events around the roofline kernel's launches
     l0 = lib.wvn_launch_count()
-    total_ms = timed(lambda k: step(dev_imgs[k % 3]), args.steps)
+    last = {}
+
+    def timed_step(k):
+        last["r"] = step(dev_imgs[k % 3])
+
+    total_ms = timed(timed_step, args.steps)
     launches = lib.wvn_launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        # what a caller of HotPathStep.step received from the last timed step; the padding of the per-frame arrays
+        # (rows past n_segments, edges past n_edges) is not output and is zeroed
+        r = last["r"]
+        nseg, nedge = r["n_segments"].long(), r["n_edges"].long()
+        crow = r["confidence_rows"].reshape(-1)
+        seg_rows = torch.arange(r["feat"].shape[1], device=dev)[None, :] < nseg[:, None]
+        edge_rows = torch.arange(r["edges"].shape[1], device=dev)[None, :] < nedge[:, None]
+        dump_outputs(args.dump_outputs, {
+            "trav": r["trav"], "conf": r["conf"], "seg": r["seg"],
+            "feat": r["feat"] * seg_rows[..., None], "centers": r["centers"] * seg_rows[..., None],
+            "edges": r["edges"] * edge_rows[..., None], "n_edges": nedge, "n_segments": nseg,
+            "confidence_rows": crow * (torch.arange(crow.numel(), device=dev) < nseg.sum()),   # compacted row order
+            "metrics": hp.te._trainer.metrics})
     prof_ms = (ctypes.c_float * 2)()
     prof_n = (ctypes.c_longlong * 2)()
     _C.check(lib.wvn_profile_collect(prof_ms, prof_n))
@@ -391,7 +426,7 @@ def run_b200(args):
             dist.destroy_process_group()
         return
 
-    peak_tf, peak_gbs, peak_src = read_peaks()
+    peak_tf = PEAK_BF16_TFLOPS
     n_tok = (S // PATCH) ** 2 + 1
     attn_flop_per_frame_head = 4.0 * n_tok * n_tok * 64
     attn_launches = max(1, prof_n[0])
@@ -399,10 +434,6 @@ def run_b200(args):
     attn_avg_ms = prof_ms[0] / attn_launches
     flops_per_launch = attn_flop_per_frame_head * c["heads"] * frames_per_launch
     achieved_tf = flops_per_launch / (attn_avg_ms * 1e-3) / 1e12 if attn_avg_ms > 0 else 0.0
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "attention_traffic.json")
-    if os.path.exists(tpath) and args.config == "c3":
-        traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
 
     cores = min(os.cpu_count() or 1, args.cpu_threads) if args.cpu_threads > 0 else (os.cpu_count() or 1)
     cpu_fps = None
@@ -421,10 +452,10 @@ def run_b200(args):
                 "d2h": "trav + conf maps, int32 segment image, pooled features, centers, edges (+ counts), loss metrics"},
         "gpu_launches": int(launches), "gpu_launches_per_step": launches / args.steps,
         "clocks": clocks,
-        "roofline": {"kernel": {"1": "attention_kernel", "2": "attention2_kernel", "3": "attention3_kernel", "5": "attention5_kernel"}.get(os.environ.get("WVN_ATTN_IMPL", "5"), "?") + " (fused QK^T-softmax-PV, tcgen05)", "bound": "tensor",
+        "roofline": {"kernel": "attention_kernel (fused QK^T-softmax-PV, wgmma)", "bound": "tensor",
                      "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
-                     "peak_source": f"{peak_src} bf16_tflops_sustained (kernel timed inside the step)",
-                     "traffic": traffic, "avg_launch_ms": attn_avg_ms, "launches": int(prof_n[0]),
+                     "peak_source": "H100 SXM data sheet, dense BF16 at 700 W (kernel timed inside the step)",
+                     "avg_launch_ms": attn_avg_ms, "launches": int(prof_n[0]),
                      "share_of_step": prof_ms[0] / total_ms if total_ms > 0 else None,
                      "gemm_share_of_step": prof_ms[1] / total_ms if (total_ms > 0 and prof_n[1] > 0) else None,
                      "gemm_launches": int(prof_n[1]) if prof_n[1] > 0 else None},
@@ -451,12 +482,16 @@ def main():
     ap.add_argument("--chunk", type=int, default=32, help="frames per ViT activation chunk")
     ap.add_argument("--cpu-frames", type=int, default=1, help="frames per step of the bounded CPU sample (~3-6 s per frame)")
     ap.add_argument("--cpu-threads", type=int, default=32,
-                    help="torch CPU threads for the CPU legs (0 = all host cores).  Measured on the 128-thread B200 host: the "
-                         "eager oracle runs 1 frame in ~3 s on 32 threads and in 42 s on 128 (thread sync on its many small "
-                         "ops), so 32 is what 'all the threads it can use' means for this code")
+                    help="torch CPU threads for the CPU legs (0 = all host cores).  The eager oracle is many small ops whose "
+                         "thread synchronisation makes it slower, not faster, on a very wide host, so the default is capped")
     ap.add_argument("--gpu-eager-frames", type=int, default=2, help="frames per step of the GPU-eager oracle leg (0 = skip)")
     ap.add_argument("--no-extras", action="store_true", help="skip the latency / flip-TTA / GPU-eager legs")
-    ap.add_argument("--profile-only", action="store_true", help="setup + warmup + steps only (for ncu)")
+    ap.add_argument("--profile-only", action="store_true", help="setup + warmup + steps only (for a profiler)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last of them returned (maps, segments, pooled rows, graph, "
+                         "loss metrics) as DIR/<name>.npy; the inputs are seeded, so two builds can be compared array by array.  "
+                         "CUDA arm only (--impl reference has no such outputs and rejects the option); with several ranks, "
+                         "rank 0 writes its own frames' outputs")
     ap.add_argument("--profile-gemm", action="store_true",
                     help="also time every GEMM launch with CUDA events (gemm_share_of_step; ~280 extra event pairs per step)")
     ap.add_argument("--ingest", default="f32", choices=["f32", "u8"],
@@ -464,6 +499,8 @@ def main():
                          "BASELINE.json); u8 = camera frames (B,H,W,3) uint8, ingest fused into the patch loader (SURVEY.md §8f)")
     args = ap.parse_args()
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs needs the CUDA arm (--impl b200)")
         run_reference(args)
     else:
         run_b200(args)

@@ -1,6 +1,6 @@
 /* wvn-b200 — C ABI of libwvn_b200.so
  *
- * B200-native (sm_100a) implementation of the Wild Visual Navigation per-frame hot path:
+ * H100-native (sm_90a) implementation of the Wild Visual Navigation per-frame hot path:
  * DINO ViT forward -> STEGO segmentation head / per-segment feature gather -> traversability
  * MLP (per-pixel inference with confidence, and the online train step).
  *
@@ -36,18 +36,18 @@ typedef enum {
   WVN_STATUS_OK = 0,
   WVN_STATUS_INVALID = -1,   /* bad argument / unsupported shape */
   WVN_STATUS_CUDA = -2,      /* CUDA error, see wvn_last_error() */
-  WVN_STATUS_NO_DEVICE = -3, /* no sm_100 device visible */
+  WVN_STATUS_NO_DEVICE = -3, /* no sm_90 device visible */
   WVN_STATUS_STATE = -4      /* handle not ready (e.g. a weight was never set) */
 } wvn_status;
 
 const char* wvn_last_error(void);
-/* 0 if device 0..n has compute capability 10.x, WVN_STATUS_NO_DEVICE otherwise. */
+/* 0 if device 0..n has compute capability 9.0, WVN_STATUS_NO_DEVICE otherwise. */
 int wvn_check_device(void);
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
 /* Optional CUDA-event timing of the dominant kernels inside real steps (bench.py roofline):
- * category 0 = fused attention, 1 = tcgen05 GEMMs; category_mask bit c enables category c (0 = off, 1 = the
+ * category 0 = fused attention, 1 = wgmma GEMMs; category_mask bit c enables category c (0 = off, 1 = the
  * roofline kernel only — 24 event pairs per step —, 3 = attention + the ~280 GEMM launches per step).
  * collect() synchronises and writes the summed milliseconds / launch counts per category into HOST arrays of
  * length 2 and clears the records. */
@@ -55,7 +55,7 @@ void wvn_profile_enable(int category_mask);
 int wvn_profile_collect(float* host_ms, long long* host_launches);
 
 /* ------------------------------------------------------------------------------------------
- * Primitive: bf16 tensor-core GEMM  C = A[M,K] * W[N,K]^T  (tcgen05, fp32 accumulate)
+ * Primitive: bf16 tensor-core GEMM  C = A[M,K] * W[N,K]^T  (wgmma, fp32 accumulate)
  * Replaces every nn.Linear / 1x1-conv call of the path (cuBLAS in the reference).
  * out_kind: 0 = bf16 out[M,ldo] = act(acc + bias); 1 = fp32 out = acc + bias;
  *           2 = fp32 out += acc + bias (residual).   act: 0 none, 1 ReLU, 2 GELU(erf).

@@ -9,7 +9,7 @@ The reference calls ``stego.backbones.backbone.get_backbone(cfg)`` and then ``se
 (``wild_visual_navigation/feature_extractor/dino_interface.py:12,45,84``).  That package
 (``leggedrobotics/self_supervised_segmentation``, *unpinned*, installed from a sibling clone:
 reference ``README.md:103-123``, ``docker/first_run.sh:3-4``) is NOT vendored in
-``/root/reference``; it wraps facebookresearch/dino's ``vision_transformer.py``.  This file
+the reference repository; it wraps facebookresearch/dino's ``vision_transformer.py``.  This file
 restates the published DINO algorithm [EXTERNAL-RECALLED, SURVEY.md §8 a3]:
 
 * ``PatchEmbed``: ``Conv2d(3, D, p, p)`` -> flatten -> ``(B, N, D)``

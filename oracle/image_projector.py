@@ -6,7 +6,7 @@ Follows wild_visual_navigation/image_projector/image_projector.py:
   project_and_render :152-197, and its use in TraversabilityEstimator.add_supervision_node
   (traversability_estimator/traversability_estimator.py:261-284: mask * traversability, fmin into the nodes' masks).
 
-The three kornia routines it calls are NOT in /root/reference (setup.py:11 ``kornia>=0.6.5``, unpinned, not installed
+The three kornia routines it calls are NOT in the reference repository (setup.py:11 ``kornia>=0.6.5``, unpinned, not installed
 here) -> [EXTERNAL-RECALLED], restated from kornia's published source, parity unpinned against kornia itself:
   kornia.geometry.linalg.transform_points, kornia.geometry.camera.pinhole.PinholeCamera.project
   (both end in convert_points_from_homogeneous: scale = 1 / (z + 1e-8) where |z| > 1e-8, else 1),

@@ -1,7 +1,7 @@
 """ORACLE helper — path-import of the reference's own torch-only modules.
 
-Only usable where ``/root/reference`` exists (the build container), i.e. by
-``tests/golden/make_golden.py`` and by tests marked ``needs_reference``.  A normal
+Only usable where a checkout of the reference repository exists and ``$WVN_REFERENCE_ROOT`` points at it, i.e. by
+``tests/golden/make_golden.py``; no test needs it.  A normal
 ``import wild_visual_navigation`` fails here (pytorch_lightning / omegaconf / pandas are absent),
 so stub packages are registered and the individual files are loaded with importlib, exactly as
 SURVEY.md §8c describes.  Nothing is copied: the modules execute from the read-only tree.
@@ -13,11 +13,11 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("WVN_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("WVN_REFERENCE_ROOT", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REF_ROOT, "wild_visual_navigation"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "wild_visual_navigation"))
 
 
 def _load(name: str, rel: str):

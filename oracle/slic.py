@@ -3,7 +3,7 @@
 :221-225 ``segment_slic``: ``slic.iterate(np.uint8(img * 255))``).
 
 The routine itself lives in the un-vendored ``fast-slic`` C++ package (setup.py:29, unpinned, not installed here; its
-source is not in /root/reference and it pins no numbers) -> [EXTERNAL-RECALLED]: restated as the published SLIC
+source is not in the reference repository and it pins no numbers) -> [EXTERNAL-RECALLED]: restated as the published SLIC
 algorithm (Achanta et al.) in the all-integer form fast-slic / gSLIC use — 8-bit sRGB -> CIELAB through lookup tables,
 a regular grid of ``num_components`` centres, 10 rounds of {assign every pixel to the nearest of the 3x3 neighbouring
 grid cells' centres under  d = |dLab|^2 * S^2 + |dxy|^2 * (compactness * Q)^2 ;  move every centre to the rounded

@@ -1,7 +1,7 @@
 """ORACLE (test infrastructure only) — restatement of the STEGO segmentation head and probes.
 
 The arithmetic lives in the external ``stego`` package (``stego.stego.Stego``), absent from
-``/root/reference``; call sites: ``feature_extractor/stego_interface.py:43,91-100,107-109``.
+the reference repository; call sites: ``feature_extractor/stego_interface.py:43,91-100,107-109``.
 Restated from the public STEGO code [EXTERNAL-RECALLED, SURVEY.md §8 a4]:
 
 * ``segmentation_head``: ``cluster1 = Conv2d(C, dim, 1)``; ``cluster2 = Conv2d(C, C, 1) -> ReLU ->
@@ -73,7 +73,7 @@ def postprocess(code: torch.Tensor, out_hw: tuple[int, int], hd: dict):
 @torch.no_grad()
 def image_kmeans(code: torch.Tensor, n_clusters: int, iters: int = 10) -> torch.Tensor:
     """Per-image k-means of the code, ``Stego.postprocess(image_clustering=True)`` with ``n_image_clusters`` clusters
-    (call site: stego_interface.py:43,91-100).  [EXTERNAL-RECALLED]: the upstream routine is not in /root/reference and
+    (call site: stego_interface.py:43,91-100).  [EXTERNAL-RECALLED]: the upstream routine is not in the reference repository and
     pins nothing (its initialisation is random); restated as plain Lloyd iterations — Euclidean distance, ``iters``
     iterations, initial centroids = the codes of ``n_clusters`` patches evenly spaced over the token sequence
     (index ``(2k+1) P / (2K)``), an empty cluster keeps its centroid — over the code at patch resolution.

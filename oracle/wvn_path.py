@@ -4,7 +4,7 @@ WVN hot path.  Never imported by the product package.
 Each function cites the reference code it follows (paths relative to the reference repo).
 PARITY STATUS: pinned against the reference itself — ``tests/golden/make_golden.py`` path-imports
 the reference's own ``SimpleMLP`` / ``TraversabilityLoss`` / ``ConfidenceGenerator`` /
-``SegmentExtractor`` / ``DinoInterface.inference`` wrapper code from ``/root/reference`` and
+``SegmentExtractor`` / ``DinoInterface.inference`` wrapper code from the reference repository and
 stores their outputs as fixtures; ``tests/test_oracle.py`` checks this file against them
 (plus the shipped known-answer ``assets/graph/{seg,center}.pt`` for the segment stage).
 """

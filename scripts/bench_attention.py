@@ -1,6 +1,6 @@
-"""Micro-benchmark of the fused attention kernel alone (ViT-S/8 @448 shapes), one process per
-variant: `WVN_ATTN_POLY=k python scripts/bench_attention.py`.  Prints accuracy vs fp32 torch and
-TFLOP/s (algorithmic 4*N^2*64 per (frame, head))."""
+"""Micro-benchmark of the fused attention kernel alone (ViT-S/8 @448 shapes):
+`python scripts/bench_attention.py`.  Prints accuracy vs fp32 torch and TFLOP/s (algorithmic 4*N^2*64 per
+(frame, head))."""
 import os
 import sys
 
@@ -36,4 +36,4 @@ e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / iters
 tf = 4.0 * N * N * 64 * B * H / (ms * 1e-3) / 1e12
-print(f"poly={os.environ.get('WVN_ATTN_POLY', 'default')} B={B} ms={ms:.3f} TFLOP/s={tf:.1f} rel_l2={rel:.2e}")
+print(f"B={B} ms={ms:.3f} TFLOP/s={tf:.1f} rel_l2={rel:.2e}")

@@ -1,10 +1,10 @@
 """Generate the golden fixtures in tests/golden/ by running the REFERENCE's own code.
 
-Run in the build container (``/root/reference`` present):  ``python tests/golden/make_golden.py``
+Run with a checkout of the reference repository:  ``WVN_REFERENCE_ROOT=<checkout> python tests/golden/make_golden.py``
 
 The reference is pure Python; its torch-only modules are path-imported from the read-only tree
 (oracle/ref_import.py) and executed on seeded inputs.  The results are stored as small fixtures
-so that the GPU box (which has no ``/root/reference``) can still check the oracle — and through
+so that a machine without the reference can still check the oracle — and through
 it the CUDA path — against what the reference computes.
 
 Fixtures
@@ -492,7 +492,7 @@ def make_stego_wrapper(ns):
 
 
 if __name__ == "__main__":
-    assert ref_import.available(), "needs /root/reference"
+    assert ref_import.available(), "set WVN_REFERENCE_ROOT to a checkout of the reference repository"
     ns = ref_import.load()
     make_mlp_train(ns)
     make_mlp_init(ns)

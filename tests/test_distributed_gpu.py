@@ -1,7 +1,7 @@
 """world_size-2 test of the CUDA trainer itself (``ops.MlpTrainer(process_group=...)``): two processes share cuda:0
 and exchange over gloo (NCCL refuses two ranks on one device), each holding a RAGGED shard of the rows; three steps must
 reproduce the single-process trainer on the concatenated rows — confidence statistics, loss terms, parameters (2e-5).
-The N>1 NCCL path (library-owned communicator) is exercised by bench.py / the scaling run on real multi-GPU boxes."""
+The N>1 NCCL path (library-owned communicator) is exercised by bench.py on a multi-GPU node."""
 import os
 import socket
 

@@ -84,7 +84,7 @@ def test_project_and_render_vs_oracle_448(batch, colors):
 
 
 def test_fused_supervision_update_and_label_pooling():
-    """traversability_estimator.py:261-289 as the B200 path runs it: several footprints rendered into the mission nodes'
+    """traversability_estimator.py:261-289 as the CUDA path runs it: several footprints rendered into the mission nodes'
     supervision masks (fmin with mask * traversability, in place, no temporaries), then the per-segment labels
     (update_supervision_signal) from those masks — against the oracle chain."""
     from oracle import image_projector as oip

@@ -3,10 +3,8 @@ the file the reference's learning node writes (golden ``tmp_state_dict.pt``, pro
 classes) and the reader's change-detection semantics (wvn_feature_extractor_node.py:407-446)."""
 import os
 
-import pytest
 import torch
 
-from oracle import ref_import
 from wild_visual_navigation_b200.model.simple_mlp import SimpleMLP
 from wild_visual_navigation_b200.utils import ConfidenceGenerator, read_tmp_state_dict, write_tmp_state_dict, TMP_STATE_DICT_NAME
 
@@ -48,24 +46,35 @@ def test_roundtrip_and_change_detection(tmp_path):
     assert not read_tmp_state_dict(dst_model, dst_cg, f)
 
 
-@pytest.mark.needs_reference
-def test_reference_classes_load_our_file(tmp_path):
-    if not ref_import.available():
-        pytest.skip("reference tree not present")
-    ns = ref_import.load()
+def test_reference_classes_load_our_file(golden_dir, tmp_path):
+    """Our file against the one the reference's own SimpleMLP / ConfidenceGenerator wrote (golden): the same keys, shapes
+    and dtypes, so the reference's ``load_state_dict(..., strict=False)`` takes every tensor.  ``ref_model`` below is a RESTATEMENT of the
+    reference's SimpleMLP layout (a Sequential under ``layers``), not the reference class; that it is the right layout
+    is checked against the golden's keys, which make_golden.py wrote with the reference's SimpleMLP(16, [8, 4, 1]).
+    It loads our file bit for bit."""
+    ref_file = torch.load(os.path.join(golden_dir, "tmp_state_dict.pt"), weights_only=False)
     model, cg = _pair(3)
     with torch.no_grad():
         cg.mean[0], cg.std[0] = 0.11, 0.07
     f = write_tmp_state_dict(model, cg, str(tmp_path))
     new_model_state_dict = torch.load(f, weights_only=False)
-    ref_model = ns.SimpleMLP(16, [8, 4, 1], True)
-    k = list(ref_model.state_dict().keys())[-1]
-    assert k in new_model_state_dict and (ref_model.state_dict()[k] != new_model_state_dict[k]).any()
+    assert list(new_model_state_dict.keys()) == list(ref_file.keys())
+    weight_keys = [k for k in ref_file if k != "confidence_generator"]
+    for k in weight_keys:
+        assert new_model_state_dict[k].shape == ref_file[k].shape and new_model_state_dict[k].dtype == ref_file[k].dtype, k
+    k = weight_keys[-1]
+    assert (ref_file[k] != new_model_state_dict[k]).any()   # the reader's change detection sees a new model
+    ref_model = torch.nn.Module()                            # the reference's layout: Sequential under `layers`
+    ref_model.layers = torch.nn.Sequential(torch.nn.Linear(16, 8), torch.nn.ReLU(), torch.nn.Linear(8, 4), torch.nn.ReLU(),
+                                           torch.nn.Linear(4, 17))
+    assert list(ref_model.state_dict().keys()) == weight_keys
     ref_model.load_state_dict(new_model_state_dict, strict=False)
     for name, v in ref_model.state_dict().items():
         assert torch.equal(v, model.state_dict()[name])
-    c = new_model_state_dict["confidence_generator"]
+    c, c_ref = new_model_state_dict["confidence_generator"], ref_file["confidence_generator"]
+    assert set(c.keys()) == set(c_ref.keys())
     assert abs(c["mean"].item() - 0.11) < 1e-7 and abs(c["std"].item() - 0.07) < 1e-7 and tuple(c["var"].shape) == (1, 1)
+    assert all(tuple(c[n].shape) == tuple(c_ref[n].shape) for n in c_ref if torch.is_tensor(c_ref[n]))
 
 
 def test_image_features_wire_roundtrip():

@@ -1,4 +1,4 @@
-"""GPU parity tests of the individual sm_100a kernels against plain PyTorch fp32 references.
+"""GPU parity tests of the individual sm_90a kernels against plain PyTorch fp32 references.
 
 Tolerances (stated per test): bf16 tensor-core kernels are compared with an fp32 reference
 evaluated on the SAME bf16-rounded operands, so the only differences are accumulation order and
@@ -26,7 +26,7 @@ def ops():
 @pytest.mark.parametrize("M,N,K,bn", [
     (128, 128, 64, 128), (300, 384, 384, 0), (1000, 1152, 384, 192), (777, 1536, 384, 256), (512, 384, 1536, 0),
     (130, 448, 64, 224), (4096, 64, 256, 64), (128 * 150, 384, 192, 128), (25600, 1152, 384, 0), (12800, 1536, 384, 0),
-    # CTA-pair kernel: odd 128-row block count + row tail, streaming (K=1536), 256- and 128-wide resident tiles
+    # odd 128-row block count + row tail, long K (1536), 256- and 128-wide tiles
     (25600 + 128 + 37, 1152, 384, 0), (20000, 384, 1536, 0), (19200, 512, 384, 0), (19000, 640, 128, 128),
 ])
 @pytest.mark.parametrize("out_kind,act", [(0, 0), (0, 1), (0, 2), (1, 0), (2, 0)])
@@ -85,7 +85,7 @@ def test_attention(ops, B, H, n_valid):
 
 
 def test_attention_peaked_softmax(ops):
-    """Large logit spread: exercises the lazy-rescale path (max grows by > 2^8 between tiles)."""
+    """Large logit spread: the running row maximum grows by more than 2^8 between tiles."""
     B, H, n_valid, npad = 1, 2, 640, 640
     g = torch.Generator(device="cuda").manual_seed(1)
     q = (torch.randn(B, H, npad, 64, device="cuda", generator=g) * 4).bfloat16()

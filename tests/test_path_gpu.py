@@ -125,7 +125,7 @@ def test_vit_base_logit_spread_conditioning_and_debug_mode(attn_std, monkeypatch
 
 
 def test_beats_eager_gpu_reference_path():
-    """North star: "end-to-end frames/s at 1 GPU that beats the reference's own GPU PyTorch path on the same B200".
+    """North star: "end-to-end frames/s at 1 GPU that beats the reference's own GPU PyTorch path on the same H100".
     The oracle IS that path (eager fp32 PyTorch in the reference's order of operations); it is timed here on the GPU
     for the backbone + per-pixel inference of 448x448 frames next to the product.  Prints both; asserts >= 5x."""
     import time

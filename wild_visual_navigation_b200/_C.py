@@ -2,7 +2,7 @@
 
 PyTorch is used here only for device memory and streams: every call passes raw
 ``tensor.data_ptr()`` values plus the current CUDA stream.  There is no CPU fallback — a
-missing library or a non-sm_100 device raises.
+missing library or a non-sm_90 device raises.
 """
 from __future__ import annotations
 
@@ -121,9 +121,9 @@ def check(status: int) -> None:
 
 
 def require_device() -> None:
-    """Fail loudly unless a compute-capability-10.x GPU is the current device."""
+    """Fail loudly unless a compute-capability-9.0 GPU is the current device."""
     if not torch.cuda.is_available():
-        raise WvnError("wild_visual_navigation_b200 needs a CUDA (sm_100a) device; no CPU fallback exists")
+        raise WvnError("wild_visual_navigation_b200 needs a CUDA (sm_90a) device; no CPU fallback exists")
     check(lib().wvn_check_device())
 
 

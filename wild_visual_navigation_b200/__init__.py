@@ -1,4 +1,4 @@
-"""wild_visual_navigation_b200 — B200-native (sm_100a) hot path of Wild Visual Navigation.
+"""wild_visual_navigation_b200 — H100-native (sm_90a) hot path of Wild Visual Navigation.
 
 Keeps the reference's class surface for the per-frame path (SURVEY.md §8b):
 ``FeatureExtractor`` / ``DinoInterface`` / ``StegoInterface`` / ``SegmentExtractor`` /

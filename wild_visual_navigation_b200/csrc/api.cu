@@ -121,7 +121,10 @@ int wvn_check_device(void) {
   cudaGetDevice(&dev);
   int major = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return set_error(WVN_ERR_NO_DEVICE, "device %d has compute capability %d.x, need 10.x (sm_100a)", dev, major);
+  int minor = 0;
+  cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (major != 9 || minor != 0)
+    return set_error(WVN_ERR_NO_DEVICE, "device %d has compute capability %d.%d, need 9.0 (sm_90a)", dev, major, minor);
   return WVN_OK;
 }
 
@@ -140,32 +143,7 @@ int wvn_gemm_bf16(const void* a, long long lda, const void* w, const float* bias
   g.epi = out_kind == 0 ? EPI_BF16 : (out_kind == 1 ? EPI_F32 : EPI_RESID_F32);
   WVN_REQUIRE(out_kind >= 0 && out_kind <= 2, "wvn_gemm_bf16: out_kind %d", out_kind);
   g.act = act; g.bias = bias; g.out = out; g.ldo = ldo;
-#ifdef WVN_GEMM_ABLATE
-  {
-    static int dbg = -1;  // $WVN_GEMM_DEBUG: epilogue ablations (1 = no stores, 2 = no epilogue), ablation builds only
-    if (dbg < 0) { const char* e = getenv("WVN_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
-    g.debug = dbg;
-  }
-#endif
-#ifdef WVN_GEMM_TIMING
-  static long long* tbuf = nullptr;  // device memory: the probes must not fault on managed pages
-  if (!tbuf) cudaMalloc(&tbuf, 16 * sizeof(long long));
-  cudaMemsetAsync(tbuf, 0, 16 * sizeof(long long), S(stream));
-  g.timing = tbuf;
-  const int rc = gemm_bf16(g, a, lda, w, block_n, S(stream));
-  long long t[16];
-  cudaMemcpyAsync(t, tbuf, sizeof(t), cudaMemcpyDeviceToHost, S(stream));
-  cudaStreamSynchronize(S(stream));
-  const long long nt = t[3] > 0 ? t[3] : 1;
-  fprintf(stderr, "[gemm timing M=%d N=%d K=%d kind=%d act=%d, cycles per tile of CTA 0 (%lld tiles)] mma: wait_acc_empty %lld  "
-          "wait_full(TMA) %lld  issue+commit %lld | epilogue: wait_acc_full %lld  work %lld = ldtm %lld  bias %lld  act %lld  "
-          "transpose+store %lld\n",
-          m, n, k, out_kind, act, nt, t[0] / nt, t[1] / nt, t[2] / nt, t[4] / nt, t[5] / nt, t[8] / nt, t[9] / nt, t[10] / nt,
-          t[11] / nt);
-  return rc;
-#else
   return gemm_bf16(g, a, lda, w, block_n, S(stream));
-#endif
 }
 
 int wvn_attention_bf16(const void* q, const void* k, const void* vt, void* out, int batch, int heads, int npad,
@@ -174,39 +152,7 @@ int wvn_attention_bf16(const void* q, const void* k, const void* vt, void* out, 
   a.batch = batch; a.heads = heads; a.npad = npad; a.n_valid = n_valid;
   a.scale_log2 = scale * 1.4426950408889634f;
   a.out = out; a.ldo = static_cast<long long>(heads) * 64;
-  static long long* timing_buf = nullptr;  // $WVN_ATTN_TIMING=1: phase cycle counters, printed after each call
-  static int timing_on = -1;
-  if (timing_on < 0) {
-    const char* e = getenv("WVN_ATTN_TIMING");
-    timing_on = (e && e[0] == '1') ? 1 : 0;
-    if (timing_on) cudaMallocManaged(&timing_buf, 16 * sizeof(long long));
-  }
-  a.timing = timing_on ? timing_buf : nullptr;
-  const int rc = attention_bf16(a, q, k, vt, S(stream));
-  if (timing_on && rc == 0) {
-    cudaStreamSynchronize(S(stream));
-    const int nkv = npad / 128;
-    const char* impl = getenv("WVN_ATTN_IMPL");
-    if (impl && atoi(impl) == 1)
-      fprintf(stderr, "[attn v1 timing, cycles per KV tile] softmax: wait_s %lld  ldtm %lld  math %lld  wait_pv %lld  store+fence %lld | "
-              "mma: issue_qk(+waits) %lld  wait_p %lld  wait_v+issue_pv %lld  loop %lld\n",
-              timing_buf[0] / nkv, timing_buf[1] / nkv, timing_buf[2] / nkv, timing_buf[3] / nkv, timing_buf[4] / nkv,
-              timing_buf[8] / nkv, timing_buf[9] / nkv, timing_buf[10] / nkv, timing_buf[11] / nkv);
-    else if (impl == nullptr || atoi(impl) == 5)
-      fprintf(stderr, "[attn v5 timing, cycles per 64-key tile, thread 0] wait_s %lld  ldtm %lld  max+rescale %lld  exp %lld  store %lld\n",
-              timing_buf[0] / ((n_valid + 63) / 64), timing_buf[1] / ((n_valid + 63) / 64), timing_buf[2] / ((n_valid + 63) / 64),
-              timing_buf[3] / ((n_valid + 63) / 64), timing_buf[4] / ((n_valid + 63) / 64));
-    else if (atoi(impl) == 3)
-      fprintf(stderr, "[attn v3 timing, cycles per KV tile, thread 0] wait_s %lld  ldtm %lld  max+mailbox %lld  rescale %lld  exp %lld  "
-              "probe+wait_pv+store %lld\n", timing_buf[0] / nkv, timing_buf[1] / nkv, timing_buf[2] / nkv, timing_buf[5] / nkv,
-              timing_buf[3] / nkv, timing_buf[4] / nkv);
-    else
-      fprintf(stderr, "[attn v2 timing, cycles per KV tile] softmax wg0: wait_s %lld  ldtm %lld  max+rescale %lld  token_wait %lld  exp %lld  "
-              "wait_pv+store %lld | mma: wait_v+wait_p0 %lld  pv0+wait_sfree0+qk0 %lld  wait_p1 %lld  pv1+qk1+loop %lld\n",
-              timing_buf[0] / nkv, timing_buf[1] / nkv, timing_buf[2] / nkv, timing_buf[5] / nkv, timing_buf[3] / nkv,
-              timing_buf[4] / nkv, timing_buf[8] / nkv, timing_buf[9] / nkv, timing_buf[10] / nkv, timing_buf[11] / nkv);
-  }
-  return rc;
+  return attention_bf16(a, q, k, vt, S(stream));
 }
 
 int wvn_layernorm(const float* x, const float* gamma, const float* beta, void* out_bf16, long long rows, int dim,
@@ -347,7 +293,7 @@ static int vit_check_loaded(wvn_vit* h, bool need_head) {
   return WVN_OK;
 }
 
-constexpr int kDefaultSubAttn = 1 << 30;  // frames per (LN1, QKV, attention) pass; tuned on B200
+constexpr int kDefaultSubAttn = 1 << 30;  // frames per (LN1, QKV, attention) pass: one pass over the whole chunk
 
 namespace {
 int vit_forward_impl(wvn_vit_t* h, const void* img, bool u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
@@ -409,9 +355,8 @@ int vit_forward_impl(wvn_vit_t* h, const void* img, bool u8_hwc, int src_batch, 
     LayerNormArgs la;
     la.rows = rows; la.dim = D; la.eps = c.ln_eps; la.npad = h->npad; la.n_valid = h->n_valid;
     // GEMMs / LayerNorms can run over sub-chunks of `sub` frames ($WVN_VIT_SUBCHUNK) to keep xn / hid / x
-    // L2-resident between producer and consumer.  Measured on B200 (round 1): sub-chunking LOSES (1752 -> 1719
-    // frames/s at sub = 16): what the smaller GEMMs lose to wave quantisation (the N = 384 GEMMs drop to 5.4 waves)
-    // outweighs the L2 hits, which the snake order below already collects for the hottest ~100 MB — default off.
+    // L2-resident between producer and consumer.  Smaller GEMMs lose to wave quantisation what they gain in L2
+    // hits, which the snake order below already collects for the rows written last — default off.
     static int sub_env = -1;
     if (sub_env < 0) {
       const char* e = getenv("WVN_VIT_SUBCHUNK");
@@ -420,7 +365,7 @@ int vit_forward_impl(wvn_vit_t* h, const void* img, bool u8_hwc, int src_batch, 
     }
     const int sub = std::min(sub_env, nb);
     // "Snake" order: every kernel of the chain walks its rows in the opposite direction to its producer, so it
-    // starts on the rows that were written last and are still in the 126 MB L2 ($WVN_VIT_SNAKE=0 disables).
+    // starts on the rows that were written last and are still in the 50 MB L2 ($WVN_VIT_SNAKE=0 disables).
     static int snake = -1;
     if (snake < 0) { const char* e = getenv("WVN_VIT_SNAKE"); snake = (e && atoi(e) == 0) ? 0 : 1; }
     int dir = 0;  // the patch-embed GEMM above ran first-to-last
@@ -754,7 +699,7 @@ int wvn_mlp_infer_create(int dim, int h1, int h2, int chunk_rows, wvn_mlp_infer_
     if (n <= best_n) { best_n = n; best_bn = bn; }
   }
   h->bn3 = best_bn; h->n3_p = best_n;
-  h->chunk_rows = chunk_rows > 0 ? round_up(chunk_rows, 128) : 148 * 128 * 3;
+  h->chunk_rows = chunk_rows > 0 ? round_up(chunk_rows, 128) : sm_count() * 128 * 3;  // three waves of 128-row tiles
   int rc = WVN_OK;
   auto alloc = [&](DevBuf& b, size_t bytes) { if (rc == WVN_OK) rc = b.alloc(bytes); };
   alloc(h->w1, static_cast<size_t>(h->h1_p) * h->dim_p * 2);
@@ -840,23 +785,7 @@ static int pixels_fused_chunk(wvn_mlp_infer_t* h, const void* tok_bf16, long lon
   a.sx = static_cast<float>(gw - 1) / static_cast<float>(out_w - 1);
   a.ww = ww; a.feat = h->dim;
   a.frame_rows = frame_rows; a.row0 = row0;
-#ifdef WVN_GEMM_TIMING
-  static long long* ptb = nullptr;
-  if (!ptb) cudaMalloc(&ptb, 16 * sizeof(long long));
-  a.timing = ptb;
-#endif
   WVN_PROPAGATE(pixel_head(a, h->w2.p, h->h1_p, s));
-#ifdef WVN_GEMM_TIMING
-  {
-    long long t[16];
-    cudaMemcpyAsync(t, ptb, sizeof(t), cudaMemcpyDeviceToHost, s);
-    cudaStreamSynchronize(s);
-    const long long n = t[5] > 0 ? t[5] : 1;
-    fprintf(stderr, "[pixel_head timing, cycles per tile of CTA 0 (%lld tiles)] phaseA+sync %lld  phaseB+sync %lld  mma_wait %lld  "
-            "epilogue %lld  end_sync %lld | producer: tables+bar %lld  copy %lld  pix/gram %lld\n", n, t[0] / n, t[1] / n, t[2] / n, t[3] / n,
-            t[4] / n, t[8] / n, t[9] / n, t[10] / n);
-  }
-#endif
   return WVN_OK;
 }
 

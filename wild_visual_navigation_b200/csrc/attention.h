@@ -1,4 +1,4 @@
-// wvn-b200: internal interface of the fused tcgen05 attention kernel (attention_tcgen05.cu).
+// wvn-b200: internal interface of the fused wgmma attention kernel (attention_wgmma.cu).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -13,12 +13,6 @@ struct AttnArgs {
   void* out = nullptr;     // [batch, npad, ldo] bf16, head h occupies columns [64h, 64h+64)
   long long ldo = 0;
   int reverse = 0;     // walk (frame, head, q-tile) last-to-first: start on what the QKV GEMM wrote last (L2 hits)
-  int no_token = 0;    // debug: v2 kernel without the exp-phase ordering between its two softmax warpgroups
-  // lazy rescale (impl 5): O and l are rescaled only when a row's max grew by more than 2^this.  P is bf16 and every
-  // accumulator fp32, so 2^32 is as safe as FA4's fp16-motivated 2^8 — and with the bench ViT's logit spread (std ~3) the
-  // threshold 8 still rescaled often enough to cost 3-7 % of the kernel (scripts/bench_attention.py QK_STD=1.8 / 2.5)
-  float rescale_log2 = 32.f;
-  long long* timing = nullptr;  // debug: 16 cycle counters of block (0,0) (see scripts/bench_attention.py)
 };
 
 // q, k: [batch*heads, npad, 64] bf16; vt: [batch*heads, 64, npad] bf16.

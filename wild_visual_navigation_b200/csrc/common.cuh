@@ -1,9 +1,9 @@
-// wvn-b200: shared device-side primitives for the sm_100a kernels.
+// wvn-b200: shared device-side primitives for the sm_90a kernels.
 //
-// Thin inline-PTX wrappers for the Blackwell async machinery this library is
-// built on: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit /
-// ld / st / fences) and the shared-memory / instruction descriptors that
-// tcgen05.mma consumes.  Everything here targets sm_100a only.
+// Thin inline-PTX wrappers for the Hopper async machinery this library is
+// built on: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async /
+// commit / wait) and the shared-memory matrix descriptor that wgmma consumes.
+// Everything here targets sm_90a only.
 #pragma once
 
 #include <cuda.h>
@@ -21,12 +21,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// One lane of the (fully converged) warp.  The single-thread roles (TMA producer, MMA issuer) run with ALL 32 lanes
-// in the loop and guard only the issue instructions with this: ptxas knows the predicate selects exactly one lane and
-// emits `ELECT; @P UTCHMMA`.  Under a plain `if (lane == 0)` the branch is divergent as far as the compiler can tell and
-// every uniform-datapath instruction (UTCHMMA, UTMALDG, UTCBAR) is wrapped in its own ELECT / BRA.U.ANY
-// serialisation loop preceded by R2UR moves — ~90 clk per tcgen05.mma issue, which made the attention kernel
-// MMA-ISSUE bound (12 small UMMAs per KV tile; round-2 SASS + phase timing).
+// One lane of the (fully converged) warp.  The single-thread TMA producer runs with ALL 32 lanes in its loop and guards
+// only the issue instructions with this, so the compiler sees a warp-uniform loop around one elected lane.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile(
@@ -46,26 +42,6 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
-
-// packed fp32x2 arithmetic (sm_100: FFMA2 / FADD2 halve the issue slots of elementwise epilogues)
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
 
 // ---------------------------------------------------------------------------
 // mbarrier
@@ -123,9 +99,8 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
 #endif
 
 // Up to 2^16 try_waits in a 4-instruction loop (try_wait suspends the thread in hardware for a bounded,
-// implementation-defined time; an explicit suspend-time hint was measured to delay the wake-up — see DESIGN.md): the single-thread producer / MMA-issuer warps share their SM sub-partition with the
-// math warps, and every instruction they spin on is an issue slot taken from those (round 1: 30 % of all issued
-// instructions of the attention kernel were the 12-instruction wait loops of these two warps).
+// implementation-defined time): the producer warp shares its SM sub-partition with math warps, and every instruction it
+// spins on is an issue slot taken from those.
 #ifndef WVN_MBAR_HINT_NS
 #define WVN_MBAR_HINT_NS 0
 #endif
@@ -174,14 +149,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ---------------------------------------------------------------------------
-// Proxy / tcgen05 fences
+// Proxy fence
 // ---------------------------------------------------------------------------
-// Generic-proxy writes to shared memory (st.shared) -> visible to the async proxy (UMMA / TMA).
+// Generic-proxy writes to shared memory (st.shared) -> visible to the async proxy (wgmma / TMA).
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
 // TMA: 2D tiled load, global -> shared, completion on an mbarrier (complete_tx bytes)
@@ -246,31 +219,7 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 }
 
 // ---------------------------------------------------------------------------
-// TMEM allocation (whole warp, .sync.aligned)
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-// Two allocations by one CTA: the permit is relinquished only after the last one.
-__device__ __forceinline__ void tmem_alloc_keep_permit(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_permit() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---------------------------------------------------------------------------
-// UMMA descriptors
+// wgmma: warpgroup-wide asynchronous MMA, bf16 operands, fp32 accumulator in registers
 // ---------------------------------------------------------------------------
 // Shared-memory matrix descriptor for a K-major bf16 operand tile whose rows are 64
 // elements (=128 B) wide, stored with the 128-byte swizzle exactly as TMA
@@ -278,191 +227,116 @@ __device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
 //   bits [0,14)  start address >> 4
 //   bits [16,30) leading byte offset >> 4   (unused for swizzled K-major; 1)
 //   bits [32,46) stride byte offset >> 4    (1024 B between 8-row groups -> 64)
-//   bits [46,48) descriptor version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
+//   bits [62,64) layout type: 1 = SWIZZLE_128B
+// A step of 16 elements (32 B) along K inside the swizzle atom is +2 on the descriptor.
 __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3ffff) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for tcgen05.mma.kind::f16 with bf16 A/B (both K-major) and an
-// fp32 accumulator:  c_format=F32 (bits 4-5 = 1), a_format=BF16 (bits 7-9 = 1),
-// b_format=BF16 (bits 10-12 = 1), N>>3 at bits 17-22, M>>4 at bits 24-28.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
+// Orders the warpgroup's earlier register / shared-memory accesses before its next wgmma.mma_async.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// Waits until at most N committed wgmma groups of this warpgroup are still in flight.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T   (single thread issues)
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
+// Zero-cost ordering point: ties accumulator registers to the surrounding wgmma fence / wait, so that no use of them is
+// scheduled across it while the asynchronous MMA may still write them.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Register budget of the calling warpgroup (all four warps execute it): producers give registers up, consumers take them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// D[64 x N] (+)= A[64 x 16, smem] * B[N x 16, smem]^T.  Thread t of the warpgroup (warp w = t / 32, g = lane / 4,
+// q = lane % 4) holds d[4 j + 2 h + e] = D[16 w + g + 8 h][8 j + 2 q + e].
+__device__ __forceinline__ void wgmma_m64n32k16_ss(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
-// D[tmem] (+)= A[tmem] * B[smem]^T: the A operand (bf16, K-major) is read from tensor memory — lane = row,
-// each 32-bit column holds two consecutive K elements, so one K=16 step spans 8 columns.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
+      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
-// Arrive (count 1) on an mbarrier once every previously issued tcgen05.mma of this thread
-// has completed.  Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// Same, arriving on the mbarrier at this CTA-relative offset in every CTA of cta_mask.
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// ---------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: the two CTAs of a 2-cluster sit on the two SMs of one TPC and
-// execute one 256-row UMMA together.  Each CTA stages its own 128 rows of A and its own half of
-// the B tile's N rows at the same CTA-relative shared-memory offsets; the leader (cluster rank 0)
-// issues the MMA and owns the "full" barriers, which the peer's TMA loads signal remotely.
-// ---------------------------------------------------------------------------
-// shared::cluster address of the same CTA-relative location in the leader CTA (cluster rank 0)
-__device__ __forceinline__ uint32_t leader_smem_addr(const void* p) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(smem_u32(p)));
-  return r;
-}
-
-// TMA load into this CTA's shared memory whose complete_tx lands on the LEADER CTA's mbarrier.
-__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap* map, uint32_t leader_bar, void* smem_dst, int32_t c0,
-                                                 int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// Arrive (count 1) on an mbarrier of the leader CTA (address from leader_smem_addr).
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t leader_bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(leader_bar) : "memory");
-}
-
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem of both CTAs, 256 rows] (+)= A[128 rows per CTA] * B[N/2 rows per CTA]^T   (leader thread issues)
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
+      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, "
+      "%40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, "
+      "%59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
-// Commit of the pair's MMAs, arriving on the mbarrier at this offset in both CTAs (mask 0b11) or one of them.
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// ---------------------------------------------------------------------------
-// TMEM <-> registers: 32 lanes x 32 columns of 32-bit (each thread: its lane, 32 columns)
-// The warp may only touch lanes [32*(warp_id%4), +32).
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+// Same with the A operand in registers: a0..a3 are bf16 pairs laid out like the accumulator of a 64 x 16 tile,
+// a0 = A[g][2q, 2q+1], a1 = A[g + 8][2q, 2q+1], a2 = A[g][2q + 8, 2q + 9], a3 = A[g + 8][2q + 8, 2q + 9].
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                   uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, "
+      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(desc_b), "r"(accumulate));
 }
 
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Zero-cost ordering point: ties the 32 destination registers of a tcgen05.ld to the preceding
-// tcgen05.wait::ld, so that no use of them can be scheduled ahead of the wait when loads are pipelined.
-__device__ __forceinline__ void tmem_ld_fence32(uint32_t (&r)[32]) {
-  asm volatile(""
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                 "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                 "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                 "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// single 32-bit column per lane (used as a tiny cross-warp mailbox in tensor memory)
-__device__ __forceinline__ void tmem_st1(uint32_t taddr, uint32_t v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t tmem_ld1(uint32_t taddr) {
-  uint32_t v;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(v) : "r"(taddr) : "memory");
-  return v;
-}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

@@ -1,4 +1,4 @@
-// wvn-b200: kernels between the ViT token grid and image resolution (sm_100a).
+// wvn-b200: kernels between the ViT token grid and image resolution (sm_90a).
 //
 //   upsample_tokens_dense : F.interpolate(features, (H,H), "bilinear", align_corners=True)
 //                           (reference: dino_interface.py:87-90, stego_interface.py:107) —

@@ -1,4 +1,4 @@
-// wvn-b200: internal interface of the tcgen05 GEMM family (see gemm_tcgen05.cu).
+// wvn-b200: internal interface of the wgmma GEMM family (see gemm_wgmma.cu).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -48,8 +48,6 @@ struct GemmArgs {
   // launch control
   int max_ctas = 0;             // 0 = one CTA per SM
   int reverse_m = 0;            // walk the m-blocks last-to-first (start on the rows the producer kernel wrote last: L2 hits)
-  int debug = 0;                // debug (-DWVN_GEMM_TIMING builds): 1 = skip the global stores, 2 = skip the epilogue body
-  long long* timing = nullptr;  // debug (-DWVN_GEMM_TIMING builds): phase cycle counters of CTA 0
 };
 
 int pick_block_n(int N);

@@ -90,8 +90,8 @@ int sm_count() {
   static int n = 0;
   if (n) return n;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   return n;
 }
 

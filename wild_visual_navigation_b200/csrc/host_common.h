@@ -13,7 +13,7 @@ enum : int {
   WVN_OK = 0,
   WVN_ERR_INVALID = -1,   // bad argument / unsupported shape
   WVN_ERR_CUDA = -2,      // CUDA runtime / driver error (message in wvn_last_error())
-  WVN_ERR_NO_DEVICE = -3, // no sm_100 device
+  WVN_ERR_NO_DEVICE = -3, // no sm_90 device
   WVN_ERR_STATE = -4,     // handle in the wrong state (e.g. weights missing)
 };
 

@@ -1,4 +1,4 @@
-// wvn-b200: online traversability-MLP training step in fp32 (sm_100a, latency-bound).
+// wvn-b200: online traversability-MLP training step in fp32 (sm_90a, latency-bound).
 //
 // One call sequence = the body of TraversabilityEstimator.train()
 // (traversability_estimator.py:464-477):

@@ -2,7 +2,7 @@
 //
 // Same arithmetic as mlp_train.cu (the body of TraversabilityEstimator.train(), traversability_estimator.py:464-477:
 // SimpleMLP.forward -> TraversabilityLoss.forward incl. the ConfidenceGenerator "latest_measurement" update ->
-// backward -> Adam), restructured around what round 1's launch list showed — ~20 launches of 5-30 us each, two host
+// backward -> Adam), restructured to remove what that version's launch list shows — some twenty short launches, two host
 // synchronisations (a boolean-mask gather and an .item()) and three torch.distributed calls per step:
 //
 //   K1 train_fwd_rows   : per 32-row tile the three layers run back to back out of shared memory; per-row loss terms and

@@ -1,4 +1,4 @@
-// wvn-b200: fused per-pixel traversability head (sm_100a).
+// wvn-b200: fused per-pixel traversability head (sm_90a).
 //
 // Replaces, per frame (wvn_feature_extractor_node.py:319-370, simple_mlp.py:33-39,
 // confidence_generator.py:182-193):
@@ -9,7 +9,7 @@
 // The per-pixel work is restructured algebraically so that neither x (384-d) nor pred (385-d) is
 // ever formed per pixel — only the 256-d hidden layer is:
 //   * layer 1 is affine and bilinear weights sum to 1:  W1 x + b1 = sum_k w_k (W1 t_k + b1)
-//     -> G = tokens @ W1^T + b1 is computed ONCE PER TOKEN (3136 rows/frame, tcgen05 GEMM) and the
+//     -> G = tokens @ W1^T + b1 is computed ONCE PER TOKEN (3136 rows/frame, wgmma GEMM) and the
 //        kernel below interpolates G (256 ch) instead of x (384 ch) followed by a 384->256 GEMM;
 //   * with r = R h2 + c the reconstruction (R = W3[1:], c = b3[1:]):
 //       D*loss = |r|^2 - 2 r.x + |x|^2
@@ -17,7 +17,7 @@
 //       r.x    = sum_k w_k ( h2 . (R^T t_k) + c.t_k )            (U = tokens @ R, cT = tokens @ c: per token)
 //       |x|^2  = bilinear form of the 2x2 neighbourhood's Gram    (5 dot products per token)
 // Per pixel that leaves: interpolate 256+33 channels, one 256->32 layer on the tensor core
-// (tcgen05, M=128 pixels, N=32), and ~650 fp32 FMAs — ~12x fewer FLOPs than the direct form, and
+// (wgmma, M=128 pixels, N=32), and ~650 fp32 FMAs — ~12x fewer FLOPs than the direct form, and
 // no HBM traffic beyond the two output maps.  bf16 rounding points are the same as the unfused
 // path (tokens, weights, h1); everything downstream of the layer-2 accumulator is fp32.
 #include <algorithm>
@@ -31,11 +31,13 @@ namespace wvn {
 namespace {
 
 constexpr int kH1 = 256, kH2 = 32;
-constexpr int kTileW = 64, kTileH = 2;            // 128 pixels per tile: lane/TMEM row i = r*64 + px
+constexpr int kTileW = 64, kTileH = 2;            // 128 pixels per tile: row i = r*64 + px
 constexpr int kWinMax = 10;                        // token-window columns per tile (ratio 8: 7 + 3)
 constexpr int kGvStride = 292;                     // 256 G + 32 U + cT_hi + cT_lo, padded to float4
 constexpr int kThreads = 256;
-constexpr uint32_t kOffA = 0;                      // [4 K-blocks][128 rows][128 B]  h1 tile (bf16, swizzled)
+constexpr uint32_t kOffA = 0;                      // [4 K-blocks][128 rows][128 B]  h1 tile (bf16, swizzled); once layer 2
+                                                   // has consumed it: [128 pixels][kH2Stride] fp32 layer-2 accumulator
+constexpr int kH2Stride = 36;                      // floats per pixel row of that tile (16-byte aligned, conflict-free)
 constexpr uint32_t kOffW2 = 65536;                 // [4 K-blocks][32 rows][128 B]
 constexpr uint32_t kOffGv = kOffW2 + 16384;        // [2][kWinMax][kGvStride] fp32
 constexpr uint32_t kOffN2 = kOffGv + 2 * kWinMax * kGvStride * 4;  // [2][kWinMax][2] fp32: |xv|^2, xv_c.xv_{c+1}
@@ -73,8 +75,6 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
   float* n2 = reinterpret_cast<float*>(smem + kOffN2);
   PixTables* pt = reinterpret_cast<PixTables*>(smem + kOffPix);
   uint64_t* w2_full = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  uint64_t* mma_done = w2_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(w2_full + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_x = a.W / kTileW, tiles_y = a.H / kTileH;
@@ -86,25 +86,13 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) { printf("[wvn] pixel_head: smem base not 1024B aligned\n"); __trap(); }
     mbar_init(w2_full, 1);
-    mbar_init(mma_done, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, 32);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = *tmem_slot;
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(w2_full, 4 * 32 * 128);
     for (int kb = 0; kb < 4; ++kb) tma_load_2d(&tmap_w2, w2_full, smem + kOffW2 + kb * 4096, kb * 64, 0);
   }
-
-#ifdef WVN_GEMM_TIMING  // phase cycle counters of thread 0 of CTA 0 (debug builds)
-  long long tph[5] = {0, 0, 0, 0, 0}, tprev = clock64(), ntile = 0;
-#define WVN_PH(i) if (threadIdx.x == 0) { const long long tn = clock64(); tph[i] += tn - tprev; tprev = tn; }
-#else
-#define WVN_PH(i)
-#endif
 
   // Tile geometry: pixel rows [py0, py0+2), pixel columns [px0, px0+64) of frame b; cx0 = first token column of the window.
   struct TileGeo { int b, py0, px0, cx0; };
@@ -121,17 +109,8 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
 
   // ---------------- phase A (warps 4-7, one tile AHEAD of the consumers): vertical blend of the token window
   // (G | U | cT) into gv, the |x|^2 ingredients into n2, and the per-pixel horizontal tables.
-#ifdef WVN_GEMM_TIMING
-  long long pph[4] = {0, 0, 0, 0}, pprev = 0;
-#define WVN_PP0 if (threadIdx.x == 128) pprev = clock64();
-#define WVN_PP(i) if (threadIdx.x == 128) { const long long tn = clock64(); pph[i] += tn - pprev; pprev = tn; }
-#else
-#define WVN_PP0
-#define WVN_PP(i)
-#endif
   auto phase_a = [&](const TileGeo& g) {
     const int t = threadIdx.x - 128;  // 0..127
-    WVN_PP0
     const float* gub = a.gu + (static_cast<long long>(g.b) * (a.frame_rows ? a.frame_rows : P) + a.row0) * a.ldg;
     int y0r[kTileH], y1r[kTileH];
     float wyr[kTileH];
@@ -149,7 +128,6 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
       pt->row1[t] = (y1r[r] * a.gw + tc) * static_cast<int>(a.ldg);
     }
     named_bar_sync(2, 128);
-    WVN_PP(0)
     constexpr int kV4 = kGvStride / 4;
     constexpr int kBatch = 6;  // float4 pairs in flight per thread and pass (48 registers)
     const int n_rc = kTileH * ww;
@@ -181,7 +159,6 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
         }
       }
     }
-    WVN_PP(1)
     if (t < kTileW) {  // per-pixel horizontal source column / weight, first pixel of every window cell
       int x0, xp, xl;
       float wx, wp;
@@ -213,17 +190,13 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
       n2[(r * ww + c) * 2 + 0] = nn;
       n2[(r * ww + c) * 2 + 1] = xx;
     }
-    WVN_PP(2)
   };
 
-  uint32_t mma_phase = 0;
   if (warp >= 4 && blockIdx.x < num_tiles) phase_a(tile_geo(blockIdx.x));
   for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const TileGeo g = tile_geo(tile);
     const int b = g.b, py0 = g.py0, px0 = g.px0, cx0 = g.cx0;
     __syncthreads();  // phase A of this tile is visible; the previous tile's A operand / accumulator are drained
-    tc_fence_after();
-    WVN_PH(0)
 
     // ---------------- phase B (all warps): horizontal blend -> ReLU -> bf16 -> swizzled A tile (h1)
     {
@@ -259,34 +232,30 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    WVN_PH(1)
 
     if (warp >= 4) {
-      // ---------------- layer 2 on the tensor core: D[128, 32] = h1[128, 256] @ W2^T
-      if (warp == 4) {  // whole warp waits, one elected lane issues (see elect_one_sync in common.cuh)
-        mbar_wait(w2_full, 0);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          constexpr uint32_t idesc = make_idesc_bf16(128, kH2);
-#pragma unroll
-          for (int ks = 0; ks < kH1 / 16; ++ks) {
-            const uint64_t da = make_sw128_kmajor_desc(smem_u32(smem + kOffA + (ks >> 2) * 16384)) + 2 * (ks & 3);
-            const uint64_t db = make_sw128_kmajor_desc(smem_u32(smem + kOffW2 + (ks >> 2) * 4096)) + 2 * (ks & 3);
-            umma_bf16_ss(tmem_d, da, db, idesc, ks != 0);
-          }
-          umma_commit(mma_done);
-        }
-      }
-      __syncwarp();
       // ---------------- producers: once the consumers have taken what they need from gv / n2 / the pixel
-      // tables, build the NEXT tile's while the tensor core and the epilogue work on this one
+      // tables, build the NEXT tile's while the tensor core and the epilogue warpgroup work on this one
       named_bar_sync(1, kThreads);
       if (tile + gridDim.x < num_tiles) phase_a(tile_geo(tile + gridDim.x));
     } else {
-      // ---------------- epilogue: one thread per pixel (warps 0-3 <-> TMEM lanes 0-127)
-      const int i = threadIdx.x;  // pixel / TMEM lane
+      // ---------------- layer 2 on the tensor core: D[128, 32] = h1[128, 256] @ W2^T, issued by this warpgroup
+      // (two 64-row halves) and left in flight while each thread prepares its pixel's blend terms
+      float d2[2][16];
+      mbar_wait(w2_full, 0);  // completes once; later tiles pass at once
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < kH1 / 16; ++ks) {
+        const uint64_t db = make_sw128_kmajor_desc(smem_u32(smem + kOffW2 + (ks >> 2) * 4096)) + 2 * (ks & 3);
+#pragma unroll
+        for (int half = 0; half < 2; ++half)
+          wgmma_m64n32k16_ss(d2[half], make_sw128_kmajor_desc(smem_u32(smem + kOffA + (ks >> 2) * 16384 + half * 8192)) + 2 * (ks & 3),
+                             db, ks != 0);
+      }
+      wgmma_commit();
+      // ---------------- epilogue: one thread per pixel
+      const int i = threadIdx.x;  // pixel
       const int r = i >> 6, px = i & 63;
       const float wx = pt->wx[px];
       const int c0 = pt->c0[px];
@@ -310,15 +279,30 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
       const float gram = ux * ux * nn[0] + 2.f * ux * wx * xx + wx * wx * n_c1;
       asm volatile("bar.arrive 1, %0;" ::"n"(kThreads) : "memory");  // gv / n2 / tables consumed: producers may refill
 
-      mbar_wait(mma_done, mma_phase);
-      tc_fence_after();
-      WVN_PH(2)
-      uint32_t raw[32];
-      tmem_ld32(tmem_d + (static_cast<uint32_t>(warp * 32) << 16), raw);
-      tmem_ld_wait();
+      wgmma_wait<0>();
+      wgmma_fence_regs(d2[0]);
+      wgmma_fence_regs(d2[1]);
+      // fragments -> one pixel per thread, through the h1 tile once every warp's MMAs have consumed it
+      named_bar_sync(3, 128);
+      float* h2s = reinterpret_cast<float*>(smem + kOffA);
+#pragma unroll
+      for (int half = 0; half < 2; ++half)
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+            *reinterpret_cast<float2*>(h2s + (half * 64 + warp * 16 + (lane >> 2) + 8 * hh) * kH2Stride + 8 * j + 2 * (lane & 3)) =
+                make_float2(d2[half][4 * j + 2 * hh], d2[half][4 * j + 2 * hh + 1]);
+      named_bar_sync(3, 128);
       float h2[kH2];
 #pragma unroll
-      for (int j = 0; j < kH2; ++j) h2[j] = fmaxf(__uint_as_float(raw[j]) + c_ph.b2[j], 0.f);
+      for (int j4 = 0; j4 < kH2 / 4; ++j4) {
+        const float4 raw = reinterpret_cast<const float4*>(h2s + i * kH2Stride)[j4];
+        h2[4 * j4 + 0] = fmaxf(raw.x + c_ph.b2[4 * j4 + 0], 0.f);
+        h2[4 * j4 + 1] = fmaxf(raw.y + c_ph.b2[4 * j4 + 1], 0.f);
+        h2[4 * j4 + 2] = fmaxf(raw.z + c_ph.b2[4 * j4 + 2], 0.f);
+        h2[4 * j4 + 3] = fmaxf(raw.w + c_ph.b2[4 * j4 + 3], 0.f);
+      }
       // traversability logit, |r|^2 quadratic form (upper-triangular M with doubled off-diagonals), r.x
       float t = c_ph.b0, q = c_ph.cc, cross = ub[kH2] + ub[kH2 + 1];
 #pragma unroll
@@ -339,29 +323,7 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
       a.trav[o] = 1.f / (1.f + __expf(-t));
       a.conf[o] = 1.f - (xc - lo) / (hi - lo);
       if (a.loss_reco != nullptr) a.loss_reco[o] = loss;
-      tc_fence_before();
-      WVN_PH(3)
     }
-    mma_phase ^= 1;
-#ifdef WVN_GEMM_TIMING
-    ++ntile;
-#endif
-  }
-#ifdef WVN_GEMM_TIMING
-  if (blockIdx.x == 0 && threadIdx.x == 0 && a.timing != nullptr) {
-    for (int i = 0; i < 5; ++i) a.timing[i] = tph[i];
-    a.timing[5] = ntile;
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 128 && a.timing != nullptr)
-    for (int i = 0; i < 3; ++i) a.timing[8 + i] = pph[i];
-#endif
-#undef WVN_PH
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_d, 32);
   }
 }
 
@@ -405,7 +367,7 @@ token_gram_kernel(const __nv_bfloat16* __restrict__ tok, float* __restrict__ gra
 // to match the U = tokens @ R columns the tensor core produces from bf16 operands).
 // One block of 32 x 32 threads: thread (j, k) owns M[j][k]; row 0 also produces tv / b2 / w0.  R (bf16-rounded) and c
 // are staged in shared memory in chunks of 384 channels and every thread runs four independent accumulators over the
-// chunk (the first version walked the 384 channels with two dependent global loads each: 58 us per step).
+// chunk (instead of walking the 384 channels with two dependent global loads each).
 __global__ void __launch_bounds__(1024)
 pixel_head_consts_kernel(const float* __restrict__ p, MlpOffsets o, int dim, PixelHeadConsts* out) {
   constexpr int kChunk = 384;

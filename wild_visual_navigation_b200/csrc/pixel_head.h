@@ -37,7 +37,6 @@ struct PixelHeadArgs {
   int feat = 0;                  // D
   long long frame_rows = 0;      // rows of gu / gram between two frames (0 = gh*gw): the ViT's own token buffer keeps
   int row0 = 0;                  // npad rows per frame with the patch tokens starting at row 1
-  long long* timing = nullptr;   // debug (-DWVN_GEMM_TIMING builds): phase cycle counters of CTA 0
 };
 
 // Returns the token-window width if the fused kernel supports this geometry, else 0.

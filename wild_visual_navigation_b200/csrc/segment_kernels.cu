@@ -1,4 +1,4 @@
-// wvn-b200: per-segment reductions over a segmentation map (sm_100a, HBM/L2-bound integer work).
+// wvn-b200: per-segment reductions over a segmentation map (sm_90a, HBM/L2-bound integer work).
 //
 // Replaces three Python per-segment loops of the reference, each of which costs one host
 // sync per segment:
@@ -371,7 +371,7 @@ adjacency_emit_kernel(const unsigned int* __restrict__ adj, long long* __restric
 
 // ---- relabel: compact the set of labels present in a frame to 0..S-1 (sorted order)
 // grid = (slices per frame, batch): the labels a block meets are collected in a shared-memory flag array first — letting
-// every pixel store its flag to global memory made 6.4 M stores hit ~640 addresses (75 us per 32 frames)
+// every pixel store its flag to global memory would make millions of stores hit a few hundred addresses
 __global__ void __launch_bounds__(256)
 label_presence_kernel(const long long* __restrict__ seg, int* __restrict__ present, long long pix_per_frame, int num_labels) {
   extern __shared__ int flags[];

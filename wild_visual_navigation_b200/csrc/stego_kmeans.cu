@@ -11,21 +11,20 @@
 // in the head buffer's cluster-logit columns and the existing upsample+argmax kernel (dense_kernels.cu) produces the
 // pixel labels — the (H, W, 90) tensor is never formed.
 //
-// ONE launch runs all iterations for the whole batch: a TEAM of 9 CTAs owns a frame (9 x 349 of the 3136 patches at
-// 448 px), so a batch of 32 frames fills the GPU instead of 32 SMs (16 teams = 144 of 148 SMs: two full rounds).  The team synchronises once per iteration through a
-// per-frame arrival counter in global memory (release / acquire); the partial sums travel through global memory anyway.
-// Round 2 first used hardware thread-block clusters for the team: a cluster of 8 one-CTA-per-SM blocks must sit inside one
-// GPC and fits only 15 times on a B200 (120 of 148 SMs), so 32 frames took THREE rounds with the last almost empty
-// (750 us); free CTAs of 9 fit 16 teams at a time: two full rounds (445 us).  CTAs are dispatched in block order, so a team split by the
-// residency boundary only waits for earlier teams to retire (no circular wait); the spin is bounded and traps.
+// ONE launch runs all iterations for the whole batch: a TEAM of 8 CTAs owns a frame (8 x 392 of the 3136 patches at
+// 448 px), so a batch of 32 frames fills the GPU instead of 32 SMs (16 teams = 128 of the H100's 132 SMs: two full
+// rounds).  The team synchronises once per iteration through a per-frame arrival counter in global memory (release /
+// acquire); the partial sums travel through global memory anyway.  Free CTAs rather than hardware thread-block
+// clusters: a cluster has to sit inside one GPC, which leaves SMs unused.  CTAs are dispatched in block order, so a team
+// split by the residency boundary only waits for earlier teams to retire (no circular wait); the spin is bounded and traps.
 // The CTA's code rows are staged in
 // shared memory ONCE (coalesced; the first version re-read them from L2 every pass with one row per lane — with the
-// shared-memory carve-out at its maximum there is no L1 left, and those 32-sector requests made the kernel 1.4 ms).
+// shared-memory carve-out at its maximum there is no L1 left, and every such request touches 32 sectors).
 // Per iteration and CTA:
 //   1. one thread = one patch: the 90-d code row sits in registers, the K centroids are read as float4 broadcasts from
 //      shared memory; nearest centroid -> assign[] (shared)
 //   2. one warp = one patch at a time (lane = channel): the row is added to a WARP-PRIVATE copy of the K x C sums — no
-//      atomics (shared-memory float atomics are CAS loops on sm_100, and large clusters are hot spots), deterministic
+//      atomics (large clusters are hot spots for shared-memory atomics), deterministic
 //   3. the warp copies are summed, the CTA's partial sums go to global memory; after one team barrier
 //      (release / acquire) every CTA adds the team's partials in the same order and updates its own copy of the centroids.
 #include "common.cuh"
@@ -38,10 +37,10 @@ namespace {
 
 constexpr int kThreads = 512;
 constexpr int kWarps = kThreads / 32;
-constexpr int kTeam = 9;       // CTAs per frame at large batches: 16 teams = 144 SMs, 32 frames = 2 full rounds
+constexpr int kTeam = 8;       // CTAs per frame at large batches: 16 teams = 128 SMs, 32 frames = 2 full rounds
 constexpr int kMaxTeam = 32;   // small batches (the one-camera deployment case) spread a frame over more CTAs
 
-// CTAs per frame: as many as keep every team resident in ONE round (148 SMs, one CTA each), between kTeam and kMaxTeam.
+// CTAs per frame: as many as keep every team resident in ONE round (132 SMs, one CTA each), between kTeam and kMaxTeam.
 inline int team_size(int batch) {
   const int fit = sm_count() / (batch > 0 ? batch : 1);
   return fit < kTeam ? kTeam : (fit > kMaxTeam ? kMaxTeam : fit);
@@ -74,9 +73,7 @@ constexpr int kMaxC = 128;   // code_dim <= 128 (row registers: 128)
 // CREG: code_dim rounded up (centroid rows and the per-thread code row are padded to it with zeros, so the score loop
 // has no bounds checks); ROWS_SMEM: the CTA's code rows are staged in shared memory.  Shared-memory operands of the hot
 // loops are addressed through explicit 32-bit shared addresses (lds128 / plain typed pointers that never mix with
-// global ones): with a pointer that could be either space the compiler falls back to generic loads, and in a cluster
-// launch every such access re-derives the shared window from SR_CgaCtaId — measured 51k clk per iteration for the
-// 392-patch score loop instead of ~9k.
+// global ones): with a pointer that could be either space the compiler falls back to generic loads.
 template <int CREG, bool ROWS_SMEM>
 __global__ void __launch_bounds__(kThreads, 1)
 stego_kmeans_kernel(float* __restrict__ rows, KmeansArgs a, float* __restrict__ partial) {
@@ -117,13 +114,6 @@ stego_kmeans_kernel(float* __restrict__ rows, KmeansArgs a, float* __restrict__ 
   }
   __syncthreads();
 
-#ifdef WVN_GEMM_TIMING  // phase cycle counters of thread 0 of CTA 0 (timing builds; printed by the host wrapper)
-  long long tph[6] = {0, 0, 0, 0, 0, 0}, tprev = clock64();
-#define WVN_KT(i) if (blockIdx.x == 0 && t == 0) { const long long tn = clock64(); tph[i] += tn - tprev; tprev = tn; }
-#else
-#define WVN_KT(i)
-#endif
-  WVN_KT(0)
   for (int it = 0; it <= a.iters; ++it) {
     const bool last = it == a.iters;  // the last pass only writes the scores of the final centroids
     for (int k = warp; k < K; k += kWarps) {  // |c_k|^2 / 2: one warp per centroid
@@ -138,7 +128,6 @@ stego_kmeans_kernel(float* __restrict__ rows, KmeansArgs a, float* __restrict__ 
       for (int i = t; i < n_priv * K; i += kThreads) cnt_priv[i] = 0.f;
     }
     __syncthreads();
-    WVN_KT(1)
     // ---- 1. nearest centroid per patch (one thread = one patch, row in registers)
     for (int p = p0 + t; p < p1; p += kThreads) {
       float x[CREG];
@@ -184,7 +173,6 @@ stego_kmeans_kernel(float* __restrict__ rows, KmeansArgs a, float* __restrict__ 
     }
     if (last) break;
     __syncthreads();
-    WVN_KT(2)
     // ---- 2. warp-private sums: warp w < n_priv adds the rows of patches p0 + w, p0 + w + n_priv, ...
     if (warp < n_priv) {
       float* sp = sum_priv + warp * K * CP;
@@ -219,7 +207,6 @@ stego_kmeans_kernel(float* __restrict__ rows, KmeansArgs a, float* __restrict__ 
       }
     }
     __syncthreads();
-    WVN_KT(3)
     // ---- 3. CTA partial -> global; team barrier; every CTA sums the team's partials in rank order
     float* mine = part_frame + ((it & 1) * T + rank) * (K * CP + K);
     for (int i = t; i < K * CP + K; i += kThreads) {
@@ -231,9 +218,7 @@ stego_kmeans_kernel(float* __restrict__ rows, KmeansArgs a, float* __restrict__ 
       }
       mine[i] = sacc;
     }
-    WVN_KT(4)
     team_barrier(a.frame_bar + frame, static_cast<unsigned int>(T) * (it + 1));
-    WVN_KT(5)
     const float* all = part_frame + (it & 1) * T * (K * CP + K);
     for (int k = warp; k < K; k += kWarps) {  // one warp per centroid
       float n = 0.f;
@@ -247,13 +232,7 @@ stego_kmeans_kernel(float* __restrict__ rows, KmeansArgs a, float* __restrict__ 
       }
     }
     __syncthreads();
-    WVN_KT(0)
   }
-#ifdef WVN_GEMM_TIMING
-  if (blockIdx.x == 0 && t == 0 && a.timing != nullptr)
-    for (int i = 0; i < 6; ++i) a.timing[i] = tph[i];
-#endif
-#undef WVN_KT
   if (a.centroids_out && rank == 0) {
     __syncthreads();
     for (int i = t; i < K * C; i += kThreads) {
@@ -301,22 +280,8 @@ int stego_kmeans(float* rows, const KmeansArgs& a_in, float* workspace, cudaStre
   const size_t part_floats = static_cast<size_t>(a.batch) * 2 * a.team * (static_cast<size_t>(a.k) * CP + a.k);
   a.frame_bar = reinterpret_cast<unsigned int*>(workspace + ((part_floats + 3) & ~static_cast<size_t>(3)));
   WVN_CHECK_CUDA(cudaMemsetAsync(a.frame_bar, 0, sizeof(unsigned int) * a.batch, stream));
-#ifdef WVN_GEMM_TIMING
-  static long long* tbuf = nullptr;
-  if (!tbuf) cudaMalloc(&tbuf, 8 * sizeof(long long));
-  a.timing = tbuf;
-#endif
   kern<<<a.batch * a.team, kThreads, smem, stream>>>(rows, a, workspace);
   WVN_CHECK_LAUNCH("stego_kmeans_kernel");
-#ifdef WVN_GEMM_TIMING
-  {
-    long long tt[6];
-    cudaMemcpyAsync(tt, tbuf, sizeof(tt), cudaMemcpyDeviceToHost, stream);
-    cudaStreamSynchronize(stream);
-    fprintf(stderr, "[kmeans timing, cycles of CTA 0 over %d iterations] update+sync/init %lld  zero+norm %lld  assign %lld  accumulate %lld  "
-            "reduce+store %lld  cluster_barrier %lld\n", a.iters, tt[0], tt[1], tt[2], tt[3], tt[4], tt[5]);
-  }
-#endif
   return WVN_OK;
 }
 

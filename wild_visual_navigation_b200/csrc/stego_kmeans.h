@@ -15,7 +15,6 @@ struct KmeansArgs {
   int k = 0, iters = 0;
   float* centroids_out = nullptr;   // optional [batch, k, code_dim]
   int n_priv = 0;                   // set by stego_kmeans(): warp-private sum copies per CTA
-  long long* timing = nullptr;      // debug (-DWVN_GEMM_TIMING builds): phase cycle counters of CTA 0
   int rows_in_smem = 0;             // set by stego_kmeans(): the CTA's code rows are staged in shared memory
   unsigned int* frame_bar = nullptr;  // set by stego_kmeans(): [batch] arrival counters of the per-frame barrier
   int team = 0;                       // set by stego_kmeans(): CTAs per frame

@@ -1,4 +1,4 @@
-// wvn-b200: memory-bound helper kernels of the ViT forward pass (sm_100a).
+// wvn-b200: memory-bound helper kernels of the ViT forward pass (sm_90a).
 //
 //   image_to_patches   : NEAREST resize + center crop + ImageNet normalisation + im2col -> bf16
 //                        (reference: dino_interface.py:52-59,81 transform, then the DINO
@@ -140,7 +140,7 @@ layernorm_rows_kernel(const float* __restrict__ x, const float* __restrict__ gam
 // ---- parity-debug attention (SURVEY.md §7 "an fp32 mode kept for debugging parity"; $WVN_VIT_PRECISE=1) ----------------
 // softmax(q k^T * scale) v in fp32 CUDA-core arithmetic on the fp32 QKV projections: no bf16 rounding of q, k, v, of the
 // scores or of P.  One thread = one query row (q and the output accumulator in registers), K / V tiles of 64 keys staged
-// in shared memory, online softmax per 16-key chunk.  ~40x slower than the tcgen05 kernel; it exists to separate
+// in shared memory, online softmax per 16-key chunk.  ~40x slower than the wgmma kernel; it exists to separate
 // "kernel bug" from "bf16 rounding of peaked attention logits" (tests/test_path_gpu.py::test_vit_base_default_std...).
 __global__ void __launch_bounds__(128)
 attention_f32_debug_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restrict__ out, int npad, int n_valid, int heads,

@@ -2,7 +2,7 @@
 
 Same constructor arguments, ``inference`` / ``change_device`` and properties.  The transform
 (``Resize(input_size, NEAREST) + CenterCrop + Normalize``, :52-59) is folded into the patch
-loader kernel, the backbone is the tcgen05 ViT (csrc/), and the bilinear ``align_corners=True``
+loader kernel, the backbone is the wgmma ViT (csrc/), and the bilinear ``align_corners=True``
 upsampling to ``(H, H)`` (:87-90) is only materialised by ``inference`` because its contract
 returns the dense tensor; fused consumers call ``inference_tokens`` instead.
 """
@@ -35,9 +35,9 @@ class DinoInterface:
                              patch_size=patch_size, projection_type=projection_type, dropout_p=dropout_p,
                              pretrained_weights=pretrained_weights)
         if self._cfg.backbone not in ("dino",):
-            raise ValueError(f"backbone '{self._cfg.backbone}' is outside the B200 hot path (DINO ViT only)")
+            raise ValueError(f"backbone '{self._cfg.backbone}' is outside the H100 hot path (DINO ViT only)")
         if not str(device).startswith("cuda"):
-            raise RuntimeError("wild_visual_navigation_b200 runs on CUDA (sm_100a) devices only — no CPU fallback")
+            raise RuntimeError("wild_visual_navigation_b200 runs on CUDA (sm_90a) devices only — no CPU fallback")
         self._device = device
         shp = VIT_SHAPES[self._cfg.backbone_type]
         sd = state_dict if state_dict is not None else load_dino_state_dict(

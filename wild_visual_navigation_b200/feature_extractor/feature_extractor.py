@@ -46,7 +46,7 @@ class FeatureExtractor:
             # the reference hard-codes 384 for every dino variant (feature_extractor.py:56)
             self._feature_dim = 384 if common["backbone_type"] == "vit_small" else 768
         else:
-            raise ValueError(f"Extractor[{feature_type}] is outside the B200 hot path")
+            raise ValueError(f"Extractor[{feature_type}] is outside the H100 hot path")
         if need_stego:
             self._stego = StegoInterface(device=device, input_size=input_size, run_crf=kwargs.get("run_crf", False),
                                          run_clustering=kwargs.get("run_clustering", True),  # the reference's default (:51)

@@ -1,7 +1,7 @@
 """StegoInterface (reference: wild_visual_navigation/feature_extractor/stego_interface.py:19-135).
 
 ``inference(img) -> (linear_pred, cluster_pred)`` with the ``features`` / ``cluster_segments`` /
-``linear_segments`` properties.  The STEGO head runs as three tcgen05 GEMMs on the ViT tokens
+``linear_segments`` properties.  The STEGO head runs as three wgmma GEMMs on the ViT tokens
 (csrc/api.cu: wvn_vit_stego_head); the cluster / linear probes are folded into the head's output
 columns (weights.fold_stego_head) and evaluated at patch resolution, then one kernel does the
 bilinear(align_corners=False) upsampling + argmax per pixel — algebraically the upstream
@@ -28,7 +28,7 @@ class StegoInterface:
         self._cfg = _Cfg(cfg) if cfg else _Cfg(model_path=model_path, input_size=input_size, run_crf=run_crf,
                                                run_clustering=run_clustering, n_image_clusters=n_image_clusters)
         if self._cfg.run_crf:
-            raise ValueError("run_crf (pydensecrf on the CPU) is outside the B200 hot path; WVN itself runs with "
+            raise ValueError("run_crf (pydensecrf on the CPU) is outside the H100 hot path; WVN itself runs with "
                              "run_crf=False (feature_extractor.py:52)")
         self._kmeans_iters = kmeans_iters
         self._device = device

@@ -7,7 +7,7 @@
     out_trav = prediction.reshape(H,W,-1)[:,:,0]
     loss_reco = mse(prediction[:,1:], x).mean(1);  confidence = cg.inference_without_update(loss_reco)
 
-fused as: ViT tokens -> (bilinear sample -> 3 tcgen05 GEMMs -> sigmoid / reco-loss / confidence
+fused as: ViT tokens -> (bilinear sample -> 3 wgmma GEMMs -> sigmoid / reco-loss / confidence
 epilogue) per pixel; neither ``dense_feat`` (308 MB/frame) nor the (P, 385) prediction is stored.
 """
 from __future__ import annotations

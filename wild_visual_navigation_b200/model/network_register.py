@@ -11,4 +11,4 @@ def get_model(model_cfg):
         cfg = get("simple_mlp_cfg")
         cfg = dict(cfg) if isinstance(cfg, dict) else dict(vars(cfg))
         return SimpleMLP(**cfg)
-    raise ValueError(f"model '{name}' is outside the B200 hot path (only SimpleMLP; SURVEY.md §2)")
+    raise ValueError(f"model '{name}' is outside the H100 hot path (only SimpleMLP; SURVEY.md §2)")

@@ -78,7 +78,7 @@ class TraversabilityEstimator:
                  mode=None, extraction_store_folder=None, anomaly_detection: bool = False, process_group=None,
                  max_rows: int = 4096):
         if anomaly_detection:
-            raise ValueError("anomaly_detection (LinearRnvp) is outside the B200 hot path")
+            raise ValueError("anomaly_detection (LinearRnvp) is outside the H100 hot path")
         self._device = device
         self._mode = mode
         self._extraction_store_folder = extraction_store_folder

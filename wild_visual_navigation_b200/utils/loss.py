@@ -19,7 +19,7 @@ class TraversabilityLoss(nn.Module):
                  trav_cross_entropy=False):
         super().__init__()
         if trav_cross_entropy:
-            raise ValueError("trav_cross_entropy is not supported on the B200 hot path (reference default: False)")
+            raise ValueError("trav_cross_entropy is not supported on the H100 hot path (reference default: False)")
         self._w_trav, self._w_reco, self._w_temp = w_trav, w_reco, w_temp
         # registered as a sub-module exactly as the reference does (loss.py:74: ``self._model = model``), so that
         # ``traversability_loss_state_dict`` carries ``_model.layers.{0,2,4}.{weight,bias}`` next to
