@@ -1,6 +1,7 @@
-"""Micro-benchmark of the fused attention kernel alone (ViT-S/8 @448 shapes):
-`python scripts/bench_attention.py`.  Prints accuracy vs fp32 torch and TFLOP/s (algorithmic 4*N^2*64 per
-(frame, head))."""
+"""Micro-benchmark of the fused attention kernel alone: `python scripts/bench_attention.py`.  The shape comes from
+the environment: B frames (default 8), H heads (default 6) and N tokens (default 3137), so the defaults are ViT-S/8
+@448 and `B=128 H=12 N=4097` is the c5 shape (ViT-B/8, 64x64 tokens).  Prints accuracy vs fp32 torch and TFLOP/s
+(algorithmic 4*N^2*64 per (frame, head))."""
 import os
 import sys
 
@@ -9,7 +10,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from wild_visual_navigation_b200 import ops  # noqa: E402
 
-B, H, N = int(os.environ.get("B", 8)), 6, 3137
+B, H, N = int(os.environ.get("B", 8)), int(os.environ.get("H", 6)), int(os.environ.get("N", 3137))
 npad = (N + 127) // 128 * 128
 g = torch.Generator(device="cuda").manual_seed(0)
 S = float(os.environ.get("QK_STD", 1.2))   # std of q and k: the logits have std S^2 (1.2: bland; 1.8: the bench ViT's spread)
@@ -36,4 +37,4 @@ e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / iters
 tf = 4.0 * N * N * 64 * B * H / (ms * 1e-3) / 1e12
-print(f"B={B} ms={ms:.3f} TFLOP/s={tf:.1f} rel_l2={rel:.2e}")
+print(f"B={B} H={H} N={N} ms={ms:.3f} TFLOP/s={tf:.1f} rel_l2={rel:.2e}")

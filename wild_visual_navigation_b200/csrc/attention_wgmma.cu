@@ -15,9 +15,10 @@
 //                    warpgroup gives its registers up (setmaxnreg) to the consumers
 //   warpgroups 1-2 : 64 query rows each.  Per KV tile: S = Q K^T (4 x wgmma m64n128k16, operands in shared memory),
 //                    online softmax on the fragments (a row lives in the 4 lanes of a quad: 2 shuffles per reduction),
-//                    O += P V (8 x wgmma m64n64k16 with P in registers).  P·V of tile j stays in flight while
-//                    Q·K^T of tile j+1 is issued, and the two warpgroups run out of phase, so the tensor core works
-//                    on one while the other is in its softmax.
+//                    O += P V (8 x wgmma m64n64k16 with P in registers).  Q·K^T of tile j and P·V of tile j-1 are
+//                    issued together; softmax(j) runs while P·V(j-1) is still on the tensor core, and only the O
+//                    rescale and the packing of P wait for it.  The two warpgroups take turns to issue (named
+//                    barriers), so the tensor core works on one warpgroup's MMAs while the other is in its softmax.
 // The padded last KV tile runs a separate, masked instantiation of the softmax, which keeps the other tiles free of
 // mask arithmetic.
 #include <stdlib.h>
@@ -57,11 +58,12 @@ __device__ __forceinline__ float quad_max(float v) {
 }
 
 // One KV tile of the online softmax on a 64 x 128 score fragment: s[4 j + 2 h + e] is the score of query row h
-// (of this thread's two) and key 8 j + 2 q + e.  Rescales o and l, leaves P (bf16 pairs, register-operand layout of
-// the 8 k-steps of P·V) in p.  MASKED handles the padded last tile (keys >= valid are excluded).
+// (of this thread's two) and key 8 j + 2 q + e.  Updates m and l, replaces the scores by their exponentials in place
+// and returns the rescale factor of O in alpha.  It touches neither O nor P, so it runs while P·V of the previous
+// tile is still reading P and writing O.  MASKED handles the padded last tile (keys >= valid are excluded).
 template <bool MASKED>
-__device__ __forceinline__ void softmax_tile(float (&s)[64], float (&o)[32], uint32_t (&p)[32], float (&m)[2], float (&l)[2],
-                                             const float sl2, const int valid, const int q) {
+__device__ __forceinline__ void softmax_scores(float (&s)[64], float (&m)[2], float (&l)[2], float (&alpha)[2],
+                                               const float sl2, const int valid, const int q) {
   if (MASKED) {
 #pragma unroll
     for (int j = 0; j < 16; ++j)
@@ -69,7 +71,7 @@ __device__ __forceinline__ void softmax_tile(float (&s)[64], float (&o)[32], uin
       for (int e = 0; e < 2; ++e)
         if (8 * j + 2 * q + e >= valid) s[4 * j + e] = s[4 * j + 2 + e] = -INFINITY;
   }
-  float neg_m[2], alpha[2];
+  float neg_m[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float mx = s[2 * h];
@@ -88,12 +90,17 @@ __device__ __forceinline__ void softmax_tile(float (&s)[64], float (&o)[32], uin
       const float e0 = fast_exp2(fmaf(s[4 * j + 2 * h], sl2, neg_m[h]));
       const float e1 = fast_exp2(fmaf(s[4 * j + 2 * h + 1], sl2, neg_m[h]));
       sum[h] += e0 + e1;
-      // k-step j / 2 of P·V: registers {row g | row g + 8} x {keys 2q.. | keys 2q + 8..}
-      p[4 * (j >> 1) + 2 * (j & 1) + h] = pack_bf16x2(e0, e1);
+      s[4 * j + 2 * h] = e0;
+      s[4 * j + 2 * h + 1] = e1;
     }
   }
 #pragma unroll
   for (int h = 0; h < 2; ++h) l[h] = fmaf(l[h], alpha[h], sum[h]);   // per-thread partial; the quad is summed at the end
+}
+
+// Once P·V of the previous tile has retired: O *= alpha, and the exponentials in s become P (bf16 pairs in the
+// register-operand layout of the 8 k-steps of P·V).
+__device__ __forceinline__ void rescale_o(float (&o)[32], const float (&alpha)[2]) {
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     o[4 * j + 0] *= alpha[0];
@@ -101,6 +108,14 @@ __device__ __forceinline__ void softmax_tile(float (&s)[64], float (&o)[32], uin
     o[4 * j + 2] *= alpha[1];
     o[4 * j + 3] *= alpha[1];
   }
+}
+
+__device__ __forceinline__ void pack_p(const float (&s)[64], uint32_t (&p)[32]) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)  // k-step j / 2 of P·V: registers {row g | row g + 8} x {keys 2q.. | keys 2q + 8..}
+      p[4 * (j >> 1) + 2 * (j & 1) + h] = pack_bf16x2(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]);
 }
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -165,40 +180,77 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     float s[64], o[32];
     uint32_t p[32];
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+
+    float alpha[2];
 
     mbar_wait(q_full, 0);
     const uint64_t desc_q = make_sw128_kmajor_desc(smem_u32(smem + kOffQ + wg * 64 * 128));
-    int stage = 0, prev_stage = 0;
-    uint32_t phase = 0;
-    for (int j = 0; j < num_kv; ++j) {
-      mbar_wait(&kv_full[stage], phase);
-      const uint64_t desc_k = make_sw128_kmajor_desc(smem_u32(smem + kOffK + stage * kKBytes));
-      wgmma_fence_regs(s);
-      wgmma_fence();
+    auto issue_qk = [&](int st) {  // S = Q K^T of the tile in ring slot st
+      const uint64_t desc_k = make_sw128_kmajor_desc(smem_u32(smem + kOffK + st * kKBytes));
 #pragma unroll
       for (int k = 0; k < kDh / 16; ++k) wgmma_m64n128k16_ss(s, desc_q + 2 * k, desc_k + 2 * k, k != 0 ? 1u : 0u);
       wgmma_commit();
-      wgmma_wait<0>();  // S(j) is complete, and with it P·V(j-1): that tile's ring slot is free
-      wgmma_fence_regs(s);
-      wgmma_fence_regs(o);
-      if (j > 0 && lane == 0) mbar_arrive(&kv_empty[prev_stage]);
-
-      if (j == num_kv - 1) softmax_tile<true>(s, o, p, m, l, sl2, args.n_valid - j * kTileKV, q);
-      else softmax_tile<false>(s, o, p, m, l, sl2, kTileKV, q);
-
-      const uint32_t v_addr = smem_u32(smem + kOffV + stage * kVBytes);
-      wgmma_fence_regs(o);
-      wgmma_fence();
+    };
+    auto issue_pv = [&](int st, bool accumulate) {  // O (+)= P V of the tile in ring slot st
+      const uint32_t v_addr = smem_u32(smem + kOffV + st * kVBytes);
 #pragma unroll
       for (int k = 0; k < kTileKV / 16; ++k)
         wgmma_m64n64k16_rs(o, p[4 * k], p[4 * k + 1], p[4 * k + 2], p[4 * k + 3],
-                           make_sw128_kmajor_desc(v_addr + (k >> 2) * (kVBytes / 2)) + 2 * (k & 3), 1u);
+                           make_sw128_kmajor_desc(v_addr + (k >> 2) * (kVBytes / 2)) + 2 * (k & 3),
+                           (accumulate || k != 0) ? 1u : 0u);
       wgmma_commit();
-      prev_stage = stage;
+    };
+    // Warpgroup ping-pong: named barrier 1 + wg means "warpgroup wg may issue".  Each warpgroup issues its MMAs of
+    // one step and then hands the turn over, so one warpgroup's softmax runs under the other's MMAs.  Both take
+    // num_kv + 1 turns; warpgroup 1 opens with a pass to warpgroup 0 and drops its final pass, which keeps both
+    // barriers balanced.
+    auto take_turn = [&]() { named_bar_sync(1 + wg, 256); };
+    auto pass_turn = [&](bool last) { if (!(last && wg == 1)) named_bar_arrive(2 - wg, 256); };
+    if (wg == 1) named_bar_arrive(1, 256);
+
+    // Tile 0: S(0), softmax(0).  O is not rescaled (the first P·V overwrites it).
+    mbar_wait(&kv_full[0], 0);
+    take_turn();
+    wgmma_fence_regs(s);
+    wgmma_fence();
+    issue_qk(0);
+    pass_turn(false);
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    if (num_kv == 1) softmax_scores<true>(s, m, l, alpha, sl2, args.n_valid, q);
+    else softmax_scores<false>(s, m, l, alpha, sl2, kTileKV, q);
+    pack_p(s, p);
+
+    // Tile j: S(j) and P·V(j-1) are issued together; softmax(j) runs while P·V(j-1) is on the tensor core.
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int j = 1; j < num_kv; ++j) {
+      const int prev_stage = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
+      mbar_wait(&kv_full[stage], phase);
+      take_turn();
+      wgmma_fence_regs(s);
+      wgmma_fence_regs(o);
+      wgmma_fence();
+      issue_qk(stage);
+      issue_pv(prev_stage, j > 1);
+      pass_turn(false);
+      wgmma_wait<1>();  // S(j) is complete; P·V(j-1) may still run
+      wgmma_fence_regs(s);
+      if (j == num_kv - 1) softmax_scores<true>(s, m, l, alpha, sl2, args.n_valid - j * kTileKV, q);
+      else softmax_scores<false>(s, m, l, alpha, sl2, kTileKV, q);
+      wgmma_wait<0>();  // P·V(j-1) is complete: O and P may be rewritten, and tile j-1's ring slot is free
+      wgmma_fence_regs(o);
+      wgmma_fence_regs(p);
+      if (lane == 0) mbar_arrive(&kv_empty[prev_stage]);
+      rescale_o(o, alpha);
+      pack_p(s, p);
     }
+    take_turn();
+    wgmma_fence_regs(o);
+    wgmma_fence();
+    issue_pv(stage, num_kv > 1);
+    pass_turn(true);
     wgmma_wait<0>();
     wgmma_fence_regs(o);
 

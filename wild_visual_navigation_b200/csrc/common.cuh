@@ -135,14 +135,19 @@ __device__ __forceinline__ bool mbar_try_wait_many(uint32_t bar_addr, uint32_t p
   return ok != 0;
 }
 
+// The timeout prints which barrier hung only in a build with -DWVN_MBAR_DIAG: a call (printf is one, to vprintf)
+// anywhere in a kernel that issues wgmma makes ptxas serialise every wgmma.mma_async of that kernel (C7510), even
+// when the call is never executed.  The default build traps without printing.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const uint32_t addr = smem_u32(bar);
   const long long t0 = clock64();
   while (!mbar_try_wait_many(addr, parity)) {
     if (clock64() - t0 > WVN_MBAR_TIMEOUT_CYCLES) {
+#ifdef WVN_MBAR_DIAG
       printf("[wvn] mbarrier timeout: block (%d,%d) thread %d bar@%u parity %u\n", blockIdx.x, blockIdx.y,
              threadIdx.x, addr, parity);
+#endif
       __trap();
     }
   }
@@ -253,6 +258,12 @@ template <int N>
 __device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Same for register A operands: keeps them live (unmodified) until after the wait that retires the MMA reading them.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(uint32_t (&a)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 // Register budget of the calling warpgroup (all four warps execute it): producers give registers up, consumers take them.
