@@ -185,17 +185,18 @@ __device__ __forceinline__ void tma_load_2d_mcast(const CUtensorMap* map, uint64
       : "memory");
 }
 
-// TMA store / reduce-add of a shared-memory tile into a 2D global tensor (bulk async-group completion).
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int32_t c0, int32_t c1) {
+// TMA store / reduce-add of a shared-memory tile (shared-space address, as from smem_u32) into a 2D global tensor
+// (bulk async-group completion).
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t smem_src, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               "r"(smem_src), "r"(c0), "r"(c1)
                : "memory");
 }
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, const void* smem_src, int32_t c0, int32_t c1) {
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, uint32_t smem_src, int32_t c0, int32_t c1) {
   asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               "r"(smem_src), "r"(c0), "r"(c1)
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -359,6 +360,15 @@ __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
 // back to generic LD/ST when the pointer provenance is opaque.
 __device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ void sts64(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
+}
+__device__ __forceinline__ void sts16(uint32_t addr, __nv_bfloat16 a) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(addr), "h"(__bfloat16_as_ushort(a)) : "memory");
 }
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   uint4 v;
