@@ -64,6 +64,44 @@ int wvn_profile_collect(float* host_ms, long long* host_launches);
 int wvn_gemm_bf16(const void* a_bf16, long long lda, const void* w_bf16, const float* bias, void* out, long long ldo,
                   int m, int n, int k, int out_kind, int act, int block_n, void* stream);
 
+/* Testing and diagnostics entry: runs the same GEMM with any of its fused epilogues, including the three the
+ * handles use internally (patch-embed scatter, Q / K / V^T scatter, traversability-MLP head), so that each can be
+ * checked on its own.  The fields mirror the library's internal GEMM arguments; the shape and geometry checks are the
+ * GEMM's own.  epi: 0 = bf16 out[m,ldo] = act(acc + bias); 1 = fp32 out = acc + bias; 2 = fp32 out += acc + bias;
+ *   3 = patch embed: fp32 out[frame*npad + 1 + tok, :] = acc + bias + pos[1 + tok, :] (frame = row / tokens_in);
+ *   4 = QKV: bf16 q_out, k_out [m/npad*heads, npad, 64] and vt_out [m/npad*heads, 64, npad] from the columns of [q | k | v];
+ *   5 = MLP head: columns [0, feat) reconstruct x -> loss_reco = mean((out - x)^2) -> conf, column trav_col ->
+ *       trav = sigmoid; nothing of [m, n] is stored.
+ * reverse_m = 1 walks the 64-row blocks last-to-first (the result must not change). */
+typedef struct {
+  int m, n, k;
+  int epi, act;
+  int block_n;              /* 0 = auto */
+  const void* a;            /* [m, lda] bf16 */
+  long long lda;
+  const void* w;            /* [n, k] bf16 */
+  const float* bias;        /* [n] or NULL */
+  void* out;                /* epi 0-3 */
+  long long ldo;
+  const float* pos;         /* epi 3: [1 + tokens_in, ldo] */
+  int tokens_in, npad;      /* epi 3 (npad also epi 4) */
+  int dim, heads;           /* epi 4 */
+  void* q_out;
+  void* k_out;
+  void* vt_out;
+  int feat, trav_col;       /* epi 5 */
+  const void* x;            /* [m, ldx] bf16 */
+  long long ldx;
+  float* trav;
+  float* conf;
+  float* loss_reco;         /* or NULL */
+  const float* cg_mean;     /* device scalars */
+  const float* cg_std;
+  float cg_std_factor;
+  int reverse_m;
+} wvn_gemm_ex_args;
+int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* args, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Primitive: fused multi-head attention, head dim 64, non-causal.
  * Replaces `softmax(q @ k.transpose(-2,-1) * scale) @ v` of the DINO ViT block

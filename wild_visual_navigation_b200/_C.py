@@ -27,6 +27,19 @@ class VitConfig(Structure):
     ]
 
 
+class GemmExArgs(Structure):
+    """wvn_gemm_ex_args: the arguments of the testing entry wvn_gemm_bf16_ex (every GEMM epilogue)."""
+    _fields_ = [
+        ("m", c_int), ("n", c_int), ("k", c_int), ("epi", c_int), ("act", c_int), ("block_n", c_int),
+        ("a", c_void_p), ("lda", c_longlong), ("w", c_void_p), ("bias", c_void_p), ("out", c_void_p), ("ldo", c_longlong),
+        ("pos", c_void_p), ("tokens_in", c_int), ("npad", c_int), ("dim", c_int), ("heads", c_int),
+        ("q_out", c_void_p), ("k_out", c_void_p), ("vt_out", c_void_p),
+        ("feat", c_int), ("trav_col", c_int), ("x", c_void_p), ("ldx", c_longlong), ("trav", c_void_p),
+        ("conf", c_void_p), ("loss_reco", c_void_p), ("cg_mean", c_void_p), ("cg_std", c_void_p),
+        ("cg_std_factor", c_float), ("reverse_m", c_int),
+    ]
+
+
 class TrainConfig(Structure):
     _fields_ = [
         ("w_trav", c_float), ("w_reco", c_float), ("std_factor", c_float), ("anomaly_balanced", c_int),
@@ -46,6 +59,7 @@ SIGNATURES = {
     "wvn_profile_enable": (None, [_I]),
     "wvn_profile_collect": (_I, [_P, _P]),
     "wvn_gemm_bf16": (_I, [_P, _L, _P, _P, _P, _L, _I, _I, _I, _I, _I, _I, _P]),
+    "wvn_gemm_bf16_ex": (_I, [POINTER(GemmExArgs), _P]),
     "wvn_attention_bf16": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "wvn_layernorm": (_I, [_P, _P, _P, _P, _L, _I, _F, _P]),
     "wvn_vit_create": (_I, [POINTER(VitConfig), POINTER(_P)]),

@@ -146,6 +146,19 @@ int wvn_gemm_bf16(const void* a, long long lda, const void* w, const float* bias
   return gemm_bf16(g, a, lda, w, block_n, S(stream));
 }
 
+int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* x, void* stream) {
+  WVN_REQUIRE(x, "wvn_gemm_bf16_ex: null argument");
+  GemmArgs g;
+  g.M = x->m; g.N = x->n; g.K = x->k; g.epi = x->epi; g.act = x->act;
+  g.bias = x->bias; g.out = x->out; g.ldo = x->ldo;
+  g.pos = x->pos; g.tokens_in = x->tokens_in; g.npad = x->npad;
+  g.dim = x->dim; g.heads = x->heads; g.q = x->q_out; g.k = x->k_out; g.vt = x->vt_out;
+  g.feat = x->feat; g.trav_col = x->trav_col; g.x = x->x; g.ldx = x->ldx; g.trav = x->trav; g.conf = x->conf;
+  g.loss_reco = x->loss_reco; g.cg_mean = x->cg_mean; g.cg_std = x->cg_std; g.cg_std_factor = x->cg_std_factor;
+  g.reverse_m = x->reverse_m;
+  return gemm_bf16(g, x->a, x->lda, x->w, x->block_n, S(stream));
+}
+
 int wvn_attention_bf16(const void* q, const void* k, const void* vt, void* out, int batch, int heads, int npad,
                        int n_valid, float scale, void* stream) {
   AttnArgs a;
