@@ -59,7 +59,9 @@ int wvn_profile_collect(float* host_ms, long long* host_launches);
  * Replaces every nn.Linear / 1x1-conv call of the path (cuBLAS in the reference).
  * out_kind: 0 = bf16 out[M,ldo] = act(acc + bias); 1 = fp32 out = acc + bias;
  *           2 = fp32 out += acc + bias (residual).   act: 0 none, 1 ReLU, 2 GELU(erf).
- * K % 64 == 0, N % block_n == 0, block_n in {0 (auto), 64, 128, 192, 224, 256}.
+ * Any K >= 1: lda >= K and a multiple of 8, and W's rows are round_up(K, 8) elements apart (== K whenever K % 8 == 0);
+ * columns past K of either operand are never read (the last 64-wide k-block is zero-filled past K).
+ * N % block_n == 0, block_n in {0 (auto), 64, 128, 192, 224, 256}.
  * ---------------------------------------------------------------------------------------- */
 int wvn_gemm_bf16(const void* a_bf16, long long lda, const void* w_bf16, const float* bias, void* out, long long ldo,
                   int m, int n, int k, int out_kind, int act, int block_n, void* stream);
@@ -79,7 +81,7 @@ typedef struct {
   int block_n;              /* 0 = auto */
   const void* a;            /* [m, lda] bf16 */
   long long lda;
-  const void* w;            /* [n, k] bf16 */
+  const void* w;            /* [n, k] bf16, rows round_up(k, 8) elements apart (any k >= 1, see wvn_gemm_bf16) */
   const float* bias;        /* [n] or NULL */
   void* out;                /* epi 0-3 */
   long long ldo;
@@ -125,7 +127,7 @@ typedef struct wvn_vit wvn_vit_t;
 
 typedef struct {
   int image_size;   /* side of the (square) network input after resize + center crop, e.g. 448 */
-  int patch_size;   /* 8 or 16 */
+  int patch_size;   /* 8 or 16 (DINO), 14 (DINOv2) */
   int dim;          /* 384 (vit_small) or 768 (vit_base) */
   int depth;        /* 12 */
   int heads;        /* dim / 64 */
@@ -141,7 +143,8 @@ void wvn_vit_destroy(wvn_vit_t* h);
 
 /* Weights use the DINO state-dict names (fp32, host or device memory):
  *   cls_token [dim], pos_embed [(1+P), dim] (already interpolated to this token grid),
- *   patch_embed.proj.weight [dim, 3*p*p], patch_embed.proj.bias [dim],
+ *   patch_embed.proj.weight [dim, 3*p*p] (the Conv2d weight as given; the library keeps it at its own padded pitch),
+ *   patch_embed.proj.bias [dim],
  *   blocks.{i}.norm1.{weight,bias}, blocks.{i}.attn.qkv.{weight [3dim,dim],bias},
  *   blocks.{i}.attn.proj.{weight,bias}, blocks.{i}.norm2.{weight,bias},
  *   blocks.{i}.mlp.fc1.{weight [mlp,dim],bias}, blocks.{i}.mlp.fc2.{weight [dim,mlp],bias},

@@ -9,7 +9,8 @@ output its SHA-256 plus a strided sample (every 101st element, as float32):
   * ops.gemm_bf16 at the four ViT-S GEMM shapes of c3 (M = 32 frames x 3200 rows) with the epilogues they run in the
     backbone: QKV (bf16), attention out-projection (fp32 residual add), fc1 (bf16 + GELU), fc2 (fp32 residual add);
   * DinoInterface tokens of ViT-S/8 @448 at B = 32;
-  * the fused per-pixel traversability / confidence maps of a seeded SimpleMLP on those tokens.
+  * the fused per-pixel traversability / confidence maps of a seeded SimpleMLP on those tokens;
+  * DinoInterface tokens of ViT-S/16 @448 at B = 8 (the patch-16 loader and patch-embed GEMM).
 `compare` reports, per output, whether the two builds agree bit for bit and, where not, the largest difference in
 the samples.  Every output here is deterministic for a given build (no atomics race in them), so any difference is
 the build's.
@@ -94,6 +95,14 @@ def write(out_dir):
     trav, conf = TraversabilityInference(di, model, cg).predict_from_tokens(tokens, 448)
     _record(out_dir, "pixel_trav", trav, index)
     _record(out_dir, "pixel_conf", conf, index)
+    del di, tokens
+    torch.cuda.empty_cache()
+
+    # ---- the patch-16 loader and patch-embed GEMM (K = 768): DINO ViT-S/16 @448, B = 8
+    cfg16 = ViTConfig.from_name("vit_small", 16, 448)
+    di16 = DinoInterface(dev, input_size=448, backbone_type="vit_small", patch_size=16,
+                         state_dict=synthetic_state_dict(cfg16, seed=1), max_batch=8)
+    _record(out_dir, "dino_tokens_s16", di16.inference_tokens(img[:8]), index)
     torch.cuda.synchronize()
 
     with open(os.path.join(out_dir, "index.json"), "w") as f:

@@ -75,6 +75,7 @@ struct Weight {
   long long numel = 0;
   bool bf16 = false;
   bool loaded = false;
+  int cols = 0, ld = 0;  // bf16 rows of `cols` elements stored `ld` apart (0: dense)
 };
 
 }  // namespace
@@ -84,7 +85,7 @@ struct Weight {
 // ============================================================================================
 struct wvn_vit {
   wvn_vit_config cfg;
-  int grid = 0, P = 0, n_valid = 0, npad = 0, kpe = 0, chunk = 0;
+  int grid = 0, P = 0, n_valid = 0, npad = 0, kpe = 0, kpe_ld = 0, chunk = 0;
   std::map<std::string, Weight> w;
   std::vector<DevBuf> owned;
   // workspaces (per chunk)
@@ -96,12 +97,14 @@ struct wvn_vit {
   bool forwarded = false;
   int last_batch = 0;
 
-  int add_weight(const std::string& name, long long numel, bool bf16) {
+  // cols / ld: a bf16 matrix whose rows of `cols` elements are stored `ld` apart (the pad columns stay zero)
+  int add_weight(const std::string& name, long long numel, bool bf16, int cols = 0, int ld = 0) {
     DevBuf b;
-    WVN_PROPAGATE(b.alloc(static_cast<size_t>(numel) * (bf16 ? 2 : 4)));
+    const long long stored = cols > 0 ? numel / cols * ld : numel;
+    WVN_PROPAGATE(b.alloc(static_cast<size_t>(stored) * (bf16 ? 2 : 4)));
     owned.push_back(b);
     Weight wt;
-    wt.p = b.p; wt.numel = numel; wt.bf16 = bf16;
+    wt.p = b.p; wt.numel = numel; wt.bf16 = bf16; wt.cols = cols; wt.ld = ld;
     w[name] = wt;
     return WVN_OK;
   }
@@ -181,7 +184,8 @@ int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
   WVN_PROPAGATE(wvn_check_device());
   WVN_REQUIRE(cfg->dim == 384 || cfg->dim == 768, "vit: dim %d unsupported (384, 768)", cfg->dim);
   WVN_REQUIRE(cfg->heads * 64 == cfg->dim, "vit: heads*64 must equal dim");
-  WVN_REQUIRE(cfg->patch_size == 8 || cfg->patch_size == 16, "vit: patch size %d unsupported", cfg->patch_size);
+  WVN_REQUIRE(cfg->patch_size == 8 || cfg->patch_size == 14 || cfg->patch_size == 16, "vit: patch size %d unsupported",
+              cfg->patch_size);
   WVN_REQUIRE(cfg->image_size >= cfg->patch_size, "vit: image size too small");
   WVN_REQUIRE(cfg->mlp_dim % 64 == 0 && cfg->depth > 0 && cfg->max_batch > 0, "vit: bad mlp_dim/depth/max_batch");
   WVN_REQUIRE(cfg->head_out % 64 == 0, "vit: head_out must be a multiple of 64");
@@ -193,6 +197,7 @@ int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
   h->n_valid = h->P + 1;
   h->npad = round_up(h->n_valid, 128);
   h->kpe = 3 * cfg->patch_size * cfg->patch_size;
+  h->kpe_ld = patch_pitch(cfg->patch_size);  // == gemm_w_pitch(kpe): patch rows and weight rows share one pitch
   h->chunk = cfg->chunk > 0 ? cfg->chunk : 8;
   if (h->chunk > cfg->max_batch) h->chunk = cfg->max_batch;
   const int D = cfg->dim;
@@ -200,7 +205,7 @@ int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
   auto add = [&](const std::string& n, long long numel, bool bf) { if (rc == WVN_OK) rc = h->add_weight(n, numel, bf); };
   add("cls_token", D, false);
   add("pos_embed", static_cast<long long>(h->n_valid) * D, false);
-  add("patch_embed.proj.weight", static_cast<long long>(D) * h->kpe, true);
+  if (rc == WVN_OK) rc = h->add_weight("patch_embed.proj.weight", static_cast<long long>(D) * h->kpe, true, h->kpe, h->kpe_ld);
   add("patch_embed.proj.bias", D, false);
   for (int i = 0; i < cfg->depth; ++i) {
     const std::string b = "blocks." + std::to_string(i) + ".";
@@ -236,7 +241,7 @@ int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
   alloc(h->vt, bh * 64 * h->npad * 2);
   alloc(h->attn, rows * D * 2);
   alloc(h->hid, rows * cfg->mlp_dim * 2);
-  alloc(h->ape, static_cast<size_t>(h->chunk) * h->P * h->kpe * 2);
+  alloc(h->ape, static_cast<size_t>(h->chunk) * h->P * h->kpe_ld * 2);
   alloc(h->stage, 8u << 20);
   alloc(h->tok_bf16, static_cast<size_t>(cfg->max_batch) * h->npad * D * 2);
   if (cfg->head_out > 0) alloc(h->head_hidden, static_cast<size_t>(cfg->max_batch) * h->npad * D * 2);
@@ -280,6 +285,22 @@ int wvn_vit_set_weight(wvn_vit_t* h, const char* name, const float* data, long l
   // fp32 destination: copy straight in; bf16 destination: stage (if host) + cast on device
   if (!wt.bf16) {
     WVN_CHECK_CUDA(cudaMemcpy(wt.p, data, numel * 4, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+  } else if (wt.cols > 0) {
+    // pitched rows: stage whole rows, cast each into its row of the padded storage
+    const long long chunk_rows = static_cast<long long>(h->stage.bytes / 4) / wt.cols;
+    const long long rows = numel / wt.cols;
+    for (long long r0 = 0; r0 < rows; r0 += chunk_rows) {
+      const long long n = std::min(chunk_rows, rows - r0);
+      const float* src = data + r0 * wt.cols;
+      if (!on_device) {
+        WVN_CHECK_CUDA(cudaMemcpy(h->stage.p, src, n * wt.cols * 4, cudaMemcpyHostToDevice));
+        src = reinterpret_cast<const float*>(h->stage.p);
+      }
+      const int blocks = static_cast<int>(std::min<long long>((n * wt.cols + 255) / 256, 4096));
+      cast_rows_kernel<<<blocks, 256, 0, 0>>>(src, reinterpret_cast<__nv_bfloat16*>(wt.p) + r0 * wt.ld, n, wt.cols, wt.ld);
+      WVN_CHECK_LAUNCH("cast_rows_kernel");
+      WVN_CHECK_CUDA(cudaStreamSynchronize(0));
+    }
   } else {
     const long long chunk_elems = static_cast<long long>(h->stage.bytes / 4);
     for (long long off = 0; off < numel; off += chunk_elems) {
@@ -363,7 +384,7 @@ int vit_forward_impl(wvn_vit_t* h, const void* img, bool u8_hwc, int src_batch, 
       GemmArgs g;
       g.M = nb * h->P; g.N = D; g.K = h->kpe; g.epi = EPI_PATCH; g.bias = h->wp<float>("patch_embed.proj.bias");
       g.out = x; g.ldo = D; g.pos = h->wp<float>("pos_embed"); g.tokens_in = h->P; g.npad = h->npad;
-      WVN_PROPAGATE(gemm_bf16(g, h->ape.p, h->kpe, h->wp<void>("patch_embed.proj.weight"), 0, s));
+      WVN_PROPAGATE(gemm_bf16(g, h->ape.p, h->kpe_ld, h->wp<void>("patch_embed.proj.weight"), 0, s));
     }
     LayerNormArgs la;
     la.rows = rows; la.dim = D; la.eps = c.ln_eps; la.npad = h->npad; la.n_valid = h->n_valid;

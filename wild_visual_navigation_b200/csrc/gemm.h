@@ -52,7 +52,11 @@ struct GemmArgs {
 
 int pick_block_n(int N);
 
-// A: [M, K] bf16 with row pitch lda (elements); W: [N, K] bf16 contiguous.
+// Row pitch (elements) of the W operand: K rounded up to 8, the 16-byte multiple TMA needs (K itself when K % 64 == 0).
+inline long long gemm_w_pitch(int K) { return (static_cast<long long>(K) + 7) / 8 * 8; }
+
+// Any K >= 1.  A: [M, K] bf16 with row pitch lda >= K (elements, a multiple of 8); W: [N, K] bf16 at row pitch
+// gemm_w_pitch(K).  Columns past K of either operand are never read.
 int gemm_bf16(const GemmArgs& args, const void* A, long long lda, const void* W, int block_n, cudaStream_t stream);
 
 }  // namespace wvn

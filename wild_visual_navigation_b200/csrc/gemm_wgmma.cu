@@ -256,7 +256,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 
   const int num_m = (args.M + BM - 1) / BM;
   const int num_n = args.N / BN;
-  const int num_k = args.K / BK;
+  // the last k-block may run past K: the tensor maps' inner extent is K, so TMA fills those columns with zeros
+  const int num_k = (args.K + BK - 1) / BK;
   constexpr bool ROW_OWNER = (EPI == EPI_MLP_HEAD);
 
   if (threadIdx.x == 0) {
@@ -486,7 +487,7 @@ int pick_block_n(int N) {
 
 int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, int block_n, cudaStream_t stream) {
   WVN_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "gemm: empty problem (M=%d N=%d K=%d)", a.M, a.N, a.K);
-  WVN_REQUIRE(a.K % BK == 0, "gemm: K=%d must be a multiple of %d (pad the operands)", a.K, BK);
+  WVN_REQUIRE(lda >= a.K, "gemm: lda=%lld is smaller than K=%d", lda, a.K);
   if (block_n == 0) block_n = pick_block_n(a.N);
   WVN_REQUIRE(block_n == 64 || block_n == 128 || block_n == 192 || block_n == 224 || block_n == 256,
               "gemm: bad block_n %d", block_n);
@@ -504,8 +505,10 @@ int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, in
   if (a.epi == EPI_F32 || a.epi == EPI_RESID_F32) WVN_REQUIRE(a.ldo % 4 == 0, "gemm: fp32 output pitch must be a multiple of 4");
   if (a.epi == EPI_BF16) WVN_REQUIRE(a.ldo % 8 == 0, "gemm: bf16 output pitch must be a multiple of 8");
   CUtensorMap ta, tb, tc[3] = {};
+  // Both maps take the true K as their inner extent, so the pad columns of a K that is not a multiple of 64 are never
+  // read (TMA zero-fills the last k-block past K, whatever the pad columns hold).  W's rows sit at a 16-byte pitch.
   WVN_PROPAGATE(make_tmap_bf16_2d(&ta, A, a.K, a.M, static_cast<uint64_t>(lda) * 2, BK, BM));
-  WVN_PROPAGATE(make_tmap_bf16_2d(&tb, W, a.K, a.N, static_cast<uint64_t>(a.K) * 2, BK, block_n));
+  WVN_PROPAGATE(make_tmap_bf16_2d(&tb, W, a.K, a.N, static_cast<uint64_t>(gemm_w_pitch(a.K)) * 2, BK, block_n));
   // output maps for the staged epilogues: 32-column x 64-row boxes (store_frag's layouts); rows past M are clipped
   if (a.epi == EPI_BF16)
     WVN_PROPAGATE(make_tmap_2d(&tc[0], a.out, 2, a.N, a.M, static_cast<uint64_t>(a.ldo) * 2, kSliceCols, BM, 64));

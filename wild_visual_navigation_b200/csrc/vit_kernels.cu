@@ -18,16 +18,18 @@ namespace wvn {
 
 namespace {
 
-// One thread produces 8 consecutive K-elements (one patch row of one channel for p=8):
-// reads 8 floats that are contiguous in the source row when no resize happens.
-template <bool U8_HWC>
+// One thread produces G consecutive K-elements of one patch row of one channel (G = 8 for p = 8 / 16, a whole row of
+// 14 for p = 14): reads G floats that are contiguous in the source row when no resize happens.  Output rows are
+// patch_pitch(p) elements apart; the pad columns [3 p p, pitch) are never written (the GEMM does not read them).
+template <bool U8_HWC, int G>
 __global__ void image_to_patches_kernel(const void* __restrict__ img_raw, __nv_bfloat16* __restrict__ out,
                                         ImagePatchArgs a) {
   const float* img = reinterpret_cast<const float*>(img_raw);
   const unsigned char* img8 = reinterpret_cast<const unsigned char*>(img_raw);
   const int ps = a.patch;
   const int k_total = 3 * ps * ps;
-  const int groups_per_row = k_total / 8;
+  const int pitch = patch_pitch(ps);
+  const int groups_per_row = k_total / G;
   const long long total = static_cast<long long>(a.batch) * a.grid_h * a.grid_w * groups_per_row;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -36,7 +38,7 @@ __global__ void image_to_patches_kernel(const void* __restrict__ img_raw, __nv_b
     const int pw = static_cast<int>(prow % a.grid_w);
     const int ph = static_cast<int>((prow / a.grid_w) % a.grid_h);
     const int b = static_cast<int>(prow / (static_cast<long long>(a.grid_w) * a.grid_h));
-    const int k0 = g * 8;  // k = c*ps*ps + ky*ps + kx
+    const int k0 = g * G;  // k = c*ps*ps + ky*ps + kx
     const int c = k0 / (ps * ps);
     const int ky = (k0 / ps) % ps;
     const int kx0 = k0 % ps;
@@ -51,9 +53,9 @@ __global__ void image_to_patches_kernel(const void* __restrict__ img_raw, __nv_b
     const int crop_w = a.grid_w * ps;
     const float* src_row = img + ((static_cast<long long>(sb) * 3 + c) * a.in_h + sy) * a.in_w;
     const unsigned char* src_row8 = img8 + (static_cast<long long>(sb) * a.in_h + sy) * a.in_w * 3 + c;
-    float v[8];
+    float v[G];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < G; ++i) {
       const int xo = pw * ps + kx0 + i;
       const int x = flip ? crop_w - 1 - xo : xo;
       const int sx = min(static_cast<int>(floorf((x + a.crop_left) * a.scale_x)), a.in_w - 1);
@@ -61,8 +63,15 @@ __global__ void image_to_patches_kernel(const void* __restrict__ img_raw, __nv_b
       const float px = U8_HWC ? static_cast<float>(__ldg(src_row8 + 3 * sx)) / 255.f : __ldg(src_row + sx);
       v[i] = (px - mean) * inv_std;
     }
-    st_global_v4(out + prow * k_total + k0, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
-                 pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+    __nv_bfloat16* dst = out + prow * pitch + k0;
+    if (G == 8) {
+      st_global_v4(dst, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+                   pack_bf16x2(v[6], v[7]));
+    } else {
+      // 14 elements at a 28-byte offset inside the row: 4-byte aligned pairs
+#pragma unroll
+      for (int i = 0; i < G; i += 2) *reinterpret_cast<uint32_t*>(dst + i) = pack_bf16x2(v[i], v[i + 1]);
+    }
   }
 }
 
@@ -205,18 +214,22 @@ attention_f32_debug_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restr
 }  // namespace
 
 int image_to_patches(const void* img, bool u8_hwc, void* out_bf16, const ImagePatchArgs& a, cudaStream_t stream) {
-  WVN_REQUIRE(a.patch == 8 || a.patch == 16, "image_to_patches: patch size %d unsupported", a.patch);
-  const long long total = static_cast<long long>(a.batch) * a.grid_h * a.grid_w * (3 * a.patch * a.patch / 8);
+  WVN_REQUIRE(a.patch == 8 || a.patch == 14 || a.patch == 16, "image_to_patches: patch size %d unsupported", a.patch);
+  const int group = a.patch == 14 ? 14 : 8;
+  const long long total = static_cast<long long>(a.batch) * a.grid_h * a.grid_w * (3 * a.patch * a.patch / group);
   const int threads = 256;
   long long blocks = (total + threads - 1) / threads;
   const long long max_blocks = static_cast<long long>(sm_count()) * 16;
   if (blocks > max_blocks) blocks = max_blocks;
-  if (u8_hwc)
-    image_to_patches_kernel<true><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(
-        img, reinterpret_cast<__nv_bfloat16*>(out_bf16), a);
-  else
-    image_to_patches_kernel<false><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(
-        img, reinterpret_cast<__nv_bfloat16*>(out_bf16), a);
+  __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(out_bf16);
+  const unsigned nb = static_cast<unsigned>(blocks);
+  if (group == 14) {
+    if (u8_hwc) image_to_patches_kernel<true, 14><<<nb, threads, 0, stream>>>(img, out, a);
+    else image_to_patches_kernel<false, 14><<<nb, threads, 0, stream>>>(img, out, a);
+  } else {
+    if (u8_hwc) image_to_patches_kernel<true, 8><<<nb, threads, 0, stream>>>(img, out, a);
+    else image_to_patches_kernel<false, 8><<<nb, threads, 0, stream>>>(img, out, a);
+  }
   WVN_CHECK_LAUNCH("image_to_patches_kernel");
   return WVN_OK;
 }

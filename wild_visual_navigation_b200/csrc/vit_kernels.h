@@ -29,7 +29,12 @@ struct LayerNormArgs {
   int reverse = 0;  // walk the rows last-to-first (start where the producer kernel finished: those rows are still in L2)
 };
 
+// Row pitch (elements) of a patch row of 3 * p * p K-elements in (c, ky, kx) order: rounded up to the 16 bytes TMA
+// needs (p = 14: 588 -> 592; p = 8 / 16: 192 / 768, unpadded).  The patch-embed weight is stored at the same pitch.
+__host__ __device__ inline int patch_pitch(int p) { return (3 * p * p + 7) / 8 * 8; }
+
 // img: [batch, 3, in_h, in_w] fp32 in [0,1], or (u8_hwc) [batch, in_h, in_w, 3] uint8 RGB
+// out_bf16: [batch * grid_h * grid_w, patch_pitch(patch)] bf16; patch in {8, 14, 16}
 int image_to_patches(const void* img, bool u8_hwc, void* out_bf16, const ImagePatchArgs& a, cudaStream_t stream);
 int init_token_rows(float* x, const float* cls, const float* pos, int batch, int npad, int n_valid, int dim,
                     cudaStream_t stream);

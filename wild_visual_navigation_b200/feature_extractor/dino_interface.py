@@ -11,7 +11,7 @@ from __future__ import annotations
 import torch
 
 from .. import ops
-from .weights import VIT_SHAPES, load_dino_state_dict
+from .weights import DINOV2_PATCH, VIT_SHAPES, check_backbone_family, load_dino_state_dict
 
 
 class _Cfg(dict):
@@ -24,6 +24,11 @@ class _Cfg(dict):
 
 
 class DinoInterface:
+    """``backbone="dino"``: DINO ViT-S / ViT-B at ``patch_size`` 8 or 16.  ``backbone="dinov2"``: DINOv2 ViT-S/14 /
+    ViT-B/14 (no register tokens).  DINOv2 is released at patch 14 only, so it runs at patch 14 whatever ``patch_size``
+    says (the reference's ROS default passes ``patch_size=8`` with ``dinov2``); ``vit_patch_size`` still returns the
+    configured value, as the reference's property does, while ``grid`` is the token grid actually run."""
+
     def __init__(self, device: str, backbone: str = "dino", input_size: int = 448, backbone_type: str = "vit_small",
                  patch_size: int = 8, projection_type: str = None, dropout_p: float = 0,
                  pretrained_weights: str = None, cfg=None, max_batch: int = 32, chunk: int = 0, state_dict=None,
@@ -34,16 +39,20 @@ class DinoInterface:
             self._cfg = _Cfg(backbone=backbone, backbone_type=backbone_type, input_size=input_size,
                              patch_size=patch_size, projection_type=projection_type, dropout_p=dropout_p,
                              pretrained_weights=pretrained_weights)
-        if self._cfg.backbone not in ("dino",):
-            raise ValueError(f"backbone '{self._cfg.backbone}' is outside the H100 hot path (DINO ViT only)")
+        if self._cfg.backbone not in ("dino", "dinov2"):
+            raise ValueError(f"backbone '{self._cfg.backbone}' is outside the H100 hot path (DINO / DINOv2 ViT only)")
         if not str(device).startswith("cuda"):
             raise RuntimeError("wild_visual_navigation_b200 runs on CUDA (sm_90a) devices only — no CPU fallback")
         self._device = device
         shp = VIT_SHAPES[self._cfg.backbone_type]
-        sd = state_dict if state_dict is not None else load_dino_state_dict(
-            self._cfg.backbone_type, self._cfg.patch_size, self._cfg.pretrained_weights)
+        backbone = self._cfg.backbone
+        patch = DINOV2_PATCH if backbone == "dinov2" else self._cfg.patch_size
+        if state_dict is not None:
+            sd = check_backbone_family(state_dict, backbone)
+        else:
+            sd = load_dino_state_dict(self._cfg.backbone_type, patch, self._cfg.pretrained_weights, backbone=backbone)
         with torch.cuda.device(torch.device(device)):
-            self._model = ops.ViTBackbone(self._cfg.input_size, self._cfg.patch_size, shp["dim"], shp["depth"],
+            self._model = ops.ViTBackbone(self._cfg.input_size, patch, shp["dim"], shp["depth"],
                                           shp["heads"], shp["mlp_dim"], sd, max_batch=max_batch, chunk=chunk,
                                           head_weights=head_weights)
 

@@ -7,9 +7,10 @@
     when ``return_dense_features=True`` asks for it;
   * adjacency + centroids come from the same pass (no per-segment Python loops / host syncs);
   * when segmentation and features are both "stego"/"dino" on the same backbone, one ViT forward
-    serves both (the reference runs two backbones).
+    serves both (the reference runs two backbones); with "dinov2" features, STEGO's DINO backbone segments and a
+    second, DINOv2 handle gives the features.
 Supported: segmentation_type in {"slic" (the constructor default), "stego", "grid", "random", "none"/None},
-feature_type in {"dino", "stego"}.  "slic" is an all-integer SLIC kernel (csrc/slic_kernels.cu; fast_slic itself is an
+feature_type in {"dino", "dinov2", "stego"}.  "slic" is an all-integer SLIC kernel (csrc/slic_kernels.cu; fast_slic itself is an
 un-vendored C++ package, see oracle/slic.py for what is and is not restated).  "sift", "torchvision", "histogram"
 features are out of scope (SURVEY.md §2) and raise.
 """
@@ -47,19 +48,27 @@ class FeatureExtractor:
             self._feature_dim = 384 if common["backbone_type"] == "vit_small" else 768
         else:
             raise ValueError(f"Extractor[{feature_type}] is outside the H100 hot path")
+        # the feature backbone, as the reference picks it (feature_extractor.py:61): "dino" or "dinov2"
+        backbone = kwargs.get("backbone", feature_type)
+        # STEGO's own backbone is DINO; it serves the features too unless they come from another backbone
+        share = feature_type == "stego" or backbone == "dino"
         if need_stego:
             self._stego = StegoInterface(device=device, input_size=input_size, run_crf=kwargs.get("run_crf", False),
                                          run_clustering=kwargs.get("run_clustering", True),  # the reference's default (:51)
                                          n_image_clusters=kwargs.get("n_image_clusters", 20),
                                          head_state_dict=kwargs.get("head_state_dict"),
-                                         backbone_state_dict=kwargs.get("state_dict"),
+                                         backbone_state_dict=kwargs.get("state_dict" if share else "stego_state_dict"),
                                          flip_tta=kwargs.get("flip_tta", True),
                                          kmeans_iters=kwargs.get("kmeans_iters", 10), **common)
+        else:
+            self._stego = None
+        if need_stego and share:
             self._dino = self._stego._dino
             self._extractor = self._stego if feature_type == "stego" else self._dino
         else:
-            self._stego = None
-            self._dino = DinoInterface(device=device, input_size=input_size, backbone=kwargs.get("backbone", "dino"),
+            # with segmentation_type="stego" and DINOv2 features: a second handle; `state_dict` is this backbone's
+            # and `stego_state_dict` STEGO's
+            self._dino = DinoInterface(device=device, input_size=input_size, backbone=backbone,
                                        state_dict=kwargs.get("state_dict"),
                                        pretrained_weights=kwargs.get("pretrained_weights"), **common)
             self._extractor = self._dino
@@ -131,7 +140,11 @@ class FeatureExtractor:
             seg = self._stego.cluster_ids.contiguous()
             smax = self._stego.max_segments
             counts = ops.relabel(seg, smax)
-            tokens = self._stego.code_tokens if self._feature_type == "stego" else self._stego.backbone_tokens
+            if self._feature_type == "stego":
+                tokens = self._stego.code_tokens
+            elif self._dino is self._stego._dino:
+                tokens = self._stego.backbone_tokens
+            # otherwise the features come from their own backbone (DINOv2), run in step 2
         elif self._segmentation_type == "grid":
             cell = kwargs.get("cell_size", 32)
             ys = torch.arange(H, device=img.device) // cell

@@ -7,6 +7,8 @@ The reference downloads DINO checkpoints from dl.fbaipublicfiles.com at construc
     (keys cls_token, pos_embed, patch_embed.proj.*, blocks.N.*, norm.*), which is used as is;
   * otherwise seeded DINO-style random weights are generated (SURVEY.md §8d) — results are then
     numerically meaningful only for parity / throughput work, and a warning says so.
+DINOv2 (``backbone="dinov2"``, the ``dinov2_vit{s,b}14_pretrain.pth`` checkpoints) uses the same key names plus the
+LayerScale gammas ``blocks.N.ls{1,2}.gamma`` and an unused ``mask_token``.
 """
 from __future__ import annotations
 
@@ -52,7 +54,47 @@ def synthetic_dino_state_dict(dim, depth, mlp_dim, patch_size, pretrain_grid, se
     return sd
 
 
-def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights=None, seed: int = 1):
+# DINOv2 is released at patch 14 only, pre-trained at 518 x 518 (a 37 x 37 position-embedding grid)
+DINOV2_PATCH, DINOV2_PRETRAIN_GRID = 14, 37
+
+
+def synthetic_dinov2_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09):
+    """Seeded DINOv2-layout weights: the DINO layout at patch 14 / grid 37 plus ``blocks.N.ls{1,2}.gamma`` and the
+    (unused) ``mask_token``.  The LayerScale gammas vary per channel and are drawn independently for ls1 and ls2, so a
+    missing or swapped LayerScale changes the tokens far beyond the parity tolerance."""
+    sd = synthetic_dino_state_dict(dim, depth, mlp_dim, DINOV2_PATCH, DINOV2_PRETRAIN_GRID, seed, attn_std)
+    g = torch.Generator().manual_seed(seed + 1)
+    for i in range(depth):
+        sd[f"blocks.{i}.ls1.gamma"] = 0.1 + 0.9 * torch.rand(dim, generator=g)
+        sd[f"blocks.{i}.ls2.gamma"] = 0.1 + 0.9 * torch.rand(dim, generator=g)
+    sd["mask_token"] = torch.zeros(1, dim)
+    return sd
+
+
+def check_backbone_family(sd: dict, backbone: str) -> dict:
+    """Checks that a ViT state dict belongs to ``backbone`` ("dino": DINO v1, "dinov2": DINOv2 without registers) and
+    returns it with the keys the backbone does not use dropped (DINOv2's ``mask_token``).  Raises ValueError on a
+    checkpoint of the other family or on register tokens (the ``_reg`` variants are not supported)."""
+    sd = {k.replace("module.", "").replace("backbone.", ""): v for k, v in sd.items()}
+    if "register_tokens" in sd:
+        raise ValueError("ViT checkpoints with register tokens (DINOv2 *_reg) are not supported")
+    has_ls = "blocks.0.ls1.gamma" in sd
+    patch = int(sd["patch_embed.proj.weight"].shape[-1])
+    if backbone == "dinov2":
+        if not has_ls or patch != DINOV2_PATCH:
+            raise ValueError(f"backbone 'dinov2' needs a DINOv2 checkpoint (LayerScale 'ls1.gamma' and a 14x14 patch "
+                             f"conv); got one with{'' if has_ls else 'out'} LayerScale and a {patch}x{patch} patch conv")
+        return {k: v for k, v in sd.items() if k != "mask_token"}
+    if has_ls or "mask_token" in sd:
+        raise ValueError("backbone 'dino' got a DINOv2 checkpoint (LayerScale gammas / mask_token): pass "
+                         "backbone='dinov2'")
+    return sd
+
+
+def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights=None, seed: int = 1,
+                         backbone: str = "dino"):
+    """DINO (``backbone="dino"``) or DINOv2 (``"dinov2"``, always patch 14) weights, from ``pretrained_weights`` /
+    ``$WVN_DINO_WEIGHTS`` or seeded.  A checkpoint is checked against the family (check_backbone_family)."""
     shp = VIT_SHAPES[backbone_type]
     path = pretrained_weights or os.environ.get("WVN_DINO_WEIGHTS")
     if path:
@@ -61,9 +103,11 @@ def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights
             sd = sd["state_dict"]
         if "teacher" in sd:
             sd = sd["teacher"]
-        return {k.replace("module.", "").replace("backbone.", ""): v for k, v in sd.items()}
-    warnings.warn("no DINO checkpoint given (pretrained_weights / $WVN_DINO_WEIGHTS): using seeded random "
-                  "DINO-style weights — fine for parity and throughput work, not for real traversability")
+        return check_backbone_family(sd, backbone)
+    warnings.warn(f"no {backbone.upper()} checkpoint given (pretrained_weights / $WVN_DINO_WEIGHTS): using seeded random "
+                  f"{backbone.upper()}-style weights — fine for parity and throughput work, not for real traversability")
+    if backbone == "dinov2":
+        return synthetic_dinov2_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], seed)
     return synthetic_dino_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], patch_size, 224 // patch_size, seed)
 
 

@@ -24,9 +24,10 @@ ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
 # primitives
 # --------------------------------------------------------------------------------------------
 def gemm_bf16(a, w, bias=None, out_kind=OUT_BF16, act=ACT_NONE, out=None, block_n=0):
-    """out = act(a @ w.T + bias).  a: [M,K] bf16, w: [N,K] bf16, bias: [N] f32."""
+    """out = act(a @ w.T + bias).  a: [M,K] bf16, w: [N,K] bf16 with rows round_up(K, 8) apart, bias: [N] f32."""
     M, K = a.shape
     N = w.shape[0]
+    assert w.stride(0) == (K + 7) // 8 * 8 and w.stride(1) == 1, "gemm_bf16: w rows must be round_up(K, 8) elements apart"
     if out is None:
         out = torch.empty(M, N, device=a.device, dtype=torch.bfloat16 if out_kind == OUT_BF16 else torch.float32)
     check(lib().wvn_gemm_bf16(ptr(a), a.stride(0), ptr(w), ptr(bias), ptr(out), out.stride(0), M, N, K, out_kind, act,
@@ -222,7 +223,8 @@ def relabel(seg, num_labels):
 # ViT backbone handle
 # --------------------------------------------------------------------------------------------
 def interpolate_pos_embed(pos_embed: torch.Tensor, grid: int) -> torch.Tensor:
-    """DINO's interpolate_pos_encoding (bicubic, +0.1 trick), done once at weight-load time."""
+    """DINO's interpolate_pos_encoding (bicubic, +0.1 trick), done once at weight-load time.  DINOv2's is the same
+    formula from its 37 x 37 pre-training grid (the side is read off ``pos_embed``)."""
     n_pre = pos_embed.shape[1] - 1
     if n_pre == grid * grid:
         return pos_embed
@@ -235,8 +237,26 @@ def interpolate_pos_embed(pos_embed: torch.Tensor, grid: int) -> torch.Tensor:
     return torch.cat((pos_embed[:, :1], patch), dim=1)
 
 
+def fold_layerscale(sd: dict, depth: int) -> dict:
+    """DINOv2's LayerScale ``x += gamma * f(x)`` folded into the layer that ends f, in fp32 before any bf16 cast:
+    ``attn.proj`` weight rows and bias times ``ls1.gamma``, ``mlp.fc2`` weight rows and bias times ``ls2.gamma``
+    (at least fp32; a float64 state dict stays float64).  A state dict without gammas (DINO) is returned unchanged."""
+    if "blocks.0.ls1.gamma" not in sd:
+        return sd
+    out = {k: v for k, v in sd.items() if ".ls1.gamma" not in k and ".ls2.gamma" not in k}
+    for i in range(depth):
+        b = f"blocks.{i}."
+        for ls, layer in (("ls1", "attn.proj"), ("ls2", "mlp.fc2")):
+            w, bias, gamma = sd[b + layer + ".weight"], sd[b + layer + ".bias"], sd[b + ls + ".gamma"]
+            dt = torch.promote_types(w.dtype, torch.float32)
+            gamma = gamma.to(w.device, dt)
+            out[b + layer + ".weight"] = w.to(dt) * gamma[:, None]
+            out[b + layer + ".bias"] = bias.to(dt) * gamma
+    return out
+
+
 class ViTBackbone:
-    """Owns a ``wvn_vit_t``: DINO ViT weights (bf16 on device) + L2-sized activation workspaces."""
+    """Owns a ``wvn_vit_t``: DINO / DINOv2 ViT weights (bf16 on device) + L2-sized activation workspaces."""
 
     def __init__(self, image_size, patch_size, dim, depth, heads, mlp_dim, state_dict, max_batch=32, chunk=0,
                  head_weights=None, ln_eps=1e-6):
@@ -262,6 +282,7 @@ class ViTBackbone:
 
     def _load(self, sd, depth):
         sd = {k.replace("module.", "").replace("backbone.", ""): v for k, v in sd.items()}
+        sd = fold_layerscale(sd, depth)
         self._set("cls_token", sd["cls_token"].reshape(-1))
         self._set("pos_embed", interpolate_pos_embed(sd["pos_embed"].float().cpu(), self.grid).reshape(-1))
         self._set("patch_embed.proj.weight", sd["patch_embed.proj.weight"].reshape(self.dim, -1))
