@@ -43,6 +43,8 @@ typedef enum {
 const char* wvn_last_error(void);
 /* 0 if device 0..n has compute capability 9.0, WVN_STATUS_NO_DEVICE otherwise. */
 int wvn_check_device(void);
+/* ABI version.  101: wvn_vit_config and wvn_gemm_ex_args gained a trailing `int registers` (0 = the layout of 100), so
+ * callers that fill these structs by layout (ctypes mirrors, code compiled against an older header) must add the field. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -70,7 +72,8 @@ int wvn_gemm_bf16(const void* a_bf16, long long lda, const void* w_bf16, const f
  * handles use internally (patch-embed scatter, Q / K / V^T scatter, traversability-MLP head), so that each can be
  * checked on its own.  The fields mirror the library's internal GEMM arguments; the shape and geometry checks are the
  * GEMM's own.  epi: 0 = bf16 out[m,ldo] = act(acc + bias); 1 = fp32 out = acc + bias; 2 = fp32 out += acc + bias;
- *   3 = patch embed: fp32 out[frame*npad + 1 + tok, :] = acc + bias + pos[1 + tok, :] (frame = row / tokens_in);
+ *   3 = patch embed: fp32 out[frame*npad + 1 + registers + tok, :] = acc + bias + pos[1 + tok, :] (frame = row / tokens_in;
+ *       rows [frame*npad, frame*npad + 1 + registers) — CLS and register tokens — are not written);
  *   4 = QKV: bf16 q_out, k_out [m/npad*heads, npad, 64] and vt_out [m/npad*heads, 64, npad] from the columns of [q | k | v];
  *   5 = MLP head: columns [0, feat) reconstruct x -> loss_reco = mean((out - x)^2) -> conf, column trav_col ->
  *       trav = sigmoid; nothing of [m, n] is stored.
@@ -101,6 +104,7 @@ typedef struct {
   const float* cg_std;
   float cg_std_factor;
   int reverse_m;
+  int registers;            /* epi 3: register tokens between CLS and the first patch row (0 = DINO / DINOv2 layout) */
 } wvn_gemm_ex_args;
 int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* args, void* stream);
 
@@ -136,13 +140,17 @@ typedef struct {
   int chunk;        /* frames processed together (activations stay L2-resident); 0 = default */
   float ln_eps;     /* 1e-6 */
   int head_out;     /* columns of the STEGO head output matrix (multiple of 64), 0 = no head */
+  int registers;    /* register tokens R (DINOv2 *_reg: 4), 0 = none.  Token rows of a frame: [CLS, reg_0 .. reg_{R-1},
+                       patch_0 ..], so patch p sits in row 1 + R + p and n_valid = 1 + R + P.  R > 0 needs head_out == 0
+                       (the STEGO consumers below address patch p as row 1 + p). */
 } wvn_vit_config;
 
 int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out);
 void wvn_vit_destroy(wvn_vit_t* h);
 
 /* Weights use the DINO state-dict names (fp32, host or device memory):
- *   cls_token [dim], pos_embed [(1+P), dim] (already interpolated to this token grid),
+ *   cls_token [dim], pos_embed [(1+P), dim] (CLS + patches, already interpolated to this token grid),
+ *   register_tokens [registers, dim] (only when registers > 0; they get no position embedding),
  *   patch_embed.proj.weight [dim, 3*p*p] (the Conv2d weight as given; the library keeps it at its own padded pitch),
  *   patch_embed.proj.bias [dim],
  *   blocks.{i}.norm1.{weight,bias}, blocks.{i}.attn.qkv.{weight [3dim,dim],bias},
@@ -157,7 +165,7 @@ int wvn_vit_set_weight(wvn_vit_t* h, const char* name, const float* data, long l
 /* img: [batch, 3, in_h, in_w] fp32 in [0,1].  Applies the interface's transform
  * (Resize(image_size, NEAREST) + CenterCrop(image_size) + ImageNet Normalize,
  *  dino_interface.py:52-59) inside the patch loader, runs the backbone, and writes the final
- * LayerNorm output of the patch tokens (CLS dropped): tokens_out [batch, P, dim] fp32.
+ * LayerNorm output of the patch tokens (CLS and register tokens dropped): tokens_out [batch, P, dim] fp32.
  * resized_h/resized_w: size after the virtual NEAREST resize (== in_h/in_w when no resize). */
 int wvn_vit_forward(wvn_vit_t* h, const float* img, int batch, int in_h, int in_w, int resized_h, int resized_w,
                     float* tokens_out, void* stream);
@@ -292,7 +300,8 @@ int wvn_mlp_infer_pixels(wvn_mlp_infer_t* h, const float* tokens, int batch, int
                          const float* cg_mean, const float* cg_std, float std_factor, float* trav, float* conf,
                          void* stream);
 /* The same maps straight from the backbone's own bf16 token buffer (the tokens of the last wvn_vit_forward* call, frames
- * [0, batch)): no fp32 -> bf16 re-cast of the tokens.  Needs dim == the backbone's width and the fused geometry. */
+ * [0, batch)): no fp32 -> bf16 re-cast of the tokens; patch p of a frame is read from row 1 + registers + p.  Needs
+ * dim == the backbone's width and the fused geometry. */
 int wvn_mlp_infer_pixels_vit(wvn_mlp_infer_t* h, wvn_vit_t* vit, int batch, int out_h, int out_w, const float* cg_mean,
                              const float* cg_std, float std_factor, float* trav, float* conf, void* stream);
 /* Same arithmetic on explicit rows x: [rows, dim] fp32 (segment-wise prediction mode). */

@@ -24,6 +24,7 @@ class VitConfig(Structure):
     _fields_ = [
         ("image_size", c_int), ("patch_size", c_int), ("dim", c_int), ("depth", c_int), ("heads", c_int),
         ("mlp_dim", c_int), ("max_batch", c_int), ("chunk", c_int), ("ln_eps", c_float), ("head_out", c_int),
+        ("registers", c_int),
     ]
 
 
@@ -36,7 +37,7 @@ class GemmExArgs(Structure):
         ("q_out", c_void_p), ("k_out", c_void_p), ("vt_out", c_void_p),
         ("feat", c_int), ("trav_col", c_int), ("x", c_void_p), ("ldx", c_longlong), ("trav", c_void_p),
         ("conf", c_void_p), ("loss_reco", c_void_p), ("cg_mean", c_void_p), ("cg_std", c_void_p),
-        ("cg_std_factor", c_float), ("reverse_m", c_int),
+        ("cg_std_factor", c_float), ("reverse_m", c_int), ("registers", c_int),
     ]
 
 

@@ -85,7 +85,8 @@ struct Weight {
 // ============================================================================================
 struct wvn_vit {
   wvn_vit_config cfg;
-  int grid = 0, P = 0, n_valid = 0, npad = 0, kpe = 0, kpe_ld = 0, chunk = 0;
+  // t0: first patch row of a frame (1 + register tokens); rows [t0, n_valid) are the P patches
+  int grid = 0, P = 0, t0 = 1, n_valid = 0, npad = 0, kpe = 0, kpe_ld = 0, chunk = 0;
   std::map<std::string, Weight> w;
   std::vector<DevBuf> owned;
   // workspaces (per chunk)
@@ -115,7 +116,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 100; }
+int wvn_version(void) { return 101; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -158,7 +159,7 @@ int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* x, void* stream) {
   g.dim = x->dim; g.heads = x->heads; g.q = x->q_out; g.k = x->k_out; g.vt = x->vt_out;
   g.feat = x->feat; g.trav_col = x->trav_col; g.x = x->x; g.ldx = x->ldx; g.trav = x->trav; g.conf = x->conf;
   g.loss_reco = x->loss_reco; g.cg_mean = x->cg_mean; g.cg_std = x->cg_std; g.cg_std_factor = x->cg_std_factor;
-  g.reverse_m = x->reverse_m;
+  g.reverse_m = x->reverse_m; g.registers = x->registers;
   return gemm_bf16(g, x->a, x->lda, x->w, x->block_n, S(stream));
 }
 
@@ -189,12 +190,16 @@ int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
   WVN_REQUIRE(cfg->image_size >= cfg->patch_size, "vit: image size too small");
   WVN_REQUIRE(cfg->mlp_dim % 64 == 0 && cfg->depth > 0 && cfg->max_batch > 0, "vit: bad mlp_dim/depth/max_batch");
   WVN_REQUIRE(cfg->head_out % 64 == 0, "vit: head_out must be a multiple of 64");
+  WVN_REQUIRE(cfg->registers >= 0, "vit: registers must be >= 0");
+  // the STEGO head's consumers (wvn_flip_average, wvn_logits_argmax, wvn_stego_kmeans) read patch p at row 1 + p
+  WVN_REQUIRE(cfg->registers == 0 || cfg->head_out == 0, "vit: register tokens and a STEGO head cannot be combined");
   wvn_vit* h = new wvn_vit();
   h->cfg = *cfg;
   if (h->cfg.ln_eps <= 0.f) h->cfg.ln_eps = 1e-6f;
   h->grid = cfg->image_size / cfg->patch_size;  // conv-floor semantics for non-divisible sizes
   h->P = h->grid * h->grid;
-  h->n_valid = h->P + 1;
+  h->t0 = 1 + cfg->registers;
+  h->n_valid = h->t0 + h->P;
   h->npad = round_up(h->n_valid, 128);
   h->kpe = 3 * cfg->patch_size * cfg->patch_size;
   h->kpe_ld = patch_pitch(cfg->patch_size);  // == gemm_w_pitch(kpe): patch rows and weight rows share one pitch
@@ -204,7 +209,8 @@ int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
   int rc = WVN_OK;
   auto add = [&](const std::string& n, long long numel, bool bf) { if (rc == WVN_OK) rc = h->add_weight(n, numel, bf); };
   add("cls_token", D, false);
-  add("pos_embed", static_cast<long long>(h->n_valid) * D, false);
+  add("pos_embed", static_cast<long long>(1 + h->P) * D, false);
+  if (cfg->registers > 0) add("register_tokens", static_cast<long long>(cfg->registers) * D, false);
   if (rc == WVN_OK) rc = h->add_weight("patch_embed.proj.weight", static_cast<long long>(D) * h->kpe, true, h->kpe, h->kpe_ld);
   add("patch_embed.proj.bias", D, false);
   for (int i = 0; i < cfg->depth; ++i) {
@@ -379,15 +385,18 @@ int vit_forward_impl(wvn_vit_t* h, const void* img, bool u8_hwc, int src_batch, 
     ia.batch = nb;
     ia.frame0 = b0; ia.src_frames = src_batch; ia.flip_from = flip_tta ? src_batch : (1 << 30);
     WVN_PROPAGATE(image_to_patches(img, u8_hwc, h->ape.p, ia, s));
-    WVN_PROPAGATE(init_token_rows(x, h->wp<float>("cls_token"), h->wp<float>("pos_embed"), nb, h->npad, h->n_valid, D, s));
+    const float* reg = c.registers > 0 ? h->wp<float>("register_tokens") : nullptr;
+    WVN_PROPAGATE(init_token_rows(x, h->wp<float>("cls_token"), h->wp<float>("pos_embed"), reg, c.registers, nb, h->npad,
+                                  h->n_valid, D, s));
     {
       GemmArgs g;
       g.M = nb * h->P; g.N = D; g.K = h->kpe; g.epi = EPI_PATCH; g.bias = h->wp<float>("patch_embed.proj.bias");
       g.out = x; g.ldo = D; g.pos = h->wp<float>("pos_embed"); g.tokens_in = h->P; g.npad = h->npad;
+      g.registers = c.registers;
       WVN_PROPAGATE(gemm_bf16(g, h->ape.p, h->kpe_ld, h->wp<void>("patch_embed.proj.weight"), 0, s));
     }
     LayerNormArgs la;
-    la.rows = rows; la.dim = D; la.eps = c.ln_eps; la.npad = h->npad; la.n_valid = h->n_valid;
+    la.rows = rows; la.dim = D; la.eps = c.ln_eps; la.npad = h->npad; la.n_valid = h->n_valid; la.row0 = h->t0;
     // GEMMs / LayerNorms can run over sub-chunks of `sub` frames ($WVN_VIT_SUBCHUNK) to keep xn / hid / x
     // L2-resident between producer and consumer.  Smaller GEMMs lose to wave quantisation what they gain in L2
     // hits, which the snake order below already collects for the rows written last — default off.
@@ -840,7 +849,7 @@ int wvn_mlp_infer_pixels_vit(wvn_mlp_infer_t* h, wvn_vit_t* vit, int batch, int 
     const int nb = std::min(kFusedFrames, batch - b0);
     const __nv_bfloat16* tok = reinterpret_cast<const __nv_bfloat16*>(vit->tok_bf16.p) +
                                static_cast<long long>(b0) * vit->npad * vit->cfg.dim;
-    WVN_PROPAGATE(pixels_fused_chunk(h, tok, vit->npad, 1, b0, nb, g, g, out_h, out_w, ww, cg_mean, cg_std, std_factor, trav,
+    WVN_PROPAGATE(pixels_fused_chunk(h, tok, vit->npad, vit->t0, b0, nb, g, g, out_h, out_w, ww, cg_mean, cg_std, std_factor, trav,
                                      conf, S(stream)));
   }
   return WVN_OK;

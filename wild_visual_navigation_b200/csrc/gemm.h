@@ -9,7 +9,7 @@ enum GemmEpilogue : int {
   EPI_BF16 = 0,       // out(bf16)[row, col]  = act(acc + bias)
   EPI_F32 = 1,        // out(f32)[row, col]   = acc + bias
   EPI_RESID_F32 = 2,  // out(f32)[row, col] += acc + bias            (residual stream, in place)
-  EPI_PATCH = 3,      // out(f32)[frame*npad + 1 + tok, col] = acc + bias + pos[1 + tok, col]
+  EPI_PATCH = 3,      // out(f32)[frame*npad + 1 + registers + tok, col] = acc + bias + pos[1 + tok, col]
   EPI_QKV = 4,        // scatter to Q/K [b,h,npad,64] and V^T [b,h,64,npad] (bf16)
   EPI_MLP_HEAD = 5,   // last layer of the traversability MLP fused with its consumers:
                       //   cols [0,feat) reconstruct x -> loss_reco = mean((out - x)^2) -> confidence,
@@ -27,6 +27,7 @@ struct GemmArgs {
   // EPI_PATCH
   const float* pos = nullptr;   // [1 + tokens_in, ldo] positional embedding (row 0 = CLS)
   int tokens_in = 0;            // patches per frame (rows of A per frame)
+  int registers = 0;            // register tokens between CLS and the first patch row (no position embedding)
   // EPI_PATCH / EPI_QKV
   int npad = 0;                 // padded tokens per frame in the activation layout
   // EPI_QKV

@@ -121,10 +121,10 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& args, const float 
     orow[h] = row;
     tok[h] = 0;
     if (EPI == EPI_PATCH) {
-      // patch row -> token row (frame * npad + 1 + token) of the residual stream
+      // patch row -> token row (frame * npad + 1 + registers + token) of the residual stream
       const int frame = row / args.tokens_in;
       tok[h] = row - frame * args.tokens_in;
-      orow[h] = static_cast<long long>(frame) * args.npad + 1 + tok[h];
+      orow[h] = static_cast<long long>(frame) * args.npad + (1 + args.registers) + tok[h];
     }
   }
 #pragma unroll
@@ -502,6 +502,11 @@ int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, in
     WVN_REQUIRE(a.dim % 64 == 0 && a.N == 3 * a.dim && a.heads * 64 == a.dim && a.npad % 8 == 0 && a.npad % BM == 0 &&
                     a.M % a.npad == 0,
                 "gemm: bad QKV epilogue geometry (dim=%d heads=%d npad=%d N=%d M=%d)", a.dim, a.heads, a.npad, a.N, a.M);
+  // patch embed: the CLS row, the register rows and the patch rows of a frame fit in its npad rows
+  if (a.epi == EPI_PATCH)
+    WVN_REQUIRE(a.tokens_in > 0 && a.registers >= 0 && 1 + a.registers + a.tokens_in <= a.npad,
+                "gemm: bad patch-embed epilogue geometry (tokens_in=%d registers=%d npad=%d)", a.tokens_in, a.registers,
+                a.npad);
   if (a.epi == EPI_F32 || a.epi == EPI_RESID_F32) WVN_REQUIRE(a.ldo % 4 == 0, "gemm: fp32 output pitch must be a multiple of 4");
   if (a.epi == EPI_BF16) WVN_REQUIRE(a.ldo % 8 == 0, "gemm: bf16 output pitch must be a multiple of 8");
   CUtensorMap ta, tb, tc[3] = {};

@@ -76,9 +76,12 @@ __global__ void image_to_patches_kernel(const void* __restrict__ img_raw, __nv_b
 }
 
 __global__ void init_token_rows_kernel(float* __restrict__ x, const float* __restrict__ cls,
-                                       const float* __restrict__ pos, int batch, int npad, int n_valid, int dim) {
-  // rows handled per frame: row 0 (CLS) and rows [n_valid, npad) (padding)
-  const int rows_per_frame = 1 + (npad - n_valid);
+                                       const float* __restrict__ pos, const float* __restrict__ reg, int registers,
+                                       int batch, int npad, int n_valid, int dim) {
+  // rows handled per frame: row 0 (CLS), rows [1, 1 + registers) (register tokens, no position embedding) and rows
+  // [n_valid, npad) (padding)
+  const int head_rows = 1 + registers;
+  const int rows_per_frame = head_rows + (npad - n_valid);
   const long long total = static_cast<long long>(batch) * rows_per_frame * dim;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -86,8 +89,9 @@ __global__ void init_token_rows_kernel(float* __restrict__ x, const float* __res
     const long long r = idx / dim;
     const int rr = static_cast<int>(r % rows_per_frame);
     const int b = static_cast<int>(r / rows_per_frame);
-    const int row = (rr == 0) ? 0 : (n_valid + rr - 1);
-    x[(static_cast<long long>(b) * npad + row) * dim + d] = (rr == 0) ? (cls[d] + pos[d]) : 0.f;
+    const int row = (rr < head_rows) ? rr : (n_valid + rr - head_rows);
+    const float v = (rr == 0) ? (cls[d] + pos[d]) : (rr < head_rows ? reg[static_cast<long long>(rr - 1) * dim + d] : 0.f);
+    x[(static_cast<long long>(b) * npad + row) * dim + d] = v;
   }
 }
 
@@ -119,12 +123,12 @@ layernorm_rows_kernel(const float* __restrict__ x, const float* __restrict__ gam
       q += (dx * dx + dy * dy) + (dz * dz + dw * dw);
     }
     const float rstd = rsqrtf(warp_sum(q) * (1.f / D) + a.eps);
-    // optional fp32 output: only real patch tokens (CLS and padding dropped)
+    // optional fp32 output: only real patch tokens (CLS, register and padding rows dropped)
     long long f32_row = -1;
     if (out_f32 != nullptr) {
       const int tok = static_cast<int>(row % a.npad);
       const long long frame = row / a.npad;
-      if (tok >= 1 && tok < a.n_valid) f32_row = frame * (a.n_valid - 1) + (tok - 1);
+      if (tok >= a.row0 && tok < a.n_valid) f32_row = frame * (a.n_valid - a.row0) + (tok - a.row0);
     }
 #pragma unroll
     for (int i = 0; i < ITERS; ++i) {
@@ -234,13 +238,16 @@ int image_to_patches(const void* img, bool u8_hwc, void* out_bf16, const ImagePa
   return WVN_OK;
 }
 
-int init_token_rows(float* x, const float* cls, const float* pos, int batch, int npad, int n_valid, int dim,
-                    cudaStream_t stream) {
-  const long long total = static_cast<long long>(batch) * (1 + npad - n_valid) * dim;
+int init_token_rows(float* x, const float* cls, const float* pos, const float* reg, int registers, int batch, int npad,
+                    int n_valid, int dim, cudaStream_t stream) {
+  WVN_REQUIRE(registers >= 0 && (registers == 0 || reg != nullptr), "init_token_rows: %d registers without their weights",
+              registers);
+  const long long total = static_cast<long long>(batch) * (1 + registers + npad - n_valid) * dim;
   const int threads = 256;
   long long blocks = (total + threads - 1) / threads;
   if (blocks > 4096) blocks = 4096;
-  init_token_rows_kernel<<<static_cast<unsigned>(blocks), threads, 0, stream>>>(x, cls, pos, batch, npad, n_valid, dim);
+  init_token_rows_kernel<<<static_cast<unsigned>(blocks), threads, 0, stream>>>(x, cls, pos, reg, registers, batch, npad,
+                                                                                n_valid, dim);
   WVN_CHECK_LAUNCH("init_token_rows_kernel");
   return WVN_OK;
 }

@@ -24,8 +24,9 @@ struct LayerNormArgs {
   long long rows = 0;
   int dim = 0;
   float eps = 1e-6f;
-  // only used when an fp32 output is requested (drops CLS + padding rows)
-  int npad = 0, n_valid = 0;
+  // only used when an fp32 output is requested: keeps rows [row0, n_valid) of each npad-row frame (drops CLS, register
+  // and padding rows); row0 = 1 + register tokens
+  int npad = 0, n_valid = 0, row0 = 1;
   int reverse = 0;  // walk the rows last-to-first (start where the producer kernel finished: those rows are still in L2)
 };
 
@@ -36,8 +37,10 @@ __host__ __device__ inline int patch_pitch(int p) { return (3 * p * p + 7) / 8 *
 // img: [batch, 3, in_h, in_w] fp32 in [0,1], or (u8_hwc) [batch, in_h, in_w, 3] uint8 RGB
 // out_bf16: [batch * grid_h * grid_w, patch_pitch(patch)] bf16; patch in {8, 14, 16}
 int image_to_patches(const void* img, bool u8_hwc, void* out_bf16, const ImagePatchArgs& a, cudaStream_t stream);
-int init_token_rows(float* x, const float* cls, const float* pos, int batch, int npad, int n_valid, int dim,
-                    cudaStream_t stream);
+// Per frame: row 0 = cls + pos[0], rows [1, 1 + registers) = reg (no position embedding), rows [n_valid, npad) = 0;
+// the patch rows [1 + registers, n_valid) are left to the patch-embed GEMM.
+int init_token_rows(float* x, const float* cls, const float* pos, const float* reg, int registers, int batch, int npad,
+                    int n_valid, int dim, cudaStream_t stream);
 int layernorm_rows(const float* x, const float* gamma, const float* beta, void* out_bf16, float* out_f32,
                    const LayerNormArgs& a, cudaStream_t stream);
 

@@ -25,9 +25,10 @@ class _Cfg(dict):
 
 class DinoInterface:
     """``backbone="dino"``: DINO ViT-S / ViT-B at ``patch_size`` 8 or 16.  ``backbone="dinov2"``: DINOv2 ViT-S/14 /
-    ViT-B/14 (no register tokens).  DINOv2 is released at patch 14 only, so it runs at patch 14 whatever ``patch_size``
-    says (the reference's ROS default passes ``patch_size=8`` with ``dinov2``); ``vit_patch_size`` still returns the
-    configured value, as the reference's property does, while ``grid`` is the token grid actually run."""
+    ViT-B/14 (no register tokens).  ``backbone="dinov2_reg"``: DINOv2 ViT-S/14-reg / ViT-B/14-reg (4 register tokens;
+    only the patch tokens are returned).  DINOv2 is released at patch 14 only, so both run at patch 14 whatever
+    ``patch_size`` says (the reference's ROS default passes ``patch_size=8`` with ``dinov2``); ``vit_patch_size`` still
+    returns the configured value, as the reference's property does, while ``grid`` is the token grid actually run."""
 
     def __init__(self, device: str, backbone: str = "dino", input_size: int = 448, backbone_type: str = "vit_small",
                  patch_size: int = 8, projection_type: str = None, dropout_p: float = 0,
@@ -39,14 +40,14 @@ class DinoInterface:
             self._cfg = _Cfg(backbone=backbone, backbone_type=backbone_type, input_size=input_size,
                              patch_size=patch_size, projection_type=projection_type, dropout_p=dropout_p,
                              pretrained_weights=pretrained_weights)
-        if self._cfg.backbone not in ("dino", "dinov2"):
+        if self._cfg.backbone not in ("dino", "dinov2", "dinov2_reg"):
             raise ValueError(f"backbone '{self._cfg.backbone}' is outside the H100 hot path (DINO / DINOv2 ViT only)")
         if not str(device).startswith("cuda"):
             raise RuntimeError("wild_visual_navigation_b200 runs on CUDA (sm_90a) devices only — no CPU fallback")
         self._device = device
         shp = VIT_SHAPES[self._cfg.backbone_type]
         backbone = self._cfg.backbone
-        patch = DINOV2_PATCH if backbone == "dinov2" else self._cfg.patch_size
+        patch = DINOV2_PATCH if backbone in ("dinov2", "dinov2_reg") else self._cfg.patch_size
         if state_dict is not None:
             sd = check_backbone_family(state_dict, backbone)
         else:

@@ -7,10 +7,10 @@
     when ``return_dense_features=True`` asks for it;
   * adjacency + centroids come from the same pass (no per-segment Python loops / host syncs);
   * when segmentation and features are both "stego"/"dino" on the same backbone, one ViT forward
-    serves both (the reference runs two backbones); with "dinov2" features, STEGO's DINO backbone segments and a
-    second, DINOv2 handle gives the features.
+    serves both (the reference runs two backbones); with "dinov2" / "dinov2_reg" features, STEGO's DINO backbone
+    segments and a second, DINOv2 handle gives the features.
 Supported: segmentation_type in {"slic" (the constructor default), "stego", "grid", "random", "none"/None},
-feature_type in {"dino", "dinov2", "stego"}.  "slic" is an all-integer SLIC kernel (csrc/slic_kernels.cu; fast_slic itself is an
+feature_type in {"dino", "dinov2", "dinov2_reg", "stego"}.  "slic" is an all-integer SLIC kernel (csrc/slic_kernels.cu; fast_slic itself is an
 un-vendored C++ package, see oracle/slic.py for what is and is not restated).  "sift", "torchvision", "histogram"
 features are out of scope (SURVEY.md §2) and raise.
 """
@@ -48,7 +48,7 @@ class FeatureExtractor:
             self._feature_dim = 384 if common["backbone_type"] == "vit_small" else 768
         else:
             raise ValueError(f"Extractor[{feature_type}] is outside the H100 hot path")
-        # the feature backbone, as the reference picks it (feature_extractor.py:61): "dino" or "dinov2"
+        # the feature backbone, as the reference picks it (feature_extractor.py:61): "dino", "dinov2" or "dinov2_reg"
         backbone = kwargs.get("backbone", feature_type)
         # STEGO's own backbone is DINO; it serves the features too unless they come from another backbone
         share = feature_type == "stego" or backbone == "dino"

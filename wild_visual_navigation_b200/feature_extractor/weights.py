@@ -8,7 +8,8 @@ The reference downloads DINO checkpoints from dl.fbaipublicfiles.com at construc
   * otherwise seeded DINO-style random weights are generated (SURVEY.md §8d) — results are then
     numerically meaningful only for parity / throughput work, and a warning says so.
 DINOv2 (``backbone="dinov2"``, the ``dinov2_vit{s,b}14_pretrain.pth`` checkpoints) uses the same key names plus the
-LayerScale gammas ``blocks.N.ls{1,2}.gamma`` and an unused ``mask_token``.
+LayerScale gammas ``blocks.N.ls{1,2}.gamma`` and an unused ``mask_token``; DINOv2 with registers
+(``backbone="dinov2_reg"``, ``dinov2_vit{s,b}14_reg4_pretrain.pth``) adds ``register_tokens`` (1, R, D).
 """
 from __future__ import annotations
 
@@ -71,30 +72,54 @@ def synthetic_dinov2_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09):
     return sd
 
 
+# Every released DINOv2 *_reg checkpoint has 4 register tokens
+DINOV2_REGISTERS = 4
+# std of the seeded register tokens, that of cls_token and pos_embed.  The final LayerNorm and every block's norm1 see
+# only a register's direction, so its scale barely sets how much the patch tokens attend to it; what it sets is how
+# much an added pos[0] turns it: at 0.02 that moves the ViT-S/14 tokens at 224 by about 0.1 rel-L2, as much as zeroing
+# (0.1) or dropping (0.08) the registers, while at std 1 the same pos[0] moves them by less than 5e-3.
+DINOV2_REGISTER_STD = 0.02
+
+
+def synthetic_dinov2_reg_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09, registers=DINOV2_REGISTERS):
+    """Seeded DINOv2-with-registers weights: ``synthetic_dinov2_state_dict`` plus ``register_tokens`` (1, R, dim), drawn
+    from their own generator (seed + 2) with std DINOV2_REGISTER_STD."""
+    sd = synthetic_dinov2_state_dict(dim, depth, mlp_dim, seed, attn_std)
+    g = torch.Generator().manual_seed(seed + 2)
+    sd["register_tokens"] = torch.randn(1, registers, dim, generator=g) * DINOV2_REGISTER_STD
+    return sd
+
+
 def check_backbone_family(sd: dict, backbone: str) -> dict:
-    """Checks that a ViT state dict belongs to ``backbone`` ("dino": DINO v1, "dinov2": DINOv2 without registers) and
-    returns it with the keys the backbone does not use dropped (DINOv2's ``mask_token``).  Raises ValueError on a
-    checkpoint of the other family or on register tokens (the ``_reg`` variants are not supported)."""
+    """Checks that a ViT state dict belongs to ``backbone`` ("dino": DINO v1, "dinov2": DINOv2 without registers,
+    "dinov2_reg": DINOv2 with register tokens) and returns it with the keys the backbone does not use dropped (DINOv2's
+    ``mask_token``).  Raises ValueError on a checkpoint of another family."""
     sd = {k.replace("module.", "").replace("backbone.", ""): v for k, v in sd.items()}
-    if "register_tokens" in sd:
-        raise ValueError("ViT checkpoints with register tokens (DINOv2 *_reg) are not supported")
+    has_reg = "register_tokens" in sd
     has_ls = "blocks.0.ls1.gamma" in sd
     patch = int(sd["patch_embed.proj.weight"].shape[-1])
-    if backbone == "dinov2":
+    if backbone in ("dinov2", "dinov2_reg"):
         if not has_ls or patch != DINOV2_PATCH:
-            raise ValueError(f"backbone 'dinov2' needs a DINOv2 checkpoint (LayerScale 'ls1.gamma' and a 14x14 patch "
+            raise ValueError(f"backbone '{backbone}' needs a DINOv2 checkpoint (LayerScale 'ls1.gamma' and a 14x14 patch "
                              f"conv); got one with{'' if has_ls else 'out'} LayerScale and a {patch}x{patch} patch conv")
+        if backbone == "dinov2" and has_reg:
+            raise ValueError("backbone 'dinov2' got a checkpoint with register tokens (DINOv2 *_reg): pass "
+                             "backbone='dinov2_reg'")
+        if backbone == "dinov2_reg" and not has_reg:
+            raise ValueError("backbone 'dinov2_reg' needs a checkpoint with register tokens ('register_tokens'): pass "
+                             "backbone='dinov2' for the DINOv2 checkpoints without them")
         return {k: v for k, v in sd.items() if k != "mask_token"}
-    if has_ls or "mask_token" in sd:
-        raise ValueError("backbone 'dino' got a DINOv2 checkpoint (LayerScale gammas / mask_token): pass "
-                         "backbone='dinov2'")
+    if has_ls or has_reg or "mask_token" in sd:
+        raise ValueError("backbone 'dino' got a DINOv2 checkpoint (LayerScale gammas / mask_token / register tokens): "
+                         "pass backbone='dinov2' or backbone='dinov2_reg'")
     return sd
 
 
 def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights=None, seed: int = 1,
                          backbone: str = "dino"):
-    """DINO (``backbone="dino"``) or DINOv2 (``"dinov2"``, always patch 14) weights, from ``pretrained_weights`` /
-    ``$WVN_DINO_WEIGHTS`` or seeded.  A checkpoint is checked against the family (check_backbone_family)."""
+    """DINO (``backbone="dino"``), DINOv2 (``"dinov2"``) or DINOv2 with registers (``"dinov2_reg"``; both always patch
+    14) weights, from ``pretrained_weights`` / ``$WVN_DINO_WEIGHTS`` or seeded.  A checkpoint is checked against the
+    family (check_backbone_family)."""
     shp = VIT_SHAPES[backbone_type]
     path = pretrained_weights or os.environ.get("WVN_DINO_WEIGHTS")
     if path:
@@ -108,6 +133,8 @@ def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights
                   f"{backbone.upper()}-style weights — fine for parity and throughput work, not for real traversability")
     if backbone == "dinov2":
         return synthetic_dinov2_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], seed)
+    if backbone == "dinov2_reg":
+        return synthetic_dinov2_reg_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], seed)
     return synthetic_dino_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], patch_size, 224 // patch_size, seed)
 
 

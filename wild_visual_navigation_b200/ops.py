@@ -237,6 +237,20 @@ def interpolate_pos_embed(pos_embed: torch.Tensor, grid: int) -> torch.Tensor:
     return torch.cat((pos_embed[:, :1], patch), dim=1)
 
 
+def interpolate_pos_embed_antialias(pos_embed: torch.Tensor, grid: int) -> torch.Tensor:
+    """The interpolation of the DINOv2 register models (hub ``interpolate_antialias=True, interpolate_offset=0``):
+    bicubic with antialias straight to ``size=(grid, grid)``, no +0.1 trick.  The CLS row passes through."""
+    n_pre = pos_embed.shape[1] - 1
+    if n_pre == grid * grid:
+        return pos_embed
+    dim = pos_embed.shape[-1]
+    side = int(math.sqrt(n_pre))
+    patch = F.interpolate(pos_embed[:, 1:].reshape(1, side, side, dim).permute(0, 3, 1, 2).float(),
+                          size=(grid, grid), mode="bicubic", antialias=True)
+    patch = patch.permute(0, 2, 3, 1).reshape(1, -1, dim)
+    return torch.cat((pos_embed[:, :1], patch), dim=1)
+
+
 def fold_layerscale(sd: dict, depth: int) -> dict:
     """DINOv2's LayerScale ``x += gamma * f(x)`` folded into the layer that ends f, in fp32 before any bf16 cast:
     ``attn.proj`` weight rows and bias times ``ls1.gamma``, ``mlp.fc2`` weight rows and bias times ``ls2.gamma``
@@ -256,7 +270,9 @@ def fold_layerscale(sd: dict, depth: int) -> dict:
 
 
 class ViTBackbone:
-    """Owns a ``wvn_vit_t``: DINO / DINOv2 ViT weights (bf16 on device) + L2-sized activation workspaces."""
+    """Owns a ``wvn_vit_t``: DINO / DINOv2 ViT weights (bf16 on device) + L2-sized activation workspaces.  A state dict
+    with ``register_tokens`` (1, R, D) (DINOv2 *_reg) gives a handle with R register tokens after CLS, whose position
+    embeddings are interpolated by the register models' antialiased form."""
 
     def __init__(self, image_size, patch_size, dim, depth, heads, mlp_dim, state_dict, max_batch=32, chunk=0,
                  head_weights=None, ln_eps=1e-6):
@@ -266,7 +282,10 @@ class ViTBackbone:
         self.P = self.grid * self.grid
         self.max_batch = max_batch
         self.head_out = 0 if head_weights is None else int(head_weights["head_a.weight"].shape[0])
-        cfg = VitConfig(image_size, patch_size, dim, depth, heads, mlp_dim, max_batch, chunk, ln_eps, self.head_out)
+        reg = next((v for k, v in state_dict.items() if k.endswith("register_tokens")), None)
+        self.registers = 0 if reg is None else int(reg.shape[-2])
+        cfg = VitConfig(image_size, patch_size, dim, depth, heads, mlp_dim, max_batch, chunk, ln_eps, self.head_out,
+                        self.registers)
         h = c_void_p()
         check(lib().wvn_vit_create(byref(cfg), byref(h)))
         self._h = h
@@ -284,7 +303,10 @@ class ViTBackbone:
         sd = {k.replace("module.", "").replace("backbone.", ""): v for k, v in sd.items()}
         sd = fold_layerscale(sd, depth)
         self._set("cls_token", sd["cls_token"].reshape(-1))
-        self._set("pos_embed", interpolate_pos_embed(sd["pos_embed"].float().cpu(), self.grid).reshape(-1))
+        interp = interpolate_pos_embed_antialias if self.registers > 0 else interpolate_pos_embed
+        self._set("pos_embed", interp(sd["pos_embed"].float().cpu(), self.grid).reshape(-1))
+        if self.registers > 0:
+            self._set("register_tokens", sd["register_tokens"].reshape(-1))
         self._set("patch_embed.proj.weight", sd["patch_embed.proj.weight"].reshape(self.dim, -1))
         self._set("patch_embed.proj.bias", sd["patch_embed.proj.bias"])
         for i in range(depth):
