@@ -222,20 +222,31 @@ def mlp_head_ref(y, eps_y, x, feat, trav_col, cg_mean, cg_std, std_factor):
              lo / hi are computed in fp32 from the fp32 scalars (error <= eta = 8 u (|mean| + std (|f| + 2))):
              |dconf| <= (|dloss| + 2 eta) / (hi - lo) + 4 u.
     Returns dict(trav, loss, conf, *_bound)."""
-    logit = y[:, trav_col]
-    trav = torch.sigmoid(logit)
     d = y[:, :feat] - x[:, :feat].double()
     eps = eps_y[:, :feat]
     loss = (d * d).sum(1) / feat
     u = U24
     dloss = ((2 * d.abs() * eps + eps * eps).sum(1) + (feat + 4) * u * ((d.abs() + eps) ** 2).sum(1)) / feat + u * loss
+    out = {"loss": loss, "loss_bound": dloss}
+    out.update(trav_ref(y[:, trav_col], eps_y[:, trav_col]))
+    out.update(conf_ref(loss, dloss, cg_mean, cg_std, std_factor))
+    return out
+
+
+def trav_ref(logit, eps_logit):
+    """mlp_head_ref's trav rule: sigmoid of the float64 logit, bound eps_logit / 4 + 2^-19."""
+    return {"trav": torch.sigmoid(logit), "trav_bound": eps_logit / 4 + 2.0 ** -19}
+
+
+def conf_ref(loss, dloss, cg_mean, cg_std, std_factor):
+    """mlp_head_ref's conf rule: conf of the float64 loss and its 1 / (hi - lo)-Lipschitz bound from dloss."""
+    u = U24
     mean, sd = float(cg_mean), float(cg_std)
     shifted = mean + sd * std_factor
     lo, hi = max(shifted - sd, 0.0), shifted + sd
     conf = 1 - (loss.clamp(lo, hi) - lo) / (hi - lo)
     eta = 8 * u * (abs(mean) + sd * (abs(std_factor) + 2))
-    return {"trav": trav, "trav_bound": eps_y[:, trav_col] / 4 + 2.0 ** -19, "loss": loss, "loss_bound": dloss,
-            "conf": conf, "conf_bound": (dloss + 2 * eta) / (hi - lo) + 4 * u, "lo": lo, "hi": hi}
+    return {"conf": conf, "conf_bound": (dloss + 2 * eta) / (hi - lo) + 4 * u, "lo": lo, "hi": hi}
 
 
 # ------------------------------------------------------------------------------------------------ CPU negative controls
