@@ -44,7 +44,8 @@ const char* wvn_last_error(void);
 /* 0 if device 0..n has compute capability 9.0, WVN_STATUS_NO_DEVICE otherwise. */
 int wvn_check_device(void);
 /* ABI version.  101: wvn_vit_config and wvn_gemm_ex_args gained a trailing `int registers` (0 = the layout of 100), so
- * callers that fill these structs by layout (ctypes mirrors, code compiled against an older header) must add the field. */
+ * callers that fill these structs by layout (ctypes mirrors, code compiled against an older header) must add the field.
+ * 102: adds wvn_mlp_trainer_copy_confidence (no layout change). */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -373,6 +374,10 @@ int wvn_mlp_trainer_init_comm(wvn_mlp_trainer_t* t, const void* id128, int rank,
  * running_n / running_sum / running_sum_of_squares (1,) fp64 — each may be NULL (the trainer then keeps a private copy). */
 int wvn_mlp_trainer_set_confidence(wvn_mlp_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
                                    double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov);
+/* Copies the confidence state src keeps itself (moving_average's window of 5 steps; var / running sums given as NULL to
+ * set_confidence) into dst, ordered on `stream`.  For replacing a trainer by a larger one: create the new one, copy,
+ * then destroy the old one; the generator continues as if nothing had changed. */
+int wvn_mlp_trainer_copy_confidence(wvn_mlp_trainer_t* dst, const wvn_mlp_trainer_t* src, void* stream);
 int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                        const float* x, int groups, int rows_per_group, const int* n_rows, const float* y,
                        const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,

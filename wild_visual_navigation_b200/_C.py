@@ -106,6 +106,7 @@ SIGNATURES = {
     "wvn_comm_unique_id": (_I, [_P]),
     "wvn_mlp_trainer_init_comm": (_I, [_P, _P, _I, _I]),
     "wvn_mlp_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
+    "wvn_mlp_trainer_copy_confidence": (_I, [_P, _P, _P]),
     "wvn_mlp_train_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
 }
 

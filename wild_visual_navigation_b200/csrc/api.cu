@@ -116,7 +116,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 101; }
+int wvn_version(void) { return 102; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -1020,6 +1020,11 @@ int wvn_mlp_trainer_set_confidence(wvn_mlp_trainer_t* t, int method, float* var,
   WVN_REQUIRE(t, "wvn_mlp_trainer_set_confidence: null trainer");
   return fused_trainer_set_confidence(t->impl, method, var, running_n, running_sum, running_sum_of_squares, kf_proc_cov,
                                       kf_meas_cov);
+}
+
+int wvn_mlp_trainer_copy_confidence(wvn_mlp_trainer_t* dst, const wvn_mlp_trainer_t* src, void* stream) {
+  WVN_REQUIRE(dst && src, "wvn_mlp_trainer_copy_confidence: null trainer");
+  return fused_trainer_copy_confidence(dst->impl, src->impl, S(stream));
 }
 
 int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,

@@ -723,6 +723,13 @@ int fused_trainer_set_confidence(FusedTrainer* t, int method, float* var, double
   return WVN_OK;
 }
 
+int fused_trainer_copy_confidence(FusedTrainer* dst, const FusedTrainer* src, cudaStream_t stream) {
+  WVN_REQUIRE(dst && src, "trainer: null handle");
+  // ordered after src's last step on the caller's stream; destroying src afterwards (cudaFree) waits for the copy
+  WVN_CHECK_CUDA(cudaMemcpyAsync(dst->conf_priv, src->conf_priv, sizeof(double) * 32, cudaMemcpyDeviceToDevice, stream));
+  return WVN_OK;
+}
+
 int fused_comm_unique_id(void* id128) {
   WVN_REQUIRE(id128, "comm: null id buffer");
   NcclApi& api = nccl();

@@ -51,6 +51,9 @@ int fused_trainer_init_comm(FusedTrainer* t, const void* id128, int rank, int wo
 // method: ConfMethod; pointers may be null for methods that do not use them (the trainer then keeps private state).
 int fused_trainer_set_confidence(FusedTrainer* t, int method, float* var, double* running_n, double* running_sum,
                                  double* running_sumsq, float kf_proc_cov, float kf_meas_cov);
+// Copies src's private confidence state (moving_average's window; var / running sums not bound to caller buffers) into
+// dst, on `stream`: a caller that replaces a trainer by a larger one keeps the generator where it was.
+int fused_trainer_copy_confidence(FusedTrainer* dst, const FusedTrainer* src, cudaStream_t stream);
 // phase_mask: 1 = forward + statistics (+ their all-reduce), 2 = backward + weight gradients (+ gradient all-reduce),
 // 4 = loss metrics + Adam; 7 = the whole step.
 int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,

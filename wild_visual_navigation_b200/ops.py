@@ -464,14 +464,17 @@ class MlpTrainer:
 
     # ---- fused path ---------------------------------------------------------------------------
     def _create(self, max_rows):
-        if self._h is not None:
-            lib().wvn_mlp_trainer_destroy(self._h)
-            self._h = None
-        self.max_rows = int(max_rows)
         h = c_void_p()
-        check(lib().wvn_mlp_trainer_create(self.dim, self.h1, self.h2, self.max_rows, byref(self.cfg), ptr(self.scalars),
+        check(lib().wvn_mlp_trainer_create(self.dim, self.h1, self.h2, int(max_rows), byref(self.cfg), ptr(self.scalars),
                                            ptr(self.grads), byref(h)))
+        if self._h is not None:
+            # both handles' workspaces are alive until the old one is destroyed: peak memory briefly doubles here.
+            # A larger trainer replaces this one: the confidence state it keeps itself (moving_average's window, var and
+            # running sums not bound to caller tensors) moves over, so the generator does not restart
+            check(lib().wvn_mlp_trainer_copy_confidence(h, self._h, stream()))
+            lib().wvn_mlp_trainer_destroy(self._h)
         self._h = h
+        self.max_rows = int(max_rows)
         if self._conf is not None:
             self.set_confidence(*self._conf)
         self.conf = torch.empty(self.max_rows + 32, device=self.params.device, dtype=torch.float32)
