@@ -45,7 +45,9 @@ const char* wvn_last_error(void);
 int wvn_check_device(void);
 /* ABI version.  101: wvn_vit_config and wvn_gemm_ex_args gained a trailing `int registers` (0 = the layout of 100), so
  * callers that fill these structs by layout (ctypes mirrors, code compiled against an older header) must add the field.
- * 102: adds wvn_mlp_trainer_copy_confidence (no layout change). */
+ * 102: adds wvn_mlp_trainer_copy_confidence (no layout change).
+ * 103: wvn_gemm_ex_args gained trailing `residual` / `ldr` (epi 6); adds the ResNet handle, the im2col / max-pool
+ * primitives and wvn_segment_pool_pyramid. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -77,7 +79,8 @@ int wvn_gemm_bf16(const void* a_bf16, long long lda, const void* w_bf16, const f
  *       rows [frame*npad, frame*npad + 1 + registers) — CLS and register tokens — are not written);
  *   4 = QKV: bf16 q_out, k_out [m/npad*heads, npad, 64] and vt_out [m/npad*heads, 64, npad] from the columns of [q | k | v];
  *   5 = MLP head: columns [0, feat) reconstruct x -> loss_reco = mean((out - x)^2) -> conf, column trav_col ->
- *       trav = sigmoid; nothing of [m, n] is stored.
+ *       trav = sigmoid; nothing of [m, n] is stored;
+ *   6 = residual: bf16 out[m,ldo] = act(acc + bias + residual[m,ldr]) (residual bf16, ldr even and >= n; act 0 or 1).
  * reverse_m = 1 walks the 64-row blocks last-to-first (the result must not change). */
 typedef struct {
   int m, n, k;
@@ -106,6 +109,8 @@ typedef struct {
   float cg_std_factor;
   int reverse_m;
   int registers;            /* epi 3: register tokens between CLS and the first patch row (0 = DINO / DINOv2 layout) */
+  const void* residual;     /* epi 6: [m, ldr] bf16 */
+  long long ldr;
 } wvn_gemm_ex_args;
 int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* args, void* stream);
 
@@ -196,6 +201,49 @@ int wvn_vit_stego_head(wvn_vit_t* h, int batch, float* out, void* stream);
 int wvn_vit_npad(const wvn_vit_t* h);
 
 /* ------------------------------------------------------------------------------------------
+ * ResNet backbone handle — replaces TorchVisionInterface's model (wild_visual_navigation/feature_extractor/
+ * torchvision_interface.py:22-101: torchvision resnet18 / resnet50 behind create_feature_extractor).
+ * Activations are NHWC bf16 with fp32 accumulation; every conv is one wgmma GEMM over its output pixels (1 x 1 /
+ * stride 1 convs straight on the activation rows, the others after an im2col pass whose rows are round_up(K, 8)
+ * elements apart), with bias, residual and ReLU in the GEMM's epilogue.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct wvn_resnet wvn_resnet_t;
+
+typedef struct {
+  int image_size;   /* side of the square input, a multiple of 32 (e.g. 448) */
+  int depth;        /* 18 (BasicBlock [2,2,2,2]) or 50 (Bottleneck [3,4,6,3]) */
+  int max_batch;    /* largest batch a forward call may carry; the workspaces are sized for it at create */
+} wvn_resnet_config;
+
+int wvn_resnet_create(const wvn_resnet_config* cfg, wvn_resnet_t** out);
+void wvn_resnet_destroy(wvn_resnet_t* h);
+/* Bytes of activation and im2col workspace the handle allocated at create. */
+size_t wvn_resnet_workspace_bytes(const wvn_resnet_t* h);
+/* Weights use the torchvision state-dict names of the convolutions, with eval-mode batch norm already folded in
+ * (w * gamma / sqrt(var + eps) per output channel, bias = beta - mean * gamma / sqrt(var + eps)), fp32, host or device:
+ *   conv1.{weight,bias}, layer{L}.{B}.conv{1,2[,3]}.{weight,bias}, layer{L}.0.downsample.{weight,bias}
+ * (the downsample conv + its batch norm, where the block has one).  A weight is given in (out, ky, kx, in) order —
+ * torch's [out, in, ky, kx] tensor permuted to (0, 2, 3, 1) — and a bias has `out` elements. */
+int wvn_resnet_set_weight(wvn_resnet_t* h, const char* name, const float* data, long long numel);
+/* img: [batch, 3, image_size, image_size] fp32 in [0, 1]; ImageNet Normalize is applied in the stem's loader, before
+ * the zero padding.  taps: host array of four device pointers, each an NHWC bf16 map [batch, h_l, w_l, c_l]:
+ *   depth 18: layer{1,2,3,4}.1.relu_1 (the stage outputs): 64 @ S/4, 128 @ S/8, 256 @ S/16, 512 @ S/32;
+ *   depth 50: layer{2,3,4}.0.relu (after bn1 of each stage's first block): 128 @ S/4, 256 @ S/8, 512 @ S/16,
+ *             and layer4.2.relu_2 (the trunk output): 2048 @ S/32. */
+int wvn_resnet_forward(wvn_resnet_t* h, const float* img, int batch, void* const* taps, void* stream);
+
+/* The ResNet path's primitives, exposed for testing.  im2col rows of an NHWC bf16 map [batch, h, w, c] (c % 8 == 0):
+ * row (b, oy, ox) holds the k x k window at (oy * stride - pad, ox * stride - pad) in (ky, kx, channel) order, zero
+ * outside the map; rows are `pitch` elements apart and columns [k*k*c, pitch) are left as they are.
+ * wvn_im2col_image: the same rows (k*k*3 columns) from the fp32 NCHW image [batch, 3, h, w] after ImageNet Normalize.
+ * wvn_maxpool3s2_bf16_nhwc: 3 x 3 / stride 2 / pad 1 max-pool with -inf padding, out [batch, (h+1)/2, (w+1)/2, c]. */
+int wvn_im2col_bf16_nhwc(const void* in, int batch, int h, int w, int c, int k, int stride, int pad, void* out,
+                         long long pitch, void* stream);
+int wvn_im2col_image(const float* img, int batch, int h, int w, int k, int stride, int pad, void* out, long long pitch,
+                     void* stream);
+int wvn_maxpool3s2_bf16_nhwc(const void* in, int batch, int h, int w, int c, void* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Token grid -> image resolution
  * ---------------------------------------------------------------------------------------- */
 /* F.interpolate(features, (out,out), "bilinear", align_corners=True) (dino_interface.py:87-90).
@@ -239,6 +287,16 @@ size_t wvn_segment_workspace_bytes(int batch, int smax, int gh, int gw);
 int wvn_segment_reduce(const long long* seg, int batch, int h, int w, int smax, const float* tokens, int gh, int gw,
                        int dim, float* feat, float* centers, long long* edges, int* n_edges, int max_edges,
                        void* workspace, void* stream);
+/* Multiscale segment pooling — replaces the feature-pyramid branch of FeatureExtractor.sparsify_features
+ * (feature_extractor.py:314-366).  seg: [batch, h, w] int64 (ids outside [0, smax) ignored); taps: host array of four
+ * device pointers to NHWC bf16 maps [batch, tap_h[l], tap_w[l], tap_c[l]] (host int arrays), each level dividing h x w;
+ * centers: [batch, smax, 2] fp32 (col, row) as wvn_segment_reduce returns them.  out: [batch, smax, sum(tap_c)] fp32 —
+ * per level, the mean of the level's cells whose nearest-downsampled id seg[i*h/tap_h, j*w/tap_w] is the segment;
+ * a segment with no such cell takes the cell (clamp(floor(row*tap_h/h)), clamp(floor(col*tap_w/w))) under its centroid
+ * (the reference raises AttributeError there); a segment without pixels gets a NaN row, as wvn_segment_reduce's feat. */
+int wvn_segment_pool_pyramid(const long long* seg, int batch, int h, int w, int smax, const float* centers,
+                             void* const* taps, const int* tap_h, const int* tap_w, const int* tap_c, float* out,
+                             void* stream);
 /* In-place relabel of each frame to 0..S-1; scratch: [batch*num_labels] int32; counts: [batch] int32. */
 int wvn_segment_relabel(long long* seg, int batch, long long pix_per_frame, int num_labels, int* scratch, int* counts,
                         void* stream);

@@ -37,8 +37,12 @@ class GemmExArgs(Structure):
         ("q_out", c_void_p), ("k_out", c_void_p), ("vt_out", c_void_p),
         ("feat", c_int), ("trav_col", c_int), ("x", c_void_p), ("ldx", c_longlong), ("trav", c_void_p),
         ("conf", c_void_p), ("loss_reco", c_void_p), ("cg_mean", c_void_p), ("cg_std", c_void_p),
-        ("cg_std_factor", c_float), ("reverse_m", c_int), ("registers", c_int),
+        ("cg_std_factor", c_float), ("reverse_m", c_int), ("registers", c_int), ("residual", c_void_p), ("ldr", c_longlong),
     ]
+
+
+class ResnetConfig(Structure):
+    _fields_ = [("image_size", c_int), ("depth", c_int), ("max_batch", c_int)]
 
 
 class TrainConfig(Structure):
@@ -71,6 +75,15 @@ SIGNATURES = {
     "wvn_vit_forward_tta": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),
     "wvn_vit_stego_head": (_I, [_P, _I, _P, _P]),
     "wvn_vit_npad": (_I, [_P]),
+    "wvn_resnet_create": (_I, [POINTER(ResnetConfig), POINTER(_P)]),
+    "wvn_resnet_destroy": (None, [_P]),
+    "wvn_resnet_workspace_bytes": (_S, [_P]),
+    "wvn_resnet_set_weight": (_I, [_P, c_char_p, _P, _L]),
+    "wvn_resnet_forward": (_I, [_P, _P, _I, _P, _P]),
+    "wvn_im2col_bf16_nhwc": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
+    "wvn_im2col_image": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
+    "wvn_maxpool3s2_bf16_nhwc": (_I, [_P, _I, _I, _I, _I, _P, _P]),
+    "wvn_segment_pool_pyramid": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "wvn_upsample_dense": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "wvn_logits_argmax": (_I, [_P, _L, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "wvn_flip_average": (_I, [_P, _I, _I, _I, _L, _P]),

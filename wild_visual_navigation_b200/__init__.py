@@ -1,7 +1,7 @@
 """wild_visual_navigation_b200 — H100-native (sm_90a) hot path of Wild Visual Navigation.
 
 Keeps the reference's class surface for the per-frame path (SURVEY.md §8b):
-``FeatureExtractor`` / ``DinoInterface`` / ``StegoInterface`` / ``SegmentExtractor`` /
+``FeatureExtractor`` / ``DinoInterface`` / ``TorchVisionInterface`` / ``StegoInterface`` / ``SegmentExtractor`` /
 ``SimpleMLP`` / ``get_model`` / ``Data`` / ``Batch`` / ``ConfidenceGenerator`` /
 ``TraversabilityLoss`` / ``TraversabilityEstimator`` — implemented on hand-written CUDA
 kernels behind the C ABI in ``include/wvn_b200.h``.  No CPU fallback.
@@ -17,6 +17,7 @@ from .feature_extractor import (  # noqa: E402,F401
     StegoInterface,
     SegmentExtractor,
     FeatureExtractor,
+    TorchVisionInterface,
 )
 from .traversability_estimator import TraversabilityEstimator  # noqa: E402,F401
 from .image_projector import ImageProjector  # noqa: E402,F401

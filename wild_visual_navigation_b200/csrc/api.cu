@@ -16,6 +16,7 @@
 #include "mlp_train.h"
 #include "mlp_train_fused.h"
 #include "pixel_head.h"
+#include "resnet_kernels.h"
 #include "segment_kernels.h"
 #include "footprint_kernels.h"
 #include "slic_kernels.h"
@@ -116,7 +117,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 102; }
+int wvn_version(void) { return 103; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -160,6 +161,7 @@ int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* x, void* stream) {
   g.feat = x->feat; g.trav_col = x->trav_col; g.x = x->x; g.ldx = x->ldx; g.trav = x->trav; g.conf = x->conf;
   g.loss_reco = x->loss_reco; g.cg_mean = x->cg_mean; g.cg_std = x->cg_std; g.cg_std_factor = x->cg_std_factor;
   g.reverse_m = x->reverse_m; g.registers = x->registers;
+  g.residual = x->residual; g.ldr = x->ldr;
   return gemm_bf16(g, x->a, x->lda, x->w, x->block_n, S(stream));
 }
 
@@ -276,12 +278,10 @@ void wvn_vit_destroy(wvn_vit_t* h) {
 
 int wvn_vit_npad(const wvn_vit_t* h) { return h ? h->npad : 0; }
 
-int wvn_vit_set_weight(wvn_vit_t* h, const char* name, const float* data, long long numel) {
-  WVN_REQUIRE(h && name && data, "wvn_vit_set_weight: null argument");
-  auto it = h->w.find(name);
-  WVN_REQUIRE(it != h->w.end(), "wvn_vit_set_weight: unknown weight '%s'", name);
-  Weight& wt = it->second;
-  WVN_REQUIRE(wt.numel == numel, "wvn_vit_set_weight: '%s' expects %lld elements, got %lld", name, wt.numel, numel);
+// Copies fp32 `data` (host or device) into a handle's weight: fp32 storage as is, bf16 storage cast on the device (through
+// the `stage` buffer when the source is host memory), pitched rows into their padded rows.
+static int load_weight(Weight& wt, DevBuf& stage, const char* name, const float* data, long long numel) {
+  WVN_REQUIRE(wt.numel == numel, "set_weight: '%s' expects %lld elements, got %lld", name, wt.numel, numel);
   cudaPointerAttributes attr;
   bool on_device = false;
   if (cudaPointerGetAttributes(&attr, data) == cudaSuccess)
@@ -293,14 +293,14 @@ int wvn_vit_set_weight(wvn_vit_t* h, const char* name, const float* data, long l
     WVN_CHECK_CUDA(cudaMemcpy(wt.p, data, numel * 4, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
   } else if (wt.cols > 0) {
     // pitched rows: stage whole rows, cast each into its row of the padded storage
-    const long long chunk_rows = static_cast<long long>(h->stage.bytes / 4) / wt.cols;
+    const long long chunk_rows = static_cast<long long>(stage.bytes / 4) / wt.cols;
     const long long rows = numel / wt.cols;
     for (long long r0 = 0; r0 < rows; r0 += chunk_rows) {
       const long long n = std::min(chunk_rows, rows - r0);
       const float* src = data + r0 * wt.cols;
       if (!on_device) {
-        WVN_CHECK_CUDA(cudaMemcpy(h->stage.p, src, n * wt.cols * 4, cudaMemcpyHostToDevice));
-        src = reinterpret_cast<const float*>(h->stage.p);
+        WVN_CHECK_CUDA(cudaMemcpy(stage.p, src, n * wt.cols * 4, cudaMemcpyHostToDevice));
+        src = reinterpret_cast<const float*>(stage.p);
       }
       const int blocks = static_cast<int>(std::min<long long>((n * wt.cols + 255) / 256, 4096));
       cast_rows_kernel<<<blocks, 256, 0, 0>>>(src, reinterpret_cast<__nv_bfloat16*>(wt.p) + r0 * wt.ld, n, wt.cols, wt.ld);
@@ -308,13 +308,13 @@ int wvn_vit_set_weight(wvn_vit_t* h, const char* name, const float* data, long l
       WVN_CHECK_CUDA(cudaStreamSynchronize(0));
     }
   } else {
-    const long long chunk_elems = static_cast<long long>(h->stage.bytes / 4);
+    const long long chunk_elems = static_cast<long long>(stage.bytes / 4);
     for (long long off = 0; off < numel; off += chunk_elems) {
       const long long n = std::min(chunk_elems, numel - off);
       const float* src = data + off;
       if (!on_device) {
-        WVN_CHECK_CUDA(cudaMemcpy(h->stage.p, src, n * 4, cudaMemcpyHostToDevice));
-        src = reinterpret_cast<const float*>(h->stage.p);
+        WVN_CHECK_CUDA(cudaMemcpy(stage.p, src, n * 4, cudaMemcpyHostToDevice));
+        src = reinterpret_cast<const float*>(stage.p);
       }
       WVN_PROPAGATE(cast_to_bf16(src, reinterpret_cast<__nv_bfloat16*>(wt.p) + off, n, 0));
       WVN_CHECK_CUDA(cudaStreamSynchronize(0));
@@ -322,6 +322,14 @@ int wvn_vit_set_weight(wvn_vit_t* h, const char* name, const float* data, long l
   }
   wt.loaded = true;
   return WVN_OK;
+}
+
+
+int wvn_vit_set_weight(wvn_vit_t* h, const char* name, const float* data, long long numel) {
+  WVN_REQUIRE(h && name && data, "wvn_vit_set_weight: null argument");
+  auto it = h->w.find(name);
+  WVN_REQUIRE(it != h->w.end(), "wvn_vit_set_weight: unknown weight '%s'", name);
+  return load_weight(it->second, h->stage, name, data, numel);
 }
 
 static int vit_check_loaded(wvn_vit* h, bool need_head) {
@@ -636,6 +644,234 @@ int wvn_project_and_render(const float* K, const float* pose_camera_in_world, co
   a.batch = batch; a.n_points = n_points; a.h = h; a.w = w; a.color_batched = color_batched;
   return footprint_render(a, K, pose_camera_in_world, points, colors, traversability, masks, projected, valid,
                           supervision_inout, S(stream));
+}
+
+// ============================================================================================
+// ResNet backbone handle (torchvision ResNet-18 / ResNet-50 trunks; reference torchvision_interface.py)
+// ============================================================================================
+}  // extern "C"
+
+struct wvn_resnet {
+  wvn_resnet_config cfg;
+  int bottleneck = 0;
+  std::map<std::string, Weight> w;
+  std::vector<DevBuf> owned;
+  DevBuf stage, col;
+  DevBuf act[5];  // block input / output (two, alternating), conv1 out, conv2 out, downsample out
+};
+
+namespace {
+
+enum ResnetPass { RN_REGISTER, RN_SIZE, RN_RUN };
+
+// Blocks per stage of the two supported depths (torchvision resnet18 / resnet50)
+const int kBlocks18[4] = {2, 2, 2, 2};
+const int kBlocks50[4] = {3, 4, 6, 3};
+
+struct ResnetRun {
+  wvn_resnet* h;
+  ResnetPass pass;
+  int batch;
+  cudaStream_t s;
+  size_t need_col = 0, need_act[5] = {0, 0, 0, 0, 0};
+  int rc = WVN_OK;
+
+  // k x k convolution of the NHWC map `in` [batch, H, W, C] (batch norm folded in) -> `out` [batch, Ho, Wo, Cout];
+  // `role` is the workspace buffer the output lives in (-1: a caller's tap buffer), `residual` is added before the ReLU.
+  void conv(const std::string& name, const void* in, int H, int W, int C, int k, int stride, int pad, int Cout,
+            void* out, int role, bool relu, const void* residual, int* Ho_, int* Wo_, const float* img = nullptr,
+            bool stem = false) {
+    const int Ho = (H + 2 * pad - k) / stride + 1, Wo = (W + 2 * pad - k) / stride + 1;
+    *Ho_ = Ho; *Wo_ = Wo;
+    if (rc != WVN_OK) return;
+    const int K = k * k * C;
+    const long long M = static_cast<long long>(batch) * Ho * Wo;
+    const bool direct = k == 1 && stride == 1 && !stem;
+    const long long pitch = gemm_w_pitch(K);
+    if (pass == RN_REGISTER) {
+      wvn_resnet& r = *h;
+      DevBuf b;
+      if ((rc = b.alloc(static_cast<size_t>(Cout) * pitch * 2)) != WVN_OK) return;
+      r.owned.push_back(b);
+      Weight wt;
+      wt.p = b.p; wt.numel = static_cast<long long>(Cout) * K; wt.bf16 = true; wt.cols = K; wt.ld = static_cast<int>(pitch);
+      r.w[name + ".weight"] = wt;
+      DevBuf bb;
+      if ((rc = bb.alloc(static_cast<size_t>(Cout) * 4)) != WVN_OK) return;
+      r.owned.push_back(bb);
+      Weight wb;
+      wb.p = bb.p; wb.numel = Cout;
+      r.w[name + ".bias"] = wb;
+      return;
+    }
+    if (pass == RN_SIZE) {
+      if (!direct) need_col = std::max(need_col, static_cast<size_t>(M * pitch * 2));
+      if (role >= 0) need_act[role] = std::max(need_act[role], static_cast<size_t>(M * Cout * 2));
+      return;
+    }
+    const void* A = in;
+    long long lda = C;
+    if (!direct) {
+      rc = stem ? im2col_image(img, batch, H, W, k, stride, pad, h->col.p, pitch, s)
+               : im2col_nhwc(in, batch, H, W, C, k, stride, pad, h->col.p, pitch, s);
+      if (rc != WVN_OK) return;
+      A = h->col.p;
+      lda = pitch;
+    }
+    if (M > 0x7fffffff) {
+      rc = set_error(WVN_ERR_INVALID, "resnet: %lld output rows", M);
+      return;
+    }
+    GemmArgs g;
+    g.M = static_cast<int>(M); g.N = Cout; g.K = K;
+    g.epi = residual ? EPI_BF16_RESID : EPI_BF16;
+    g.act = relu ? ACT_RELU : ACT_NONE;
+    g.bias = reinterpret_cast<const float*>(h->w[name + ".bias"].p);
+    g.out = out; g.ldo = Cout;
+    g.residual = residual; g.ldr = Cout;
+    rc = gemm_bf16(g, A, lda, h->w[name + ".weight"].p, 0, s);
+  }
+
+  // The whole trunk; in RN_RUN the four taps are written to taps[0..3] (NHWC bf16).
+  void walk(const float* img, void* const* taps) {
+    const int S = h->cfg.image_size;
+    const bool bn = h->bottleneck != 0;
+    const int* blocks = bn ? kBlocks50 : kBlocks18;
+    void* A[5];
+    for (int i = 0; i < 5; ++i) A[i] = h->act[i].p;
+    void* T[4] = {nullptr, nullptr, nullptr, nullptr};
+    if (taps) for (int i = 0; i < 4; ++i) T[i] = taps[i];
+    int Ho, Wo;
+    // stem: conv1 7x7/2 + bn1 + relu (output in buffer 2), max-pool 3x3/2 into buffer 0
+    conv("conv1", nullptr, S, S, 3, 7, 2, 3, 64, A[2], 2, true, nullptr, &Ho, &Wo, img, true);
+    int H = (Ho - 1) / 2 + 1, W = (Wo - 1) / 2 + 1, C = 64;
+    if (pass == RN_SIZE) need_act[0] = std::max(need_act[0], static_cast<size_t>(batch) * H * W * C * 2);
+    if (pass == RN_RUN && rc == WVN_OK) rc = maxpool3s2_nhwc(A[2], batch, Ho, Wo, 64, A[0], s);
+    const void* cur = A[0];
+    int cur_role = 0;
+    for (int L = 1; L <= 4; ++L) {
+      const int planes = 64 << (L - 1), out_c = bn ? planes * 4 : planes;
+      for (int blk = 0; blk < blocks[L - 1]; ++blk) {
+        const std::string p = "layer" + std::to_string(L) + "." + std::to_string(blk) + ".";
+        const int stride = (blk == 0 && L > 1) ? 2 : 1;
+        const int out_role = cur_role == 0 ? 1 : 0;
+        const bool out_tap = bn ? (L == 4 && blk == blocks[3] - 1) : (blk == blocks[L - 1] - 1);
+        void* out = out_tap ? T[bn ? 3 : L - 1] : A[out_role];
+        int h1, w1, h2, w2, hd, wd;
+        const void* res = cur;
+        if (blk == 0 && (stride != 1 || C != out_c)) {
+          conv(p + "downsample", cur, H, W, C, 1, stride, 0, out_c, A[4], 4, false, nullptr, &hd, &wd);
+          res = A[4];
+        }
+        if (bn) {
+          // taps feat1..feat3: layer{2,3,4}.0.relu, the ReLU after bn1 of each stage's first block
+          const bool t1_tap = blk == 0 && L >= 2;
+          void* t1 = t1_tap ? T[L - 2] : A[2];
+          conv(p + "conv1", cur, H, W, C, 1, 1, 0, planes, t1, t1_tap ? -1 : 2, true, nullptr, &h1, &w1);
+          conv(p + "conv2", t1, h1, w1, planes, 3, stride, 1, planes, A[3], 3, true, nullptr, &h2, &w2);
+          conv(p + "conv3", A[3], h2, w2, planes, 1, 1, 0, out_c, out, out_tap ? -1 : out_role, true, res, &H, &W);
+        } else {
+          conv(p + "conv1", cur, H, W, C, 3, stride, 1, planes, A[2], 2, true, nullptr, &h1, &w1);
+          conv(p + "conv2", A[2], h1, w1, planes, 3, 1, 1, out_c, out, out_tap ? -1 : out_role, true, res, &H, &W);
+        }
+        C = out_c;
+        cur = out;
+        cur_role = out_tap ? -1 : out_role;
+      }
+    }
+  }
+};
+
+}  // namespace
+
+extern "C" {
+
+int wvn_resnet_create(const wvn_resnet_config* cfg, wvn_resnet_t** out) {
+  WVN_REQUIRE(cfg && out, "wvn_resnet_create: null argument");
+  WVN_PROPAGATE(wvn_check_device());
+  WVN_REQUIRE(cfg->depth == 18 || cfg->depth == 50, "resnet: depth %d unsupported (18, 50)", cfg->depth);
+  WVN_REQUIRE(cfg->image_size >= 32 && cfg->image_size % 32 == 0, "resnet: image size %d must be a multiple of 32",
+              cfg->image_size);
+  WVN_REQUIRE(cfg->max_batch > 0, "resnet: max_batch must be positive");
+  wvn_resnet* h = new wvn_resnet();
+  h->cfg = *cfg;
+  h->bottleneck = cfg->depth == 50;
+  ResnetRun reg{h, RN_REGISTER, cfg->max_batch, 0};
+  reg.walk(nullptr, nullptr);
+  ResnetRun size{h, RN_SIZE, cfg->max_batch, 0};
+  size.walk(nullptr, nullptr);
+  int rc = reg.rc;
+  auto alloc = [&](DevBuf& b, size_t bytes) { if (rc == WVN_OK) rc = b.alloc(bytes); };
+  alloc(h->stage, 8u << 20);
+  alloc(h->col, size.need_col);
+  for (int i = 0; i < 5; ++i) alloc(h->act[i], size.need_act[i]);
+  if (rc != WVN_OK) {
+    wvn_resnet_destroy(h);
+    return rc;
+  }
+  *out = h;
+  return WVN_OK;
+}
+
+void wvn_resnet_destroy(wvn_resnet_t* h) {
+  if (!h) return;
+  for (auto& b : h->owned) b.release();
+  h->stage.release();
+  h->col.release();
+  for (auto& b : h->act) b.release();
+  delete h;
+}
+
+size_t wvn_resnet_workspace_bytes(const wvn_resnet_t* h) {
+  if (!h) return 0;
+  size_t n = h->col.bytes;
+  for (const auto& b : h->act) n += b.bytes;
+  return n;
+}
+
+int wvn_resnet_set_weight(wvn_resnet_t* h, const char* name, const float* data, long long numel) {
+  WVN_REQUIRE(h && name && data, "wvn_resnet_set_weight: null argument");
+  auto it = h->w.find(name);
+  WVN_REQUIRE(it != h->w.end(), "wvn_resnet_set_weight: unknown weight '%s'", name);
+  return load_weight(it->second, h->stage, name, data, numel);
+}
+
+int wvn_resnet_forward(wvn_resnet_t* h, const float* img, int batch, void* const* taps, void* stream) {
+  WVN_REQUIRE(h && img && taps, "wvn_resnet_forward: null argument");
+  WVN_REQUIRE(batch > 0 && batch <= h->cfg.max_batch, "wvn_resnet_forward: batch %d outside (0, %d]", batch,
+              h->cfg.max_batch);
+  for (int i = 0; i < 4; ++i) WVN_REQUIRE(taps[i], "wvn_resnet_forward: tap %d is null", i);
+  for (auto& kv : h->w)
+    if (!kv.second.loaded) return set_error(WVN_ERR_STATE, "resnet: weight '%s' was never set", kv.first.c_str());
+  ResnetRun run{h, RN_RUN, batch, S(stream)};
+  run.walk(img, taps);
+  return run.rc;
+}
+
+int wvn_im2col_bf16_nhwc(const void* in, int batch, int h, int w, int c, int k, int stride, int pad, void* out,
+                         long long pitch, void* stream) {
+  return im2col_nhwc(in, batch, h, w, c, k, stride, pad, out, pitch, S(stream));
+}
+
+int wvn_im2col_image(const float* img, int batch, int h, int w, int k, int stride, int pad, void* out, long long pitch,
+                     void* stream) {
+  return im2col_image(img, batch, h, w, k, stride, pad, out, pitch, S(stream));
+}
+
+int wvn_maxpool3s2_bf16_nhwc(const void* in, int batch, int h, int w, int c, void* out, void* stream) {
+  return maxpool3s2_nhwc(in, batch, h, w, c, out, S(stream));
+}
+
+int wvn_segment_pool_pyramid(const long long* seg, int batch, int h, int w, int smax, const float* centers,
+                             void* const* taps, const int* tap_h, const int* tap_w, const int* tap_c, float* out,
+                             void* stream) {
+  WVN_REQUIRE(taps && tap_h && tap_w && tap_c, "wvn_segment_pool_pyramid: null argument");
+  PyramidArgs a;
+  a.batch = batch; a.h = h; a.w = w; a.smax = smax;
+  for (int l = 0; l < 4; ++l) {
+    a.taps[l] = taps[l]; a.th[l] = tap_h[l]; a.tw[l] = tap_w[l]; a.tc[l] = tap_c[l];
+  }
+  return segment_pool_pyramid(seg, centers, a, out, S(stream));
 }
 
 }  // extern "C"

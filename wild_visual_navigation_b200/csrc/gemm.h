@@ -14,6 +14,7 @@ enum GemmEpilogue : int {
   EPI_MLP_HEAD = 5,   // last layer of the traversability MLP fused with its consumers:
                       //   cols [0,feat) reconstruct x -> loss_reco = mean((out - x)^2) -> confidence,
                       //   col feat = traversability logit -> sigmoid.  Nothing of [M,N] is stored.
+  EPI_BF16_RESID = 6, // out(bf16)[row, col]  = act(acc + bias + residual(bf16)[row, col])  (a residual block's last conv)
 };
 
 enum GemmAct : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2 };
@@ -46,6 +47,9 @@ struct GemmArgs {
   const float* cg_mean = nullptr;  // device scalars of the ConfidenceGenerator
   const float* cg_std = nullptr;
   float cg_std_factor = 0.5f;
+  // EPI_BF16_RESID
+  const void* residual = nullptr;  // [M, ldr] bf16
+  long long ldr = 0;
   // launch control
   int max_ctas = 0;             // 0 = one CTA per SM
   int reverse_m = 0;            // walk the m-blocks last-to-first (start on the rows the producer kernel wrote last: L2 hits)

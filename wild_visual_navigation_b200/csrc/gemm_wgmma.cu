@@ -41,6 +41,7 @@ constexpr int kMaxSmemBytes = 227 * 1024;
 constexpr int kMaxStages = 8;
 constexpr int kFixedSmemBytes = 1024 /*barriers*/ + 1024 /*align slack*/;
 constexpr int kSliceCols = 32;                // columns per staged store
+constexpr int kResidMaxBlockN = 192;          // widest tile of EPI_BF16_RESID
 
 // Tile enumeration.  Default: tile ids run n-fastest over the whole (m, n)
 // grid and are dealt round-robin to CTAs (neighbouring CTAs share the A tile through L2).  ROW_OWNER
@@ -61,7 +62,7 @@ struct TileIter {
 };
 
 template <int EPI>
-constexpr bool kStaged = EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_RESID_F32 || EPI == EPI_QKV;
+constexpr bool kStaged = EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_RESID_F32 || EPI == EPI_QKV || EPI == EPI_BF16_RESID;
 
 template <int BN, int EPI>
 struct GemmCfg {
@@ -196,8 +197,16 @@ __device__ __forceinline__ void store_frag(const GemmArgs& args, const CUtensorM
       if (args.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(args.bias + c));
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const float v0 = activate<ACT>(d[4 * j + 2 * h] + b.x), v1 = activate<ACT>(d[4 * j + 2 * h + 1] + b.y);
         const int r = row_local + 8 * h;
+        float a0 = d[4 * j + 2 * h] + b.x, a1 = d[4 * j + 2 * h + 1] + b.y;
+        if (EPI == EPI_BF16_RESID && row_tile + r < args.M) {
+          // the residual is added before the activation: out = act(conv + bias + shortcut)
+          const uint32_t rv = __ldg(reinterpret_cast<const uint32_t*>(
+              reinterpret_cast<const __nv_bfloat16*>(args.residual) + static_cast<long long>(row_tile + r) * args.ldr + c));
+          a0 += bf16_lo(rv);
+          a1 += bf16_hi(rv);
+        }
+        const float v0 = activate<ACT>(a0), v1 = activate<ACT>(a1);
         if (EPI == EPI_F32 || EPI == EPI_RESID_F32) {
           sts64(buf + r * 128 + ((((2 * js + (q >> 1)) ^ (r & 7))) << 4) + (q & 1) * 8, v0, v1);
         } else if (EPI == EPI_QKV && which == 2) {
@@ -213,7 +222,7 @@ __device__ __forceinline__ void store_frag(const GemmArgs& args, const CUtensorM
     fence_proxy_async_smem();
     named_bar_sync(bar_id, 128);
     if (leader) {
-      if (EPI == EPI_BF16 || EPI == EPI_F32) {
+      if (EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_BF16_RESID) {
         tma_store_2d(tm0, buf, col, row_tile);
       } else if (EPI == EPI_RESID_F32) {
         // x += acc + bias: one fp32 add per element, performed at L2
@@ -470,6 +479,14 @@ int dispatch_epi(const GemmArgs& a, const CUtensorMap& ta, const CUtensorMap& tb
     case EPI_MLP_HEAD:
       if (a.act == ACT_NONE) return launch_gemm<BN, EPI_MLP_HEAD, ACT_NONE>(a, ta, tb, tc, s);
       break;
+    case EPI_BF16_RESID:
+      // the residual's loads do not fit beside 224- and 256-column accumulators without spilling (gemm_bf16 keeps
+      // block_n <= kResidMaxBlockN for this epilogue)
+      if constexpr (BN <= kResidMaxBlockN) {
+        if (a.act == ACT_NONE) return launch_gemm<BN, EPI_BF16_RESID, ACT_NONE>(a, ta, tb, tc, s);
+        if (a.act == ACT_RELU) return launch_gemm<BN, EPI_BF16_RESID, ACT_RELU>(a, ta, tb, tc, s);
+      }
+      break;
   }
   return set_error(WVN_ERR_INVALID, "gemm: unsupported epilogue/activation combination (%d, %d)", a.epi, a.act);
 }
@@ -488,7 +505,12 @@ int pick_block_n(int N) {
 int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, int block_n, cudaStream_t stream) {
   WVN_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "gemm: empty problem (M=%d N=%d K=%d)", a.M, a.N, a.K);
   WVN_REQUIRE(lda >= a.K, "gemm: lda=%lld is smaller than K=%d", lda, a.K);
-  if (block_n == 0) block_n = pick_block_n(a.N);
+  if (block_n == 0) {
+    block_n = pick_block_n(a.N);
+    if (a.epi == EPI_BF16_RESID && block_n > kResidMaxBlockN) block_n = a.N % 192 == 0 ? 192 : (a.N % 128 == 0 ? 128 : 64);
+  }
+  WVN_REQUIRE(a.epi != EPI_BF16_RESID || block_n <= kResidMaxBlockN, "gemm: the residual epilogue takes block_n <= %d",
+              kResidMaxBlockN);
   WVN_REQUIRE(block_n == 64 || block_n == 128 || block_n == 192 || block_n == 224 || block_n == 256,
               "gemm: bad block_n %d", block_n);
   WVN_REQUIRE(a.N % block_n == 0, "gemm: N=%d must be a multiple of block_n=%d (pad the weights)", a.N, block_n);
@@ -508,14 +530,17 @@ int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, in
                 "gemm: bad patch-embed epilogue geometry (tokens_in=%d registers=%d npad=%d)", a.tokens_in, a.registers,
                 a.npad);
   if (a.epi == EPI_F32 || a.epi == EPI_RESID_F32) WVN_REQUIRE(a.ldo % 4 == 0, "gemm: fp32 output pitch must be a multiple of 4");
-  if (a.epi == EPI_BF16) WVN_REQUIRE(a.ldo % 8 == 0, "gemm: bf16 output pitch must be a multiple of 8");
+  if (a.epi == EPI_BF16 || a.epi == EPI_BF16_RESID) WVN_REQUIRE(a.ldo % 8 == 0, "gemm: bf16 output pitch must be a multiple of 8");
+  if (a.epi == EPI_BF16_RESID)
+    WVN_REQUIRE(a.residual != nullptr && a.ldr >= a.N && a.ldr % 2 == 0,
+                "gemm: the residual epilogue needs a bf16 residual with an even pitch ldr >= N (ldr=%lld N=%d)", a.ldr, a.N);
   CUtensorMap ta, tb, tc[3] = {};
   // Both maps take the true K as their inner extent, so the pad columns of a K that is not a multiple of 64 are never
   // read (TMA zero-fills the last k-block past K, whatever the pad columns hold).  W's rows sit at a 16-byte pitch.
   WVN_PROPAGATE(make_tmap_bf16_2d(&ta, A, a.K, a.M, static_cast<uint64_t>(lda) * 2, BK, BM));
   WVN_PROPAGATE(make_tmap_bf16_2d(&tb, W, a.K, a.N, static_cast<uint64_t>(gemm_w_pitch(a.K)) * 2, BK, block_n));
   // output maps for the staged epilogues: 32-column x 64-row boxes (store_frag's layouts); rows past M are clipped
-  if (a.epi == EPI_BF16)
+  if (a.epi == EPI_BF16 || a.epi == EPI_BF16_RESID)
     WVN_PROPAGATE(make_tmap_2d(&tc[0], a.out, 2, a.N, a.M, static_cast<uint64_t>(a.ldo) * 2, kSliceCols, BM, 64));
   if (a.epi == EPI_F32 || a.epi == EPI_RESID_F32)
     WVN_PROPAGATE(make_tmap_2d(&tc[0], a.out, 4, a.N, a.M, static_cast<uint64_t>(a.ldo) * 4, kSliceCols, BM, 128));

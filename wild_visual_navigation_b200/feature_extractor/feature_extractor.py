@@ -8,10 +8,14 @@
   * adjacency + centroids come from the same pass (no per-segment Python loops / host syncs);
   * when segmentation and features are both "stego"/"dino" on the same backbone, one ViT forward
     serves both (the reference runs two backbones); with "dinov2" / "dinov2_reg" features, STEGO's DINO backbone
-    segments and a second, DINOv2 handle gives the features.
+    segments and a second, DINOv2 handle gives the features;
+  * "torchvision" features (``model_type`` resnet18 / resnet50 / resnet50_dino) are a feature pyramid pooled per
+    segment level by level (csrc/resnet_kernels.cu), as sparsify_features' dict branch does.  Where a segment has no
+    cell at a coarse level the reference raises AttributeError; here it takes the cell under its centroid.  "random" and
+    "none" segmentation crash in the reference with a pyramid and raise ValueError here.
 Supported: segmentation_type in {"slic" (the constructor default), "stego", "grid", "random", "none"/None},
-feature_type in {"dino", "dinov2", "dinov2_reg", "stego"}.  "slic" is an all-integer SLIC kernel (csrc/slic_kernels.cu; fast_slic itself is an
-un-vendored C++ package, see oracle/slic.py for what is and is not restated).  "sift", "torchvision", "histogram"
+feature_type in {"dino", "dinov2", "dinov2_reg", "stego", "torchvision"}.  "slic" is an all-integer SLIC kernel (csrc/slic_kernels.cu; fast_slic itself is an
+un-vendored C++ package, see oracle/slic.py for what is and is not restated).  "sift", "histogram"
 features are out of scope (SURVEY.md §2) and raise.
 """
 from __future__ import annotations
@@ -22,6 +26,7 @@ from .. import ops
 from .dino_interface import DinoInterface
 from .segment_extractor import SegmentExtractor
 from .stego_interface import StegoInterface
+from .torchvision_interface import PYRAMID_KEYS, TorchVisionInterface
 
 
 class FeatureExtractor:
@@ -43,6 +48,12 @@ class FeatureExtractor:
         need_stego = feature_type == "stego" or segmentation_type == "stego"
         if feature_type == "stego":
             self._feature_dim = 90
+        elif feature_type == "torchvision":
+            if segmentation_type in ("random", "none", None):
+                # the reference indexes / returns the pyramid dict as a tensor there and crashes
+                raise ValueError(f"segmentation_type [{segmentation_type}] does not work with torchvision features")
+            if "model_type" not in kwargs:
+                raise ValueError("feature_type 'torchvision' needs model_type (resnet18, resnet50, resnet50_dino)")
         elif "dino" in feature_type:
             # the reference hard-codes 384 for every dino variant (feature_extractor.py:56)
             self._feature_dim = 384 if common["backbone_type"] == "vit_small" else 768
@@ -62,7 +73,17 @@ class FeatureExtractor:
                                          kmeans_iters=kwargs.get("kmeans_iters", 10), **common)
         else:
             self._stego = None
-        if need_stego and share:
+        self._tv = None
+        if feature_type == "torchvision":
+            # with segmentation_type="stego", STEGO segments on its own DINO backbone (`stego_state_dict`)
+            self._dino = None
+            self._tv = TorchVisionInterface(device, kwargs["model_type"], input_size, max_batch=common["max_batch"],
+                                            state_dict=kwargs.get("state_dict"),
+                                            pretrained_weights=kwargs.get("pretrained_weights"))
+            self._extractor = self._tv
+            # the reference never sets it for torchvision (reading it raises); the pooled row width
+            self._feature_dim = self._tv.feature_dim
+        elif need_stego and share:
             self._dino = self._stego._dino
             self._extractor = self._stego if feature_type == "stego" else self._dino
         else:
@@ -130,7 +151,7 @@ class FeatureExtractor:
         else:
             img = img.to(self._device, dtype=torch.float32)
             B, _, H, W = img.shape
-        g = self._dino.grid
+        g = self._dino.grid if self._dino is not None else None
         # 1. segmentation (+ the one backbone pass)
         tokens = None
         if self._segmentation_type == "stego":
@@ -189,6 +210,17 @@ class FeatureExtractor:
             return {"seg": seg, "feat": dense, "centers": centers, "edges": edges, "n_edges": None, "n_segments": None,
                     "tokens": tokens, "dense": dense}
         # 2. features
+        if self._tv is not None:
+            # feature pyramid: per segment and level, the mean over the level's nearest-downsampled segmentation
+            taps = self._tv.inference_taps(img)
+            want_graph = self._segmentation_type != "random"
+            r = ops.segment_reduce(seg, smax, want_centers=True, want_edges=want_graph)
+            feat = ops.segment_pool_pyramid(seg, smax, taps, r["centers"])
+            out = {"seg": seg, "feat": feat, "centers": r["centers"], "edges": r["edges"], "n_edges": r["n_edges"],
+                   "n_segments": counts, "tokens": None, "dense": None}
+            if kwargs.get("return_dense_features", False):
+                out["dense"] = {k: t.permute(0, 3, 1, 2).float().contiguous() for k, t in zip(PYRAMID_KEYS, taps)}
+            return out
         if tokens is None:
             if self._feature_type == "stego":
                 self._stego._forward(img, want_linear=False)

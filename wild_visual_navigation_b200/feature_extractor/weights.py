@@ -10,9 +10,12 @@ The reference downloads DINO checkpoints from dl.fbaipublicfiles.com at construc
 DINOv2 (``backbone="dinov2"``, the ``dinov2_vit{s,b}14_pretrain.pth`` checkpoints) uses the same key names plus the
 LayerScale gammas ``blocks.N.ls{1,2}.gamma`` and an unused ``mask_token``; DINOv2 with registers
 (``backbone="dinov2_reg"``, ``dinov2_vit{s,b}14_reg4_pretrain.pth``) adds ``register_tokens`` (1, R, D).
+The torchvision ResNets (``TorchVisionInterface``) take torchvision-layout state dicts (``resnet18`` / ``resnet50``
+ImageNet checkpoints, or DINO's ``dino_resnet50_pretrain.pth`` for ``resnet50_dino``); ``fc.*`` is not needed.
 """
 from __future__ import annotations
 
+import math
 import os
 import warnings
 
@@ -184,3 +187,148 @@ def fold_stego_head(hd: dict) -> dict:
     a_b[HEAD_LINEAR_COL : HEAD_LINEAR_COL + C] = wl @ (b1 + b2) + bl
     return {"head_a.weight": a_w, "head_a.bias": a_b, "hidden.weight": hd["cluster2.0.weight"].float(),
             "hidden.bias": hd["cluster2.0.bias"].float(), "head_b.weight": b_w}
+
+
+# --------------------------------------------------------------------------------------------
+# torchvision ResNets
+# --------------------------------------------------------------------------------------------
+RESNET_MODELS = {"resnet18": 18, "resnet50": 50, "resnet50_dino": 50}
+RESNET_BLOCKS = {18: (2, 2, 2, 2), 50: (3, 4, 6, 3)}
+RESNET_BN_EPS = 1e-5
+RESNET_RESIDUAL_GAMMA = 0.2
+
+
+def resnet_convs(depth: int):
+    """(conv, batch norm, in, out, kernel, stride) of every conv of the torchvision ResNet trunk, in forward order.
+    The downsample conv of a stage's first block comes before the block's own convs."""
+    convs = [("conv1", "bn1", 3, 64, 7, 2)]
+    bottleneck = depth == 50
+    cin = 64
+    for L, n in enumerate(RESNET_BLOCKS[depth], start=1):
+        planes = 64 << (L - 1)
+        cout = planes * 4 if bottleneck else planes
+        for blk in range(n):
+            p = f"layer{L}.{blk}."
+            stride = 2 if blk == 0 and L > 1 else 1
+            if blk == 0 and (stride != 1 or cin != cout):
+                convs.append((p + "downsample.0", p + "downsample.1", cin, cout, 1, stride))
+            if bottleneck:
+                # torchvision >= 0.13 (ResNet v1.5): the stride sits in the 3 x 3 conv
+                convs += [(p + "conv1", p + "bn1", cin, planes, 1, 1), (p + "conv2", p + "bn2", planes, planes, 3, stride),
+                          (p + "conv3", p + "bn3", planes, cout, 1, 1)]
+            else:
+                convs += [(p + "conv1", p + "bn1", cin, planes, 3, stride), (p + "conv2", p + "bn2", planes, cout, 3, 1)]
+            cin = cout
+    return convs
+
+
+def _resnet_calibrate(sd: dict, depth: int, img: torch.Tensor):
+    """Runs the trunk in training-mode batch norm on ``img`` and stores each batch norm's batch statistics as its running
+    statistics (momentum 1, each layer seeing the already calibrated layers before it)."""
+    import torch.nn.functional as F
+
+    def cbr(x, conv, bn, stride, k, relu=True, res=None):
+        x = F.conv2d(x, sd[conv + ".weight"], stride=stride, padding=k // 2)
+        mean, var = x.mean((0, 2, 3)), x.var((0, 2, 3), unbiased=False)
+        sd[bn + ".running_mean"], sd[bn + ".running_var"] = mean, var
+        x = F.batch_norm(x, mean, var, sd[bn + ".weight"], sd[bn + ".bias"], False, 0.0, RESNET_BN_EPS)
+        if res is not None:
+            x = x + res
+        return F.relu(x) if relu else x
+
+    x = (img - torch.tensor([0.485, 0.456, 0.406])[:, None, None]) / torch.tensor([0.229, 0.224, 0.225])[:, None, None]
+    x = F.max_pool2d(cbr(x, "conv1", "bn1", 2, 7), 3, 2, 1)
+    for L, n in enumerate(RESNET_BLOCKS[depth], start=1):
+        for blk in range(n):
+            p = f"layer{L}.{blk}."
+            stride = 2 if blk == 0 and L > 1 else 1
+            res = x
+            if p + "downsample.0.weight" in sd:
+                res = cbr(x, p + "downsample.0", p + "downsample.1", stride, 1, relu=False)
+            if depth == 50:
+                y = cbr(x, p + "conv1", p + "bn1", 1, 1)
+                y = cbr(y, p + "conv2", p + "bn2", stride, 3)
+                x = cbr(y, p + "conv3", p + "bn3", 1, 1, res=res)
+            else:
+                y = cbr(x, p + "conv1", p + "bn1", stride, 3)
+                x = cbr(y, p + "conv2", p + "bn2", 1, 3, res=res)
+
+
+def synthetic_resnet_state_dict(depth: int, seed: int = 1):
+    """Seeded torchvision-layout ResNet weights (no ``fc``).  Convs are Kaiming-normal (fan_out, as torchvision
+    initialises them), batch-norm affine parameters are drawn around (1, 0), and the running statistics are calibrated
+    on four seeded 128 x 128 images, so every tap keeps an RMS of order 1 at any input size instead of growing through
+    the residual sums as it does with identity statistics."""
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    with torch.no_grad():
+        for conv, bn, cin, cout, k, _ in resnet_convs(depth):
+            sd[conv + ".weight"] = torch.randn(cout, cin, k, k, generator=g) * math.sqrt(2.0 / (cout * k * k))
+            # the batch norm closing a residual branch starts small (torchvision's zero_init_residual takes it to 0):
+            # each block adds a correction to its input instead of replacing it.  With gamma 1 a random calibrated
+            # trunk amplifies any perturbation about 1.2x per conv, so bf16 activations would end 47% off fp32 at
+            # ResNet-50's trunk output; at 0.2 they end 3.8% off (DESIGN.md §3.9)
+            last = bn.endswith(".bn3" if depth == 50 else ".bn2")
+            sd[bn + ".weight"] = (RESNET_RESIDUAL_GAMMA if last else 1.0) * (1.0 + 0.2 * torch.randn(cout, generator=g))
+            sd[bn + ".bias"] = 0.2 * torch.randn(cout, generator=g)
+            sd[bn + ".running_mean"] = torch.zeros(cout)
+            sd[bn + ".running_var"] = torch.ones(cout)
+            sd[bn + ".num_batches_tracked"] = torch.tensor(0)
+        _resnet_calibrate(sd, depth, torch.rand(4, 3, 128, 128, generator=g))
+    return sd
+
+
+def check_resnet_family(sd: dict, model_type: str) -> dict:
+    """Checks that a torchvision-layout state dict is a ``model_type`` ResNet and returns the trunk's tensors (the
+    reference loads with ``strict=False``, so a missing ``fc.*`` is fine).  Raises ValueError on another family."""
+    if model_type not in RESNET_MODELS:
+        raise ValueError(f"model_type '{model_type}' is not supported (resnet18, resnet50, resnet50_dino)")
+    depth = RESNET_MODELS[model_type]
+    sd = {k.replace("module.", ""): v for k, v in sd.items()}
+    missing, bad = [], []
+    for conv, bn, cin, cout, k, _ in resnet_convs(depth):
+        w = sd.get(conv + ".weight")
+        if w is None:
+            missing.append(conv + ".weight")
+        elif tuple(w.shape) != (cout, cin, k, k):
+            bad.append(f"{conv}.weight {tuple(w.shape)} != {(cout, cin, k, k)}")
+        for leaf in ("weight", "bias", "running_mean", "running_var"):
+            if bn + "." + leaf not in sd:
+                missing.append(bn + "." + leaf)
+    if missing or bad:
+        detail = "; ".join((bad + [f"missing {m}" for m in missing])[:3])
+        raise ValueError(f"model_type '{model_type}' needs a torchvision ResNet-{depth} state dict; got another ({detail})")
+    keep = {c + ".weight" for c, *_ in resnet_convs(depth)}
+    keep |= {b + "." + leaf for _, b, *_ in resnet_convs(depth) for leaf in ("weight", "bias", "running_mean", "running_var")}
+    return {k: v for k, v in sd.items() if k in keep}
+
+
+def load_resnet_state_dict(model_type: str, pretrained_weights=None, seed: int = 1):
+    """ResNet weights for ``model_type`` from ``pretrained_weights`` / ``$WVN_RESNET_WEIGHTS`` (checked by
+    check_resnet_family), or seeded (synthetic_resnet_state_dict) with a warning."""
+    if model_type not in RESNET_MODELS:
+        raise ValueError(f"model_type '{model_type}' is not supported (resnet18, resnet50, resnet50_dino)")
+    path = pretrained_weights or os.environ.get("WVN_RESNET_WEIGHTS")
+    if path:
+        sd = torch.load(path, map_location="cpu", weights_only=False)
+        if "state_dict" in sd:
+            sd = sd["state_dict"]
+        return check_resnet_family(sd, model_type)
+    warnings.warn(f"no {model_type} checkpoint given (pretrained_weights / $WVN_RESNET_WEIGHTS): using seeded random "
+                  f"weights with calibrated batch-norm statistics — fine for parity and throughput work, not for real "
+                  f"traversability")
+    return synthetic_resnet_state_dict(RESNET_MODELS[model_type], seed)
+
+
+def fold_resnet_bn(sd: dict, depth: int) -> dict:
+    """Eval-mode batch norm folded into the conv before it, in at least fp32 (fp64 stays fp64):
+    w' = w * gamma / sqrt(var + eps) per output channel, b' = beta - mean * gamma / sqrt(var + eps).
+    Returns {conv name: (w', b')} with the downsample conv named ``layer{L}.0.downsample``."""
+    out = {}
+    for conv, bn, *_ in resnet_convs(depth):
+        w = sd[conv + ".weight"]
+        dt = torch.promote_types(w.dtype, torch.float32)
+        gamma, beta, mean, var = (sd[bn + "." + k].to(dt) for k in ("weight", "bias", "running_mean", "running_var"))
+        scale = gamma / torch.sqrt(var + RESNET_BN_EPS)
+        out[conv.replace("downsample.0", "downsample")] = (w.to(dt) * scale[:, None, None, None], beta - mean * scale)
+    return out

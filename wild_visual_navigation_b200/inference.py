@@ -25,8 +25,10 @@ class TraversabilityInference:
         self._dino = dino
         self._model = model
         self._cg = confidence_generator
+        # a feature-pyramid backbone (TorchVisionInterface) has no token grid: only the segment-wise mode applies
+        grid = getattr(dino, "grid", 0)
         self._mlp = ops.MlpInference(model.input_size, model.hidden[0], model.hidden[1], chunk_rows,
-                                       tokens_per_frame=max(dino.grid * dino.grid, getattr(dino._model, "npad", 0)))
+                                       tokens_per_frame=max(grid * grid, getattr(dino._model, "npad", 0)))
         self.refresh_weights()
 
     def refresh_weights(self):

@@ -14,7 +14,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _C
-from ._C import TrainConfig, VitConfig, check, lib, ptr, stream
+from ._C import ResnetConfig, TrainConfig, VitConfig, check, lib, ptr, stream
 
 OUT_BF16, OUT_F32, OUT_RESID_F32 = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
@@ -350,6 +350,97 @@ class ViTBackbone:
         try:
             if getattr(self, "_h", None):
                 lib().wvn_vit_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+# --------------------------------------------------------------------------------------------
+# ResNet backbone handle and its primitives
+# --------------------------------------------------------------------------------------------
+# (channels, stride) of the four taps: torchvision_interface.py's return nodes feat1..feat4
+RESNET_TAPS = {18: ((64, 4), (128, 8), (256, 16), (512, 32)), 50: ((128, 4), (256, 8), (512, 16), (2048, 32))}
+
+
+def _ptr_array(tensors):
+    return (c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
+
+
+def im2col_nhwc(x, k, stride, pad, pitch=None, out=None):
+    """x: [B,H,W,C] bf16 NHWC -> rows [B*Ho*Wo, pitch] bf16 in (ky, kx, channel) order; pad columns are left as they are."""
+    B, H, W, C = x.shape
+    Ho, Wo, K = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1, k * k * C
+    pitch = pitch or (K + 7) // 8 * 8
+    if out is None:
+        out = torch.empty(B * Ho * Wo, pitch, device=x.device, dtype=torch.bfloat16)
+    check(lib().wvn_im2col_bf16_nhwc(ptr(x.contiguous()), B, H, W, C, k, stride, pad, ptr(out), pitch, stream()))
+    return out
+
+
+def im2col_image(img, k, stride, pad, pitch=None, out=None):
+    """img: [B,3,H,W] fp32 in [0,1] -> ImageNet-normalised, zero-padded rows [B*Ho*Wo, pitch] bf16 (ky, kx, channel)."""
+    B, _, H, W = img.shape
+    Ho, Wo, K = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1, k * k * 3
+    pitch = pitch or (K + 7) // 8 * 8
+    if out is None:
+        out = torch.empty(B * Ho * Wo, pitch, device=img.device, dtype=torch.bfloat16)
+    check(lib().wvn_im2col_image(ptr(img.contiguous()), B, H, W, k, stride, pad, ptr(out), pitch, stream()))
+    return out
+
+
+def maxpool3s2_nhwc(x):
+    """3 x 3 / stride 2 / pad 1 max-pool of x [B,H,W,C] bf16 NHWC."""
+    B, H, W, C = x.shape
+    out = torch.empty(B, (H + 1) // 2, (W + 1) // 2, C, device=x.device, dtype=torch.bfloat16)
+    check(lib().wvn_maxpool3s2_bf16_nhwc(ptr(x.contiguous()), B, H, W, C, ptr(out), stream()))
+    return out
+
+
+def segment_pool_pyramid(seg, smax, taps, centers):
+    """Multiscale segment pooling (sparsify_features' pyramid branch).  seg [B,H,W] int64, taps: four NHWC bf16 maps
+    [B,h_l,w_l,c_l], centers [B,smax,2] fp32 (col, row) -> feat [B,smax,sum c_l] fp32 (see include/wvn_b200.h)."""
+    B, H, W = seg.shape
+    taps = [t.contiguous() for t in taps]
+    D = sum(t.shape[3] for t in taps)
+    out = torch.empty(B, smax, D, device=seg.device, dtype=torch.float32)
+    ints = ctypes.c_int * 4
+    th, tw, tc = ints(*[t.shape[1] for t in taps]), ints(*[t.shape[2] for t in taps]), ints(*[t.shape[3] for t in taps])
+    check(lib().wvn_segment_pool_pyramid(ptr(seg.contiguous()), B, H, W, smax, ptr(centers.contiguous()),
+                                         _ptr_array(taps), th, tw, tc, ptr(out), stream()))
+    return out
+
+
+class ResNetBackbone:
+    """Owns a ``wvn_resnet_t``: a torchvision ResNet-18 / ResNet-50 trunk with batch norm folded into its convs (bf16 on
+    device) and activation / im2col workspaces sized for ``max_batch``.  ``folded`` maps each conv's name to its
+    (weight [out, in, kh, kw], bias [out]) after folding (weights.fold_resnet_bn)."""
+
+    def __init__(self, image_size, depth, folded, max_batch=32):
+        _C.require_device()
+        self.image_size, self.depth, self.max_batch = image_size, depth, max_batch
+        h = c_void_p()
+        check(lib().wvn_resnet_create(byref(ResnetConfig(image_size, depth, max_batch)), byref(h)))
+        self._h = h
+        self.workspace_bytes = lib().wvn_resnet_workspace_bytes(h)
+        self.taps = [(c, image_size // s) for c, s in RESNET_TAPS[depth]]
+        for name, (w, b) in folded.items():
+            w = w.detach().to(dtype=torch.float32, device="cpu").permute(0, 2, 3, 1).contiguous()
+            b = b.detach().to(dtype=torch.float32, device="cpu").contiguous()
+            check(lib().wvn_resnet_set_weight(h, (name + ".weight").encode(), c_void_p(w.data_ptr()), w.numel()))
+            check(lib().wvn_resnet_set_weight(h, (name + ".bias").encode(), c_void_p(b.data_ptr()), b.numel()))
+
+    def forward(self, img: torch.Tensor):
+        """img (B,3,S,S) fp32 CUDA in [0,1] -> the four taps, NHWC bf16 [B, S/s_l, S/s_l, c_l]."""
+        B = img.shape[0]
+        assert img.dtype == torch.float32 and tuple(img.shape[1:]) == (3, self.image_size, self.image_size)
+        taps = [torch.empty(B, n, n, c, device=img.device, dtype=torch.bfloat16) for c, n in self.taps]
+        check(lib().wvn_resnet_forward(self._h, ptr(img.contiguous()), B, _ptr_array(taps), stream()))
+        return taps
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().wvn_resnet_destroy(self._h)
                 self._h = None
         except Exception:
             pass
