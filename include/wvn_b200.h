@@ -47,7 +47,8 @@ int wvn_check_device(void);
  * callers that fill these structs by layout (ctypes mirrors, code compiled against an older header) must add the field.
  * 102: adds wvn_mlp_trainer_copy_confidence (no layout change).
  * 103: wvn_gemm_ex_args gained trailing `residual` / `ldr` (epi 6); adds the ResNet handle, the im2col / max-pool
- * primitives and wvn_segment_pool_pyramid. */
+ * primitives and wvn_segment_pool_pyramid.
+ * 104: adds the LinearRnvp flow handles, their functions wvn_flow_* and the struct wvn_flow_buffers; no layout change. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -440,6 +441,66 @@ int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, floa
                        const float* x, int groups, int rows_per_group, const int* n_rows, const float* y,
                        const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
                        float* metrics_out, int phase_mask, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * LinearRnvp anomaly-detection learner (model/linear_rnvp.py, fp32): LinearRnvp(dim, [hidden]) with flow_n = 2,
+ * use_permutation = True — coupling 0, permutation 1, coupling 2, permutation 3; every coupling has nets s and t, each
+ * Linear(dim, hidden) ReLU Linear(hidden, hidden) ReLU Linear(hidden, dim).  Bounds: 2 <= dim <= 4096, hidden <= 512
+ * and a multiple of 8.  params / exp_avg / exp_avg_sq: flat fp32 buffers of wvn_flow_param_count floats in the
+ * module's parameters() order (flows.0.s, flows.0.t, flows.2.s, flows.2.t; each net 0.weight, 0.bias, 2.weight,
+ * 2.bias, 4.weight, 4.bias), i.e. torch.optim.Adam's state.  The masks and permutations are read from the model's
+ * buffers on every call, so "odds" and "half" masks and a loaded permutation cost nothing.
+ * The handle owns the workspaces for max_rows rows (allocated at create, nothing per call).
+ * ---------------------------------------------------------------------------------------- */
+typedef struct wvn_flow wvn_flow_t;
+typedef struct {
+  const float* mask0;       /* flows.0.mask [dim] fp32 */
+  const float* mask1;       /* flows.2.mask [dim] fp32 */
+  const long long* p1;      /* flows.1.p / flows.1.invp [dim] int64 */
+  const long long* invp1;
+  const long long* p3;      /* flows.3.p / flows.3.invp [dim] int64 */
+  const long long* invp3;
+} wvn_flow_buffers;
+size_t wvn_flow_param_count(int dim, int hidden);
+/* cfg: std_factor (the ConfidenceGenerator's) and Adam's lr / betas / eps are used; grads: optional caller-owned device
+ * buffer of wvn_flow_param_count floats (NULL: the handle allocates it). */
+int wvn_flow_create(int dim, int hidden, int max_rows, const wvn_train_config* cfg, float* grads, wvn_flow_t** out);
+void wvn_flow_destroy(wvn_flow_t* h);
+/* The ConfidenceGenerator method and state of the train step, as wvn_mlp_trainer_set_confidence. */
+int wvn_flow_set_confidence(wvn_flow_t* h, int method, float* var, double* running_n, double* running_sum,
+                            double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov);
+/* As wvn_mlp_trainer_copy_confidence: a larger handle takes over the generator state src keeps itself. */
+int wvn_flow_copy_confidence(wvn_flow_t* dst, const wvn_flow_t* src, void* stream);
+/* One step of TraversabilityEstimator.train() with AnomalyLoss on the rows of x [rows, dim] whose y_valid [rows] uint8
+ * is set (NULL: every row): forward, loss -mean(sum(logprob) + log_det), the ConfidenceGenerator update with the
+ * per-row NLL, backward, Adam.  No host synchronisation.  confidence_out [rows]: the labelled rows in order;
+ * metrics_out (device, 6 floats, may be NULL): loss_total, loss_trav (0), loss_reco (0), labelled rows, cg_mean, cg_std.
+ * phase_mask: 7 = whole step; 1 = forward + statistics + generator update, 2 = backward (gradient), 4 = Adam. */
+int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                        const wvn_flow_buffers* buffers, const float* x, int rows, const unsigned char* y_valid,
+                        float* cg_mean, float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
+                        void* stream);
+
+/* Inference handle (no backward workspaces, no gradient buffer).  max_rows: rows of wvn_flow_infer_rows per call;
+ * chunk_pixels: pixels per wgmma chunk of wvn_flow_infer_pixels (0 = 8192). */
+typedef struct wvn_flow_infer wvn_flow_infer_t;
+int wvn_flow_infer_create(int dim, int hidden, int max_rows, int chunk_pixels, wvn_flow_infer_t** out);
+void wvn_flow_infer_destroy(wvn_flow_infer_t* h);
+/* Packs the bf16 operands of the per-pixel path from the flat fp32 parameters: call again after they change. */
+int wvn_flow_infer_set_params(wvn_flow_infer_t* h, const float* params, void* stream);
+/* LinearRnvp.forward on x [rows, dim] fp32 in fp32 (rows <= max_rows): z / logprob [rows, dim], log_det [rows], each may
+ * be NULL.  trav [rows] (may be NULL): ConfidenceGenerator.inference_without_update of the NLL
+ * -(sum(logprob) + log_det) with the generator's mean / std (device scalars) and std_factor. */
+int wvn_flow_infer_rows(wvn_flow_infer_t* h, const float* params, const wvn_flow_buffers* buffers, const float* x, int rows,
+                        float* z, float* log_det, float* logprob, const float* cg_mean, const float* cg_std,
+                        float std_factor, float* trav, void* stream);
+/* The per-pixel anomaly map (wvn_feature_extractor_node.py:332-338): tokens [batch, gh * gw, dim] fp32 are upsampled
+ * bilinearly (align_corners = True) to out_h x out_w, every net layer runs as a wgmma GEMM (bf16 operands, fp32
+ * accumulation), the coupling arithmetic in fp32.  trav [batch, out_h, out_w]: inference_without_update of the NLL;
+ * nll (may be NULL): the per-pixel NLL.  Masks / permutations are read from `buffers` on every call. */
+int wvn_flow_infer_pixels(wvn_flow_infer_t* h, const wvn_flow_buffers* buffers, const float* tokens, int batch, int gh,
+                          int gw, int out_h, int out_w, const float* cg_mean, const float* cg_std, float std_factor,
+                          float* trav, float* nll, void* stream);
 
 #ifdef __cplusplus
 }

@@ -52,6 +52,12 @@ class TrainConfig(Structure):
     ]
 
 
+class FlowBuffers(Structure):
+    """wvn_flow_buffers: the LinearRnvp buffers the flow kernels read (coupling masks, permutations)."""
+    _fields_ = [("mask0", c_void_p), ("mask1", c_void_p), ("p1", c_void_p), ("invp1", c_void_p), ("p3", c_void_p),
+                ("invp3", c_void_p)]
+
+
 _lib = None
 
 # name -> (restype, argtypes); every symbol of include/wvn_b200.h
@@ -121,6 +127,17 @@ SIGNATURES = {
     "wvn_mlp_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
     "wvn_mlp_trainer_copy_confidence": (_I, [_P, _P, _P]),
     "wvn_mlp_train_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "wvn_flow_param_count": (_S, [_I, _I]),
+    "wvn_flow_create": (_I, [_I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
+    "wvn_flow_destroy": (None, [_P]),
+    "wvn_flow_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
+    "wvn_flow_copy_confidence": (_I, [_P, _P, _P]),
+    "wvn_flow_infer_create": (_I, [_I, _I, _I, _I, POINTER(_P)]),
+    "wvn_flow_infer_destroy": (None, [_P]),
+    "wvn_flow_infer_set_params": (_I, [_P, _P, _P]),
+    "wvn_flow_infer_rows": (_I, [_P, _P, POINTER(FlowBuffers), _P, _I, _P, _P, _P, _P, _P, _F, _P, _P]),
+    "wvn_flow_infer_pixels": (_I, [_P, POINTER(FlowBuffers), _P, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P]),
+    "wvn_flow_train_step": (_I, [_P, _P, _P, _P, _P, POINTER(FlowBuffers), _P, _I, _P, _P, _P, _P, _P, _I, _P]),
 }
 
 

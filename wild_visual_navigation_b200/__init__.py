@@ -2,16 +2,16 @@
 
 Keeps the reference's class surface for the per-frame path (SURVEY.md §8b):
 ``FeatureExtractor`` / ``DinoInterface`` / ``TorchVisionInterface`` / ``StegoInterface`` / ``SegmentExtractor`` /
-``SimpleMLP`` / ``get_model`` / ``Data`` / ``Batch`` / ``ConfidenceGenerator`` /
-``TraversabilityLoss`` / ``TraversabilityEstimator`` — implemented on hand-written CUDA
+``SimpleMLP`` / ``LinearRnvp`` / ``get_model`` / ``Data`` / ``Batch`` / ``ConfidenceGenerator`` /
+``TraversabilityLoss`` / ``AnomalyLoss`` / ``TraversabilityEstimator`` — implemented on hand-written CUDA
 kernels behind the C ABI in ``include/wvn_b200.h``.  No CPU fallback.
 """
 import os
 
 WVN_ROOT_DIR = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-from .utils import Data, Batch, ConfidenceGenerator, TraversabilityLoss  # noqa: E402,F401
-from .model import SimpleMLP, get_model  # noqa: E402,F401
+from .utils import Data, Batch, ConfidenceGenerator, TraversabilityLoss, AnomalyLoss  # noqa: E402,F401
+from .model import SimpleMLP, LinearRnvp, get_model  # noqa: E402,F401
 from .feature_extractor import (  # noqa: E402,F401
     DinoInterface,
     StegoInterface,

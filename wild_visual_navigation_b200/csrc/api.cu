@@ -18,6 +18,7 @@
 #include "pixel_head.h"
 #include "resnet_kernels.h"
 #include "segment_kernels.h"
+#include "flow_train.h"
 #include "footprint_kernels.h"
 #include "slic_kernels.h"
 #include "stego_kmeans.h"
@@ -117,7 +118,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 103; }
+int wvn_version(void) { return 104; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -1270,6 +1271,125 @@ int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, floa
   WVN_REQUIRE(t, "wvn_mlp_train_step: null trainer");
   return fused_train_step(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows, y, y_valid,
                           cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
+}
+
+}  // extern "C"
+
+// ============================================================================================
+// LinearRnvp flow: fp32 row forward and online train step (flow_train.cu)
+// ============================================================================================
+struct wvn_flow {
+  FlowTrainer* impl = nullptr;
+};
+
+// inference only: the fp32 row forward (forward workspaces only) and the per-pixel wgmma path
+struct wvn_flow_infer {
+  FlowTrainer* rows = nullptr;
+  FlowPixels* pix = nullptr;
+};
+
+namespace {
+FlowBuffers buffers_of(const wvn_flow_buffers* b) {
+  FlowBuffers f;
+  if (b) {
+    f.mask0 = b->mask0; f.mask1 = b->mask1; f.p1 = b->p1; f.invp1 = b->invp1; f.p3 = b->p3; f.invp3 = b->invp3;
+  }
+  return f;
+}
+}  // namespace
+
+extern "C" {
+
+size_t wvn_flow_param_count(int dim, int hidden) {
+  FlowShape s;
+  s.dim = dim; s.hidden = hidden;
+  return flow_param_count(s);
+}
+
+int wvn_flow_create(int dim, int hidden, int max_rows, const wvn_train_config* cfg, float* grads, wvn_flow_t** out) {
+  WVN_REQUIRE(cfg && out, "wvn_flow_create: null argument");
+  WVN_PROPAGATE(wvn_check_device());
+  FlowShape s;
+  s.dim = dim; s.hidden = hidden;
+  AdamCfg a;
+  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
+  FlowTrainer* impl = nullptr;
+  WVN_PROPAGATE(flow_trainer_create(s, max_rows, cfg->std_factor, a, grads, false, &impl));
+  wvn_flow* h = new wvn_flow();
+  h->impl = impl;
+  *out = h;
+  return WVN_OK;
+}
+
+void wvn_flow_destroy(wvn_flow_t* h) {
+  if (!h) return;
+  flow_trainer_destroy(h->impl);
+  delete h;
+}
+
+int wvn_flow_set_confidence(wvn_flow_t* h, int method, float* var, double* running_n, double* running_sum,
+                            double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
+  WVN_REQUIRE(h, "wvn_flow_set_confidence: null handle");
+  return flow_trainer_set_confidence(h->impl, method, var, running_n, running_sum, running_sum_of_squares, kf_proc_cov,
+                                     kf_meas_cov);
+}
+
+int wvn_flow_copy_confidence(wvn_flow_t* dst, const wvn_flow_t* src, void* stream) {
+  WVN_REQUIRE(dst && src, "wvn_flow_copy_confidence: null handle");
+  return flow_trainer_copy_confidence(dst->impl, src->impl, S(stream));
+}
+
+int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                        const wvn_flow_buffers* buffers, const float* x, int rows, const unsigned char* y_valid,
+                        float* cg_mean, float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
+                        void* stream) {
+  WVN_REQUIRE(h && buffers, "wvn_flow_train_step: null argument");
+  return flow_train_step(h->impl, params, exp_avg, exp_avg_sq, step_counter, buffers_of(buffers), x, rows, y_valid,
+                         cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
+}
+
+int wvn_flow_infer_create(int dim, int hidden, int max_rows, int chunk_pixels, wvn_flow_infer_t** out) {
+  WVN_REQUIRE(out && max_rows > 0, "wvn_flow_infer_create: bad arguments");
+  WVN_PROPAGATE(wvn_check_device());
+  FlowShape s;
+  s.dim = dim; s.hidden = hidden;
+  wvn_flow_infer* h = new wvn_flow_infer();
+  int rc = flow_trainer_create(s, max_rows, 0.5f, AdamCfg(), nullptr, true, &h->rows);
+  if (rc == WVN_OK) rc = flow_pixels_create(s, chunk_pixels, &h->pix);
+  if (rc != WVN_OK) {
+    wvn_flow_infer_destroy(h);
+    return rc;
+  }
+  *out = h;
+  return WVN_OK;
+}
+
+void wvn_flow_infer_destroy(wvn_flow_infer_t* h) {
+  if (!h) return;
+  flow_trainer_destroy(h->rows);
+  flow_pixels_destroy(h->pix);
+  delete h;
+}
+
+int wvn_flow_infer_set_params(wvn_flow_infer_t* h, const float* params, void* stream) {
+  WVN_REQUIRE(h, "wvn_flow_infer_set_params: null handle");
+  return flow_pixels_set_params(h->pix, params, S(stream));
+}
+
+int wvn_flow_infer_rows(wvn_flow_infer_t* h, const float* params, const wvn_flow_buffers* buffers, const float* x, int rows,
+                        float* z, float* log_det, float* logprob, const float* cg_mean, const float* cg_std,
+                        float std_factor, float* trav, void* stream) {
+  WVN_REQUIRE(h && buffers, "wvn_flow_infer_rows: null argument");
+  return flow_forward_rows(h->rows, params, buffers_of(buffers), x, rows, z, log_det, logprob, cg_mean, cg_std,
+                           std_factor, trav, S(stream));
+}
+
+int wvn_flow_infer_pixels(wvn_flow_infer_t* h, const wvn_flow_buffers* buffers, const float* tokens, int batch, int gh,
+                          int gw, int out_h, int out_w, const float* cg_mean, const float* cg_std, float std_factor,
+                          float* trav, float* nll, void* stream) {
+  WVN_REQUIRE(h && buffers, "wvn_flow_infer_pixels: null argument");
+  return flow_pixels_run(h->pix, buffers_of(buffers), tokens, batch, gh, gw, out_h, out_w, cg_mean, cg_std, std_factor,
+                         trav, nll, S(stream));
 }
 
 }  // extern "C"

@@ -24,6 +24,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "conf_update.cuh"
 #include "host_common.h"
 #include "mlp_train.h"
 #include "mlp_train_fused.h"
@@ -242,66 +243,15 @@ train_fwd_rows_kernel(MlpShape s, MlpOffsets o, const float* __restrict__ params
 }
 
 // ------------------------------------------------------------------------------------------------ K1b
-// ConfidenceGenerator.update from the (all-reduced) sums of this step: one thread.  utils/confidence_generator.py:
-// latest_measurement :78-82, running_mean :94-115, moving_average :117-129, kalman_filter :131-145 (+ KalmanFilter,
-// utils/kalman_filter.py:78-111 with D = 1, F = H = 1).
+// ConfidenceGenerator.update from the (all-reduced) sums of this step: one thread (conf_update.cuh).
 __global__ void train_conf_kernel(LossCfg cfg, ConfState cs, int dim, FusedScalars* __restrict__ sc,
                                   float* __restrict__ cg_mean, float* __restrict__ cg_std,
                                   long long* __restrict__ step_counter) {
   if (threadIdx.x != 0) return;
-  const double n = sc->n_valid, s1 = sc->sum_lr, s2 = sc->sum_lr2;
-  float m, sd;
-  float lo, hi, cmin = 0.f, cmax = 0.f;
-  if (cs.method == CONF_RUNNING_MEAN) {
-    const double rn = *cs.running_n + n, rs = *cs.running_sum + s1, rq = *cs.running_sumsq + s2;
-    *cs.running_n = rn; *cs.running_sum = rs; *cs.running_sumsq = rq;
-    m = static_cast<float>(rs / rn);
-    const float var = static_cast<float>(rq / rn - static_cast<double>(m * m));   // float64 - float32^2, stored as fp32
-    sd = sqrtf(var);
-    if (cs.var) *cs.var = var;
-  } else if (cs.method == CONF_KALMAN) {
-    float state = cg_mean ? *cg_mean : 0.f, cov = cs.var ? *cs.var : 1.f;
-    if (n > 0.0) {
-      const float meas = static_cast<float>(s1 / n);
-      cov = cov + cs.kf_proc_cov;                      // prediction: F = 1
-      const float gain = cov / (cov + cs.kf_meas_cov);
-      state = state + gain * (meas - state);
-      cov = (1.f - gain) * cov;
-      if (cs.var) *cs.var = cov;
-    }
-    m = state;
-    sd = sqrtf(cov);
-  } else if (cs.method == CONF_MOVING_AVERAGE) {
-    // the deque of the last kConfWindow positive sets, kept as (n, sum, sum of squares) per step
-    double* ring = cs.ring;
-    const int count = static_cast<int>(ring[3 * kConfWindow]);
-    const int slot = count % kConfWindow;
-    ring[3 * slot] = n; ring[3 * slot + 1] = s1; ring[3 * slot + 2] = s2;
-    ring[3 * kConfWindow] = count + 1;
-    double N = 0.0, S1 = 0.0, S2 = 0.0;
-    for (int i = 0; i < (count + 1 < kConfWindow ? count + 1 : kConfWindow); ++i) { N += ring[3 * i]; S1 += ring[3 * i + 1]; S2 += ring[3 * i + 2]; }
-    const double mean = S1 / N;
-    m = static_cast<float>(mean);
-    sd = N > 1.0 ? static_cast<float>(sqrt(fmax((S2 - N * mean * mean) / (N - 1.0), 0.0))) : nanf("");
-  } else {
-    const double mean = s1 / n;                                   // n == 0 -> NaN, like torch's mean of empty
-    const double var = (s2 - n * mean * mean) / (n - 1.0);        // n == 1 -> NaN, like torch.std
-    m = static_cast<float>(mean);
-    sd = (n > 1.0) ? static_cast<float>(sqrt(fmax(var, 0.0))) : nanf("");
-  }
-  if (cs.method == CONF_KALMAN) {
-    lo = m;
-    hi = 1.f / (sd * cfg.std_factor);
-  } else if (cs.method == CONF_MOVING_AVERAGE) {
-    lo = m - 2.f * sd;
-    hi = m + 2.f * sd;
-    cmin = fminf(fmaxf(static_cast<float>(sc->x_min), lo), hi);   // min / max of the clipped losses = clipped extrema
-    cmax = fminf(fmaxf(static_cast<float>(sc->x_max), lo), hi);
-  } else {
-    const float shifted = m + sd * cfg.std_factor;
-    lo = fmaxf(shifted - sd, 0.f);
-    hi = shifted + sd;
-  }
+  const double n = sc->n_valid;
+  const ConfUpdate u = conf_generator_update(cs, cfg.std_factor, n, sc->sum_lr, sc->sum_lr2, sc->x_min, sc->x_max,
+                                             cg_mean);
+  const float m = u.mean, sd = u.std, lo = u.lo, hi = u.hi, cmin = u.cmin, cmax = u.cmax;
   sc->lo = lo; sc->hi = hi; sc->cmin = cmin; sc->cmax = cmax;
   sc->g_reco = cfg.w_reco * 2.f / (static_cast<float>(n) * static_cast<float>(dim));
   sc->g_trav = cfg.w_trav * 2.f / static_cast<float>(sc->n_rows);
@@ -310,16 +260,6 @@ __global__ void train_conf_kernel(LossCfg cfg, ConfState cs, int dim, FusedScala
   if (cg_mean) *cg_mean = m;
   if (cg_std) *cg_std = sd;
   *step_counter += 1;  // torch.optim.Adam counts from 1; K4 reads the bumped value
-}
-
-__device__ __forceinline__ float row_confidence(int method, float lr, float lo, float hi, float cmin, float cmax) {
-  if (method == CONF_KALMAN) {   // lo = mean, hi = 1 / (std * std_factor)
-    const float z = (lr - lo) * hi;
-    return lr < lo ? 1.f : expf(-(z * z) * 0.5f);
-  }
-  const float xc = fminf(fmaxf(lr, lo), hi);
-  if (method == CONF_MOVING_AVERAGE) return (xc - cmin) / (cmax - cmin);
-  return 1.f - (xc - lo) / (hi - lo);
 }
 
 // ------------------------------------------------------------------------------------------------ K2

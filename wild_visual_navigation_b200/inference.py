@@ -9,18 +9,33 @@
 
 fused as: ViT tokens -> (bilinear sample -> 3 wgmma GEMMs -> sigmoid / reco-loss / confidence
 epilogue) per pixel; neither ``dense_feat`` (308 MB/frame) nor the (P, 385) prediction is stored.
+
+In anomaly-detection mode (a ``LinearRnvp`` model, wvn_feature_extractor_node.py:332-338) traversability is the
+generator's ``inference_without_update`` of the per-row NLL and there is no confidence map (the node forces
+``publish_confidence = False``): per pixel, the tokens are upsampled in a sampling kernel and every layer of the four
+nets runs as a wgmma GEMM (bf16 operands, fp32 accumulation) over chunks of pixels, with the coupling arithmetic, NLL and
+confidence in fp32 kernels (csrc/flow_train.cu); ``predict_segments`` runs the fp32 flow on the pooled rows.
 """
 from __future__ import annotations
 
 import torch
 
 from . import ops
+from .model.linear_rnvp import LinearRnvp
 from .model.simple_mlp import SimpleMLP
 from .utils.confidence_generator import ConfidenceGenerator
 
 
 class TraversabilityInference:
     def __init__(self, dino, model: SimpleMLP, confidence_generator: ConfidenceGenerator, chunk_rows: int = 0):
+        self._flow = isinstance(model, LinearRnvp)
+        if self._flow:
+            if model.flat_params is None or not model.flat_params.is_cuda:
+                raise ValueError("TraversabilityInference: the LinearRnvp must be on a CUDA device")
+            self._dino, self._model, self._cg = dino, model, confidence_generator
+            self._flow_infer = ops.FlowInference(model.input_size, model.hidden, max_rows=1024, chunk_pixels=chunk_rows)
+            self.refresh_weights()
+            return
         assert model.fused_ok(), "model must be the hot-path SimpleMLP(D,[256,32,1],reconstruction=True) on CUDA"
         self._dino = dino
         self._model = model
@@ -33,7 +48,11 @@ class TraversabilityInference:
 
     def refresh_weights(self):
         """Re-pack the bf16 GEMM operands after the MLP parameters changed (the node's ``load_model``,
-        wvn_feature_extractor_node.py:407-450, runs at <= 1 Hz)."""
+        wvn_feature_extractor_node.py:407-450, runs at <= 1 Hz).  For a LinearRnvp the bf16 operands of the per-pixel
+        path are re-packed; masks and permutations are read from the module's buffers on every call."""
+        if self._flow:
+            self._flow_infer.set_params(self._model.flat_params)
+            return
         self._mlp.set_params(self._model.flat_params)
 
     def load_model(self, path: str) -> bool:
@@ -55,6 +74,9 @@ class TraversabilityInference:
     @torch.no_grad()
     def predict_from_tokens(self, tokens: torch.Tensor, out_size: int):
         g = self._dino.grid
+        if self._flow:   # anomaly mode: (trav, None) — the node publishes no confidence map here
+            return self._flow_infer.pixels(self._model, tokens, (g, g), (out_size, out_size), self._cg.mean.data,
+                                           self._cg.std.data, self._cg.std_factor), None
         vit = self._dino._model
         last = getattr(vit, "last_tokens", None)
         if (last is not None and tokens.data_ptr() == last.data_ptr() and tokens.shape[1:] == last.shape[1:]
@@ -68,6 +90,9 @@ class TraversabilityInference:
     @torch.no_grad()
     def predict_segments(self, feat: torch.Tensor, seg: torch.Tensor):
         """Segment-wise mode (``prediction_per_pixel=False``, node :324-327): MLP on the S pooled rows,
-        scattered back through ``seg``."""
+        scattered back through ``seg``.  For a LinearRnvp: (trav[seg], None), trav the confidence of each row's NLL."""
+        if self._flow:
+            return self._flow_infer.trav(self._model, feat, self._cg.mean.data, self._cg.std.data,
+                                         self._cg.std_factor)[seg], None
         trav, conf = self._mlp.rows(feat, self._cg.mean.data, self._cg.std.data, self._cg.std_factor)
         return trav[seg], conf[seg]

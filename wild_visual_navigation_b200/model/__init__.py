@@ -1,2 +1,3 @@
 from .simple_mlp import SimpleMLP
+from .linear_rnvp import LinearRnvp
 from .network_register import get_model

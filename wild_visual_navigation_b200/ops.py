@@ -14,7 +14,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _C
-from ._C import ResnetConfig, TrainConfig, VitConfig, check, lib, ptr, stream
+from ._C import FlowBuffers, ResnetConfig, TrainConfig, VitConfig, check, lib, ptr, stream
 
 OUT_BF16, OUT_F32, OUT_RESID_F32 = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
@@ -686,3 +686,176 @@ class MlpTrainer:
                 self._h = None
         except Exception:
             pass
+
+
+# --------------------------------------------------------------------------------------------
+# LinearRnvp flow (anomaly-detection learner): fp32 row forward and online train step
+# --------------------------------------------------------------------------------------------
+def flow_buffers(model):
+    """The wvn_flow_buffers of a LinearRnvp: its masks and permutations, read by the kernels on every call."""
+    f = model.flows
+    for t in (f[0].mask, f[2].mask, f[1].p, f[1].invp, f[3].p, f[3].invp):
+        assert t.is_cuda and t.is_contiguous()
+    assert f[0].mask.dtype == torch.float32 and f[1].p.dtype == torch.int64
+    return FlowBuffers(f[0].mask.data_ptr(), f[2].mask.data_ptr(), f[1].p.data_ptr(), f[1].invp.data_ptr(),
+                       f[3].p.data_ptr(), f[3].invp.data_ptr())
+
+
+class _FlowHandle:
+    """Owns a ``wvn_flow_t`` (workspaces for ``max_rows`` rows); grows it when a call needs more rows."""
+
+    def __init__(self, dim, hidden, max_rows, cfg, grads=None):
+        _C.require_device()
+        self.dim, self.hidden, self.cfg, self._grads = dim, hidden, cfg, grads
+        self.n_params = lib().wvn_flow_param_count(dim, hidden)
+        self._h = None
+        self._conf = None
+        self._create(max_rows)
+
+    def _create(self, max_rows):
+        h = c_void_p()
+        check(lib().wvn_flow_create(self.dim, self.hidden, int(max_rows), byref(self.cfg), ptr(self._grads), byref(h)))
+        if self._h is not None:
+            # the larger handle takes over the generator state the old one kept itself (moving_average's window, ...)
+            check(lib().wvn_flow_copy_confidence(h, self._h, stream()))
+            lib().wvn_flow_destroy(self._h)
+        self._h = h
+        self.max_rows = int(max_rows)
+        if self._conf is not None:
+            self.set_confidence(*self._conf)
+
+    def _reserve(self, rows):
+        if rows > self.max_rows:
+            self._create(int(rows * 1.5))
+
+    def set_confidence(self, method=0, var=None, running_n=None, running_sum=None, running_sum_of_squares=None,
+                       kf_proc_cov=0.2, kf_meas_cov=1.0):
+        self._conf = (int(method), var, running_n, running_sum, running_sum_of_squares, float(kf_proc_cov), float(kf_meas_cov))
+        check(lib().wvn_flow_set_confidence(self._h, int(method), ptr(var), ptr(running_n), ptr(running_sum),
+                                            ptr(running_sum_of_squares), float(kf_proc_cov), float(kf_meas_cov)))
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().wvn_flow_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+class FlowInference:
+    """Owns a ``wvn_flow_infer_t`` (forward workspaces only): LinearRnvp.forward on rows in fp32, and the per-pixel
+    anomaly map on wgmma (bf16 operands, fp32 accumulation; ``set_params`` re-packs them).  Traversability is
+    ``ConfidenceGenerator.inference_without_update`` of the NLL ``-(logprob.sum(1) + log_det)``."""
+
+    def __init__(self, dim=384, hidden=200, max_rows=1024, chunk_pixels=0):
+        _C.require_device()
+        self.dim, self.hidden, self.chunk_pixels = dim, hidden, chunk_pixels
+        self._h = None
+        self._params = None
+        self._create(max_rows)
+
+    def _create(self, max_rows):
+        h = c_void_p()
+        check(lib().wvn_flow_infer_create(self.dim, self.hidden, int(max_rows), int(self.chunk_pixels), byref(h)))
+        if self._h is not None:
+            lib().wvn_flow_infer_destroy(self._h)
+        self._h = h
+        self.max_rows = int(max_rows)
+        if self._params is not None:
+            self.set_params(self._params)
+
+    def _reserve(self, rows):
+        if rows > self.max_rows:
+            self._create(int(rows * 1.5))
+
+    def set_params(self, flat_params):
+        """Re-pack the bf16 operands of the per-pixel path (after the parameters changed)."""
+        assert flat_params.is_cuda and flat_params.dtype == torch.float32 and flat_params.is_contiguous()
+        self._params = flat_params
+        check(lib().wvn_flow_infer_set_params(self._h, ptr(flat_params), stream()))
+
+    def rows(self, model, x, want_z=True, want_logprob=True):
+        """x (R, D) fp32 -> dict(z (R,D), log_det (R,), logprob (R,D)), the reference's forward outputs."""
+        R = x.shape[0]
+        self._reserve(R)
+        x = x.contiguous().float()
+        z = torch.empty(R, self.dim, device=x.device) if want_z else None
+        ld = torch.empty(R, device=x.device)
+        lp = torch.empty(R, self.dim, device=x.device) if want_logprob else None
+        check(lib().wvn_flow_infer_rows(self._h, ptr(model.flat_params), byref(flow_buffers(model)), ptr(x), R, ptr(z),
+                                        ptr(ld), ptr(lp), None, None, 0.0, None, stream()))
+        return {"z": z, "log_det": ld, "logprob": lp}
+
+    def trav(self, model, x, cg_mean, cg_std, std_factor):
+        """x (R, D) fp32 -> the confidence of each row's NLL under the generator (R,) fp32."""
+        R = x.shape[0]
+        self._reserve(R)
+        x = x.contiguous().float()
+        out = torch.empty(R, device=x.device)
+        check(lib().wvn_flow_infer_rows(self._h, ptr(model.flat_params), byref(flow_buffers(model)), ptr(x), R, None,
+                                        None, None, ptr(cg_mean), ptr(cg_std), float(std_factor), ptr(out), stream()))
+        return out
+
+    def pixels(self, model, tokens, grid, out_hw, cg_mean, cg_std, std_factor, want_nll=False):
+        """tokens (B, gh*gw, D) fp32 -> trav (B, H, W) fp32 (and the per-pixel NLL with want_nll).  Uses the operands
+        of the last ``set_params``."""
+        assert self._params is not None, "FlowInference.pixels: set_params was never called"
+        B = tokens.shape[0]
+        tokens = tokens.contiguous().float()
+        trav = torch.empty(B, out_hw[0], out_hw[1], device=tokens.device)
+        nll = torch.empty_like(trav) if want_nll else None
+        check(lib().wvn_flow_infer_pixels(self._h, byref(flow_buffers(model)), ptr(tokens), B, grid[0], grid[1],
+                                          out_hw[0], out_hw[1], ptr(cg_mean), ptr(cg_std), float(std_factor), ptr(trav),
+                                          ptr(nll), stream()))
+        return (trav, nll) if want_nll else trav
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().wvn_flow_infer_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+class FlowTrainer(_FlowHandle):
+    """The anomaly-detection train step on a LinearRnvp's flat fp32 parameters (csrc/flow_train.cu): forward, loss
+    ``-mean(logprob.sum(1) + log_det)`` over the labelled rows, ConfidenceGenerator update with the per-row NLL,
+    backward and Adam as one fixed launch sequence without host synchronisation.  ``exp_avg`` / ``exp_avg_sq`` /
+    ``step_counter`` are torch.optim.Adam's state over the 24 parameter tensors, flattened in ``parameters()`` order."""
+
+    def __init__(self, model, max_rows=4096, std_factor=0.5, lr=1e-3, betas=(0.9, 0.999), eps=1e-8):
+        params = model.flat_params
+        assert params.is_cuda and params.dtype == torch.float32
+        dev = params.device
+        self.model = model
+        grads = torch.zeros(lib().wvn_flow_param_count(model.input_size, model.hidden), device=dev)
+        super().__init__(model.input_size, model.hidden, max_rows,
+                         TrainConfig(0.0, 0.0, float(std_factor), 0, float(lr), betas[0], betas[1], float(eps)), grads)
+        self.grads = grads
+        self.exp_avg = torch.zeros(self.n_params, device=dev)
+        self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
+        self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
+        self.metrics = torch.zeros(6, device=dev)
+        self.cg_mean = torch.zeros(1, device=dev)
+        self.cg_std = torch.ones(1, device=dev)
+        self.conf = torch.empty(self.max_rows, device=dev)
+
+    def _create(self, max_rows):
+        super()._create(max_rows)
+        if hasattr(self, "conf"):
+            self.conf = torch.empty(self.max_rows, device=self.conf.device)
+
+    def step(self, x, y_valid=None, phase_mask=7):
+        """x (R, D) fp32; y_valid (R,) bool or None (every row).  Returns the confidence of the labelled rows in
+        order (a view of length R whose first n entries are live; n is metrics[3])."""
+        R = x.shape[0]
+        self._reserve(R)
+        x = x.contiguous().float()
+        yv = None if y_valid is None else y_valid.contiguous().to(torch.uint8)
+        check(lib().wvn_flow_train_step(self._h, ptr(self.model.flat_params), ptr(self.exp_avg), ptr(self.exp_avg_sq),
+                                        ptr(self.step_counter), byref(flow_buffers(self.model)), ptr(x), R, ptr(yv),
+                                        ptr(self.cg_mean), ptr(self.cg_std), ptr(self.conf), ptr(self.metrics),
+                                        int(phase_mask), stream()))
+        return self.conf[:R]

@@ -1,8 +1,8 @@
 """TraversabilityEstimator — the online learner
 (reference: wild_visual_navigation/traversability_estimator/traversability_estimator.py:33-505).
 
-On the hot path and implemented: ``__init__`` (seed 42, SimpleMLP, TraversabilityLoss, Adam —
-:78-105), ``make_batch`` (:431-446), ``train`` (:448-497, same return dict), ``save_checkpoint`` /
+On the hot path and implemented: ``__init__`` (seed 42, SimpleMLP + TraversabilityLoss, or with
+``anomaly_detection=True`` LinearRnvp + AnomalyLoss, Adam — :78-105), ``make_batch`` (:431-446), ``train`` (:448-497, same return dict), ``save_checkpoint`` /
 ``load_checkpoint`` (:377-429, same file format incl. a torch.optim.Adam-compatible
 ``optimizer_state_dict``), ``pause_learning`` / ``step`` / ``loss``.
 The mission / supervision graphs (networkx + liegroups, nodes.py / graphs.py), footprint
@@ -12,6 +12,8 @@ list and must already carry their per-segment features and supervision (``Missio
 ``train()`` runs forward + loss + backward + Adam as one fixed sequence of fp32 CUDA kernels
 (csrc/mlp_train.cu) with all scalars on the device; with a ``process_group`` the three confidence
 statistics and the flat gradient are all-reduced (NCCL over NVLink) for a global-batch step.
+In anomaly-detection mode the step is the LinearRnvp flow's (csrc/flow_train.cu: forward, NLL, confidence update,
+backward, Adam) on the labelled rows only; it is single-GPU.
 """
 from __future__ import annotations
 
@@ -23,16 +25,20 @@ import torch
 
 from .. import ops
 from ..model import get_model
-from ..utils import Batch, Data, TraversabilityLoss
+from ..utils import AnomalyLoss, Batch, Data, TraversabilityLoss
 
 
-def default_params():
-    """The defaults of ``ExperimentParams`` that define the hot path (cfg/experiment_params.py:44-56,91,104-112)."""
+def default_params(anomaly_detection: bool = False):
+    """The defaults of ``ExperimentParams`` that define the hot path (cfg/experiment_params.py:44-65,91,104-140); with
+    ``anomaly_detection`` the model is ``LinearRnvp`` (what the nodes select with ``model.name = "LinearRnvp"``)."""
     return {
-        "model": {"name": "SimpleMLP",
-                  "simple_mlp_cfg": {"input_size": 384, "hidden_sizes": [256, 32, 1], "reconstruction": True}},
+        "model": {"name": "LinearRnvp" if anomaly_detection else "SimpleMLP",
+                  "simple_mlp_cfg": {"input_size": 384, "hidden_sizes": [256, 32, 1], "reconstruction": True},
+                  "linear_rnvp_cfg": {"input_size": 384, "coupling_topology": [200], "mask_type": "odds",
+                                      "conditioning_size": 0, "use_permutation": True, "single_function": False}},
         "loss": {"anomaly_balanced": True, "w_trav": 0.03, "w_temp": 0.0, "w_reco": 0.5, "method": "latest_measurement",
                  "confidence_std_factor": 0.5, "trav_cross_entropy": False},
+        "loss_anomaly": {"method": "latest_measurement", "confidence_std_factor": 0.5},
         "optimizer": {"name": "ADAM", "lr": 0.001},
         "ablation_data_module": {"batch_size": 8},
         "general": {"log_confidence": False, "model_path": "/tmp"},
@@ -65,6 +71,9 @@ class MissionNode:
         self.supervision_signal, self.supervision_signal_valid = y[0], valid[0]
 
     def as_pyg_data(self, anomaly_detection: bool = False):
+        if anomaly_detection:   # the flow learns from the labelled rows only (nodes.py:207-214)
+            v = self.supervision_signal_valid
+            return Data(x=self.features[v], y=self.supervision_signal[v], y_valid=v[v])
         return Data(x=self.features, y=self.supervision_signal, y_valid=self.supervision_signal_valid)
 
 
@@ -77,14 +86,14 @@ class TraversabilityEstimator:
                  supervision_distance_thr: float = None, min_samples_for_training: int = 10, vis_node_index: int = 10,
                  mode=None, extraction_store_folder=None, anomaly_detection: bool = False, process_group=None,
                  max_rows: int = 4096):
-        if anomaly_detection:
-            raise ValueError("anomaly_detection (LinearRnvp) is outside the H100 hot path")
+        if anomaly_detection and process_group is not None:
+            raise ValueError("anomaly_detection (LinearRnvp) trains on one GPU: process_group is not supported")
         self._device = device
         self._mode = mode
         self._extraction_store_folder = extraction_store_folder
         self._min_samples_for_training = min_samples_for_training
         self._vis_node_index = vis_node_index
-        self._params = params if params is not None else default_params()
+        self._params = params if params is not None else default_params(anomaly_detection)
         self._anomaly_detection = anomaly_detection
         self._mission_nodes = []
         self._learning_lock = Lock()
@@ -92,14 +101,30 @@ class TraversabilityEstimator:
 
         torch.manual_seed(42)  # seed_everything(42) (:78) — same init as the reference's get_model
         random.seed(42)
-        self._model = get_model(_get(self._params, "model")).to(self._device)
+        model_cfg = _get(self._params, "model")
+        if anomaly_detection != (_get(model_cfg, "name") == "LinearRnvp"):
+            raise ValueError("anomaly_detection=True goes with model.name 'LinearRnvp' (and only with it), got "
+                             f"{_get(model_cfg, 'name')!r}")
+        self._model = get_model(model_cfg).to(self._device)
         self._model.train()
-        lp = dict(_get(self._params, "loss"))
         gp = _get(self._params, "general")
+        self._lr = float(_get(_get(self._params, "optimizer"), "lr"))
+        self._loss = torch.tensor([torch.inf])
+        self._step = 0
+        self._last_confidence = None
+        if anomaly_detection:
+            la = dict(_get(self._params, "loss_anomaly"))
+            self._traversability_loss = AnomalyLoss(**la, log_enabled=_get(gp, "log_confidence"),
+                                                    log_folder=_get(gp, "model_path"))
+            self._traversability_loss.to(self._device)
+            cg = self._traversability_loss._confidence_generator
+            self._trainer = ops.FlowTrainer(self._model, max_rows=max_rows, std_factor=cg.std_factor, lr=self._lr)
+            self._bind_confidence_state()
+            return
+        lp = dict(_get(self._params, "loss"))
         self._traversability_loss = TraversabilityLoss(
             **lp, model=self._model, log_enabled=_get(gp, "log_confidence"), log_folder=_get(gp, "model_path"))
         self._traversability_loss.to(self._device)
-        self._lr = float(_get(_get(self._params, "optimizer"), "lr"))
         m = self._model
         cg = self._traversability_loss._confidence_generator
         self._trainer = ops.MlpTrainer(m.flat_params, m.input_size, m.hidden[0], m.hidden[1], max_rows=max_rows,
@@ -108,9 +133,6 @@ class TraversabilityEstimator:
         # the train step writes the ConfidenceGenerator's mean / std straight into the module's parameters
         self._trainer.cg_mean, self._trainer.cg_std = cg.mean.data, cg.std.data
         self._bind_confidence_state()
-        self._loss = torch.tensor([torch.inf])
-        self._step = 0
-        self._last_confidence = None
 
     def _bind_confidence_state(self):
         """Points the fused step at the ConfidenceGenerator's own parameters (mean / std / var / running sums), so the
@@ -167,7 +189,10 @@ class TraversabilityEstimator:
         """forward + TraversabilityLoss + backward + Adam on ``graph`` (x, y, y_valid).  Metrics stay
         on the device in ``self._trainer.metrics``; returns the per-row confidence."""
         with self._learning_lock:
-            conf = self._trainer.step(graph.x, graph.y, graph.y_valid, n_total=n_total)
+            if self._anomaly_detection:   # AnomalyLoss: the flow's step on the labelled rows of the batch
+                conf = self._trainer.step(graph.x, graph.y_valid)
+            else:
+                conf = self._trainer.step(graph.x, graph.y, graph.y_valid, n_total=n_total)
             self._last_confidence = conf
         self._step += 1
         return conf
@@ -176,6 +201,8 @@ class TraversabilityEstimator:
         """The same step on rows that are still padded per frame, as ``FeatureExtractor.extract_batch`` returns them:
         ``feat`` (B, smax, D), ``n_rows`` (B,) int32 on the device; ``y`` / ``y_valid`` are indexed by the compacted row
         number (what ``feat[mask]`` would give).  No host synchronisation (the gather happens inside the kernels)."""
+        if self._anomaly_detection:
+            raise ValueError("train_on_padded is the SimpleMLP step; in anomaly-detection mode use train_on_batch")
         with self._learning_lock:
             conf = self._trainer.step_padded(feat, n_rows, y, y_valid)
             self._last_confidence = conf
@@ -205,9 +232,13 @@ class TraversabilityEstimator:
         return return_dict
 
     # ---- checkpoints (same on-disk format as the reference, :377-429) --------------------------
+    def _optimizer_params(self):
+        """The tensors torch.optim.Adam(model.parameters()) would hold, in its order."""
+        return list(self._model.parameters())
+
     def _optimizer_state_dict(self):
         tr, off, state = self._trainer, 0, {}
-        for i, p in enumerate(self._model.layers.parameters()):
+        for i, p in enumerate(self._optimizer_params()):
             n = p.numel()
             state[i] = {"step": tr.step_counter.float().cpu().reshape(()).clone(),
                         "exp_avg": tr.exp_avg[off : off + n].view_as(p).clone(),
@@ -220,7 +251,7 @@ class TraversabilityEstimator:
 
     def _load_optimizer_state_dict(self, sd):
         tr, off = self._trainer, 0
-        for i, p in enumerate(self._model.layers.parameters()):
+        for i, p in enumerate(self._optimizer_params()):
             n = p.numel()
             st = sd["state"].get(i)
             if st is not None:

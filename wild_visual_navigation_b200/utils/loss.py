@@ -1,4 +1,4 @@
-"""TraversabilityLoss (reference: wild_visual_navigation/utils/loss.py:57-164).
+"""TraversabilityLoss (reference: wild_visual_navigation/utils/loss.py:57-164) and AnomalyLoss (:16-54).
 
 Holds the loss weights and the ConfidenceGenerator.  In the reference ``forward`` builds an
 autograd graph; here the whole fwd + loss + bwd + Adam step is one fused kernel sequence driven
@@ -57,3 +57,28 @@ class TraversabilityLoss(nn.Module):
     def update_node_confidence(self, node):
         reco_loss = ((node.prediction[:, 1:] - node.features) ** 2).mean(dim=1)
         node.confidence = self._confidence_generator.inference_without_update(reco_loss)
+
+
+class AnomalyLoss(nn.Module):
+    """The LinearRnvp learner's loss (reference: utils/loss.py:16-54): ``-mean(logprob.sum(1) + log_det)``, with the
+    ConfidenceGenerator updated on the per-row NLL (``x = x_positive``: the batch holds only labelled rows).  The
+    training step itself runs fused in csrc/flow_train.cu (``ops.FlowTrainer``); ``forward`` keeps the reference's
+    signature and return triple for direct use (no grad)."""
+
+    def __init__(self, confidence_std_factor: float, method: str, log_enabled: bool = False, log_folder: str = "/tmp"):
+        super().__init__()
+        self._confidence_generator = ConfidenceGenerator(
+            std_factor=confidence_std_factor, method=method, log_enabled=log_enabled, log_folder=log_folder)
+
+    @torch.no_grad()
+    def forward(self, graph, res: dict, update_generator: bool = True, step: int = 0, log_step: bool = False):
+        loss_aux = {"loss_trav": torch.tensor([0.0]), "loss_reco": torch.tensor([0.0])}
+        losses = res["logprob"].sum(1) + res["log_det"]
+        confidence = None
+        if update_generator:
+            confidence = self._confidence_generator.update(x=-losses.clone(), x_positive=-losses.clone(), step=step)
+        loss_aux["confidence"] = confidence
+        return -torch.mean(losses), loss_aux, confidence
+
+    def update_node_confidence(self, node):
+        node.confidence = 0
