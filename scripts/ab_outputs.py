@@ -10,7 +10,11 @@ output its SHA-256 plus a strided sample (every 101st element, as float32):
     backbone: QKV (bf16), attention out-projection (fp32 residual add), fc1 (bf16 + GELU), fc2 (fp32 residual add);
   * DinoInterface tokens of ViT-S/8 @448 at B = 32;
   * the fused per-pixel traversability / confidence maps of a seeded SimpleMLP on those tokens;
-  * DinoInterface tokens of ViT-S/16 @448 at B = 8 (the patch-16 loader and patch-embed GEMM).
+  * DinoInterface tokens of ViT-S/16 @448 at B = 8 (the patch-16 loader and patch-embed GEMM);
+  * ops.mlp_forward_f32 of that SimpleMLP at R = 4096 and 65536 rows;
+  * FlowInference.rows (z, log_det, logprob) of a seeded LinearRnvp(384, [200]) at R = 4096;
+  * after three FlowTrainer steps at R = 1024, per confidence method: the parameters, Adam's moments, the confidence
+    vector, the metrics and the generator's mean / std / var / running sums.
 `compare` reports, per output, whether the two builds agree bit for bit and, where not, the largest difference in
 the samples.  Every output here is deterministic for a given build (no atomics race in them), so any difference is
 the build's.
@@ -34,7 +38,7 @@ def _record(out_dir, name, t, index):
     digest = hashlib.sha256(raw.view(-1).view(torch.uint8).numpy().tobytes()).hexdigest()
     np.save(os.path.join(out_dir, name + ".npy"), raw.reshape(-1)[::STRIDE].float().numpy())
     index[name] = {"sha256": digest, "shape": list(raw.shape), "dtype": str(raw.dtype)}
-    print(f"{name:28s} {tuple(raw.shape)} {digest[:16]}", flush=True)
+    print(f"{name:44s} {tuple(raw.shape)} {digest[:16]}", flush=True)
 
 
 def write(out_dir):
@@ -103,6 +107,45 @@ def write(out_dir):
     di16 = DinoInterface(dev, input_size=448, backbone_type="vit_small", patch_size=16,
                          state_dict=synthetic_state_dict(cfg16, seed=1), max_batch=8)
     _record(out_dir, "dino_tokens_s16", di16.inference_tokens(img[:8]), index)
+    del di16
+    torch.cuda.empty_cache()
+
+    # ---- the fp32 CUDA-core paths: SimpleMLP forward, LinearRnvp row forward and train step
+    g = torch.Generator(device=dev).manual_seed(13)
+    for R in (4096, 65536):
+        x = torch.randn(R, 384, device=dev, generator=g) * 0.5
+        _record(out_dir, f"mlp_forward_f32_{R}", ops.mlp_forward_f32(model.flat_params, x, 384, 256, 32), index)
+
+    from wild_visual_navigation_b200 import LinearRnvp
+    from wild_visual_navigation_b200.utils import AnomalyLoss
+
+    torch.manual_seed(42)
+    flow = LinearRnvp(384, [200], use_permutation=True).to(dev)
+    x = torch.randn(4096, 384, device=dev, generator=g) * 0.5
+    rows = ops.FlowInference(384, 200, max_rows=4096).rows(flow, x)
+    for k in ("z", "log_det", "logprob"):
+        _record(out_dir, f"flow_rows_{k}", rows[k], index)
+    for method in ("latest_measurement", "running_mean", "kalman_filter", "moving_average"):
+        torch.manual_seed(42)
+        flow = LinearRnvp(384, [200], use_permutation=True).to(dev)
+        cg = AnomalyLoss(0.5, method).to(dev)._confidence_generator
+        tr = ops.FlowTrainer(flow, max_rows=1024)
+        tr.cg_mean, tr.cg_std = cg.mean.data, cg.std.data
+        kf = getattr(cg, "_kalman_filter", None)
+        tr.set_confidence(cg.method_id, cg.var.data, getattr(cg, "running_n", None), getattr(cg, "running_sum", None),
+                          getattr(cg, "running_sum_of_squares", None),
+                          kf_proc_cov=float(kf.proc_cov.item()) if kf is not None else 0.2,
+                          kf_meas_cov=float(kf.meas_cov.item()) if kf is not None else 1.0)
+        gs = torch.Generator(device=dev).manual_seed(14)
+        for _ in range(3):
+            conf = tr.step(torch.randn(1024, 384, device=dev, generator=gs) * 0.5)
+        out = {"params": flow.flat_params, "exp_avg": tr.exp_avg, "exp_avg_sq": tr.exp_avg_sq, "conf": conf,
+               "metrics": tr.metrics, "cg_mean": cg.mean, "cg_std": cg.std, "cg_var": cg.var}
+        for k in ("running_n", "running_sum", "running_sum_of_squares"):
+            if hasattr(cg, k):
+                out["cg_" + k] = getattr(cg, k)
+        for k, t in out.items():
+            _record(out_dir, f"flow_train_{method}_{k}", t, index)
     torch.cuda.synchronize()
 
     with open(os.path.join(out_dir, "index.json"), "w") as f:
@@ -115,16 +158,16 @@ def compare(dir_a, dir_b):
     same = True
     for name in ia:
         if name not in ib:
-            print(f"{name:28s} missing in {dir_b}")
+            print(f"{name:44s} missing in {dir_b}")
             same = False
             continue
         if ia[name]["sha256"] == ib[name]["sha256"]:
-            print(f"{name:28s} bit-identical")
+            print(f"{name:44s} bit-identical")
             continue
         same = False
         sa, sb = np.load(os.path.join(dir_a, name + ".npy")), np.load(os.path.join(dir_b, name + ".npy"))
         d = np.abs(sa.astype(np.float64) - sb.astype(np.float64))
-        print(f"{name:28s} DIFFERENT: sampled max |diff| {d.max():.3e}, {int((d > 0).sum())} of {d.size} samples differ")
+        print(f"{name:44s} DIFFERENT: sampled max |diff| {d.max():.3e}, {int((d > 0).sum())} of {d.size} samples differ")
     print("ALL BIT-IDENTICAL" if same else "OUTPUTS DIFFER")
     return 0 if same else 1
 

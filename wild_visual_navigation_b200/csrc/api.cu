@@ -22,6 +22,7 @@
 #include "footprint_kernels.h"
 #include "slic_kernels.h"
 #include "stego_kmeans.h"
+#include "train_core.h"
 #include "vit_kernels.h"
 
 using namespace wvn;
@@ -1255,13 +1256,13 @@ int wvn_mlp_trainer_init_comm(wvn_mlp_trainer_t* t, const void* id128, int rank,
 int wvn_mlp_trainer_set_confidence(wvn_mlp_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
                                    double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
   WVN_REQUIRE(t, "wvn_mlp_trainer_set_confidence: null trainer");
-  return fused_trainer_set_confidence(t->impl, method, var, running_n, running_sum, running_sum_of_squares, kf_proc_cov,
-                                      kf_meas_cov);
+  return trainer_conf_bind(fused_trainer_conf(t->impl), method, var, running_n, running_sum, running_sum_of_squares,
+                           kf_proc_cov, kf_meas_cov);
 }
 
 int wvn_mlp_trainer_copy_confidence(wvn_mlp_trainer_t* dst, const wvn_mlp_trainer_t* src, void* stream) {
   WVN_REQUIRE(dst && src, "wvn_mlp_trainer_copy_confidence: null trainer");
-  return fused_trainer_copy_confidence(dst->impl, src->impl, S(stream));
+  return trainer_conf_copy(fused_trainer_conf(dst->impl), fused_trainer_conf(src->impl), S(stream));
 }
 
 int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
@@ -1330,13 +1331,13 @@ void wvn_flow_destroy(wvn_flow_t* h) {
 int wvn_flow_set_confidence(wvn_flow_t* h, int method, float* var, double* running_n, double* running_sum,
                             double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
   WVN_REQUIRE(h, "wvn_flow_set_confidence: null handle");
-  return flow_trainer_set_confidence(h->impl, method, var, running_n, running_sum, running_sum_of_squares, kf_proc_cov,
-                                     kf_meas_cov);
+  return trainer_conf_bind(flow_trainer_conf(h->impl), method, var, running_n, running_sum, running_sum_of_squares,
+                           kf_proc_cov, kf_meas_cov);
 }
 
 int wvn_flow_copy_confidence(wvn_flow_t* dst, const wvn_flow_t* src, void* stream) {
   WVN_REQUIRE(dst && src, "wvn_flow_copy_confidence: null handle");
-  return flow_trainer_copy_confidence(dst->impl, src->impl, S(stream));
+  return trainer_conf_copy(flow_trainer_conf(dst->impl), flow_trainer_conf(src->impl), S(stream));
 }
 
 int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,

@@ -9,9 +9,10 @@
 //
 // The step is one fixed sequence of ~24 launches with every scalar on the device (no host synchronisation):
 //   compact (labelled rows from y_valid) -> gather -> per coupling 3 batched GEMMs (s | t) + the coupling kernel
-//   -> NLL statistics + confidence update (conf_update.cuh) + per-row confidence -> per coupling (last first): dx / ds / dt, 2-3 batched
+//   -> NLL statistics + confidence update (train_core.cuh) + per-row confidence -> per coupling (last first): dx / ds / dt, 2-3 batched
 //   data-gradient GEMMs, du -> one batched launch of all 12 weight-gradient products (+ bias gradients) -> Adam
-//   (mlp_adam_step).
+//   (mlp_adam_step).  The GEMMs, Adam and the generator's state are the training core shared with the MLP trainers
+//   (train_core.h / train_core.cuh).
 // Training batches are small (~8 nodes x ~16 labelled segments), so the step is latency-bound: the GEMMs are plain
 // fp32 CUDA-core tiles, every output element is summed by one thread in a fixed order (no atomics: bit-reproducible).
 // The weight-gradient columns that see masked-out inputs (mu = 0) and the last-layer rows that feed masked-out outputs
@@ -22,11 +23,10 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "conf_update.cuh"
 #include "flow_train.h"
 #include "gemm.h"
 #include "host_common.h"
-#include "mlp_train_fused.h"
+#include "train_core.cuh"
 
 namespace wvn {
 
@@ -34,7 +34,6 @@ namespace {
 
 constexpr float kLogSqrt2Pi = 0.91893853320467274178f;   // math.log(math.sqrt(2 * math.pi)), torch.distributions.Normal
 constexpr int kRowThreads = 128;
-constexpr int kMaxProblems = 12;
 constexpr int kStatThreads = 256;
 
 // ------------------------------------------------------------------------------------------------ row compaction
@@ -81,92 +80,6 @@ flow_gather_kernel(const float* __restrict__ x, const int* __restrict__ comp, co
     const float u = xr[j];
     u0[static_cast<long long>(r) * dim + j] = u;
     mu0[static_cast<long long>(r) * dim + j] = u * mask[j];
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ batched fp32 GEMM
-// C(m, n) = epilogue(sum_k A(m, k) B(k, n)) with A(m, k) = a[m a_rs + k a_cs], B(k, n) = b[k b_rs + n b_cs]: the same
-// kernel does X W^T (forward), dY W (data gradients) and dY^T X (weight gradients).  live = 1: M is capped by the live
-// row count, live = 2: K is.  Epilogue: + bias[n]; relu (NaN passes, like torch.relu); * (ref(m, n) > 0) (ReLU's
-// backward).  db (weight-gradient problems): db[m] = sum_k A(m, k), the bias gradient.
-struct GemmProblem {
-  const float* a; long long a_rs, a_cs;
-  const float* b; long long b_rs, b_cs;
-  float* c; long long ldc;
-  const float* bias;
-  const float* ref; long long ld_ref;
-  float* db;
-  int M, N, K, relu, live;
-};
-struct GemmBatch {
-  GemmProblem p[kMaxProblems];
-  const int* n_live;
-};
-
-constexpr int GT = 64, GK = 16;
-
-__global__ void __launch_bounds__(256)
-flow_gemm_kernel(GemmBatch g) {
-  const GemmProblem& p = g.p[blockIdx.z];
-  int M = p.M, K = p.K;
-  if (p.live == 1) M = min(M, *g.n_live);
-  if (p.live == 2) K = min(K, *g.n_live);
-  const int m0 = blockIdx.y * GT, n0 = blockIdx.x * GT;
-  if (m0 >= M || n0 >= p.N) return;
-  __shared__ float As[GK][GT + 1];
-  __shared__ float Bs[GK][GT + 1];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const bool a_kfast = p.a_cs == 1, b_nfast = p.b_cs == 1;
-  float acc[4][4], bsum[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-  for (int k0 = 0; k0 < K; k0 += GK) {
-#pragma unroll
-    for (int rr = 0; rr < 4; ++rr) {
-      const int idx = tid + 256 * rr;
-      int mm, kk;
-      if (a_kfast) { mm = idx >> 4; kk = idx & 15; } else { kk = idx >> 6; mm = idx & 63; }
-      const int gm = m0 + mm, gk = k0 + kk;
-      As[kk][mm] = (gm < M && gk < K) ? p.a[gm * p.a_rs + gk * p.a_cs] : 0.f;
-      int nn;
-      if (b_nfast) { kk = idx >> 6; nn = idx & 63; } else { nn = idx >> 4; kk = idx & 15; }
-      const int gn = n0 + nn, gk2 = k0 + kk;
-      Bs[kk][nn] = (gn < p.N && gk2 < K) ? p.b[gk2 * p.b_rs + gn * p.b_cs] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < GK; ++k) {
-      float av[4], bv[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) av[i] = As[k][ty + 16 * i];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) bv[j] = Bs[k][tx + 16 * j];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        bsum[i] += av[i];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-      }
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int gm = m0 + ty + 16 * i;
-    if (gm >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int gn = n0 + tx + 16 * j;
-      if (gn >= p.N) continue;
-      float v = acc[i][j];
-      if (p.bias) v += p.bias[gn];
-      if (p.relu) v = v < 0.f ? 0.f : v;
-      if (p.ref) v = p.ref[gm * p.ld_ref + gn] > 0.f ? v : 0.f;
-      p.c[gm * p.ldc + gn] = v;
-    }
-    if (p.db && blockIdx.x == 0 && tx == 0) p.db[gm] = bsum[i];
   }
 }
 
@@ -241,10 +154,10 @@ flow_coupling_fwd_kernel(CouplingFwd c, int dim, const int* __restrict__ n_live)
 
 // ------------------------------------------------------------------------------------------------ statistics + confidence
 // One block of kStatThreads: sums / extrema of the NLL over the live rows; then one thread updates the generator
-// (conf_update.cuh) and writes the metrics and the loss gradient scale 1 / n for the backward kernels.
+// (train_core.cuh) and writes the metrics and the loss gradient scale 1 / n for the backward kernels.
 struct FlowScalars {
   float inv_n;
-  float lo, hi, cmin, cmax;   // the updated generator, for the per-row confidence (conf_update.cuh)
+  float lo, hi, cmin, cmax;   // the updated generator, for the per-row confidence (train_core.cuh)
   float pad[3];
 };
 
@@ -386,8 +299,7 @@ struct FlowTrainer {
   float *dx = nullptr, *dso[2] = {nullptr, nullptr}, *d2[2] = {nullptr, nullptr}, *d1[2] = {nullptr, nullptr},
         *dmu[2] = {nullptr, nullptr}, *du = nullptr;
   bool forward_only = false;   // inference: no backward workspaces, no gradient buffer
-  ConfState conf;
-  double* conf_priv = nullptr;
+  TrainerConf conf;
 };
 
 int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, const AdamCfg& adam, float* grads_ext,
@@ -398,7 +310,7 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
               "multiple of 8)", s.dim, s.hidden);
   FlowTrainer* t = new FlowTrainer();
   t->s = s; t->adam = adam; t->std_factor = std_factor; t->forward_only = forward_only;
-  t->max_rows = (max_rows + GT - 1) / GT * GT;
+  t->max_rows = (max_rows + 63) / 64 * 64;   // whole 64-row GEMM tiles
   const size_t R = t->max_rows, D = s.dim, h = s.hidden, np = flow_param_count(s);
   const size_t floats = R * D * 4 + R * h * 8 + R * D * 4 + R * D + 2 * R       // forward
                         + (forward_only ? 0 : R * D * 3 + R * h * 4 + R * D * 2 + R * D   // backward
@@ -409,16 +321,13 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
     delete t;
     return set_error(WVN_ERR_CUDA, "flow trainer: cudaMalloc of %zu bytes failed", bytes);
   }
-  if (cudaMalloc(&t->conf_priv, sizeof(double) * 32) != cudaSuccess) {
+  const int rc = trainer_conf_create(&t->conf);
+  if (rc != WVN_OK) {
     cudaFree(t->arena);
     delete t;
-    return set_error(WVN_ERR_CUDA, "flow trainer: cudaMalloc of the confidence state failed");
+    return rc;
   }
   cudaMemset(t->arena, 0, bytes);
-  cudaMemset(t->conf_priv, 0, sizeof(double) * 32);
-  const float one = 1.f;   // private var = 1 (the reference's initial value) unless the caller binds its own
-  cudaMemcpy(reinterpret_cast<float*>(t->conf_priv + 3), &one, sizeof(float), cudaMemcpyHostToDevice);
-  flow_trainer_set_confidence(t, CONF_LATEST, nullptr, nullptr, nullptr, nullptr, 0.2f, 1.0f);
   char* base = reinterpret_cast<char*>(t->arena);
   t->sc = reinterpret_cast<FlowScalars*>(base);
   t->n_live = reinterpret_cast<int*>(base + 128);
@@ -455,60 +364,13 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
 void flow_trainer_destroy(FlowTrainer* t) {
   if (!t) return;
   if (t->arena) cudaFree(t->arena);
-  if (t->conf_priv) cudaFree(t->conf_priv);
+  trainer_conf_destroy(&t->conf);
   delete t;
 }
 
-int flow_trainer_set_confidence(FlowTrainer* t, int method, float* var, double* running_n, double* running_sum,
-                                double* running_sumsq, float kf_proc_cov, float kf_meas_cov) {
-  WVN_REQUIRE(t, "flow trainer: null handle");
-  WVN_REQUIRE(method >= CONF_LATEST && method <= CONF_MOVING_AVERAGE, "flow trainer: confidence method %d (0 "
-              "latest_measurement, 1 running_mean, 2 kalman_filter, 3 moving_average)", method);
-  ConfState& c = t->conf;
-  c.method = method;
-  c.running_n = running_n ? running_n : t->conf_priv;
-  c.running_sum = running_sum ? running_sum : t->conf_priv + 1;
-  c.running_sumsq = running_sumsq ? running_sumsq : t->conf_priv + 2;
-  c.var = var ? var : reinterpret_cast<float*>(t->conf_priv + 3);
-  c.kf_proc_cov = kf_proc_cov;
-  c.kf_meas_cov = kf_meas_cov;
-  c.ring = t->conf_priv + 4;
-  return WVN_OK;
-}
-
-int flow_trainer_copy_confidence(FlowTrainer* dst, const FlowTrainer* src, cudaStream_t stream) {
-  WVN_REQUIRE(dst && src, "flow trainer: null handle");
-  WVN_CHECK_CUDA(cudaMemcpyAsync(dst->conf_priv, src->conf_priv, sizeof(double) * 32, cudaMemcpyDeviceToDevice, stream));
-  return WVN_OK;
-}
+TrainerConf* flow_trainer_conf(FlowTrainer* t) { return &t->conf; }
 
 namespace {
-
-GemmProblem problem(const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs,
-                    float* c, long long ldc, int M, int N, int K, int live) {
-  GemmProblem p;
-  memset(&p, 0, sizeof(p));
-  p.a = a; p.a_rs = a_rs; p.a_cs = a_cs;
-  p.b = b; p.b_rs = b_rs; p.b_cs = b_cs;
-  p.c = c; p.ldc = ldc;
-  p.M = M; p.N = N; p.K = K; p.live = live;
-  return p;
-}
-
-int launch_gemms(const GemmProblem* ps, int count, const int* n_live, cudaStream_t stream) {
-  GemmBatch g;
-  memset(&g, 0, sizeof(g));
-  int gx = 1, gy = 1;
-  for (int i = 0; i < count; ++i) {
-    g.p[i] = ps[i];
-    gx = std::max(gx, (ps[i].N + GT - 1) / GT);
-    gy = std::max(gy, (ps[i].M + GT - 1) / GT);
-  }
-  g.n_live = n_live;
-  flow_gemm_kernel<<<dim3(gx, gy, count), 256, 0, stream>>>(g);
-  WVN_CHECK_LAUNCH("flow_gemm_kernel");
-  return WVN_OK;
-}
 
 // compaction + both couplings' forward; the last coupling writes z / logprob / log_det / nll / trav as given
 int flow_forward(FlowTrainer* t, const float* params, const FlowBuffers& b, const float* x, int rows,
@@ -524,21 +386,21 @@ int flow_forward(FlowTrainer* t, const float* params, const FlowBuffers& b, cons
     GemmProblem ps[2];
     for (int k = 0; k < 2; ++k) {
       const NetOffsets o = net_offsets(t->s, c, k);
-      ps[k] = problem(t->mu[c], D, 1, params + o.w0, 1, D, t->s1[c][k], h, rows, h, D, 1);
+      ps[k] = gemm_problem(t->mu[c], D, 1, params + o.w0, 1, D, t->s1[c][k], h, rows, h, D, 1);
       ps[k].bias = params + o.b0;
-      ps[k].relu = 1;
+      ps[k].act = F32_RELU;
     }
     WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
     for (int k = 0; k < 2; ++k) {
       const NetOffsets o = net_offsets(t->s, c, k);
-      ps[k] = problem(t->s1[c][k], h, 1, params + o.w2, 1, h, t->s2[c][k], h, rows, h, h, 1);
+      ps[k] = gemm_problem(t->s1[c][k], h, 1, params + o.w2, 1, h, t->s2[c][k], h, rows, h, h, 1);
       ps[k].bias = params + o.b2;
-      ps[k].relu = 1;
+      ps[k].act = F32_RELU;
     }
     WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
     for (int k = 0; k < 2; ++k) {
       const NetOffsets o = net_offsets(t->s, c, k);
-      ps[k] = problem(t->s2[c][k], h, 1, params + o.w4, 1, h, t->so[c][k], D, rows, D, h, 1);
+      ps[k] = gemm_problem(t->s2[c][k], h, 1, params + o.w4, 1, h, t->so[c][k], D, rows, D, h, 1);
       ps[k].bias = params + o.b4;
     }
     WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
@@ -593,10 +455,10 @@ int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_av
   if (phase_mask & 1) {
     WVN_PROPAGATE(flow_forward(t, params, b, x, rows, y_valid, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f,
                                stream));
-    flow_stats_kernel<<<1, kStatThreads, 0, stream>>>(t->nll, t->n_live, t->conf, t->std_factor, cg_mean, cg_std, metrics,
+    flow_stats_kernel<<<1, kStatThreads, 0, stream>>>(t->nll, t->n_live, t->conf.cs, t->std_factor, cg_mean, cg_std, metrics,
                                                       t->sc);
     WVN_CHECK_LAUNCH("flow_stats_kernel");
-    flow_conf_rows_kernel<<<(R + 255) / 256, 256, 0, stream>>>(t->nll, t->n_live, t->conf.method, t->sc, conf_out);
+    flow_conf_rows_kernel<<<(R + 255) / 256, 256, 0, stream>>>(t->nll, t->n_live, t->conf.cs.method, t->sc, conf_out);
     WVN_CHECK_LAUNCH("flow_conf_rows_kernel");
   }
   if (phase_mask & 2) {
@@ -611,20 +473,20 @@ int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_av
       GemmProblem ps[2];
       for (int k = 0; k < 2; ++k) {   // d2 = (dso W4) * (s2 > 0)
         const NetOffsets o = net_offsets(t->s, c, k);
-        ps[k] = problem(t->dso[k], D, 1, params + o.w4, h, 1, t->d2[k], h, R, h, D, 1);
+        ps[k] = gemm_problem(t->dso[k], D, 1, params + o.w4, h, 1, t->d2[k], h, R, h, D, 1);
         ps[k].ref = t->s2[c][k]; ps[k].ld_ref = h;
       }
       WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
       for (int k = 0; k < 2; ++k) {   // d1 = (d2 W2) * (s1 > 0)
         const NetOffsets o = net_offsets(t->s, c, k);
-        ps[k] = problem(t->d2[k], h, 1, params + o.w2, h, 1, t->d1[k], h, R, h, h, 1);
+        ps[k] = gemm_problem(t->d2[k], h, 1, params + o.w2, h, 1, t->d1[k], h, R, h, h, 1);
         ps[k].ref = t->s1[c][k]; ps[k].ld_ref = h;
       }
       WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
       if (c == 1) {
         for (int k = 0; k < 2; ++k) {   // dmu = d1 W0
           const NetOffsets o = net_offsets(t->s, c, k);
-          ps[k] = problem(t->d1[k], h, 1, params + o.w0, D, 1, t->dmu[k], D, R, D, h, 1);
+          ps[k] = gemm_problem(t->d1[k], h, 1, params + o.w0, D, 1, t->dmu[k], D, R, D, h, 1);
         }
         WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
         flow_coupling_bwd_post_kernel<<<R, kRowThreads, 0, stream>>>(D, t->n_live, t->dx, t->so[1][0], mask, t->dmu[0],
@@ -635,11 +497,11 @@ int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_av
       GemmProblem wg[6];
       for (int k = 0; k < 2; ++k) {
         const NetOffsets o = net_offsets(t->s, c, k);
-        wg[3 * k + 0] = problem(t->dso[k], 1, D, t->s2[c][k], h, 1, t->grads + o.w4, h, D, h, R, 2);
+        wg[3 * k + 0] = gemm_problem(t->dso[k], 1, D, t->s2[c][k], h, 1, t->grads + o.w4, h, D, h, R, 2);
         wg[3 * k + 0].db = t->grads + o.b4;
-        wg[3 * k + 1] = problem(t->d2[k], 1, h, t->s1[c][k], h, 1, t->grads + o.w2, h, h, h, R, 2);
+        wg[3 * k + 1] = gemm_problem(t->d2[k], 1, h, t->s1[c][k], h, 1, t->grads + o.w2, h, h, h, R, 2);
         wg[3 * k + 1].db = t->grads + o.b2;
-        wg[3 * k + 2] = problem(t->d1[k], 1, h, t->mu[c], D, 1, t->grads + o.w0, D, h, D, R, 2);
+        wg[3 * k + 2] = gemm_problem(t->d1[k], 1, h, t->mu[c], D, 1, t->grads + o.w0, D, h, D, R, 2);
         wg[3 * k + 2].db = t->grads + o.b0;
       }
       WVN_PROPAGATE(launch_gemms(wg, 6, t->n_live, stream));

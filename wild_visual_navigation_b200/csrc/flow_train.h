@@ -5,7 +5,7 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 
-#include "mlp_train.h"
+#include "train_core.h"
 
 namespace wvn {
 
@@ -40,9 +40,8 @@ struct FlowTrainer;
 int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, const AdamCfg& adam, float* grads_ext,
                         bool forward_only, FlowTrainer** out);
 void flow_trainer_destroy(FlowTrainer* t);
-int flow_trainer_set_confidence(FlowTrainer* t, int method, float* var, double* running_n, double* running_sum,
-                                double* running_sumsq, float kf_proc_cov, float kf_meas_cov);
-int flow_trainer_copy_confidence(FlowTrainer* dst, const FlowTrainer* src, cudaStream_t stream);
+// The trainer's ConfidenceGenerator (bound and copied with trainer_conf_bind / trainer_conf_copy).
+TrainerConf* flow_trainer_conf(FlowTrainer* t);
 
 // LinearRnvp.forward on rows x [rows, dim]: z / logprob [rows, dim], log_det [rows] (each may be NULL); with trav
 // non-NULL also ConfidenceGenerator.inference_without_update of the per-row NLL -(sum(logprob) + log_det) from the

@@ -16,103 +16,11 @@
 #include "common.cuh"
 #include "host_common.h"
 #include "mlp_train.h"
+#include "train_core.h"
 
 namespace wvn {
 
 namespace {
-
-constexpr int TS = 64;  // C tile
-constexpr int TK = 16;
-
-enum { SACT_NONE = 0, SACT_RELU = 1, SACT_SIGMOID_COL0 = 2 };
-
-struct SgemmArgs {
-  const float* A; long long sam, sak;   // A(m,k) = A[m*sam + k*sak]
-  const float* B; long long sbk, sbn;   // B(k,n) = B[k*sbk + n*sbn]
-  float* C; long long ldc;
-  int M, N, K;
-  const float* bias;                    // [N] or null
-  int act;
-  const float* relu_mask; long long ld_mask;  // multiply by (mask[m,n] > 0) or null
-  int k_per_split;                      // K range per blockIdx.z; > 0 and < K => atomic accumulate into C
-};
-
-__global__ void __launch_bounds__(256)
-sgemm_kernel(SgemmArgs a) {
-  __shared__ float As[TK][TS + 1];
-  __shared__ float Bs[TK][TS + 1];
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int m0 = blockIdx.y * TS, n0 = blockIdx.x * TS;
-  const int kbeg = blockIdx.z * a.k_per_split;
-  const int kend = min(a.K, kbeg + a.k_per_split);
-  float acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-
-  for (int k0 = kbeg; k0 < kend; k0 += TK) {
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      const int idx = threadIdx.x + 256 * r;  // 0..1023
-      int m, k;
-      if (a.sak == 1) { m = idx >> 4; k = idx & 15; } else { k = idx >> 6; m = idx & 63; }
-      const int gm = m0 + m, gk = k0 + k;
-      As[k][m] = (gm < a.M && gk < kend) ? a.A[gm * a.sam + gk * a.sak] : 0.f;
-      int n, kk;
-      if (a.sbk == 1) { n = idx >> 4; kk = idx & 15; } else { kk = idx >> 6; n = idx & 63; }
-      const int gn = n0 + n, gk2 = k0 + kk;
-      Bs[kk][n] = (gn < a.N && gk2 < kend) ? a.B[gk2 * a.sbk + gn * a.sbn] : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < TK; ++k) {
-      float av[4], bv[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) av[i] = As[k][ty + 16 * i];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) bv[j] = Bs[k][tx + 16 * j];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  const bool atomic = a.k_per_split < a.K;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int gm = m0 + ty + 16 * i;
-    if (gm >= a.M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int gn = n0 + tx + 16 * j;
-      if (gn >= a.N) continue;
-      float v = acc[i][j];
-      if (atomic) {
-        atomicAdd(&a.C[gm * a.ldc + gn], v);
-      } else {
-        if (a.bias) v += a.bias[gn];
-        if (a.act == SACT_RELU) v = fmaxf(v, 0.f);
-        if (a.act == SACT_SIGMOID_COL0 && gn == 0) v = 1.f / (1.f + expf(-v));
-        if (a.relu_mask) v = (a.relu_mask[gm * a.ld_mask + gn] > 0.f) ? v : 0.f;
-        a.C[gm * a.ldc + gn] = v;
-      }
-    }
-  }
-}
-
-int sgemm(const SgemmArgs& a, int splits, cudaStream_t s) {
-  SgemmArgs b = a;
-  if (splits < 1) splits = 1;
-  b.k_per_split = ((a.K + splits - 1) / splits + TK - 1) / TK * TK;
-  const int z = (a.K + b.k_per_split - 1) / b.k_per_split;
-  if (z <= 1) b.k_per_split = a.K;
-  dim3 grid((a.N + TS - 1) / TS, (a.M + TS - 1) / TS, z < 1 ? 1 : z);
-  sgemm_kernel<<<grid, 256, 0, s>>>(b);
-  WVN_CHECK_LAUNCH("sgemm_kernel");
-  return WVN_OK;
-}
 
 // ---- per-row loss terms + global statistics -------------------------------------------------
 // One warp per row: loss_reco_i = mean_d (out[i,1+d] - x[i,d])^2 ; raw_i = (out[i,0] - y_i)^2.
@@ -224,28 +132,6 @@ colsum_kernel(const float* __restrict__ a, long long lda, int rows, int cols, fl
   atomicAdd(&out[c], s);
 }
 
-__global__ void __launch_bounds__(256)
-adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-            long long n, AdamCfg cfg, const long long* __restrict__ step_ptr) {
-  // torch.optim.Adam (no amsgrad, no weight decay): step t counts from 1
-  const double t = static_cast<double>(*step_ptr);
-  const float bc1 = static_cast<float>(1.0 - pow(static_cast<double>(cfg.beta1), t));
-  const float bc2_sqrt = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(cfg.beta2), t)));
-  const float step_size = cfg.lr / bc1;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float gi = g[i];
-    const float mi = m[i] + (gi - m[i]) * (1.f - cfg.beta1);      // lerp form used by torch
-    const float vi = v[i] * cfg.beta2 + (1.f - cfg.beta2) * gi * gi;
-    m[i] = mi;
-    v[i] = vi;
-    const float denom = sqrtf(vi) / bc2_sqrt + cfg.eps;
-    p[i] -= step_size * (mi / denom);
-  }
-}
-
-__global__ void bump_step_kernel(long long* step) { *step += 1; }
-
 }  // namespace
 
 size_t mlp_param_count(const MlpShape& s) {
@@ -293,16 +179,15 @@ Ws carve(float* ws, const MlpShape& s, int max_rows) {
 int mlp_forward_f32(const MlpShape& s, const float* params, const float* x, int rows, float* h1, float* h2, float* out,
                     cudaStream_t stream) {
   const MlpOffsets o = mlp_offsets(s);
-  SgemmArgs g{};
-  g.A = x; g.sam = s.dim; g.sak = 1; g.B = params + o.w1; g.sbk = 1; g.sbn = s.dim; g.C = h1; g.ldc = s.h1;
-  g.M = rows; g.N = s.h1; g.K = s.dim; g.bias = params + o.b1; g.act = SACT_RELU; g.relu_mask = nullptr; g.ld_mask = 0;
-  WVN_PROPAGATE(sgemm(g, 1, stream));
-  g.A = h1; g.sam = s.h1; g.B = params + o.w2; g.sbn = s.h1; g.C = h2; g.ldc = s.h2; g.N = s.h2; g.K = s.h1;
-  g.bias = params + o.b2;
-  WVN_PROPAGATE(sgemm(g, 1, stream));
-  g.A = h2; g.sam = s.h2; g.B = params + o.w3; g.sbn = s.h2; g.C = out; g.ldc = s.dim + 1; g.N = s.dim + 1; g.K = s.h2;
-  g.bias = params + o.b3; g.act = SACT_SIGMOID_COL0;
-  WVN_PROPAGATE(sgemm(g, 1, stream));
+  GemmProblem g = gemm_problem(x, s.dim, 1, params + o.w1, 1, s.dim, h1, s.h1, rows, s.h1, s.dim);
+  g.bias = params + o.b1; g.act = F32_RELU_FMAX;
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream));
+  g = gemm_problem(h1, s.h1, 1, params + o.w2, 1, s.h1, h2, s.h2, rows, s.h2, s.h1);
+  g.bias = params + o.b2; g.act = F32_RELU_FMAX;
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream));
+  g = gemm_problem(h2, s.h2, 1, params + o.w3, 1, s.h2, out, s.dim + 1, rows, s.dim + 1, s.h2);
+  g.bias = params + o.b3; g.act = F32_SIGMOID_COL0;
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream));
   return WVN_OK;
 }
 
@@ -338,31 +223,27 @@ int mlp_train_backward(const MlpShape& s, const float* params, const float* x, c
 
   const int nout = s.dim + 1;
   const int splits = rows >= 512 ? 16 : (rows >= 128 ? 4 : 1);
-  SgemmArgs g{};
   // dW3[nout, h2] = dOut^T · H2
-  g.A = w.d_out; g.sam = 1; g.sak = nout; g.B = w.h2; g.sbk = s.h2; g.sbn = 1; g.C = grads + o.w3; g.ldc = s.h2;
-  g.M = nout; g.N = s.h2; g.K = rows; g.bias = nullptr; g.act = SACT_NONE; g.relu_mask = nullptr; g.ld_mask = 0;
-  WVN_PROPAGATE(sgemm(g, splits, stream));
+  GemmProblem g = gemm_problem(w.d_out, 1, nout, w.h2, s.h2, 1, grads + o.w3, s.h2, nout, s.h2, rows);
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream, splits));
   colsum_kernel<<<dim3((nout + 127) / 128, 16), 128, 0, stream>>>(w.d_out, nout, rows, nout, grads + o.b3);
   WVN_CHECK_LAUNCH("colsum_kernel");
   // dH2[rows, h2] = (dOut · W3) * (H2 > 0)
-  g.A = w.d_out; g.sam = nout; g.sak = 1; g.B = params + o.w3; g.sbk = s.h2; g.sbn = 1; g.C = w.d_h2; g.ldc = s.h2;
-  g.M = rows; g.N = s.h2; g.K = nout; g.relu_mask = w.h2; g.ld_mask = s.h2;
-  WVN_PROPAGATE(sgemm(g, 1, stream));
+  g = gemm_problem(w.d_out, nout, 1, params + o.w3, s.h2, 1, w.d_h2, s.h2, rows, s.h2, nout);
+  g.ref = w.h2; g.ld_ref = s.h2;
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream));
   // dW2[h2, h1] = dH2^T · H1
-  g.A = w.d_h2; g.sam = 1; g.sak = s.h2; g.B = w.h1; g.sbk = s.h1; g.sbn = 1; g.C = grads + o.w2; g.ldc = s.h1;
-  g.M = s.h2; g.N = s.h1; g.K = rows; g.relu_mask = nullptr; g.ld_mask = 0;
-  WVN_PROPAGATE(sgemm(g, splits, stream));
+  g = gemm_problem(w.d_h2, 1, s.h2, w.h1, s.h1, 1, grads + o.w2, s.h1, s.h2, s.h1, rows);
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream, splits));
   colsum_kernel<<<dim3((s.h2 + 127) / 128, 16), 128, 0, stream>>>(w.d_h2, s.h2, rows, s.h2, grads + o.b2);
   WVN_CHECK_LAUNCH("colsum_kernel");
   // dH1[rows, h1] = (dH2 · W2) * (H1 > 0)
-  g.A = w.d_h2; g.sam = s.h2; g.sak = 1; g.B = params + o.w2; g.sbk = s.h1; g.sbn = 1; g.C = w.d_h1; g.ldc = s.h1;
-  g.M = rows; g.N = s.h1; g.K = s.h2; g.relu_mask = w.h1; g.ld_mask = s.h1;
-  WVN_PROPAGATE(sgemm(g, 1, stream));
+  g = gemm_problem(w.d_h2, s.h2, 1, params + o.w2, s.h1, 1, w.d_h1, s.h1, rows, s.h1, s.h2);
+  g.ref = w.h1; g.ld_ref = s.h1;
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream));
   // dW1[h1, dim] = dH1^T · X
-  g.A = w.d_h1; g.sam = 1; g.sak = s.h1; g.B = x; g.sbk = s.dim; g.sbn = 1; g.C = grads + o.w1; g.ldc = s.dim;
-  g.M = s.h1; g.N = s.dim; g.K = rows; g.relu_mask = nullptr; g.ld_mask = 0;
-  WVN_PROPAGATE(sgemm(g, splits, stream));
+  g = gemm_problem(w.d_h1, 1, s.h1, x, s.dim, 1, grads + o.w1, s.dim, s.h1, s.dim, rows);
+  WVN_PROPAGATE(launch_gemms(&g, 1, nullptr, stream, splits));
   colsum_kernel<<<dim3((s.h1 + 127) / 128, 16), 128, 0, stream>>>(w.d_h1, s.h1, rows, s.h1, grads + o.b1);
   WVN_CHECK_LAUNCH("colsum_kernel");
   return WVN_OK;
@@ -372,17 +253,6 @@ int mlp_train_finalize(TrainScalars* scalars, const float* grads, long long n_pa
                        const LossCfg& cfg, cudaStream_t stream) {
   loss_finalize_kernel<<<1, 1, 0, stream>>>(scalars, grads + n_params, cfg, n_total);
   WVN_CHECK_LAUNCH("loss_finalize_kernel");
-  return WVN_OK;
-}
-
-int mlp_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
-                  const AdamCfg& cfg, long long* step_counter, cudaStream_t stream) {
-  bump_step_kernel<<<1, 1, 0, stream>>>(step_counter);
-  WVN_CHECK_LAUNCH("bump_step_kernel");
-  int blocks = static_cast<int>((n + 255) / 256);
-  if (blocks > sm_count() * 4) blocks = sm_count() * 4;
-  adam_kernel<<<blocks, 256, 0, stream>>>(params, grads, exp_avg, exp_avg_sq, n, cfg, step_counter);
-  WVN_CHECK_LAUNCH("adam_kernel");
   return WVN_OK;
 }
 

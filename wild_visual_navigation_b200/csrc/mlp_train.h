@@ -26,10 +26,6 @@ struct LossCfg {
   int anomaly_balanced = 1;
 };
 
-struct AdamCfg {
-  float lr = 1e-3f, beta1 = 0.9f, beta2 = 0.999f, eps = 1e-8f;
-};
-
 // Device-resident scalars of one step.  The five leading doubles are plain sums so a
 // data-parallel caller can all-reduce them in one call between the phases.
 struct TrainScalars {
@@ -58,10 +54,8 @@ int mlp_train_backward(const MlpShape& s, const float* params, const float* x, c
                        const unsigned char* y_valid, int rows, int max_rows, long long n_total, const LossCfg& cfg,
                        float* workspace, TrainScalars* scalars, float* cg_mean, float* cg_std, float* grads,
                        float* conf_out, cudaStream_t stream);
-// phase 3: loss metrics from the (possibly all-reduced) sums, then Adam.
+// phase 3: loss metrics from the (possibly all-reduced) sums; then Adam (mlp_adam_step, train_core.h).
 int mlp_train_finalize(TrainScalars* scalars, const float* grads, long long n_params, long long n_total,
                        const LossCfg& cfg, cudaStream_t stream);
-int mlp_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
-                  const AdamCfg& cfg, long long* step_counter, cudaStream_t stream);
 
 }  // namespace wvn

@@ -24,10 +24,10 @@
 #include <algorithm>
 
 #include "common.cuh"
-#include "conf_update.cuh"
 #include "host_common.h"
 #include "mlp_train.h"
 #include "mlp_train_fused.h"
+#include "train_core.cuh"
 
 namespace wvn {
 
@@ -243,7 +243,7 @@ train_fwd_rows_kernel(MlpShape s, MlpOffsets o, const float* __restrict__ params
 }
 
 // ------------------------------------------------------------------------------------------------ K1b
-// ConfidenceGenerator.update from the (all-reduced) sums of this step: one thread (conf_update.cuh).
+// ConfidenceGenerator.update from the (all-reduced) sums of this step: one thread (train_core.cuh).
 __global__ void train_conf_kernel(LossCfg cfg, ConfState cs, int dim, FusedScalars* __restrict__ sc,
                                   float* __restrict__ cg_mean, float* __restrict__ cg_std,
                                   long long* __restrict__ step_counter) {
@@ -513,21 +513,7 @@ train_apply_kernel(float* __restrict__ p, const float* __restrict__ g, float* __
     sc->x_max = 0.0;
     sc->sum_lr = sc->sum_lr2 = sc->sum_raw = sc->n_valid = sc->n_rows = sc->reserved = 0.0;
   }
-  // torch.optim.Adam (no amsgrad, no weight decay): step t counts from 1
-  const double t = static_cast<double>(*step_ptr);
-  const float bc1 = static_cast<float>(1.0 - pow(static_cast<double>(cfg.beta1), t));
-  const float bc2_sqrt = static_cast<float>(sqrt(1.0 - pow(static_cast<double>(cfg.beta2), t)));
-  const float step_size = cfg.lr / bc1;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float gi = g[i];
-    const float mi = m[i] + (gi - m[i]) * (1.f - cfg.beta1);      // lerp form used by torch
-    const float vi = v[i] * cfg.beta2 + (1.f - cfg.beta2) * gi * gi;
-    m[i] = mi;
-    v[i] = vi;
-    const float denom = sqrtf(vi) / bc2_sqrt + cfg.eps;
-    p[i] -= step_size * (mi / denom);
-  }
+  adam_update(p, g, m, v, n, cfg, step_ptr);
 }
 
 // ------------------------------------------------------------------------------------------------ NCCL (dlopen)
@@ -577,8 +563,7 @@ struct FusedTrainer {
   NcclComm comm = nullptr;
   int world = 1;
   size_t smem_fwd = 0, smem_bwd = 0;
-  ConfState conf;          // ConfidenceGenerator method + where its state lives
-  double* conf_priv = nullptr;   // [3 running | 1 var as float | ring 3 * kConfWindow + 1]: private state / the ring
+  TrainerConf conf;        // ConfidenceGenerator method + where its state lives
 };
 
 int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, void* scalars_ext,
@@ -604,15 +589,12 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
     memset(&init, 0, sizeof(init));
     init.x_min = INFINITY;
     cudaMemcpy(t->sc, &init, sizeof(init), cudaMemcpyHostToDevice);
-    if (cudaMalloc(&t->conf_priv, sizeof(double) * 32) != cudaSuccess) {
-      cudaFree(t->arena);
-      delete t;
-      return set_error(WVN_ERR_CUDA, "trainer: cudaMalloc of the confidence state failed");
-    }
-    cudaMemset(t->conf_priv, 0, sizeof(double) * 32);
-    const float one = 1.f;   // private var = 1 (the reference's initial value) unless the caller binds its own
-    cudaMemcpy(reinterpret_cast<float*>(t->conf_priv + 3), &one, sizeof(float), cudaMemcpyHostToDevice);
-    fused_trainer_set_confidence(t, CONF_LATEST, nullptr, nullptr, nullptr, nullptr, 0.2f, 1.0f);
+  }
+  const int rc = trainer_conf_create(&t->conf);
+  if (rc != WVN_OK) {
+    cudaFree(t->arena);
+    delete t;
+    return rc;
   }
   float* f = reinterpret_cast<float*>(reinterpret_cast<char*>(t->arena) + 256);
   t->h1 = f; f += R * s.h1;
@@ -628,8 +610,7 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
                                  s.h2 * TR + TR + TR);
   t->smem_bwd = sizeof(float) * (((n3 * TRP + 3) & ~size_t(3)) + s.h2 * TR + TR + 8);
   if (t->smem_fwd > 227 * 1024 || t->smem_bwd > 227 * 1024) {
-    cudaFree(t->arena);
-    delete t;
+    fused_trainer_destroy(t);
     return set_error(WVN_ERR_INVALID, "trainer: shared memory need exceeds 227 KB");
   }
   cudaFuncSetAttribute(train_fwd_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(t->smem_fwd));
@@ -642,33 +623,11 @@ void fused_trainer_destroy(FusedTrainer* t) {
   if (!t) return;
   if (t->comm && nccl().ok) nccl().CommDestroy(t->comm);
   if (t->arena) cudaFree(t->arena);
-  if (t->conf_priv) cudaFree(t->conf_priv);
+  trainer_conf_destroy(&t->conf);
   delete t;
 }
 
-int fused_trainer_set_confidence(FusedTrainer* t, int method, float* var, double* running_n, double* running_sum,
-                                 double* running_sumsq, float kf_proc_cov, float kf_meas_cov) {
-  WVN_REQUIRE(t, "trainer: null handle");
-  WVN_REQUIRE(method >= CONF_LATEST && method <= CONF_MOVING_AVERAGE, "trainer: confidence method %d (0 latest_measurement, "
-              "1 running_mean, 2 kalman_filter, 3 moving_average)", method);
-  ConfState& c = t->conf;
-  c.method = method;
-  c.running_n = running_n ? running_n : t->conf_priv;
-  c.running_sum = running_sum ? running_sum : t->conf_priv + 1;
-  c.running_sumsq = running_sumsq ? running_sumsq : t->conf_priv + 2;
-  c.var = var ? var : reinterpret_cast<float*>(t->conf_priv + 3);
-  c.kf_proc_cov = kf_proc_cov;
-  c.kf_meas_cov = kf_meas_cov;
-  c.ring = t->conf_priv + 4;
-  return WVN_OK;
-}
-
-int fused_trainer_copy_confidence(FusedTrainer* dst, const FusedTrainer* src, cudaStream_t stream) {
-  WVN_REQUIRE(dst && src, "trainer: null handle");
-  // ordered after src's last step on the caller's stream; destroying src afterwards (cudaFree) waits for the copy
-  WVN_CHECK_CUDA(cudaMemcpyAsync(dst->conf_priv, src->conf_priv, sizeof(double) * 32, cudaMemcpyDeviceToDevice, stream));
-  return WVN_OK;
-}
+TrainerConf* fused_trainer_conf(FusedTrainer* t) { return &t->conf; }
 
 int fused_comm_unique_id(void* id128) {
   WVN_REQUIRE(id128, "comm: null id buffer");
@@ -715,7 +674,7 @@ int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_
     if (t->comm) {
       const int rc = api.AllReduce(t->sc, t->sc, 6, kNcclFloat64, kNcclSum, t->comm, stream);
       if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclAllReduce(stats): %s", api.GetErrorString(rc));
-      if (t->conf.method == CONF_MOVING_AVERAGE) {
+      if (t->conf.cs.method == CONF_MOVING_AVERAGE) {
         int r2 = api.AllReduce(&t->sc->x_min, &t->sc->x_min, 1, kNcclFloat64, kNcclMin, t->comm, stream);
         if (r2 == 0) r2 = api.AllReduce(&t->sc->x_max, &t->sc->x_max, 1, kNcclFloat64, kNcclMax, t->comm, stream);
         if (r2 != 0) return set_error(WVN_ERR_CUDA, "ncclAllReduce(extrema): %s", api.GetErrorString(r2));
@@ -723,12 +682,12 @@ int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_
     }
   }
   if (phase_mask & 2) {
-    if (t->conf.method != CONF_LATEST) {   // generators with memory: one thread updates the state once
-      train_conf_kernel<<<1, 32, 0, stream>>>(t->loss, t->conf, s.dim, t->sc, cg_mean, cg_std, step_counter);
+    if (t->conf.cs.method != CONF_LATEST) {   // generators with memory: one thread updates the state once
+      train_conf_kernel<<<1, 32, 0, stream>>>(t->loss, t->conf.cs, s.dim, t->sc, cg_mean, cg_std, step_counter);
       WVN_CHECK_LAUNCH("train_conf_kernel");
     }
     train_bwd_rows_kernel<<<tiles, kThreads, t->smem_bwd, stream>>>(
-        s, t->o, t->loss, t->conf.method, params, x, y, y_valid, n_rows, groups, rpg, t->h1, t->h2, t->out, t->loss_reco,
+        s, t->o, t->loss, t->conf.cs.method, params, x, y, y_valid, n_rows, groups, rpg, t->h1, t->h2, t->out, t->loss_reco,
         t->raw, t->d_out, t->d_h2, t->d_h1, conf_out, t->sc, cg_mean, cg_std, t->grads + np, step_counter, t->grads, np);
     WVN_CHECK_LAUNCH("train_bwd_rows_kernel");
     WgradArgs w;

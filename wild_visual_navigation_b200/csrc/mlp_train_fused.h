@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include "mlp_train.h"
+#include "train_core.h"
 
 namespace wvn {
 
@@ -26,19 +27,6 @@ struct FusedScalars {
   float lo, hi, cmin, cmax, g_reco, g_trav;
 };
 
-// ConfidenceGenerator methods (utils/confidence_generator.py:49-76)
-enum ConfMethod : int { CONF_LATEST = 0, CONF_RUNNING_MEAN = 1, CONF_KALMAN = 2, CONF_MOVING_AVERAGE = 3 };
-constexpr int kConfWindow = 5;   // moving_average's deque(maxlen=5)
-
-// State the reference keeps in the ConfidenceGenerator module, updated in place on the device.
-struct ConfState {
-  int method = CONF_LATEST;
-  float* var = nullptr;                                        // (1,1) fp32 parameter
-  double *running_n = nullptr, *running_sum = nullptr, *running_sumsq = nullptr;   // (1,) fp64 parameters
-  float kf_proc_cov = 0.2f, kf_meas_cov = 1.0f;                // the 1-D Kalman filter's Q and R (F = H = 1)
-  double* ring = nullptr;                                      // trainer-owned: [kConfWindow][3] (n, sum, sum^2) + count
-};
-
 struct FusedTrainer;
 
 // scalars_ext (sizeof(FusedScalars) bytes) / grads_ext (n_params + 1 floats): caller-owned device buffers, or NULL to
@@ -48,12 +36,8 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
 void fused_trainer_destroy(FusedTrainer* t);
 int fused_comm_unique_id(void* id128);
 int fused_trainer_init_comm(FusedTrainer* t, const void* id128, int rank, int world);
-// method: ConfMethod; pointers may be null for methods that do not use them (the trainer then keeps private state).
-int fused_trainer_set_confidence(FusedTrainer* t, int method, float* var, double* running_n, double* running_sum,
-                                 double* running_sumsq, float kf_proc_cov, float kf_meas_cov);
-// Copies src's private confidence state (moving_average's window; var / running sums not bound to caller buffers) into
-// dst, on `stream`: a caller that replaces a trainer by a larger one keeps the generator where it was.
-int fused_trainer_copy_confidence(FusedTrainer* dst, const FusedTrainer* src, cudaStream_t stream);
+// The trainer's ConfidenceGenerator (bound and copied with trainer_conf_bind / trainer_conf_copy).
+TrainerConf* fused_trainer_conf(FusedTrainer* t);
 // phase_mask: 1 = forward + statistics (+ their all-reduce), 2 = backward + weight gradients (+ gradient all-reduce),
 // 4 = loss metrics + Adam; 7 = the whole step.
 int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,

@@ -1,0 +1,74 @@
+// wvn-b200: the fp32 training core shared by the MLP trainers (mlp_train.cu, mlp_train_fused.cu) and the LinearRnvp
+// trainer (flow_train.cu): the ConfidenceGenerator state a trainer keeps, Adam, and the batched fp32 tile GEMM.
+#pragma once
+
+#include <cuda_runtime.h>
+
+namespace wvn {
+
+struct AdamCfg {
+  float lr = 1e-3f, beta1 = 0.9f, beta2 = 0.999f, eps = 1e-8f;
+};
+
+// torch.optim.Adam's update (no amsgrad, no weight decay): bumps *step_counter, then one update of n parameters.
+int mlp_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n,
+                  const AdamCfg& cfg, long long* step_counter, cudaStream_t stream);
+
+// ConfidenceGenerator methods (utils/confidence_generator.py:49-76)
+enum ConfMethod : int { CONF_LATEST = 0, CONF_RUNNING_MEAN = 1, CONF_KALMAN = 2, CONF_MOVING_AVERAGE = 3 };
+constexpr int kConfWindow = 5;   // moving_average's deque(maxlen=5)
+
+// State the reference keeps in the ConfidenceGenerator module, updated in place on the device.
+struct ConfState {
+  int method = CONF_LATEST;
+  float* var = nullptr;                                        // (1,1) fp32 parameter
+  double *running_n = nullptr, *running_sum = nullptr, *running_sumsq = nullptr;   // (1,) fp64 parameters
+  float kf_proc_cov = 0.2f, kf_meas_cov = 1.0f;                // the 1-D Kalman filter's Q and R (F = H = 1)
+  double* ring = nullptr;                                      // trainer-owned: [kConfWindow][3] (n, sum, sum^2) + count
+};
+
+// A trainer's generator: where its state lives (cs, passed to the kernels) and the device block holding what no caller
+// buffer holds: moving_average's window, and var / the running sums when the caller binds none (var starts at 1, the
+// reference's initial value).
+struct TrainerConf {
+  ConfState cs;
+  double* priv = nullptr;
+};
+int trainer_conf_create(TrainerConf* c);   // allocates the block and binds latest_measurement to it
+void trainer_conf_destroy(TrainerConf* c);
+// method: ConfMethod; pointers may be null for methods that do not use them (the private block then holds that state).
+int trainer_conf_bind(TrainerConf* c, int method, float* var, double* running_n, double* running_sum,
+                      double* running_sumsq, float kf_proc_cov, float kf_meas_cov);
+// Copies src's private block into dst's, on `stream`: a caller that replaces a trainer by a larger one keeps the
+// generator where it was.  Ordered after src's last step; destroying src afterwards (cudaFree) waits for the copy.
+int trainer_conf_copy(TrainerConf* dst, const TrainerConf* src, cudaStream_t stream);
+
+// ---- batched fp32 GEMM: 64 x 64 tiles, K step 16, 4 x 4 outputs per thread, CUDA cores
+// C(m, n) = epilogue(sum_k A(m, k) B(k, n)) with A(m, k) = a[m a_rs + k a_cs], B(k, n) = b[k b_rs + n b_cs]: the same
+// kernel does X W^T (forward), dY W (data gradients) and dY^T X (weight gradients).  live = 1: M is capped by *n_live,
+// live = 2: K is.  Epilogue: + bias[n], then act, then * (ref(m, n) > 0) (ReLU's backward).  db (weight-gradient
+// problems): db[m] = sum_k A(m, k), the bias gradient.
+enum GemmF32Act : int {
+  F32_LINEAR = 0,
+  F32_RELU = 1,          // v < 0 ? 0 : v: NaN passes, like torch.relu
+  F32_RELU_FMAX = 2,     // fmaxf(v, 0): NaN becomes 0
+  F32_SIGMOID_COL0 = 3,  // column 0 through the sigmoid (SimpleMLP's traversability output)
+};
+struct GemmProblem {
+  const float* a; long long a_rs, a_cs;
+  const float* b; long long b_rs, b_cs;
+  float* c; long long ldc;
+  const float* bias;
+  const float* ref; long long ld_ref;
+  float* db;
+  int M, N, K, act, live;
+};
+constexpr int kMaxGemmProblems = 12;
+
+GemmProblem gemm_problem(const float* a, long long a_rs, long long a_cs, const float* b, long long b_rs, long long b_cs,
+                         float* c, long long ldc, int M, int N, int K, int live = 0);
+// One launch for `count` problems.  splits > 1 (one problem, no live bound, no epilogue, no db): K is cut into up to
+// `splits` ranges of a multiple of 16 whose partial products are added into C with fp32 atomics (C zeroed by the caller).
+int launch_gemms(const GemmProblem* ps, int count, const int* n_live, cudaStream_t stream, int splits = 1);
+
+}  // namespace wvn

@@ -515,7 +515,50 @@ def mlp_forward_f32(flat_params, x, dim, h1, h2):
     return out
 
 
-class MlpTrainer:
+class _TrainerHandle:
+    """Owns a library trainer handle with workspaces for ``max_rows`` rows and replaces it by a larger one when a call
+    needs more.  Remembers the ConfidenceGenerator binding, so the replacement keeps the generator where it was.
+    Subclasses name their ABI functions and make the handle in ``_new_handle``."""
+
+    _DESTROY = _SET_CONFIDENCE = _COPY_CONFIDENCE = None
+
+    def _create(self, max_rows):
+        h = self._new_handle(int(max_rows))
+        if self._h is not None:
+            # both handles' workspaces are alive until the old one is destroyed: peak memory briefly doubles here.
+            # The confidence state the old handle kept itself (moving_average's window, var and running sums not bound
+            # to caller tensors) moves over, so the generator does not restart
+            check(getattr(lib(), self._COPY_CONFIDENCE)(h, self._h, stream()))
+            getattr(lib(), self._DESTROY)(self._h)
+        self._h = h
+        self.max_rows = int(max_rows)
+        if self._conf is not None:
+            self.set_confidence(*self._conf)
+
+    def _reserve(self, rows):
+        if rows > self.max_rows:
+            self._create(int(rows * 1.5))
+
+    def set_confidence(self, method=0, var=None, running_n=None, running_sum=None, running_sum_of_squares=None,
+                       kf_proc_cov=0.2, kf_meas_cov=1.0):
+        """ConfidenceGenerator method of the step (0 latest_measurement, 1 running_mean, 2 kalman_filter, 3
+        moving_average) and the device tensors holding its state (updated in place by the step; None = private)."""
+        self._conf = (int(method), var, running_n, running_sum, running_sum_of_squares, float(kf_proc_cov), float(kf_meas_cov))
+        if self._h is not None:
+            check(getattr(lib(), self._SET_CONFIDENCE)(self._h, int(method), ptr(var), ptr(running_n), ptr(running_sum),
+                                                       ptr(running_sum_of_squares), float(kf_proc_cov),
+                                                       float(kf_meas_cov)))
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                getattr(lib(), self._DESTROY)(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+class MlpTrainer(_TrainerHandle):
     """Fused online train step on a flat fp32 parameter buffer (csrc/mlp_train_fused.cu): four kernels, no host
     synchronisation, rows may arrive padded per frame (``step_padded``) exactly as the segment pooling leaves them.
 
@@ -554,20 +597,18 @@ class MlpTrainer:
         self._create(max_rows)
 
     # ---- fused path ---------------------------------------------------------------------------
-    def _create(self, max_rows):
+    _DESTROY = "wvn_mlp_trainer_destroy"
+    _SET_CONFIDENCE = "wvn_mlp_trainer_set_confidence"
+    _COPY_CONFIDENCE = "wvn_mlp_trainer_copy_confidence"
+
+    def _new_handle(self, max_rows):
         h = c_void_p()
-        check(lib().wvn_mlp_trainer_create(self.dim, self.h1, self.h2, int(max_rows), byref(self.cfg), ptr(self.scalars),
+        check(lib().wvn_mlp_trainer_create(self.dim, self.h1, self.h2, max_rows, byref(self.cfg), ptr(self.scalars),
                                            ptr(self.grads), byref(h)))
-        if self._h is not None:
-            # both handles' workspaces are alive until the old one is destroyed: peak memory briefly doubles here.
-            # A larger trainer replaces this one: the confidence state it keeps itself (moving_average's window, var and
-            # running sums not bound to caller tensors) moves over, so the generator does not restart
-            check(lib().wvn_mlp_trainer_copy_confidence(h, self._h, stream()))
-            lib().wvn_mlp_trainer_destroy(self._h)
-        self._h = h
-        self.max_rows = int(max_rows)
-        if self._conf is not None:
-            self.set_confidence(*self._conf)
+        return h
+
+    def _create(self, max_rows):
+        super()._create(max_rows)
         self.conf = torch.empty(self.max_rows + 32, device=self.params.device, dtype=torch.float32)
         self._lib_comm = False
         if self.pg is not None:
@@ -585,19 +626,12 @@ class MlpTrainer:
                 check(lib().wvn_mlp_trainer_init_comm(self._h, raw, rank, world))
                 self._lib_comm = True
 
-    def set_confidence(self, method=0, var=None, running_n=None, running_sum=None, running_sum_of_squares=None,
-                       kf_proc_cov=0.2, kf_meas_cov=1.0):
-        """ConfidenceGenerator method of the step (0 latest_measurement, 1 running_mean, 2 kalman_filter, 3
-        moving_average) and the device tensors holding its state (updated in place by the step; None = private)."""
+    def set_confidence(self, method=0, *args, **kwargs):
         assert not self.legacy or method == 0, "the round-1 kernels implement latest_measurement only"
-        self._conf = (int(method), var, running_n, running_sum, running_sum_of_squares, float(kf_proc_cov), float(kf_meas_cov))
-        if self._h is not None:
-            check(lib().wvn_mlp_trainer_set_confidence(self._h, int(method), ptr(var), ptr(running_n), ptr(running_sum),
-                                                       ptr(running_sum_of_squares), float(kf_proc_cov), float(kf_meas_cov)))
+        super().set_confidence(method, *args, **kwargs)
 
     def _run(self, x, groups, rpg, n_rows, y, yv):
-        if groups * rpg > self.max_rows:
-            self._create(int(groups * rpg * 1.5))
+        self._reserve(groups * rpg)
         x = x.contiguous()
         y = y.contiguous().float()
         yv = yv.contiguous().to(torch.uint8)
@@ -679,14 +713,6 @@ class MlpTrainer:
         check(lib().wvn_mlp_train_read_metrics(ptr(self.scalars), ptr(self.metrics), s))
         return self.conf[:R]
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                lib().wvn_mlp_trainer_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
 
 # --------------------------------------------------------------------------------------------
 # LinearRnvp flow (anomaly-detection learner): fp32 row forward and online train step
@@ -699,48 +725,6 @@ def flow_buffers(model):
     assert f[0].mask.dtype == torch.float32 and f[1].p.dtype == torch.int64
     return FlowBuffers(f[0].mask.data_ptr(), f[2].mask.data_ptr(), f[1].p.data_ptr(), f[1].invp.data_ptr(),
                        f[3].p.data_ptr(), f[3].invp.data_ptr())
-
-
-class _FlowHandle:
-    """Owns a ``wvn_flow_t`` (workspaces for ``max_rows`` rows); grows it when a call needs more rows."""
-
-    def __init__(self, dim, hidden, max_rows, cfg, grads=None):
-        _C.require_device()
-        self.dim, self.hidden, self.cfg, self._grads = dim, hidden, cfg, grads
-        self.n_params = lib().wvn_flow_param_count(dim, hidden)
-        self._h = None
-        self._conf = None
-        self._create(max_rows)
-
-    def _create(self, max_rows):
-        h = c_void_p()
-        check(lib().wvn_flow_create(self.dim, self.hidden, int(max_rows), byref(self.cfg), ptr(self._grads), byref(h)))
-        if self._h is not None:
-            # the larger handle takes over the generator state the old one kept itself (moving_average's window, ...)
-            check(lib().wvn_flow_copy_confidence(h, self._h, stream()))
-            lib().wvn_flow_destroy(self._h)
-        self._h = h
-        self.max_rows = int(max_rows)
-        if self._conf is not None:
-            self.set_confidence(*self._conf)
-
-    def _reserve(self, rows):
-        if rows > self.max_rows:
-            self._create(int(rows * 1.5))
-
-    def set_confidence(self, method=0, var=None, running_n=None, running_sum=None, running_sum_of_squares=None,
-                       kf_proc_cov=0.2, kf_meas_cov=1.0):
-        self._conf = (int(method), var, running_n, running_sum, running_sum_of_squares, float(kf_proc_cov), float(kf_meas_cov))
-        check(lib().wvn_flow_set_confidence(self._h, int(method), ptr(var), ptr(running_n), ptr(running_sum),
-                                            ptr(running_sum_of_squares), float(kf_proc_cov), float(kf_meas_cov)))
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                lib().wvn_flow_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
 
 class FlowInference:
@@ -819,33 +803,44 @@ class FlowInference:
             pass
 
 
-class FlowTrainer(_FlowHandle):
+class FlowTrainer(_TrainerHandle):
     """The anomaly-detection train step on a LinearRnvp's flat fp32 parameters (csrc/flow_train.cu): forward, loss
     ``-mean(logprob.sum(1) + log_det)`` over the labelled rows, ConfidenceGenerator update with the per-row NLL,
     backward and Adam as one fixed launch sequence without host synchronisation.  ``exp_avg`` / ``exp_avg_sq`` /
     ``step_counter`` are torch.optim.Adam's state over the 24 parameter tensors, flattened in ``parameters()`` order."""
 
+    _DESTROY = "wvn_flow_destroy"
+    _SET_CONFIDENCE = "wvn_flow_set_confidence"
+    _COPY_CONFIDENCE = "wvn_flow_copy_confidence"
+
     def __init__(self, model, max_rows=4096, std_factor=0.5, lr=1e-3, betas=(0.9, 0.999), eps=1e-8):
+        _C.require_device()
         params = model.flat_params
         assert params.is_cuda and params.dtype == torch.float32
         dev = params.device
         self.model = model
-        grads = torch.zeros(lib().wvn_flow_param_count(model.input_size, model.hidden), device=dev)
-        super().__init__(model.input_size, model.hidden, max_rows,
-                         TrainConfig(0.0, 0.0, float(std_factor), 0, float(lr), betas[0], betas[1], float(eps)), grads)
-        self.grads = grads
+        self.dim, self.hidden = model.input_size, model.hidden
+        self.cfg = TrainConfig(0.0, 0.0, float(std_factor), 0, float(lr), betas[0], betas[1], float(eps))
+        self.n_params = lib().wvn_flow_param_count(self.dim, self.hidden)
+        self.grads = torch.zeros(self.n_params, device=dev)
         self.exp_avg = torch.zeros(self.n_params, device=dev)
         self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
         self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
         self.metrics = torch.zeros(6, device=dev)
         self.cg_mean = torch.zeros(1, device=dev)
         self.cg_std = torch.ones(1, device=dev)
-        self.conf = torch.empty(self.max_rows, device=dev)
+        self._h = None
+        self._conf = None
+        self._create(max_rows)
+
+    def _new_handle(self, max_rows):
+        h = c_void_p()
+        check(lib().wvn_flow_create(self.dim, self.hidden, max_rows, byref(self.cfg), ptr(self.grads), byref(h)))
+        return h
 
     def _create(self, max_rows):
         super()._create(max_rows)
-        if hasattr(self, "conf"):
-            self.conf = torch.empty(self.max_rows, device=self.conf.device)
+        self.conf = torch.empty(self.max_rows, device=self.grads.device)
 
     def step(self, x, y_valid=None, phase_mask=7):
         """x (R, D) fp32; y_valid (R,) bool or None (every row).  Returns the confidence of the labelled rows in

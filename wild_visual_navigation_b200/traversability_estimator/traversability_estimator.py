@@ -130,8 +130,6 @@ class TraversabilityEstimator:
         self._trainer = ops.MlpTrainer(m.flat_params, m.input_size, m.hidden[0], m.hidden[1], max_rows=max_rows,
                                        w_trav=lp["w_trav"], w_reco=lp["w_reco"], std_factor=cg.std_factor,
                                        anomaly_balanced=lp["anomaly_balanced"], lr=self._lr, process_group=process_group)
-        # the train step writes the ConfidenceGenerator's mean / std straight into the module's parameters
-        self._trainer.cg_mean, self._trainer.cg_std = cg.mean.data, cg.std.data
         self._bind_confidence_state()
 
     def _bind_confidence_state(self):
