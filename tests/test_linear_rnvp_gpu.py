@@ -21,8 +21,8 @@ U = 2.0**-24
 METHODS = ("latest_measurement", "running_mean", "moving_average", "kalman_filter")
 
 
-def _model(dim, hidden, mask="odds", seed=42, spread=0.05):
-    """A LinearRnvp on the GPU whose t nets differ from the s nets (as after training)."""
+def _model(dim, hidden, mask="odds", seed=42, spread=0.05, device="cuda"):
+    """A LinearRnvp (on the GPU by default) whose t nets differ from the s nets (as after training)."""
     from wild_visual_navigation_b200 import LinearRnvp
 
     torch.manual_seed(seed)
@@ -32,7 +32,7 @@ def _model(dim, hidden, mask="odds", seed=42, spread=0.05):
         for n, p in m.named_parameters():
             if ".t." in n:
                 p.add_(torch.randn(p.shape, generator=g) * spread)
-    return m.cuda()
+    return m.to(device)
 
 
 def _sd64(m):
@@ -330,11 +330,22 @@ class _Grid:
         self.grid = g
 
 
+# size: a square frame from a g = size / 8 grid through TraversabilityInference, or a name in _PIXEL_GEOMETRY: a
+# (gh, gw) grid to an (H, W) output through ops.FlowInference with its own pixel chunk
+_PIXEL_GEOMETRY = {
+    "grid28x42-224x336": (28, 42, 224, 336, 0),        # non-square grid and output: a swapped gh / gw or sy / sx shows
+    "grid1x7-16x56": (1, 7, 16, 56, 0),                # degenerate grid: one token row, sy = 0
+    "grid5x7-37x53-chunk384": (5, 7, 37, 53, 384),     # 1961 pixels a frame: chunks of 384 straddle the frames
+}
+
+
 @pytest.mark.parametrize("size,dim,batch", [(224, 384, 1), (224, 384, 3), (448, 384, 1), (448, 384, 3), (224, 90, 3),
-                                            (448, 90, 1)])
+                                            (448, 90, 1), ("grid28x42-224x336", 384, 1), ("grid1x7-16x56", 90, 2),
+                                            ("grid5x7-37x53-chunk384", 384, 3)])
 def test_pixel_map_matches_float64(size, dim, batch):
-    """Per-pixel maps from a (B, g*g, D) token grid (DINO ViT-S/8 tokens: D = 384; the STEGO code: D = 90), pixel by
-    pixel against float64.
+    """Per-pixel maps from a (B, gh*gw, D) token grid (DINO ViT-S/8 tokens: D = 384; the STEGO code: D = 90), pixel by
+    pixel against float64, for square frames and for the non-square, degenerate and chunk-straddling geometries of
+    _PIXEL_GEOMETRY.
 
     Bound.  The path rounds to bf16 at fixed points: every weight, mu = u * mask and the two hidden activations of each
     net; everything else is fp32.  ``oracle.linear_rnvp.nll_bf16`` applies exactly these roundings in float64, so
@@ -344,29 +355,46 @@ def test_pixel_map_matches_float64(size, dim, batch):
     typical e.  An element passes when |nll_gpu - nll64| <= 3 e + 6 rms_frame(e) + 64 u (1 + |nll64|).  The factors
     are not derived: with 3 rms_frame(e) the worst of 602k pixels (448^2, B = 3, D = 384) measured 1.11 times the bound
     on an H100, so the flip term was doubled.  The same bound
-    must reject the first permutation dropped and the map shifted by one pixel.  (Dropping the last permutation cannot
-    show: sum(z^2) does not depend on it.  Swapping s and t of these nets, which differ by 0.05-sized weight noise, moves
-    the NLL by less than the bf16 resolution; the fp32 row test holds the swap.)"""
+    must reject the first permutation dropped, the map shifted by one pixel and, for a non-square grid, the tokens read
+    as a (gw, gh) grid.  (Dropping the last permutation cannot show: sum(z^2) does not depend on it.  Swapping s and t
+    of these nets, which differ by 0.05-sized weight noise, moves the NLL by less than the bf16 resolution; the fp32 row
+    test holds the swap.)"""
     import torch.nn.functional as F
 
-    from wild_visual_navigation_b200 import ConfidenceGenerator, TraversabilityInference
+    from wild_visual_navigation_b200 import ConfidenceGenerator, TraversabilityInference, ops
 
-    g = size // 8
+    if isinstance(size, int):
+        gh = gw = size // 8
+        H = W = size
+        seed = size + dim + batch
+    else:
+        gh, gw, H, W, chunk = _PIXEL_GEOMETRY[size]
+        seed = H + W + dim + batch
     m = _model(dim, 200)
-    gen = torch.Generator().manual_seed(size + dim + batch)
-    tokens = (torch.randn(batch, g * g, dim, generator=gen) * 0.5).cuda()
+    gen = torch.Generator().manual_seed(seed)
+    tokens = (torch.randn(batch, gh * gw, dim, generator=gen) * 0.5).cuda()
     sd = {k: (v.detach().double() if v.is_floating_point() else v) for k, v in m.state_dict().items()}
-    dense = F.interpolate(tokens.double().view(batch, g, g, dim).permute(0, 3, 1, 2), (size, size), mode="bilinear",
-                          align_corners=True).permute(0, 2, 3, 1).reshape(-1, dim)
-    ref = orn.nll(sd, dense).view(batch, size, size)
-    emu = orn.nll_bf16(sd, dense).view(batch, size, size)
+
+    def upsampled(rows, cols):
+        return F.interpolate(tokens.double().view(batch, rows, cols, dim).permute(0, 3, 1, 2), (H, W), mode="bilinear",
+                             align_corners=True).permute(0, 2, 3, 1).reshape(-1, dim)
+
+    dense = upsampled(gh, gw)
+    ref = orn.nll(sd, dense).view(batch, H, W)
+    emu = orn.nll_bf16(sd, dense).view(batch, H, W)
     cg = ConfidenceGenerator(0.5, "latest_measurement").cuda()
     with torch.no_grad():
         cg.mean[0], cg.std[0] = ref.mean().item() - 0.5 * ref.std().item(), ref.std().item()
-    ti = TraversabilityInference(_Grid(g), m, cg)
-    trav, conf = ti.predict_from_tokens(tokens, size)
-    assert conf is None and trav.shape == (batch, size, size)
-    _, nll = ti._flow_infer.pixels(m, tokens, (g, g), (size, size), cg.mean.data, cg.std.data, 0.5, want_nll=True)
+    if isinstance(size, int):
+        ti = TraversabilityInference(_Grid(gh), m, cg)
+        trav, conf = ti.predict_from_tokens(tokens, size)
+        assert conf is None and trav.shape == (batch, H, W)
+        _, nll = ti._flow_infer.pixels(m, tokens, (gh, gw), (H, W), cg.mean.data, cg.std.data, 0.5, want_nll=True)
+    else:
+        fi = ops.FlowInference(dim, 200, chunk_pixels=chunk)
+        fi.set_params(m.flat_params)
+        trav, nll = fi.pixels(m, tokens, (gh, gw), (H, W), cg.mean.data, cg.std.data, 0.5, want_nll=True)
+        assert trav.shape == (batch, H, W)
     e = (emu - ref).abs()
     bound = 3 * e + 6 * e.pow(2).mean().sqrt() + 64 * U * (1 + ref.abs())
     err = (nll.double() - ref).abs()
@@ -376,8 +404,11 @@ def test_pixel_map_matches_float64(size, dim, batch):
     # negative controls under the same bound
     noperm = dict(sd)
     noperm["flows.1.p"] = torch.arange(dim, device="cuda")
-    assert not bool(((nll.double() - orn.nll(noperm, dense).view(batch, size, size)).abs() <= bound).all())
+    assert not bool(((nll.double() - orn.nll(noperm, dense).view(batch, H, W)).abs() <= bound).all())
     assert not bool(((nll.double() - torch.roll(ref, 1, 2)).abs() <= bound).all())
+    if gh != gw:   # the tokens read as a (gw, gh) grid: what a kernel with gh and gw swapped computes
+        swapped = orn.nll(sd, upsampled(gw, gh)).view(batch, H, W)
+        assert not bool(((nll.double() - swapped).abs() <= bound).all())
 
 
 def test_pixel_map_follows_refresh_and_loaded_permutation():

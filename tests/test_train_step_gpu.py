@@ -107,10 +107,11 @@ def _t(v, like):
     return torch.as_tensor(v, dtype=torch.float64, device=like.device)
 
 
-def check(got, ref, bound, tag, b0=None):
+def check(got, ref, bound, tag, b0=None, c=C_TRAIN):
     """NaN in exactly the same places, every other element within its bound (edges.assert_within records the ratio).
-    b0: the same bound at c = 0.  The bound is affine in c to first order, so (|err| - b0) / (bound - b0) * C_TRAIN is
-    the smallest c that covers the element: its maximum is recorded as the c this check needs."""
+    b0: the same bound at c = 0, bound itself being taken at c.  The bound is affine in c to first order, so
+    (|err| - b0) / (bound - b0) * c is the smallest c that covers the element: its maximum is recorded as the c this
+    check needs."""
     got, ref = torch.as_tensor(got).double(), torch.as_tensor(ref).double()
     bound = torch.as_tensor(bound, dtype=torch.float64, device=ref.device).expand_as(ref)
     got = got.to(ref.device)
@@ -128,7 +129,7 @@ def check(got, ref, bound, tag, b0=None):
     if b0 is not None and bool(ok.any()):
         b0 = torch.as_tensor(b0, dtype=torch.float64, device=ref.device).expand_as(ref)[ok]
         err, span = (got[ok] - ref[ok]).abs(), (bound[ok] - b0).clamp_min(1e-300)
-        need = ((err - b0).clamp_min(0) / span) * C_TRAIN
+        need = ((err - b0).clamp_min(0) / span) * c
         i = int(need.argmax())
         if need[i].item() > _NEED.get(tag, (0.0, ""))[0]:
             _NEED[tag] = (need[i].item(), f"{_CTX[0]} element {i}")
@@ -229,13 +230,14 @@ def generator_ref(method, st, before, window, f):
     elif method == "running_mean":
         rn0, rs0, rq0 = before["running"]
         rn, rs, rq = rn0 + n, rs0 + s1, rq0 + s2
-        with np.errstate(all="ignore"):
+        with np.errstate(all="ignore"):   # rn = 0 (no labelled row yet): NaN, as 0 / 0 in the kernel
             m = float(np.float64(rs) / rn)
             var = float(np.float64(rq) / rn - m * m)
-        em = e1 / rn + U * abs(m)
-        evar = (e2 + 2 * abs(m) * e1) / rn + 3 * U * m * m + U * abs(var) + 2.0 ** -50 * rq / rn
-        sd = math.sqrt(var) if var >= 0 else float("nan")
-        esd = evar / (2 * sd) + U * sd
+            em = float(e1 / np.float64(rn)) + U * abs(m)
+            evar = float((e2 + 2 * abs(m) * e1) / np.float64(rn) + 3 * U * m * m + U * abs(var)
+                         + 2.0 ** -50 * rq / np.float64(rn))
+            sd = math.sqrt(var) if var >= 0 else float("nan")
+            esd = float(evar / (2 * np.float64(sd))) + U * sd
         out.update(var=(var, evar), running_n=(rn, 0.0), running_sum=(rs, e1 + 2.0 ** -50 * abs(rs)),
                    running_sumsq=(rq, e2 + 2.0 ** -50 * rq))
         out["lo"], out["hi"] = _lohi(m, em, sd, esd, f)

@@ -186,6 +186,9 @@ int launch_gemms(const GemmProblem* ps, int count, const int* n_live, cudaStream
   int gx = 1, gy = 1, kmax = 0;
   bool db = false;
   for (int i = 0; i < count; ++i) {
+    // split-K adds raw partial sums with atomics: an epilogue would be dropped and a db column sum overwritten
+    WVN_REQUIRE(splits <= 1 || (!ps[i].bias && ps[i].act == F32_LINEAR && !ps[i].ref && !ps[i].db),
+                "gemm: split-K (%d splits) with a bias, activation, ReLU mask or bias gradient (problem %d)", splits, i);
     g.p[i] = ps[i];
     gx = std::max(gx, (ps[i].N + GT - 1) / GT);
     gy = std::max(gy, (ps[i].M + GT - 1) / GT);
