@@ -367,6 +367,14 @@ int wvn_mlp_infer_pixels_vit(wvn_mlp_infer_t* h, wvn_vit_t* vit, int batch, int 
 /* Same arithmetic on explicit rows x: [rows, dim] fp32 (segment-wise prediction mode). */
 int wvn_mlp_infer_rows(wvn_mlp_infer_t* h, const float* x, long long rows, const float* cg_mean,
                        const float* cg_std, float std_factor, float* trav, float* conf, void* stream);
+/* The same handle for a DoubleMLP(dim, [h1, h2, 1]) (bounds of wvn_double_mlp_trainer_create): set_params takes its
+ * flat parameters (networks.0.{0,2,4}.{weight,bias}, then networks.1's) and packs the two nets as one block-structured
+ * MLP of widths 2 h1 / 2 h2 — layer 1 [W1_0; W1_1], layer 2 diag(W2_0, W2_1), layer 3 [w3_0 | 0] for traversability and
+ * [0 | W3_1] for the reconstruction — so pixels / rows compute sigmoid(net0(x)), the reconstruction error of net1(x)
+ * and its confidence with the GEMM chain above.  For h1 in {64, 128} and h2 = 32, pixels and pixels_vit take the fused
+ * per-pixel head at its geometries (per-token GEMM columns G_0 | G_1 | U | cT, layer 2 as one wgmma chain per network);
+ * other shapes and geometries take the unfused path, and pixels_vit then fails. */
+int wvn_mlp_infer_create_double(int dim, int h1, int h2, int chunk_rows, wvn_mlp_infer_t** out);
 
 /* ------------------------------------------------------------------------------------------
  * Online train step (fp32) — replaces the body of TraversabilityEstimator.train()
@@ -441,6 +449,41 @@ int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, floa
                        const float* x, int groups, int rows_per_group, const int* n_rows, const float* y,
                        const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
                        float* metrics_out, int phase_mask, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * DoubleMLP learner (model/simple_mlp.py DoubleMLP, fp32): DoubleMLP(dim, [h1, h2, 1]) — networks.0 Linear(dim, h1)
+ * ReLU Linear(h1, h2) ReLU Linear(h2, 1) through a sigmoid (traversability), networks.1 the same ending in
+ * Linear(h2, dim) (reconstruction); output [rows, 1 + dim] = [sigmoid(net0(x)) | net1(x)], SimpleMLP's layout.
+ * Bounds: 1 <= dim <= 1024, 4 <= h1 <= 256 and a multiple of 4, 1 <= h2 <= 32.  params / exp_avg / exp_avg_sq: flat
+ * fp32 buffers of wvn_double_mlp_param_count floats in parameters() order (networks.0.{0,2,4}.{weight,bias}, then
+ * networks.1's), i.e. torch.optim.Adam's state.  The trainer owns the workspaces for max_rows rows.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct wvn_double_mlp_trainer wvn_double_mlp_trainer_t;
+size_t wvn_double_mlp_param_count(int dim, int h1, int h2);
+/* DoubleMLP.forward on x [rows, dim] fp32: a1_buf [2, rows, h1], a2_buf [2, rows, h2] (net 0, then net 1) receive the
+ * hidden activations, out [rows, 1 + dim] the output. */
+int wvn_double_mlp_forward_f32(int dim, int h1, int h2, const float* params, const float* x, int rows, float* a1_buf,
+                               float* a2_buf, float* out, void* stream);
+/* cfg: the loss weights, anomaly_balanced, the generator's std_factor and Adam's lr / betas / eps; grads: optional
+ * caller-owned device buffer of wvn_double_mlp_param_count floats (NULL: the trainer allocates it). */
+int wvn_double_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_train_config* cfg, float* grads,
+                                  wvn_double_mlp_trainer_t** out);
+void wvn_double_mlp_trainer_destroy(wvn_double_mlp_trainer_t* t);
+/* The ConfidenceGenerator method and state of the train step, as wvn_mlp_trainer_set_confidence. */
+int wvn_double_mlp_trainer_set_confidence(wvn_double_mlp_trainer_t* t, int method, float* var, double* running_n,
+                                          double* running_sum, double* running_sum_of_squares, float kf_proc_cov,
+                                          float kf_meas_cov);
+/* As wvn_mlp_trainer_copy_confidence: a larger trainer takes over the generator state src keeps itself. */
+int wvn_double_mlp_trainer_copy_confidence(wvn_double_mlp_trainer_t* dst, const wvn_double_mlp_trainer_t* src,
+                                           void* stream);
+/* One step of TraversabilityEstimator.train() with TraversabilityLoss on x [rows, dim] fp32, y [rows] fp32, y_valid
+ * [rows] uint8 (0 < rows <= max_rows): forward, loss, the ConfidenceGenerator update, backward, Adam; one fixed
+ * sequence of launches, no host synchronisation, bit-reproducible.  confidence_out [rows]; metrics_out (device,
+ * 6 floats, may be NULL): loss_total, loss_trav, loss_reco, loss_trav_confidence, cg_mean, cg_std. */
+int wvn_double_mlp_train_step(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                              long long* step_counter, const float* x, int rows, const float* y,
+                              const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
+                              float* metrics_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * LinearRnvp anomaly-detection learner (model/linear_rnvp.py, fp32): LinearRnvp(dim, [hidden]) with flow_n = 2,

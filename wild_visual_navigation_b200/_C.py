@@ -111,6 +111,7 @@ SIGNATURES = {
     "wvn_mlp_infer_pixels": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P]),
     "wvn_mlp_infer_pixels_vit": (_I, [_P, _P, _I, _I, _I, _P, _P, _F, _P, _P, _P]),
     "wvn_mlp_infer_rows": (_I, [_P, _P, _L, _P, _P, _F, _P, _P, _P]),
+    "wvn_mlp_infer_create_double": (_I, [_I, _I, _I, _I, POINTER(_P)]),
     "wvn_mlp_param_count": (_S, [_I, _I, _I]),
     "wvn_mlp_train_workspace_bytes": (_S, [_I, _I, _I, _I]),
     "wvn_mlp_train_scalars_bytes": (_S, []),
@@ -127,6 +128,13 @@ SIGNATURES = {
     "wvn_mlp_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
     "wvn_mlp_trainer_copy_confidence": (_I, [_P, _P, _P]),
     "wvn_mlp_train_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "wvn_double_mlp_param_count": (_S, [_I, _I, _I]),
+    "wvn_double_mlp_forward_f32": (_I, [_I, _I, _I, _P, _P, _I, _P, _P, _P, _P]),
+    "wvn_double_mlp_trainer_create": (_I, [_I, _I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
+    "wvn_double_mlp_trainer_destroy": (None, [_P]),
+    "wvn_double_mlp_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
+    "wvn_double_mlp_trainer_copy_confidence": (_I, [_P, _P, _P]),
+    "wvn_double_mlp_train_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P]),
     "wvn_flow_param_count": (_S, [_I, _I]),
     "wvn_flow_create": (_I, [_I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
     "wvn_flow_destroy": (None, [_P]),

@@ -11,6 +11,7 @@
 #include "../../include/wvn_b200.h"
 #include "attention.h"
 #include "dense_kernels.h"
+#include "double_mlp_train.h"
 #include "gemm.h"
 #include "host_common.h"
 #include "mlp_train.h"
@@ -119,7 +120,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 104; }
+int wvn_version(void) { return 105; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -890,7 +891,13 @@ struct wvn_mlp_infer {
   // fused per-pixel head (pixel_head.cu): per-token GEMM operands + workspaces for kFusedFrames frames
   DevBuf wcat, bias_cat, head_consts, tok_bf16, gu, gram;
   int fused_tokens = 0;           // token rows the fused workspaces are sized for (grown on demand)
+  int head_n = 0;                 // columns of the per-token GEMM (G | U | cT); 0: no fused head for this handle
   int force_unfused = 0;          // debugging / A-B knob ($WVN_PIXEL_HEAD=unfused)
+  // DoubleMLP layout (wvn_mlp_infer_create_double): the two nets packed as one block-structured SimpleMLP with
+  // h1 = 2 net_h1, h2 = 2 net_h2; the unfused GEMM chain and its EPI_MLP_HEAD epilogue run it unchanged, and for
+  // net_h1 in {64, 128}, net_h2 = 32 the fused head's DoubleMLP instantiation (pixel_head_double) takes the fused
+  // geometries
+  int double_layout = 0, net_h1 = 0, net_h2 = 0;
   bool loaded = false;
 };
 
@@ -942,6 +949,49 @@ __global__ void pack_mlp_kernel(const float* __restrict__ p, MlpOffsets o, int d
   }
 }
 
+// The DoubleMLP's flat parameters as the block-structured SimpleMLP the GEMM chain runs (h1 = 2 h, h2 = 2 k for nets of
+// widths h / k): W1 = [W1_0; W1_1], W2 = diag(W2_0, W2_1), layer 3's reconstruction rows [0 | W3_1] first and its
+// traversability row [w3_0 | 0] at trav_col; the biases stacked the same way.  Padding is zero.
+__global__ void pack_double_mlp_kernel(const float* __restrict__ p, DoubleOffsets o, int dim, int h, int k, int dim_p,
+                                       int h1_p, int h2_p, int n3_p, int trav_col, __nv_bfloat16* w1, float* b1,
+                                       __nv_bfloat16* w2, float* b2, __nv_bfloat16* w3, float* b3) {
+  const long long n1 = static_cast<long long>(h1_p) * dim_p, n2 = static_cast<long long>(h2_p) * h1_p,
+                  n3 = static_cast<long long>(n3_p) * h2_p;
+  const long long total = n1 + n2 + n3 + h1_p + h2_p + n3_p;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    long long j = i;
+    float v = 0.f;
+    if (j < n1) {
+      const int r = static_cast<int>(j / dim_p), c = static_cast<int>(j % dim_p), net = r < h ? 0 : 1;
+      if (r < 2 * h && c < dim) v = p[o.w1[net] + static_cast<long long>(r - net * h) * dim + c];
+      w1[j] = __float2bfloat16_rn(v);
+      continue;
+    }
+    j -= n1;
+    if (j < n2) {
+      const int r = static_cast<int>(j / h1_p), c = static_cast<int>(j % h1_p), net = r < k ? 0 : 1;
+      if (r < 2 * k && c >= net * h && c < (net + 1) * h) v = p[o.w2[net] + static_cast<long long>(r - net * k) * h + c - net * h];
+      w2[j] = __float2bfloat16_rn(v);
+      continue;
+    }
+    j -= n2;
+    if (j < n3) {
+      const int r = static_cast<int>(j / h2_p), c = static_cast<int>(j % h2_p);
+      if (r < dim && c >= k && c < 2 * k) v = p[o.w3[1] + static_cast<long long>(r) * k + c - k];
+      else if (r == trav_col && c < k) v = p[o.w3[0] + c];
+      w3[j] = __float2bfloat16_rn(v);
+      continue;
+    }
+    j -= n3;
+    if (j < h1_p) { b1[j] = j < 2 * h ? p[(j < h ? o.b1[0] : o.b1[1] - h) + j] : 0.f; continue; }
+    j -= h1_p;
+    if (j < h2_p) { b2[j] = j < 2 * k ? p[(j < k ? o.b2[0] : o.b2[1] - k) + j] : 0.f; continue; }
+    j -= h2_p;
+    b3[j] = j < dim ? p[o.b3[1] + j] : (j == trav_col ? p[o.b3[0]] : 0.f);
+  }
+}
+
 int mlp_infer_chunk(wvn_mlp_infer* h, long long rows, long long row0, const float* cg_mean, const float* cg_std,
                     float std_factor, float* trav, float* conf, cudaStream_t s) {
   GemmArgs g1;
@@ -965,10 +1015,15 @@ int mlp_infer_chunk(wvn_mlp_infer* h, long long rows, long long row0, const floa
 
 extern "C" {
 
-int wvn_mlp_infer_create(int dim, int h1, int h2, int chunk_rows, wvn_mlp_infer_t** out) {
+static int mlp_infer_create(int dim, int h1, int h2, int chunk_rows, int double_layout, wvn_mlp_infer_t** out) {
   WVN_REQUIRE(out && dim > 0 && h1 > 0 && h2 > 0, "wvn_mlp_infer_create: bad arguments");
   WVN_PROPAGATE(wvn_check_device());
   wvn_mlp_infer* h = new wvn_mlp_infer();
+  h->double_layout = double_layout;
+  if (double_layout) {
+    h->net_h1 = h1; h->net_h2 = h2;
+    h1 *= 2; h2 *= 2;
+  }
   h->dim = dim; h->h1 = h1; h->h2 = h2;
   h->dim_p = round_up(dim, 64); h->h1_p = round_up(h1, 64); h->h2_p = round_up(h2, 64);
   h->trav_col = round_up(dim, 32);
@@ -992,9 +1047,15 @@ int wvn_mlp_infer_create(int dim, int h1, int h2, int chunk_rows, wvn_mlp_infer_
   alloc(h->x, static_cast<size_t>(h->chunk_rows) * h->dim_p * 2);
   alloc(h->a1, static_cast<size_t>(h->chunk_rows) * h->h1_p * 2);
   alloc(h->a2, static_cast<size_t>(h->chunk_rows) * h->h2_p * 2);
-  alloc(h->wcat, static_cast<size_t>(kPixelHeadN) * h->dim_p * 2);
-  alloc(h->bias_cat, static_cast<size_t>(kPixelHeadN) * 4);
-  alloc(h->head_consts, sizeof(PixelHeadConsts));
+  if (!double_layout)
+    h->head_n = kPixelHeadN;
+  else if (pixel_head_double_shape(h->net_h1, h->net_h2))
+    h->head_n = pixel_head_columns(2 * h->net_h1);
+  if (h->head_n > 0) {
+    alloc(h->wcat, static_cast<size_t>(h->head_n) * h->dim_p * 2);
+    alloc(h->bias_cat, static_cast<size_t>(h->head_n) * 4);
+    alloc(h->head_consts, sizeof(PixelHeadConsts));
+  }
   {
     const char* e = getenv("WVN_PIXEL_HEAD");
     h->force_unfused = (e && std::string(e) == "unfused") ? 1 : 0;
@@ -1005,6 +1066,17 @@ int wvn_mlp_infer_create(int dim, int h1, int h2, int chunk_rows, wvn_mlp_infer_
   }
   *out = h;
   return WVN_OK;
+}
+
+int wvn_mlp_infer_create(int dim, int h1, int h2, int chunk_rows, wvn_mlp_infer_t** out) {
+  return mlp_infer_create(dim, h1, h2, chunk_rows, 0, out);
+}
+
+int wvn_mlp_infer_create_double(int dim, int h1, int h2, int chunk_rows, wvn_mlp_infer_t** out) {
+  MlpShape s;
+  s.dim = dim; s.h1 = h1; s.h2 = h2;
+  WVN_PROPAGATE(double_mlp_check_shape(s, "wvn_mlp_infer_create_double"));
+  return mlp_infer_create(dim, h1, h2, chunk_rows, 1, out);
 }
 
 void wvn_mlp_infer_destroy(wvn_mlp_infer_t* h) {
@@ -1018,10 +1090,10 @@ void wvn_mlp_infer_destroy(wvn_mlp_infer_t* h) {
 int wvn_mlp_infer_reserve(wvn_mlp_infer_t* h, int tokens_per_frame) {
   WVN_REQUIRE(h && tokens_per_frame > 0, "wvn_mlp_infer_reserve: bad arguments");
   const int P = tokens_per_frame;
-  if (h->fused_tokens >= kFusedFrames * P) return WVN_OK;
+  if (h->head_n == 0 || h->fused_tokens >= kFusedFrames * P) return WVN_OK;   // no fused head: nothing to size
   for (DevBuf* b : {&h->tok_bf16, &h->gu, &h->gram}) b->release();
   WVN_PROPAGATE(h->tok_bf16.alloc(static_cast<size_t>(kFusedFrames) * P * h->dim_p * 2));
-  WVN_PROPAGATE(h->gu.alloc(static_cast<size_t>(kFusedFrames) * P * kPixelHeadN * 4));
+  WVN_PROPAGATE(h->gu.alloc(static_cast<size_t>(kFusedFrames) * P * h->head_n * 4));
   WVN_PROPAGATE(h->gram.alloc(static_cast<size_t>(kFusedFrames) * P * 5 * 4));
   h->fused_tokens = kFusedFrames * P;
   return WVN_OK;
@@ -1031,6 +1103,21 @@ int wvn_mlp_infer_set_params(wvn_mlp_infer_t* h, const float* params, void* stre
   WVN_REQUIRE(h && params, "wvn_mlp_infer_set_params: null argument");
   MlpShape sh;
   sh.dim = h->dim; sh.h1 = h->h1; sh.h2 = h->h2;
+  if (h->double_layout) {
+    MlpShape net;
+    net.dim = h->dim; net.h1 = h->net_h1; net.h2 = h->net_h2;
+    pack_double_mlp_kernel<<<256, 256, 0, S(stream)>>>(
+        params, double_mlp_offsets(net), h->dim, net.h1, net.h2, h->dim_p, h->h1_p, h->h2_p, h->n3_p, h->trav_col,
+        reinterpret_cast<__nv_bfloat16*>(h->w1.p), reinterpret_cast<float*>(h->b1.p),
+        reinterpret_cast<__nv_bfloat16*>(h->w2.p), reinterpret_cast<float*>(h->b2.p),
+        reinterpret_cast<__nv_bfloat16*>(h->w3.p), reinterpret_cast<float*>(h->b3.p));
+    WVN_CHECK_LAUNCH("pack_double_mlp_kernel");
+    if (h->head_n > 0)
+      WVN_PROPAGATE(pixel_head_pack_double(params, net, h->dim_p, h->wcat.p, reinterpret_cast<float*>(h->bias_cat.p),
+                                           reinterpret_cast<PixelHeadConsts*>(h->head_consts.p), S(stream)));
+    h->loaded = true;
+    return WVN_OK;
+  }
   pack_mlp_kernel<<<256, 256, 0, S(stream)>>>(
       params, mlp_offsets(sh), h->dim, h->h1, h->h2, h->dim_p, h->h1_p, h->h2_p, h->n3_p, h->trav_col,
       reinterpret_cast<__nv_bfloat16*>(h->w1.p), reinterpret_cast<float*>(h->b1.p),
@@ -1044,6 +1131,12 @@ int wvn_mlp_infer_set_params(wvn_mlp_infer_t* h, const float* params, void* stre
   return WVN_OK;
 }
 
+// Token-window width of the fused head for this handle and geometry, 0 when the fused head does not take it.
+static int fused_window(const wvn_mlp_infer_t* h, int gh, int gw, int out_h, int out_w) {
+  if (h->double_layout) return h->head_n > 0 ? pixel_head_supported_double(h->net_h1, h->net_h2, gh, gw, out_h, out_w) : 0;
+  return pixel_head_supported(h->h1, h->h2, gh, gw, out_h, out_w);
+}
+
 // Fused per-pixel head over frames [b0, b0 + nb): per-token GEMM (G | U | cT) + token Gram + one pixel kernel.
 // tok_bf16: the frames' bf16 tokens, frame_rows rows per frame with the patch tokens starting at row row0.
 static int pixels_fused_chunk(wvn_mlp_infer_t* h, const void* tok_bf16, long long frame_rows, int row0, int b0, int nb,
@@ -1051,12 +1144,12 @@ static int pixels_fused_chunk(wvn_mlp_infer_t* h, const void* tok_bf16, long lon
                               float std_factor, float* trav, float* conf, cudaStream_t s) {
   const long long rows = static_cast<long long>(nb) * frame_rows;
   GemmArgs g;
-  g.M = static_cast<int>(rows); g.N = kPixelHeadN; g.K = h->dim_p; g.epi = EPI_F32;
-  g.bias = reinterpret_cast<float*>(h->bias_cat.p); g.out = h->gu.p; g.ldo = kPixelHeadN;
+  g.M = static_cast<int>(rows); g.N = h->head_n; g.K = h->dim_p; g.epi = EPI_F32;
+  g.bias = reinterpret_cast<float*>(h->bias_cat.p); g.out = h->gu.p; g.ldo = h->head_n;
   WVN_PROPAGATE(gemm_bf16(g, tok_bf16, h->dim_p, h->wcat.p, 64, s));
   WVN_PROPAGATE(token_gram(tok_bf16, reinterpret_cast<float*>(h->gram.p), nb, gh, gw, h->dim_p, frame_rows, row0, s));
   PixelHeadArgs a;
-  a.gu = reinterpret_cast<float*>(h->gu.p); a.ldg = kPixelHeadN; a.gram = reinterpret_cast<float*>(h->gram.p);
+  a.gu = reinterpret_cast<float*>(h->gu.p); a.ldg = h->head_n; a.gram = reinterpret_cast<float*>(h->gram.p);
   a.consts = reinterpret_cast<PixelHeadConsts*>(h->head_consts.p);
   a.cg_mean = cg_mean; a.cg_std = cg_std; a.std_factor = std_factor;
   a.trav = trav + static_cast<long long>(b0) * out_h * out_w;
@@ -1066,7 +1159,8 @@ static int pixels_fused_chunk(wvn_mlp_infer_t* h, const void* tok_bf16, long lon
   a.sx = static_cast<float>(gw - 1) / static_cast<float>(out_w - 1);
   a.ww = ww; a.feat = h->dim;
   a.frame_rows = frame_rows; a.row0 = row0;
-  WVN_PROPAGATE(pixel_head(a, h->w2.p, h->h1_p, s));
+  if (h->double_layout) WVN_PROPAGATE(pixel_head_double(a, h->net_h1, h->w2.p, h->h1_p, s));
+  else WVN_PROPAGATE(pixel_head(a, h->w2.p, h->h1_p, s));
   return WVN_OK;
 }
 
@@ -1080,7 +1174,7 @@ int wvn_mlp_infer_pixels_vit(wvn_mlp_infer_t* h, wvn_vit_t* vit, int batch, int 
   WVN_REQUIRE(h->dim == vit->cfg.dim && h->dim_p == vit->cfg.dim, "wvn_mlp_infer_pixels_vit: the MLP takes %d-d features, "
               "the backbone's tokens are %d-d", h->dim, vit->cfg.dim);
   const int g = vit->grid;
-  const int ww = pixel_head_supported(h->h1, h->h2, g, g, out_h, out_w);
+  const int ww = fused_window(h, g, g, out_h, out_w);
   WVN_REQUIRE(ww > 0, "wvn_mlp_infer_pixels_vit: geometry outside the fused per-pixel head (use wvn_mlp_infer_pixels)");
   if (h->fused_tokens < kFusedFrames * vit->npad) WVN_PROPAGATE(wvn_mlp_infer_reserve(h, vit->npad));
   for (int b0 = 0; b0 < batch; b0 += kFusedFrames) {
@@ -1100,7 +1194,7 @@ int wvn_mlp_infer_pixels(wvn_mlp_infer_t* h, const float* tokens, int batch, int
   if (!h->loaded) return set_error(WVN_ERR_STATE, "wvn_mlp_infer_pixels: parameters were never set");
   cudaStream_t s = S(stream);
   // any feature width works (the 90-d STEGO code is zero-padded to 128 columns in the bf16 operands)
-  const int ww = h->force_unfused ? 0 : pixel_head_supported(h->h1, h->h2, gh, gw, out_h, out_w);
+  const int ww = h->force_unfused ? 0 : fused_window(h, gh, gw, out_h, out_w);
   if (ww > 0) {
     // ---- fused path: per-token GEMM (G | U | cT) + token Gram, then one kernel per chunk of frames
     const int P = gh * gw;
@@ -1272,6 +1366,67 @@ int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, floa
   WVN_REQUIRE(t, "wvn_mlp_train_step: null trainer");
   return fused_train_step(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows, y, y_valid,
                           cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
+}
+
+}  // extern "C"
+
+// ============================================================================================
+// DoubleMLP learner: fp32 row forward and online train step (double_mlp_train.cu)
+// ============================================================================================
+struct wvn_double_mlp_trainer {
+  DoubleTrainer* impl = nullptr;
+};
+
+extern "C" {
+
+size_t wvn_double_mlp_param_count(int dim, int h1, int h2) { return double_mlp_param_count(shape_of(dim, h1, h2)); }
+
+int wvn_double_mlp_forward_f32(int dim, int h1, int h2, const float* params, const float* x, int rows, float* a1_buf,
+                               float* a2_buf, float* out, void* stream) {
+  return double_mlp_forward_f32(shape_of(dim, h1, h2), params, x, rows, a1_buf, a2_buf, out, S(stream));
+}
+
+int wvn_double_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_train_config* cfg, float* grads,
+                                  wvn_double_mlp_trainer_t** out) {
+  WVN_REQUIRE(cfg && out, "wvn_double_mlp_trainer_create: null argument");
+  WVN_PROPAGATE(wvn_check_device());
+  AdamCfg a;
+  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
+  DoubleTrainer* impl = nullptr;
+  WVN_PROPAGATE(double_trainer_create(shape_of(dim, h1, h2), max_rows, loss_of(cfg), a, grads, &impl));
+  wvn_double_mlp_trainer* t = new wvn_double_mlp_trainer();
+  t->impl = impl;
+  *out = t;
+  return WVN_OK;
+}
+
+void wvn_double_mlp_trainer_destroy(wvn_double_mlp_trainer_t* t) {
+  if (!t) return;
+  double_trainer_destroy(t->impl);
+  delete t;
+}
+
+int wvn_double_mlp_trainer_set_confidence(wvn_double_mlp_trainer_t* t, int method, float* var, double* running_n,
+                                          double* running_sum, double* running_sum_of_squares, float kf_proc_cov,
+                                          float kf_meas_cov) {
+  WVN_REQUIRE(t, "wvn_double_mlp_trainer_set_confidence: null trainer");
+  return trainer_conf_bind(double_trainer_conf(t->impl), method, var, running_n, running_sum, running_sum_of_squares,
+                           kf_proc_cov, kf_meas_cov);
+}
+
+int wvn_double_mlp_trainer_copy_confidence(wvn_double_mlp_trainer_t* dst, const wvn_double_mlp_trainer_t* src,
+                                           void* stream) {
+  WVN_REQUIRE(dst && src, "wvn_double_mlp_trainer_copy_confidence: null trainer");
+  return trainer_conf_copy(double_trainer_conf(dst->impl), double_trainer_conf(src->impl), S(stream));
+}
+
+int wvn_double_mlp_train_step(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                              long long* step_counter, const float* x, int rows, const float* y,
+                              const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
+                              float* metrics_out, void* stream) {
+  WVN_REQUIRE(t, "wvn_double_mlp_train_step: null trainer");
+  return double_train_step(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, rows, y, y_valid, cg_mean, cg_std,
+                           confidence_out, metrics_out, S(stream));
 }
 
 }  // extern "C"

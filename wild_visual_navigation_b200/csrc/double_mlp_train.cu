@@ -1,0 +1,351 @@
+// wvn-b200: the DoubleMLP learner (model/simple_mlp.py DoubleMLP) in fp32 — the row forward and the online train step,
+// the body of TraversabilityEstimator.train() (traversability_estimator.py:464-477) with TraversabilityLoss
+// (utils/loss.py:93-160) on a DoubleMLP.
+//
+// Two networks read the same rows: net 0 (dim -> h1 -> h2 -> 1, sigmoid) gives traversability, net 1 (dim -> h1 -> h2
+// -> dim) the reconstruction; out = [sigmoid(net0(x)) | net1(x)] has SimpleMLP's (rows, 1 + dim) layout, so the loss,
+// its gradient and the confidence are SimpleMLP's.  The step is one fixed sequence of 12 launches with every scalar on
+// the device (no host synchronisation):
+//   forward: 3 batched GEMMs of two problems each (one per net; bias + ReLU, then layer 3 writes column 0 through the
+//   sigmoid and columns 1..dim) -> per-row loss terms -> statistics + generator update (train_core.cuh) -> dLoss/dOut
+//   and per-row confidence -> 2 batched data-gradient GEMMs (ReLU backward) -> ONE six-problem launch of every weight
+//   and bias gradient -> loss metrics -> Adam (mlp_adam_step).
+// Training batches are small (~8 nodes x ~100 segments), so the step is latency-bound: the GEMMs are the training core's
+// fp32 CUDA-core tiles, every output element and every sum is formed by one thread (or one fixed reduction tree) in a
+// fixed order, with no atomics: two runs of the same step are bit-identical.
+#include <string.h>
+
+#include <algorithm>
+
+#include "common.cuh"
+#include "double_mlp_train.h"
+#include "host_common.h"
+#include "train_core.cuh"
+
+namespace wvn {
+
+namespace {
+
+constexpr int kRowThreads = 256;    // one warp per row
+constexpr int kStatThreads = 256;   // the single-block reductions
+
+// The step's scalars.  The sums are the fused SimpleMLP step's (FusedScalars): over the labelled rows the sum of
+// loss_reco and of its square, over all rows the sum of (trav - y)^2, the two row counts and loss_reco's extrema.
+struct DoubleScalars {
+  double sum_lr, sum_lr2, sum_raw, n_valid, n_rows, x_min, x_max;
+  float lo, hi, cmin, cmax, g_reco, g_trav;   // the updated generator and the loss-gradient scales
+  float mean, std;
+};
+
+// loss_reco[r] = mean_d (out[r, 1 + d] - x[r, d])^2,  raw[r] = (out[r, 0] - y[r])^2
+__global__ void __launch_bounds__(kRowThreads)
+double_loss_rows_kernel(const float* __restrict__ out, const float* __restrict__ x, const float* __restrict__ y,
+                        float* __restrict__ loss_reco, float* __restrict__ raw, int rows, int dim) {
+  const int lane = threadIdx.x & 31;
+  const int r = (blockIdx.x * kRowThreads + threadIdx.x) >> 5;
+  if (r >= rows) return;
+  const float* o = out + static_cast<long long>(r) * (dim + 1);
+  const float* xr = x + static_cast<long long>(r) * dim;
+  float acc = 0.f;
+  for (int d = lane; d < dim; d += 32) {
+    const float df = o[1 + d] - xr[d];
+    acc = fmaf(df, df, acc);
+  }
+  acc = warp_sum(acc);
+  if (lane == 0) {
+    loss_reco[r] = acc / static_cast<float>(dim);
+    const float dt = o[0] - y[r];
+    raw[r] = dt * dt;
+  }
+}
+
+// One block: the statistic sums in fp64 (fixed reduction order), then one thread updates the ConfidenceGenerator.
+// loss_reco's extrema (moving_average's clip) skip NaN rows (fminf / fmaxf).  The fused SimpleMLP step skips them too,
+// except that a 32-row tile whose every live row is NaN makes its x_max NaN (mlp_train_fused.cu, atomicMax on the bits).
+__global__ void __launch_bounds__(kStatThreads, 1)
+double_stats_kernel(const float* __restrict__ loss_reco, const float* __restrict__ raw,
+                    const unsigned char* __restrict__ y_valid, int rows, int dim, LossCfg cfg, ConfState cs,
+                    float* __restrict__ cg_mean, float* __restrict__ cg_std, DoubleScalars* __restrict__ sc) {
+  __shared__ double red[4][kStatThreads / 32];
+  __shared__ float rmin[kStatThreads / 32], rmax[kStatThreads / 32];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  double s1 = 0.0, s2 = 0.0, sraw = 0.0, nv = 0.0;
+  float mn = INFINITY, mx = 0.f;
+  for (int i = t; i < rows; i += kStatThreads) {
+    const float lr = loss_reco[i];
+    sraw += static_cast<double>(raw[i]);
+    mn = fminf(mn, lr);
+    mx = fmaxf(mx, lr);
+    if (y_valid[i]) { s1 += lr; s2 += static_cast<double>(lr) * lr; nv += 1.0; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+    s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    sraw += __shfl_xor_sync(0xffffffffu, sraw, o);
+    nv += __shfl_xor_sync(0xffffffffu, nv, o);
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  if (lane == 0) { red[0][warp] = s1; red[1][warp] = s2; red[2][warp] = sraw; red[3][warp] = nv; rmin[warp] = mn; rmax[warp] = mx; }
+  __syncthreads();
+  if (t != 0) return;
+  double S1 = 0.0, S2 = 0.0, SR = 0.0, NV = 0.0;
+  float MN = INFINITY, MX = 0.f;
+  for (int w = 0; w < kStatThreads / 32; ++w) {
+    S1 += red[0][w]; S2 += red[1][w]; SR += red[2][w]; NV += red[3][w];
+    MN = fminf(MN, rmin[w]); MX = fmaxf(MX, rmax[w]);
+  }
+  const double NR = static_cast<double>(rows);
+  sc->sum_lr = S1; sc->sum_lr2 = S2; sc->sum_raw = SR; sc->n_valid = NV; sc->n_rows = NR;
+  sc->x_min = MN; sc->x_max = MX;
+  const ConfUpdate u = conf_generator_update(cs, cfg.std_factor, NV, S1, S2, MN, MX, cg_mean);
+  sc->lo = u.lo; sc->hi = u.hi; sc->cmin = u.cmin; sc->cmax = u.cmax;
+  sc->g_reco = cfg.w_reco * 2.f / (static_cast<float>(NV) * static_cast<float>(dim));
+  sc->g_trav = cfg.w_trav * 2.f / static_cast<float>(NR);
+  sc->mean = u.mean;
+  sc->std = u.std;
+  if (cg_mean) *cg_mean = u.mean;
+  if (cg_std) *cg_std = u.std;
+}
+
+// dLoss/dOut of w_trav * L_trav + w_reco * L_reco (+ w_temp * 0), the confidence of each row under the updated
+// generator (what ConfidenceGenerator.update returns) and each row's confidence-weighted traversability error.
+__global__ void __launch_bounds__(kRowThreads)
+double_dout_kernel(const float* __restrict__ out, const float* __restrict__ x, const float* __restrict__ y,
+                   const unsigned char* __restrict__ y_valid, const float* __restrict__ loss_reco,
+                   const float* __restrict__ raw, const DoubleScalars* __restrict__ sc, LossCfg cfg, int method,
+                   float* __restrict__ d_out, float* __restrict__ conf_out, float* __restrict__ wraw, int rows,
+                   int dim) {
+  const int lane = threadIdx.x & 31;
+  const int r = (blockIdx.x * kRowThreads + threadIdx.x) >> 5;
+  if (r >= rows) return;
+  const float lo = sc->lo, hi = sc->hi, cmin = sc->cmin, cmax = sc->cmax, g_reco = sc->g_reco, g_trav = sc->g_trav;
+  const bool v = y_valid[r] != 0;
+  const float conf = row_confidence(method, loss_reco[r], lo, hi, cmin, cmax);
+  const float wgt = (v || !cfg.anomaly_balanced) ? 1.f : (1.f - conf);
+  const float* o = out + static_cast<long long>(r) * (dim + 1);
+  const float* xr = x + static_cast<long long>(r) * dim;
+  float* g = d_out + static_cast<long long>(r) * (dim + 1);
+  for (int d = lane; d < dim; d += 32) g[1 + d] = v ? g_reco * (o[1 + d] - xr[d]) : 0.f;
+  if (lane == 0) {
+    const float tv = o[0];
+    g[0] = g_trav * wgt * (tv - y[r]) * tv * (1.f - tv);   // through the sigmoid
+    conf_out[r] = conf;
+    wraw[r] = raw[r] * wgt;
+  }
+}
+
+// Loss metrics (one block, fixed reduction order); leaves them in metrics[6] for the host.
+__global__ void __launch_bounds__(kStatThreads, 1)
+double_finish_kernel(const float* __restrict__ wraw, int rows, LossCfg cfg, const DoubleScalars* __restrict__ sc,
+                     float* __restrict__ metrics) {
+  __shared__ double red[kStatThreads / 32];
+  const int t = threadIdx.x;
+  double s = 0.0;
+  for (int i = t; i < rows; i += kStatThreads) s += static_cast<double>(wraw[i]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((t & 31) == 0) red[t >> 5] = s;
+  __syncthreads();
+  if (t != 0 || metrics == nullptr) return;
+  double S = 0.0;
+  for (int w = 0; w < kStatThreads / 32; ++w) S += red[w];
+  const float loss_reco = static_cast<float>(sc->sum_lr / sc->n_valid);
+  const float loss_trav_conf = static_cast<float>(S / sc->n_rows);
+  metrics[0] = cfg.w_trav * loss_trav_conf + cfg.w_reco * loss_reco;
+  metrics[1] = static_cast<float>(sc->sum_raw / sc->n_rows);
+  metrics[2] = loss_reco;
+  metrics[3] = loss_trav_conf;
+  metrics[4] = sc->mean;
+  metrics[5] = sc->std;
+}
+
+}  // namespace
+
+// ------------------------------------------------------------------------------------------------ host side
+DoubleOffsets double_mlp_offsets(const MlpShape& s) {
+  const size_t D = s.dim, h1 = s.h1, h2 = s.h2;
+  DoubleOffsets o;
+  size_t off = 0;
+  for (int k = 0; k < 2; ++k) {
+    const size_t last = k == 0 ? 1 : D;
+    o.w1[k] = off; off += h1 * D;
+    o.b1[k] = off; off += h1;
+    o.w2[k] = off; off += h2 * h1;
+    o.b2[k] = off; off += h2;
+    o.w3[k] = off; off += last * h2;
+    o.b3[k] = off; off += last;
+  }
+  o.total = off;
+  return o;
+}
+
+size_t double_mlp_param_count(const MlpShape& s) { return double_mlp_offsets(s).total; }
+
+int double_mlp_check_shape(const MlpShape& s, const char* who) {
+  WVN_REQUIRE(s.dim >= 1 && s.dim <= 1024 && s.h1 >= 4 && s.h1 <= 256 && s.h1 % 4 == 0 && s.h2 >= 1 && s.h2 <= 32,
+              "%s: DoubleMLP(%d, [%d, %d, 1]) outside the kernels' range (1 <= dim <= 1024, 4 <= h1 <= 256 and a "
+              "multiple of 4, 1 <= h2 <= 32)", who, s.dim, s.h1, s.h2);
+  return WVN_OK;
+}
+
+namespace {
+
+// The three forward launches; a1 / a2 hold net 0's block, then net 1's, `pitch` rows apart.
+int forward_gemms(const MlpShape& s, const DoubleOffsets& o, const float* params, const float* x, int rows, long long pitch,
+                  float* a1, float* a2, float* out, cudaStream_t stream) {
+  const int D = s.dim, h1 = s.h1, h2 = s.h2;
+  GemmProblem ps[2];
+  for (int k = 0; k < 2; ++k) {   // a1_k = ReLU(x W1_k^T + b1_k)
+    ps[k] = gemm_problem(x, D, 1, params + o.w1[k], 1, D, a1 + k * pitch * h1, h1, rows, h1, D);
+    ps[k].bias = params + o.b1[k]; ps[k].act = F32_RELU_FMAX;
+  }
+  WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
+  for (int k = 0; k < 2; ++k) {   // a2_k = ReLU(a1_k W2_k^T + b2_k)
+    ps[k] = gemm_problem(a1 + k * pitch * h1, h1, 1, params + o.w2[k], 1, h1, a2 + k * pitch * h2, h2, rows, h2, h1);
+    ps[k].bias = params + o.b2[k]; ps[k].act = F32_RELU_FMAX;
+  }
+  WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
+  // column 0 = sigmoid(a2_0 w3_0 + b3_0), columns 1..dim = a2_1 W3_1^T + b3_1
+  ps[0] = gemm_problem(a2, h2, 1, params + o.w3[0], 1, h2, out, D + 1, rows, 1, h2);
+  ps[0].bias = params + o.b3[0]; ps[0].act = F32_SIGMOID_COL0;
+  ps[1] = gemm_problem(a2 + pitch * h2, h2, 1, params + o.w3[1], 1, h2, out + 1, D + 1, rows, D, h2);
+  ps[1].bias = params + o.b3[1];
+  return launch_gemms(ps, 2, nullptr, stream);
+}
+
+}  // namespace
+
+int double_mlp_forward_f32(const MlpShape& s, const float* params, const float* x, int rows, float* a1, float* a2,
+                           float* out, cudaStream_t stream) {
+  WVN_PROPAGATE(double_mlp_check_shape(s, "double mlp forward"));
+  WVN_REQUIRE(params && x && a1 && a2 && out && rows > 0, "double mlp forward: bad argument");
+  return forward_gemms(s, double_mlp_offsets(s), params, x, rows, rows, a1, a2, out, stream);
+}
+
+struct DoubleTrainer {
+  MlpShape s;
+  DoubleOffsets o;
+  LossCfg loss;
+  AdamCfg adam;
+  int max_rows = 0;
+  void* arena = nullptr;
+  DoubleScalars* sc = nullptr;
+  float *a1 = nullptr, *a2 = nullptr, *out = nullptr, *d_out = nullptr, *d2 = nullptr, *d1 = nullptr;
+  float *loss_reco = nullptr, *raw = nullptr, *wraw = nullptr, *grads = nullptr;
+  TrainerConf conf;
+};
+
+int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, float* grads_ext,
+                          DoubleTrainer** out) {
+  WVN_REQUIRE(out && max_rows > 0, "double mlp trainer: bad arguments");
+  WVN_PROPAGATE(double_mlp_check_shape(s, "double mlp trainer"));
+  DoubleTrainer* t = new DoubleTrainer();
+  t->s = s; t->o = double_mlp_offsets(s); t->loss = loss; t->adam = adam;
+  t->max_rows = max_rows;
+  const size_t R = max_rows, D = s.dim, h1 = s.h1, h2 = s.h2;
+  // a1 / d1 [2][R, h1], a2 / d2 [2][R, h2], out / d_out [R, 1 + D], loss_reco / raw / wraw [R], grads
+  const size_t floats = 2 * (2 * R * h1 + 2 * R * h2 + R * (D + 1)) + 3 * R + (grads_ext ? 0 : t->o.total);
+  const size_t head = 256;
+  const size_t bytes = head + floats * sizeof(float);
+  if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
+    delete t;
+    return set_error(WVN_ERR_CUDA, "double mlp trainer: cudaMalloc of %zu bytes failed", bytes);
+  }
+  const int rc = trainer_conf_create(&t->conf);
+  if (rc != WVN_OK) {
+    cudaFree(t->arena);
+    delete t;
+    return rc;
+  }
+  if (cudaMemset(t->arena, 0, bytes) != cudaSuccess) {
+    trainer_conf_destroy(&t->conf);
+    cudaFree(t->arena);
+    delete t;
+    return set_error(WVN_ERR_CUDA, "double mlp trainer: cudaMemset of %zu bytes failed", bytes);
+  }
+  char* base = reinterpret_cast<char*>(t->arena);
+  t->sc = reinterpret_cast<DoubleScalars*>(base);
+  float* f = reinterpret_cast<float*>(base + head);
+  auto take = [&](size_t n) { float* p = f; f += n; return p; };
+  t->a1 = take(2 * R * h1);
+  t->d1 = take(2 * R * h1);
+  t->a2 = take(2 * R * h2);
+  t->d2 = take(2 * R * h2);
+  t->out = take(R * (D + 1));
+  t->d_out = take(R * (D + 1));
+  t->loss_reco = take(R);
+  t->raw = take(R);
+  t->wraw = take(R);
+  t->grads = grads_ext ? grads_ext : take(t->o.total);
+  *out = t;
+  return WVN_OK;
+}
+
+void double_trainer_destroy(DoubleTrainer* t) {
+  if (!t) return;
+  if (t->arena) cudaFree(t->arena);
+  trainer_conf_destroy(&t->conf);
+  delete t;
+}
+
+TrainerConf* double_trainer_conf(DoubleTrainer* t) { return &t->conf; }
+
+int double_train_step(DoubleTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                      const float* x, int rows, const float* y, const unsigned char* y_valid, float* cg_mean,
+                      float* cg_std, float* conf_out, float* metrics, cudaStream_t stream) {
+  WVN_REQUIRE(t && params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
+              "double mlp train step: null argument");
+  WVN_REQUIRE(rows > 0 && rows <= t->max_rows, "double mlp train step: rows=%d outside (0, %d]", rows, t->max_rows);
+  const MlpShape& s = t->s;
+  const DoubleOffsets& o = t->o;
+  const int D = s.dim, h1 = s.h1, h2 = s.h2, n3 = D + 1;
+  const long long R = t->max_rows;   // the per-net blocks of a1 / a2 / d1 / d2 are max_rows rows apart
+  WVN_PROPAGATE(forward_gemms(s, o, params, x, rows, R, t->a1, t->a2, t->out, stream));
+  // ---- loss terms, statistics + generator update, dLoss/dOut + confidence
+  const int row_blocks = (rows * 32 + kRowThreads - 1) / kRowThreads;
+  double_loss_rows_kernel<<<row_blocks, kRowThreads, 0, stream>>>(t->out, x, y, t->loss_reco, t->raw, rows, D);
+  WVN_CHECK_LAUNCH("double_loss_rows_kernel");
+  double_stats_kernel<<<1, kStatThreads, 0, stream>>>(t->loss_reco, t->raw, y_valid, rows, D, t->loss, t->conf.cs,
+                                                      cg_mean, cg_std, t->sc);
+  WVN_CHECK_LAUNCH("double_stats_kernel");
+  double_dout_kernel<<<row_blocks, kRowThreads, 0, stream>>>(t->out, x, y, y_valid, t->loss_reco, t->raw, t->sc, t->loss,
+                                                             t->conf.cs.method, t->d_out, conf_out, t->wraw, rows, D);
+  WVN_CHECK_LAUNCH("double_dout_kernel");
+  // ---- data gradients: d2_k = (dOut_k W3_k) * (a2_k > 0), d1_k = (d2_k W2_k) * (a1_k > 0)
+  {
+    GemmProblem ps[2];
+    ps[0] = gemm_problem(t->d_out, n3, 1, params + o.w3[0], h2, 1, t->d2, h2, rows, h2, 1);
+    ps[1] = gemm_problem(t->d_out + 1, n3, 1, params + o.w3[1], h2, 1, t->d2 + R * h2, h2, rows, h2, D);
+    for (int k = 0; k < 2; ++k) { ps[k].ref = t->a2 + k * R * h2; ps[k].ld_ref = h2; }
+    WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
+    for (int k = 0; k < 2; ++k) {
+      ps[k] = gemm_problem(t->d2 + k * R * h2, h2, 1, params + o.w2[k], h1, 1, t->d1 + k * R * h1, h1, rows, h1, h2);
+      ps[k].ref = t->a1 + k * R * h1; ps[k].ld_ref = h1;
+    }
+    WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
+  }
+  // ---- every weight gradient dW = dZ^T A and bias gradient db = column sums of dZ: one launch of six problems
+  {
+    GemmProblem wg[6];
+    wg[0] = gemm_problem(t->d_out, 1, n3, t->a2, h2, 1, t->grads + o.w3[0], h2, 1, h2, rows);
+    wg[0].db = t->grads + o.b3[0];
+    wg[1] = gemm_problem(t->d_out + 1, 1, n3, t->a2 + R * h2, h2, 1, t->grads + o.w3[1], h2, D, h2, rows);
+    wg[1].db = t->grads + o.b3[1];
+    for (int k = 0; k < 2; ++k) {
+      wg[2 + k] = gemm_problem(t->d2 + k * R * h2, 1, h2, t->a1 + k * R * h1, h1, 1, t->grads + o.w2[k], h1, h2, h1, rows);
+      wg[2 + k].db = t->grads + o.b2[k];
+      wg[4 + k] = gemm_problem(t->d1 + k * R * h1, 1, h1, x, D, 1, t->grads + o.w1[k], D, h1, D, rows);
+      wg[4 + k].db = t->grads + o.b1[k];
+    }
+    WVN_PROPAGATE(launch_gemms(wg, 6, nullptr, stream));
+  }
+  // ---- loss metrics, then Adam
+  double_finish_kernel<<<1, kStatThreads, 0, stream>>>(t->wraw, rows, t->loss, t->sc, metrics);
+  WVN_CHECK_LAUNCH("double_finish_kernel");
+  return mlp_adam_step(params, t->grads, exp_avg, exp_avg_sq, static_cast<long long>(o.total), t->adam, step_counter,
+                       stream);
+}
+
+}  // namespace wvn

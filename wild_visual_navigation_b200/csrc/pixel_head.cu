@@ -20,9 +20,18 @@
 // (wgmma, M=128 pixels, N=32), and ~650 fp32 FMAs — ~12x fewer FLOPs than the direct form, and
 // no HBM traffic beyond the two output maps.  bf16 rounding points are the same as the unfused
 // path (tokens, weights, h1); everything downstream of the layer-2 accumulator is fp32.
+//
+// The same kernel serves the DoubleMLP (two networks of widths h1 / 32 on the same features, net 0 -> traversability,
+// net 1 -> reconstruction): G = tokens @ [W1_0; W1_1]^T + [b1_0; b1_1] (2 h1 channels), U / cT from net 1's last layer,
+// and layer 2 as TWO m64n32 wgmma chains over the two K halves of the h1 tile, one per network.  The block-diagonal
+// alternative (one N = 64 chain over all 2 h1 channels) would spend half of its MMAs on the zero blocks and keep 64
+// accumulators live per thread; two chains keep the SimpleMLP head's instruction, W2 tile and shared-memory layout, and
+// net 0's chain (which only feeds the logit) is reduced to one partial sum per fragment row before net 1's (which only
+// feeds the reconstruction terms) is issued, so at most 32 accumulators are live, as in the SimpleMLP head.
 #include <algorithm>
 
 #include "common.cuh"
+#include "double_mlp_train.h"
 #include "host_common.h"
 #include "pixel_head.h"
 
@@ -33,7 +42,7 @@ namespace {
 constexpr int kH1 = 256, kH2 = 32;
 constexpr int kTileW = 64, kTileH = 2;            // 128 pixels per tile: row i = r*64 + px
 constexpr int kWinMax = 10;                        // token-window columns per tile (ratio 8: 7 + 3)
-constexpr int kGvStride = 292;                     // 256 G + 32 U + cT_hi + cT_lo, padded to float4
+constexpr int kGvStride = 292;                     // 256 G + 32 U + cT_hi + cT_lo, padded to float4 (the largest row)
 constexpr int kThreads = 256;
 constexpr uint32_t kOffA = 0;                      // [4 K-blocks][128 rows][128 B]  h1 tile (bf16, swizzled); once layer 2
                                                    // has consumed it: [128 pixels][kH2Stride] fp32 layer-2 accumulator
@@ -68,8 +77,15 @@ __device__ __forceinline__ uint32_t pack_bf16x2_relu(float lo, float hi) {
   return d;
 }
 
-__global__ void __launch_bounds__(kThreads, 2)
+// kK: channels of the h1 tile (= layer 2's K; 256 for the SimpleMLP head, 2 h1 for the DoubleMLP), kNets: 1 (SimpleMLP)
+// or 2 (DoubleMLP: net 0's h1 in channels [0, kK/2), net 1's in [kK/2, kK); W2's K blocks of net 1 are read from rows
+// 32..63 of the W2 operand, i.e. the block-diagonal layer 2 of the packed unfused operands).
+template <int kK, int kNets>
+__global__ void __launch_bounds__(kThreads, kNets == 1 ? 2 : 1)
 pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadArgs a) {
+  static_assert(kK % 64 == 0 && kK <= kH1 && (kNets == 1 || kK % 128 == 0), "pixel_head_kernel: h1 tile shape");
+  constexpr int kGvS = (kK + kH2 + 2 + 3) / 4 * 4;   // G | U | cT_hi | cT_lo, padded to float4 (292 for kK = 256)
+  constexpr int kKB = kK / 64;                       // 64-channel K blocks of the h1 tile
   extern __shared__ __align__(1024) uint8_t smem[];
   float* gv = reinterpret_cast<float*>(smem + kOffGv);
   float* n2 = reinterpret_cast<float*>(smem + kOffN2);
@@ -90,8 +106,9 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    mbar_arrive_expect_tx(w2_full, 4 * 32 * 128);
-    for (int kb = 0; kb < 4; ++kb) tma_load_2d(&tmap_w2, w2_full, smem + kOffW2 + kb * 4096, kb * 64, 0);
+    mbar_arrive_expect_tx(w2_full, kKB * 32 * 128);
+    for (int kb = 0; kb < kKB; ++kb)
+      tma_load_2d(&tmap_w2, w2_full, smem + kOffW2 + kb * 4096, kb * 64, (kNets == 2 && kb >= kKB / 2) ? 32 : 0);
   }
 
   // Tile geometry: pixel rows [py0, py0+2), pixel columns [px0, px0+64) of frame b; cx0 = first token column of the window.
@@ -128,11 +145,19 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
       pt->row1[t] = (y1r[r] * a.gw + tc) * static_cast<int>(a.ldg);
     }
     named_bar_sync(2, 128);
-    constexpr int kV4 = kGvStride / 4;
+    constexpr int kV4 = kGvS / 4;
     constexpr int kBatch = 6;  // float4 pairs in flight per thread and pass (48 registers)
+    constexpr int kStepRc = 128 / kV4, kStepV4 = 128 % kV4;
     const int n_rc = kTileH * ww;
-    // item i = t + 128 * k  <->  (rc, v4) = (i / 73, i % 73), advanced incrementally (128 = 73 + 55)
-    int rc = t >= kV4 ? 1 : 0, v4 = t - rc * kV4;
+    // item i = t + 128 * k  <->  (rc, v4) = (i / kV4, i % kV4), advanced incrementally (128 = kStepRc kV4 + kStepV4)
+    int rc, v4;
+    if constexpr (2 * kV4 > 128) {
+      rc = t >= kV4 ? 1 : 0;
+      v4 = t - rc * kV4;
+    } else {
+      rc = t / kV4;
+      v4 = t - rc * kV4;
+    }
     while (rc < n_rc) {
       float4 g0[kBatch], g1[kBatch];
       int rcs[kBatch], v4s[kBatch];
@@ -143,7 +168,7 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
           g0[it] = __ldg(reinterpret_cast<const float4*>(gub + pt->row0[rc]) + v4);
           g1[it] = __ldg(reinterpret_cast<const float4*>(gub + pt->row1[rc]) + v4);
         }
-        v4 += 128 - kV4; rc += 1;
+        v4 += kStepV4; rc += kStepRc;
         if (v4 >= kV4) { v4 -= kV4; rc += 1; }
       }
 #pragma unroll
@@ -202,13 +227,14 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
     {
       const int units = kTileH * (ww - 1);  // (row, cell) pairs; cell c spans window columns [c, c+1]
       for (int u = warp; u < units; u += kThreads / 32) {
+        if (kK < kH1 && 8 * lane >= kK) continue;   // lanes past the tile's channels
         const int r = u >= (ww - 1) ? 1 : 0, cell = u - r * (ww - 1);
         const int p_begin = pt->start[cell], p_end = pt->start[cell + 1];  // contiguous run of this cell's pixels
         if (p_begin >= p_end) continue;
-        const float* g0p = gv + (r * ww + cell) * kGvStride + 8 * lane;
+        const float* g0p = gv + (r * ww + cell) * kGvS + 8 * lane;
         const float4 a0 = reinterpret_cast<const float4*>(g0p)[0], a1 = reinterpret_cast<const float4*>(g0p)[1];
-        const float4 b0 = reinterpret_cast<const float4*>(g0p + kGvStride)[0];
-        const float4 b1 = reinterpret_cast<const float4*>(g0p + kGvStride)[1];
+        const float4 b0 = reinterpret_cast<const float4*>(g0p + kGvS)[0];
+        const float4 b1 = reinterpret_cast<const float4*>(g0p + kGvS)[1];
         const float gg[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
         const float dg[8] = {b0.x - a0.x, b0.y - a0.y, b0.z - a0.z, b0.w - a0.w,
                              b1.x - a1.x, b1.y - a1.y, b1.z - a1.z, b1.w - a1.w};
@@ -240,89 +266,210 @@ pixel_head_kernel(const __grid_constant__ CUtensorMap tmap_w2, const PixelHeadAr
       named_bar_sync(1, kThreads);
       if (tile + gridDim.x < num_tiles) phase_a(tile_geo(tile + gridDim.x));
     } else {
+      if constexpr (kNets == 1) {
       // ---------------- layer 2 on the tensor core: D[128, 32] = h1[128, 256] @ W2^T, issued by this warpgroup
-      // (two 64-row halves) and left in flight while each thread prepares its pixel's blend terms
-      float d2[2][16];
-      mbar_wait(w2_full, 0);  // completes once; later tiles pass at once
-      wgmma_fence();
+        // (two 64-row halves) and left in flight while each thread prepares its pixel's blend terms
+        float d2[2][16];
+        mbar_wait(w2_full, 0);  // completes once; later tiles pass at once
+        wgmma_fence();
+  #pragma unroll
+        for (int ks = 0; ks < kK / 16; ++ks) {
+          const uint64_t db = make_sw128_kmajor_desc(smem_u32(smem + kOffW2 + (ks >> 2) * 4096)) + 2 * (ks & 3);
+  #pragma unroll
+          for (int half = 0; half < 2; ++half)
+            wgmma_m64n32k16_ss(d2[half], make_sw128_kmajor_desc(smem_u32(smem + kOffA + (ks >> 2) * 16384 + half * 8192)) + 2 * (ks & 3),
+                               db, ks != 0);
+        }
+        wgmma_commit();
+        // ---------------- epilogue: one thread per pixel
+        const int i = threadIdx.x;  // pixel
+        const int r = i >> 6, px = i & 63;
+        const float wx = pt->wx[px];
+        const int c0 = pt->c0[px];
+        const bool same_x = (cx0 + c0 + 1 > a.gw - 1);
+        // U columns of the two neighbouring window columns (c0+1 is a clamped duplicate at the right border)
+        const float4* u0 = reinterpret_cast<const float4*>(gv + (r * ww + c0) * kGvS + kK);
+        const float4* u1 = u0 + kGvS / 4;
+        float ub[kH2 + 4];  // blended U (32) | cT_hi, cT_lo
+  #pragma unroll
+        for (int j4 = 0; j4 < kH2 / 4 + 1; ++j4) {
+          const float4 p0 = u0[j4], p1 = u1[j4];
+          ub[4 * j4 + 0] = fmaf(wx, p1.x - p0.x, p0.x);
+          ub[4 * j4 + 1] = fmaf(wx, p1.y - p0.y, p0.y);
+          ub[4 * j4 + 2] = fmaf(wx, p1.z - p0.z, p0.z);
+          ub[4 * j4 + 3] = fmaf(wx, p1.w - p0.w, p0.w);
+        }
+        const float* nn = n2 + (r * ww + c0) * 2;
+        const float ux = 1.f - wx;
+        const float n_c1 = same_x ? nn[0] : nn[2];
+        const float xx = same_x ? nn[0] : nn[1];
+        const float gram = ux * ux * nn[0] + 2.f * ux * wx * xx + wx * wx * n_c1;
+        asm volatile("bar.arrive 1, %0;" ::"n"(kThreads) : "memory");  // gv / n2 / tables consumed: producers may refill
+  
+        wgmma_wait<0>();
+        wgmma_fence_regs(d2[0]);
+        wgmma_fence_regs(d2[1]);
+        // fragments -> one pixel per thread, through the h1 tile once every warp's MMAs have consumed it
+        named_bar_sync(3, 128);
+        float* h2s = reinterpret_cast<float*>(smem + kOffA);
+  #pragma unroll
+        for (int half = 0; half < 2; ++half)
+  #pragma unroll
+          for (int j = 0; j < 4; ++j)
+  #pragma unroll
+            for (int hh = 0; hh < 2; ++hh)
+              *reinterpret_cast<float2*>(h2s + (half * 64 + warp * 16 + (lane >> 2) + 8 * hh) * kH2Stride + 8 * j + 2 * (lane & 3)) =
+                  make_float2(d2[half][4 * j + 2 * hh], d2[half][4 * j + 2 * hh + 1]);
+        named_bar_sync(3, 128);
+        float h2[kH2];
+  #pragma unroll
+        for (int j4 = 0; j4 < kH2 / 4; ++j4) {
+          const float4 raw = reinterpret_cast<const float4*>(h2s + i * kH2Stride)[j4];
+          h2[4 * j4 + 0] = fmaxf(raw.x + c_ph.b2[4 * j4 + 0], 0.f);
+          h2[4 * j4 + 1] = fmaxf(raw.y + c_ph.b2[4 * j4 + 1], 0.f);
+          h2[4 * j4 + 2] = fmaxf(raw.z + c_ph.b2[4 * j4 + 2], 0.f);
+          h2[4 * j4 + 3] = fmaxf(raw.w + c_ph.b2[4 * j4 + 3], 0.f);
+        }
+        // traversability logit, |r|^2 quadratic form (upper-triangular M with doubled off-diagonals), r.x
+        float t = c_ph.b0, q = c_ph.cc, cross = ub[kH2] + ub[kH2 + 1];
+  #pragma unroll
+        for (int j = 0; j < kH2; ++j) {
+          t = fmaf(c_ph.w0[j], h2[j], t);
+          float acc = c_ph.tv[j];
+  #pragma unroll
+          for (int k = j; k < kH2; ++k) acc = fmaf(c_ph.m[j * kH2 + k], h2[k], acc);
+          q = fmaf(h2[j], acc, q);
+          cross = fmaf(h2[j], ub[j], cross);
+        }
+        const float loss = fmaxf(q - 2.f * cross + gram, 0.f) / static_cast<float>(a.feat);
+        const float mean = __ldg(a.cg_mean), sd = __ldg(a.cg_std);
+        const float shifted = mean + sd * a.std_factor;
+        const float lo = fmaxf(shifted - sd, 0.f), hi = shifted + sd;
+        const float xc = fminf(fmaxf(loss, lo), hi);
+        const long long o = (static_cast<long long>(b) * a.H + py0 + r) * a.W + px0 + px;
+        a.trav[o] = 1.f / (1.f + __expf(-t));
+        a.conf[o] = 1.f - (xc - lo) / (hi - lo);
+        if (a.loss_reco != nullptr) a.loss_reco[o] = loss;
+      } else {
+        // ---------------- layer 2 on the tensor core, one m64n32 chain per network over its half of the h1 tile:
+        // D_n[128, 32] = h1_n[128, kK/2] @ W2_n^T, net 0 first
+        float d0[2][16], d1[2][16];
+        mbar_wait(w2_full, 0);  // completes once; later tiles pass at once
+        wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < kH1 / 16; ++ks) {
-        const uint64_t db = make_sw128_kmajor_desc(smem_u32(smem + kOffW2 + (ks >> 2) * 4096)) + 2 * (ks & 3);
+        for (int ks = 0; ks < kK / 32; ++ks) {
+          const uint64_t db = make_sw128_kmajor_desc(smem_u32(smem + kOffW2 + (ks >> 2) * 4096)) + 2 * (ks & 3);
+#pragma unroll
+          for (int half = 0; half < 2; ++half)
+            wgmma_m64n32k16_ss(d0[half], make_sw128_kmajor_desc(smem_u32(smem + kOffA + (ks >> 2) * 16384 + half * 8192)) + 2 * (ks & 3),
+                               db, ks != 0);
+        }
+        wgmma_commit();
+        // net 0 only feeds the logit: once its chain completes, reduce its fragments to one partial sum per fragment
+        // row, w0 . ReLU(z + b2) over this thread's 8 columns, then over the 4 lanes that share the row
+        wgmma_wait<0>();
+        wgmma_fence_regs(d0[0]);
+        wgmma_fence_regs(d0[1]);
+        float tp[2][2];
 #pragma unroll
         for (int half = 0; half < 2; ++half)
-          wgmma_m64n32k16_ss(d2[half], make_sw128_kmajor_desc(smem_u32(smem + kOffA + (ks >> 2) * 16384 + half * 8192)) + 2 * (ks & 3),
-                             db, ks != 0);
-      }
-      wgmma_commit();
-      // ---------------- epilogue: one thread per pixel
-      const int i = threadIdx.x;  // pixel
-      const int r = i >> 6, px = i & 63;
-      const float wx = pt->wx[px];
-      const int c0 = pt->c0[px];
-      const bool same_x = (cx0 + c0 + 1 > a.gw - 1);
-      // U columns of the two neighbouring window columns (c0+1 is a clamped duplicate at the right border)
-      const float4* u0 = reinterpret_cast<const float4*>(gv + (r * ww + c0) * kGvStride + kH1);
-      const float4* u1 = u0 + kGvStride / 4;
-      float ub[kH2 + 4];  // blended U (32) | cT_hi, cT_lo
 #pragma unroll
-      for (int j4 = 0; j4 < kH2 / 4 + 1; ++j4) {
-        const float4 p0 = u0[j4], p1 = u1[j4];
-        ub[4 * j4 + 0] = fmaf(wx, p1.x - p0.x, p0.x);
-        ub[4 * j4 + 1] = fmaf(wx, p1.y - p0.y, p0.y);
-        ub[4 * j4 + 2] = fmaf(wx, p1.z - p0.z, p0.z);
-        ub[4 * j4 + 3] = fmaf(wx, p1.w - p0.w, p0.w);
-      }
-      const float* nn = n2 + (r * ww + c0) * 2;
-      const float ux = 1.f - wx;
-      const float n_c1 = same_x ? nn[0] : nn[2];
-      const float xx = same_x ? nn[0] : nn[1];
-      const float gram = ux * ux * nn[0] + 2.f * ux * wx * xx + wx * wx * n_c1;
-      asm volatile("bar.arrive 1, %0;" ::"n"(kThreads) : "memory");  // gv / n2 / tables consumed: producers may refill
+          for (int hh = 0; hh < 2; ++hh) {
+            float acc = 0.f;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int col = 8 * j + 2 * (lane & 3) + e;
+                acc = fmaf(c_ph.w0[col], fmaxf(d0[half][4 * j + 2 * hh + e] + c_ph.b2[col], 0.f), acc);
+              }
+            acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+            acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+            tp[half][hh] = acc;
+          }
+        // net 1's chain, left in flight while each thread prepares its pixel's blend terms
+        wgmma_fence();
+#pragma unroll
+        for (int ks = kK / 32; ks < kK / 16; ++ks) {
+          const uint64_t db = make_sw128_kmajor_desc(smem_u32(smem + kOffW2 + (ks >> 2) * 4096)) + 2 * (ks & 3);
+#pragma unroll
+          for (int half = 0; half < 2; ++half)
+            wgmma_m64n32k16_ss(d1[half], make_sw128_kmajor_desc(smem_u32(smem + kOffA + (ks >> 2) * 16384 + half * 8192)) + 2 * (ks & 3),
+                               db, ks != kK / 32);
+        }
+        wgmma_commit();
+        // ---------------- epilogue: one thread per pixel
+        const int i = threadIdx.x;  // pixel
+        const int r = i >> 6, px = i & 63;
+        const float wx = pt->wx[px];
+        const int c0 = pt->c0[px];
+        const bool same_x = (cx0 + c0 + 1 > a.gw - 1);
+        const float4* u0 = reinterpret_cast<const float4*>(gv + (r * ww + c0) * kGvS + kK);
+        const float4* u1 = u0 + kGvS / 4;
+        float ub[kH2 + 4];  // blended U (32) | cT_hi, cT_lo
+#pragma unroll
+        for (int j4 = 0; j4 < kH2 / 4 + 1; ++j4) {
+          const float4 p0 = u0[j4], p1 = u1[j4];
+          ub[4 * j4 + 0] = fmaf(wx, p1.x - p0.x, p0.x);
+          ub[4 * j4 + 1] = fmaf(wx, p1.y - p0.y, p0.y);
+          ub[4 * j4 + 2] = fmaf(wx, p1.z - p0.z, p0.z);
+          ub[4 * j4 + 3] = fmaf(wx, p1.w - p0.w, p0.w);
+        }
+        const float* nn = n2 + (r * ww + c0) * 2;
+        const float ux = 1.f - wx;
+        const float n_c1 = same_x ? nn[0] : nn[2];
+        const float xx = same_x ? nn[0] : nn[1];
+        const float gram = ux * ux * nn[0] + 2.f * ux * wx * xx + wx * wx * n_c1;
+        asm volatile("bar.arrive 1, %0;" ::"n"(kThreads) : "memory");  // gv / n2 / tables consumed: producers may refill
 
-      wgmma_wait<0>();
-      wgmma_fence_regs(d2[0]);
-      wgmma_fence_regs(d2[1]);
-      // fragments -> one pixel per thread, through the h1 tile once every warp's MMAs have consumed it
-      named_bar_sync(3, 128);
-      float* h2s = reinterpret_cast<float*>(smem + kOffA);
+        wgmma_wait<0>();
+        wgmma_fence_regs(d1[0]);
+        wgmma_fence_regs(d1[1]);
+        // net 1's fragments and net 0's logit partials -> one pixel per thread, through the h1 tile
+        named_bar_sync(3, 128);
+        float* h2s = reinterpret_cast<float*>(smem + kOffA);
+        float* ts = h2s + 128 * kH2Stride;
 #pragma unroll
-      for (int half = 0; half < 2; ++half)
+        for (int half = 0; half < 2; ++half)
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
+          for (int hh = 0; hh < 2; ++hh) {
+            const int row = half * 64 + warp * 16 + (lane >> 2) + 8 * hh;
 #pragma unroll
-          for (int hh = 0; hh < 2; ++hh)
-            *reinterpret_cast<float2*>(h2s + (half * 64 + warp * 16 + (lane >> 2) + 8 * hh) * kH2Stride + 8 * j + 2 * (lane & 3)) =
-                make_float2(d2[half][4 * j + 2 * hh], d2[half][4 * j + 2 * hh + 1]);
-      named_bar_sync(3, 128);
-      float h2[kH2];
+            for (int j = 0; j < 4; ++j)
+              *reinterpret_cast<float2*>(h2s + row * kH2Stride + 8 * j + 2 * (lane & 3)) =
+                  make_float2(d1[half][4 * j + 2 * hh], d1[half][4 * j + 2 * hh + 1]);
+            if ((lane & 3) == 0) ts[row] = tp[half][hh];
+          }
+        named_bar_sync(3, 128);
+        const float t = c_ph.b0 + ts[i];
+        float h2[kH2];
 #pragma unroll
-      for (int j4 = 0; j4 < kH2 / 4; ++j4) {
-        const float4 raw = reinterpret_cast<const float4*>(h2s + i * kH2Stride)[j4];
-        h2[4 * j4 + 0] = fmaxf(raw.x + c_ph.b2[4 * j4 + 0], 0.f);
-        h2[4 * j4 + 1] = fmaxf(raw.y + c_ph.b2[4 * j4 + 1], 0.f);
-        h2[4 * j4 + 2] = fmaxf(raw.z + c_ph.b2[4 * j4 + 2], 0.f);
-        h2[4 * j4 + 3] = fmaxf(raw.w + c_ph.b2[4 * j4 + 3], 0.f);
+        for (int j4 = 0; j4 < kH2 / 4; ++j4) {
+          const float4 raw = reinterpret_cast<const float4*>(h2s + i * kH2Stride)[j4];
+          h2[4 * j4 + 0] = fmaxf(raw.x + c_ph.b2r[4 * j4 + 0], 0.f);
+          h2[4 * j4 + 1] = fmaxf(raw.y + c_ph.b2r[4 * j4 + 1], 0.f);
+          h2[4 * j4 + 2] = fmaxf(raw.z + c_ph.b2r[4 * j4 + 2], 0.f);
+          h2[4 * j4 + 3] = fmaxf(raw.w + c_ph.b2r[4 * j4 + 3], 0.f);
+        }
+        float q = c_ph.cc, cross = ub[kH2] + ub[kH2 + 1];
+  #pragma unroll
+        for (int j = 0; j < kH2; ++j) {
+          float acc = c_ph.tv[j];
+  #pragma unroll
+          for (int k = j; k < kH2; ++k) acc = fmaf(c_ph.m[j * kH2 + k], h2[k], acc);
+          q = fmaf(h2[j], acc, q);
+          cross = fmaf(h2[j], ub[j], cross);
+        }
+        const float loss = fmaxf(q - 2.f * cross + gram, 0.f) / static_cast<float>(a.feat);
+        const float mean = __ldg(a.cg_mean), sd = __ldg(a.cg_std);
+        const float shifted = mean + sd * a.std_factor;
+        const float lo = fmaxf(shifted - sd, 0.f), hi = shifted + sd;
+        const float xc = fminf(fmaxf(loss, lo), hi);
+        const long long o = (static_cast<long long>(b) * a.H + py0 + r) * a.W + px0 + px;
+        a.trav[o] = 1.f / (1.f + __expf(-t));
+        a.conf[o] = 1.f - (xc - lo) / (hi - lo);
+        if (a.loss_reco != nullptr) a.loss_reco[o] = loss;
       }
-      // traversability logit, |r|^2 quadratic form (upper-triangular M with doubled off-diagonals), r.x
-      float t = c_ph.b0, q = c_ph.cc, cross = ub[kH2] + ub[kH2 + 1];
-#pragma unroll
-      for (int j = 0; j < kH2; ++j) {
-        t = fmaf(c_ph.w0[j], h2[j], t);
-        float acc = c_ph.tv[j];
-#pragma unroll
-        for (int k = j; k < kH2; ++k) acc = fmaf(c_ph.m[j * kH2 + k], h2[k], acc);
-        q = fmaf(h2[j], acc, q);
-        cross = fmaf(h2[j], ub[j], cross);
-      }
-      const float loss = fmaxf(q - 2.f * cross + gram, 0.f) / static_cast<float>(a.feat);
-      const float mean = __ldg(a.cg_mean), sd = __ldg(a.cg_std);
-      const float shifted = mean + sd * a.std_factor;
-      const float lo = fmaxf(shifted - sd, 0.f), hi = shifted + sd;
-      const float xc = fminf(fmaxf(loss, lo), hi);
-      const long long o = (static_cast<long long>(b) * a.H + py0 + r) * a.W + px0 + px;
-      a.trav[o] = 1.f / (1.f + __expf(-t));
-      a.conf[o] = 1.f - (xc - lo) / (hi - lo);
-      if (a.loss_reco != nullptr) a.loss_reco[o] = loss;
     }
   }
 }
@@ -368,18 +515,25 @@ token_gram_kernel(const __nv_bfloat16* __restrict__ tok, float* __restrict__ gra
 // One block of 32 x 32 threads: thread (j, k) owns M[j][k]; row 0 also produces tv / b2 / w0.  R (bf16-rounded) and c
 // are staged in shared memory in chunks of 384 channels and every thread runs four independent accumulators over the
 // chunk (instead of walking the 384 channels with two dependent global loads each).
+// The operands, as pointers into the flat parameters: R [dim][32] and c [dim] (the reconstruction rows of the last
+// layer and their bias), w0 [32] / b0 (the traversability row and its bias), b2 / b2r [32] (layer 2's bias of the
+// traversability / reconstruction path: the same for a SimpleMLP).
+struct HeadSources {
+  const float *R, *c, *w0, *b0, *b2, *b2r;
+};
+
 __global__ void __launch_bounds__(1024)
-pixel_head_consts_kernel(const float* __restrict__ p, MlpOffsets o, int dim, PixelHeadConsts* out) {
+pixel_head_consts_kernel(HeadSources hs, int dim, PixelHeadConsts* out) {
   constexpr int kChunk = 384;
   __shared__ __nv_bfloat16 rs[kChunk * kH2];
   __shared__ float cs[kChunk];
   const int k = threadIdx.x & 31, j = threadIdx.x >> 5;
-  const float* w3 = p + o.w3 + kH2;  // rows 1.. of layers.4.weight: R[d][*]
+  const float* w3 = hs.R;
   float m4[4] = {0.f, 0.f, 0.f, 0.f}, tv4[4] = {0.f, 0.f, 0.f, 0.f}, cc4[4] = {0.f, 0.f, 0.f, 0.f};
   for (int d0 = 0; d0 < dim; d0 += kChunk) {
     const int nd = min(kChunk, dim - d0);
     for (int i = threadIdx.x; i < nd * kH2; i += 1024) rs[i] = __float2bfloat16_rn(w3[static_cast<long long>(d0) * kH2 + i]);
-    for (int i = threadIdx.x; i < nd; i += 1024) cs[i] = p[o.b3 + 1 + d0 + i];
+    for (int i = threadIdx.x; i < nd; i += 1024) cs[i] = hs.c[d0 + i];
     __syncthreads();
     auto step = [&](int d, int q) {
       const float rj = __bfloat162float(rs[d * kH2 + j]);
@@ -400,52 +554,111 @@ pixel_head_consts_kernel(const float* __restrict__ p, MlpOffsets o, int dim, Pix
   out->m[j * kH2 + k] = (k == j) ? m : (k > j ? 2.f * m : 0.f);
   if (k == 0) {
     out->tv[j] = 2.f * tv;
-    out->b2[j] = p[o.b2 + j];
-    out->w0[j] = __bfloat162float(__float2bfloat16_rn(p[o.w3 + j]));  // row 0 (bf16 like the GEMM path)
+    out->b2[j] = hs.b2[j];
+    out->b2r[j] = hs.b2r[j];
+    out->w0[j] = __bfloat162float(__float2bfloat16_rn(hs.w0[j]));  // the logit row (bf16 like the GEMM path)
   }
   if (threadIdx.x == 0) {
-    out->b0 = p[o.b3];
+    out->b0 = *hs.b0;
     out->cc = cc;
   }
 }
 
-// Wcat [320, dim_p] bf16 = [W1 ; R^T ; c_hi ; c_lo ; 0], bias [320] = [b1 ; 0]
-__global__ void pixel_head_pack_kernel(const float* __restrict__ p, MlpOffsets o, int dim, int dim_p,
-                                       __nv_bfloat16* __restrict__ wcat, float* __restrict__ bias) {
-  const long long total = static_cast<long long>(kPixelHeadN) * dim_p;
+// Wcat [n, dim_p] bf16 = [W1 ; R^T ; c_hi ; c_lo ; 0], bias [n] = [b1 ; 0], n = pixel_head_columns(ng).  The ng G rows
+// come from w1a / b1a (rows [0, ha)) and w1b / b1b (rows [ha, ng): the DoubleMLP's second network).
+__global__ void pixel_head_pack_kernel(const float* __restrict__ w1a, const float* __restrict__ b1a, int ha,
+                                       const float* __restrict__ w1b, const float* __restrict__ b1b, int ng, HeadSources hs,
+                                       int n, int dim, int dim_p, __nv_bfloat16* __restrict__ wcat, float* __restrict__ bias) {
+  const long long total = static_cast<long long>(n) * dim_p;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int r = static_cast<int>(i / dim_p), d = static_cast<int>(i % dim_p);
     float v = 0.f;
     if (d < dim) {
-      if (r < kH1) v = p[o.w1 + static_cast<long long>(r) * dim + d];
-      else if (r < kH1 + kH2) v = p[o.w3 + static_cast<long long>(1 + d) * kH2 + (r - kH1)];
-      else if (r == kH1 + kH2) v = p[o.b3 + 1 + d];
-      else if (r == kH1 + kH2 + 1) {
-        const float c = p[o.b3 + 1 + d];
+      if (r < ha) v = w1a[static_cast<long long>(r) * dim + d];
+      else if (r < ng) v = w1b[static_cast<long long>(r - ha) * dim + d];
+      else if (r < ng + kH2) v = hs.R[static_cast<long long>(d) * kH2 + (r - ng)];
+      else if (r == ng + kH2) v = hs.c[d];
+      else if (r == ng + kH2 + 1) {
+        const float c = hs.c[d];
         v = c - __bfloat162float(__float2bfloat16_rn(c));
       }
     }
     wcat[i] = __float2bfloat16_rn(v);
-    if (d == 0) bias[r] = r < kH1 ? p[o.b1 + r] : 0.f;
+    if (d == 0) bias[r] = r < ha ? b1a[r] : (r < ng ? b1b[r - ha] : 0.f);
   }
 }
 
-}  // namespace
-
-int pixel_head_supported(int h1, int h2, int gh, int gw, int H, int W) {
-  if (h1 != kH1 || h2 != kH2 || H % kTileH != 0 || W % kTileW != 0 || H < 2 || W < 2) return 0;
+int window_width(int gh, int gw, int H, int W) {
+  if (H % kTileH != 0 || W % kTileW != 0 || H < 2 || W < 2) return 0;
   const float sx = static_cast<float>(gw - 1) / static_cast<float>(W - 1);
   const int ww = static_cast<int>((kTileW - 1) * sx) + 3;
   return (ww >= 2 && ww <= kWinMax) ? ww : 0;
 }
 
+template <int kK, int kNets>
+int launch_pixel_head(const PixelHeadArgs& a, const void* w2_bf16, int w2_ld, cudaStream_t stream) {
+  constexpr int kGvS = (kK + kH2 + 2 + 3) / 4 * 4;
+  WVN_REQUIRE(a.ww >= 2 && a.ww <= kWinMax && a.W % kTileW == 0 && a.H % kTileH == 0, "pixel_head: unsupported geometry");
+  WVN_REQUIRE(a.ldg >= kGvS && a.ldg % 4 == 0, "pixel_head: ldg %lld too small", a.ldg);
+  WVN_REQUIRE(static_cast<long long>(a.gh) * a.gw * a.ldg < (1ll << 31), "pixel_head: token grid too large for 32-bit row offsets");
+  CUtensorMap tw;
+  WVN_PROPAGATE(make_tmap_bf16_2d(&tw, w2_bf16, kK, kNets * kH2, static_cast<uint64_t>(w2_ld) * 2, 64, kH2));
+  static bool attr_set = false;
+  if (!attr_set) {
+    WVN_CHECK_CUDA(cudaFuncSetAttribute(pixel_head_kernel<kK, kNets>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        kSmemBytes));
+    attr_set = true;
+  }
+  const long long tiles = static_cast<long long>(a.batch) * (a.H / kTileH) * (a.W / kTileW);
+  // one resident CTA per SM for the DoubleMLP instantiation (189 registers: it spills at the SimpleMLP head's 128)
+  int grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(sm_count()) * (kNets == 1 ? 2 : 1)));
+  WVN_CHECK_CUDA(cudaMemcpyToSymbolAsync(c_ph, a.consts, sizeof(PixelHeadConsts), 0, cudaMemcpyDeviceToDevice, stream));
+  pixel_head_kernel<kK, kNets><<<grid, kThreads, kSmemBytes, stream>>>(tw, a);
+  WVN_CHECK_LAUNCH("pixel_head_kernel");
+  return WVN_OK;
+}
+
+}  // namespace
+
+int pixel_head_supported(int h1, int h2, int gh, int gw, int H, int W) {
+  if (h1 != kH1 || h2 != kH2) return 0;
+  return window_width(gh, gw, H, W);
+}
+
+bool pixel_head_double_shape(int h1, int h2) { return (h1 == 64 || h1 == 128) && h2 == kH2; }
+
+int pixel_head_supported_double(int h1, int h2, int gh, int gw, int H, int W) {
+  return pixel_head_double_shape(h1, h2) ? window_width(gh, gw, H, W) : 0;
+}
+
+int pixel_head_columns(int g_channels) { return (g_channels + kH2 + 2 + 63) / 64 * 64; }
+
 int pixel_head_pack(const float* params, const MlpShape& s, int dim_p, void* wcat_bf16, float* bias,
                     PixelHeadConsts* consts, cudaStream_t stream) {
   const MlpOffsets o = mlp_offsets(s);
-  pixel_head_pack_kernel<<<128, 256, 0, stream>>>(params, o, s.dim, dim_p, reinterpret_cast<__nv_bfloat16*>(wcat_bf16), bias);
+  const HeadSources hs{params + o.w3 + kH2, params + o.b3 + 1, params + o.w3, params + o.b3, params + o.b2, params + o.b2};
+  pixel_head_pack_kernel<<<128, 256, 0, stream>>>(params + o.w1, params + o.b1, kH1, nullptr, nullptr, kH1, hs,
+                                                  kPixelHeadN, s.dim, dim_p, reinterpret_cast<__nv_bfloat16*>(wcat_bf16),
+                                                  bias);
   WVN_CHECK_LAUNCH("pixel_head_pack_kernel");
-  pixel_head_consts_kernel<<<1, 1024, 0, stream>>>(params, o, s.dim, consts);
+  pixel_head_consts_kernel<<<1, 1024, 0, stream>>>(hs, s.dim, consts);
+  WVN_CHECK_LAUNCH("pixel_head_consts_kernel");
+  return WVN_OK;
+}
+
+int pixel_head_pack_double(const float* params, const MlpShape& net, int dim_p, void* wcat_bf16, float* bias,
+                           PixelHeadConsts* consts, cudaStream_t stream) {
+  WVN_REQUIRE(pixel_head_double_shape(net.h1, net.h2), "pixel_head_pack_double: h1 = %d, h2 = %d outside the "
+              "fused head", net.h1, net.h2);
+  const DoubleOffsets o = double_mlp_offsets(net);
+  const HeadSources hs{params + o.w3[1], params + o.b3[1], params + o.w3[0], params + o.b3[0], params + o.b2[0],
+                       params + o.b2[1]};
+  pixel_head_pack_kernel<<<128, 256, 0, stream>>>(params + o.w1[0], params + o.b1[0], net.h1, params + o.w1[1],
+                                                  params + o.b1[1], 2 * net.h1, hs, pixel_head_columns(2 * net.h1),
+                                                  net.dim, dim_p, reinterpret_cast<__nv_bfloat16*>(wcat_bf16), bias);
+  WVN_CHECK_LAUNCH("pixel_head_pack_kernel");
+  pixel_head_consts_kernel<<<1, 1024, 0, stream>>>(hs, net.dim, consts);
   WVN_CHECK_LAUNCH("pixel_head_consts_kernel");
   return WVN_OK;
 }
@@ -463,22 +676,13 @@ int token_gram(const void* tok_bf16, float* gram, int batch, int gh, int gw, int
 }
 
 int pixel_head(const PixelHeadArgs& a, const void* w2_bf16, int w2_ld, cudaStream_t stream) {
-  WVN_REQUIRE(a.ww >= 2 && a.ww <= kWinMax && a.W % kTileW == 0 && a.H % kTileH == 0, "pixel_head: unsupported geometry");
-  WVN_REQUIRE(a.ldg >= kGvStride && a.ldg % 4 == 0, "pixel_head: ldg %lld too small", a.ldg);
-  WVN_REQUIRE(static_cast<long long>(a.gh) * a.gw * a.ldg < (1ll << 31), "pixel_head: token grid too large for 32-bit row offsets");
-  CUtensorMap tw;
-  WVN_PROPAGATE(make_tmap_bf16_2d(&tw, w2_bf16, kH1, kH2, static_cast<uint64_t>(w2_ld) * 2, 64, kH2));
-  static bool attr_set = false;
-  if (!attr_set) {
-    WVN_CHECK_CUDA(cudaFuncSetAttribute(pixel_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    attr_set = true;
-  }
-  const long long tiles = static_cast<long long>(a.batch) * (a.H / kTileH) * (a.W / kTileW);
-  int grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(sm_count()) * 2));
-  WVN_CHECK_CUDA(cudaMemcpyToSymbolAsync(c_ph, a.consts, sizeof(PixelHeadConsts), 0, cudaMemcpyDeviceToDevice, stream));
-  pixel_head_kernel<<<grid, kThreads, kSmemBytes, stream>>>(tw, a);
-  WVN_CHECK_LAUNCH("pixel_head_kernel");
-  return WVN_OK;
+  return launch_pixel_head<kH1, 1>(a, w2_bf16, w2_ld, stream);
+}
+
+int pixel_head_double(const PixelHeadArgs& a, int h1, const void* w2_bf16, int w2_ld, cudaStream_t stream) {
+  if (h1 == 64) return launch_pixel_head<128, 2>(a, w2_bf16, w2_ld, stream);
+  if (h1 == 128) return launch_pixel_head<256, 2>(a, w2_bf16, w2_ld, stream);
+  return set_error(WVN_ERR_INVALID, "pixel_head_double: h1 = %d outside the fused head (64 or 128)", h1);
 }
 
 }  // namespace wvn

@@ -18,6 +18,7 @@ struct PixelHeadConsts {
   float b0;          // layers.4.bias[0]
   float cc;          // c . c
   float pad[2];
+  float b2r[32];     // layer 2's bias of the reconstruction network (DoubleMLP: networks.1.2.bias; SimpleMLP: b2)
 };
 
 struct PixelHeadArgs {
@@ -46,5 +47,15 @@ int pixel_head_pack(const float* params, const MlpShape& s, int dim_p, void* wca
 int token_gram(const void* tok_bf16, float* gram, int batch, int gh, int gw, int dim, long long frame_rows, int row0,
                cudaStream_t stream);
 int pixel_head(const PixelHeadArgs& a, const void* w2_bf16, int w2_ld, cudaStream_t stream);
+
+// The DoubleMLP head (net widths h1 in {64, 128}, h2 = 32): per-token GEMM columns G_0 | G_1 | U | cT_hi | cT_lo, padded
+// to pixel_head_columns(2 h1) (192 / 320); U / cT from networks.1.4, the logit from networks.0.4.  w2_bf16: the packed
+// block-diagonal layer 2 [64 rows][w2_ld] (rows 0..31 net 0 on channels [0, h1), rows 32..63 net 1 on [h1, 2 h1)).
+bool pixel_head_double_shape(int h1, int h2);
+int pixel_head_supported_double(int h1, int h2, int gh, int gw, int H, int W);
+int pixel_head_columns(int g_channels);
+int pixel_head_pack_double(const float* params, const MlpShape& net, int dim_p, void* wcat_bf16, float* bias,
+                           PixelHeadConsts* consts, cudaStream_t stream);
+int pixel_head_double(const PixelHeadArgs& a, int h1, const void* w2_bf16, int w2_ld, cudaStream_t stream);
 
 }  // namespace wvn

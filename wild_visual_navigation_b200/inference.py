@@ -15,6 +15,12 @@ generator's ``inference_without_update`` of the per-row NLL and there is no conf
 ``publish_confidence = False``): per pixel, the tokens are upsampled in a sampling kernel and every layer of the four
 nets runs as a wgmma GEMM (bf16 operands, fp32 accumulation) over chunks of pixels, with the coupling arithmetic, NLL and
 confidence in fp32 kernels (csrc/flow_train.cu); ``predict_segments`` runs the fp32 flow on the pooled rows.
+
+A ``DoubleMLP`` runs through the same MLP handle.  Per pixel, for h1 in {64, 128} and h2 = 32, the fused head's
+DoubleMLP instantiation (csrc/pixel_head.cu: G of both networks interpolated, layer 2 as one wgmma chain per network);
+other shapes, and ``predict_segments``, run the two networks packed as one block-structured MLP (layer 1 both nets'
+rows, layer 2 block-diagonal, layer 3 the traversability row on net 0's half and the reconstruction rows on net 1's)
+through the unfused GEMM chain.
 """
 from __future__ import annotations
 
@@ -22,7 +28,7 @@ import torch
 
 from . import ops
 from .model.linear_rnvp import LinearRnvp
-from .model.simple_mlp import SimpleMLP
+from .model.simple_mlp import DoubleMLP, SimpleMLP
 from .utils.confidence_generator import ConfidenceGenerator
 
 
@@ -36,14 +42,19 @@ class TraversabilityInference:
             self._flow_infer = ops.FlowInference(model.input_size, model.hidden, max_rows=1024, chunk_pixels=chunk_rows)
             self.refresh_weights()
             return
-        assert model.fused_ok(), "model must be the hot-path SimpleMLP(D,[256,32,1],reconstruction=True) on CUDA"
+        self._double = isinstance(model, DoubleMLP)
+        if self._double:
+            model.check_supported()
+        else:
+            assert model.fused_ok(), "model must be the hot-path SimpleMLP(D,[256,32,1],reconstruction=True) on CUDA"
         self._dino = dino
         self._model = model
         self._cg = confidence_generator
         # a feature-pyramid backbone (TorchVisionInterface) has no token grid: only the segment-wise mode applies
         grid = getattr(dino, "grid", 0)
         self._mlp = ops.MlpInference(model.input_size, model.hidden[0], model.hidden[1], chunk_rows,
-                                       tokens_per_frame=max(grid * grid, getattr(dino._model, "npad", 0)))
+                                       tokens_per_frame=max(grid * grid, getattr(dino._model, "npad", 0)),
+                                       double=self._double)
         self.refresh_weights()
 
     def refresh_weights(self):
@@ -79,7 +90,7 @@ class TraversabilityInference:
                                            self._cg.std.data, self._cg.std_factor), None
         vit = self._dino._model
         last = getattr(vit, "last_tokens", None)
-        if (last is not None and tokens.data_ptr() == last.data_ptr() and tokens.shape[1:] == last.shape[1:]
+        if ((not self._double or self._mlp.fused_shape) and last is not None and tokens.data_ptr() == last.data_ptr() and tokens.shape[1:] == last.shape[1:]
                 and tokens.shape[0] <= last.shape[0] and self._model.input_size == vit.dim and out_size % 64 == 0):
             # these ARE the backbone's last tokens: its bf16 copy goes to the head as it is (no re-cast of 4.8 MB/frame)
             return self._mlp.pixels_from_vit(vit, tokens.shape[0], (out_size, out_size), self._cg.mean.data,

@@ -1,3 +1,3 @@
-from .simple_mlp import SimpleMLP
+from .simple_mlp import DoubleMLP, SimpleMLP
 from .linear_rnvp import LinearRnvp
 from .network_register import get_model

@@ -457,11 +457,18 @@ def _resized_size(h, w, size):
 # traversability MLP: inference handle and trainer
 # --------------------------------------------------------------------------------------------
 class MlpInference:
-    def __init__(self, dim=384, h1=256, h2=32, chunk_rows=0, tokens_per_frame=0):
+    """Per-pixel and per-row traversability / confidence of a SimpleMLP, or with ``double=True`` of a
+    DoubleMLP(dim, [h1, h2, 1]) (``set_params`` then takes its flat parameters).  ``fused_shape``: the fused per-pixel
+    head takes this shape (SimpleMLP [256, 32, 1], DoubleMLP [64 or 128, 32, 1]), so ``pixels_from_vit`` can run at
+    the fused geometries."""
+
+    def __init__(self, dim=384, h1=256, h2=32, chunk_rows=0, tokens_per_frame=0, double=False):
         _C.require_device()
-        self.dim, self.h1, self.h2 = dim, h1, h2
+        self.dim, self.h1, self.h2, self.double = dim, h1, h2, double
+        self.fused_shape = (h1 in (64, 128) and h2 == 32) if double else (h1 == 256 and h2 == 32)
         h = c_void_p()
-        check(lib().wvn_mlp_infer_create(dim, h1, h2, chunk_rows, byref(h)))
+        create = lib().wvn_mlp_infer_create_double if double else lib().wvn_mlp_infer_create
+        check(create(dim, h1, h2, chunk_rows, byref(h)))
         self._h = h
         if tokens_per_frame > 0:  # all workspaces exist before the first frame arrives
             check(lib().wvn_mlp_infer_reserve(h, tokens_per_frame))
@@ -512,6 +519,20 @@ def mlp_forward_f32(flat_params, x, dim, h1, h2):
     out = torch.empty(R, 1 + dim, device=dev, dtype=torch.float32)
     check(lib().wvn_mlp_forward_f32(dim, h1, h2, ptr(flat_params), ptr(x.contiguous()), R, ptr(b1), ptr(b2), ptr(out),
                                     stream()))
+    return out
+
+
+def double_mlp_forward_f32(flat_params, x, dim, h1, h2):
+    """DoubleMLP.forward in fp32: returns (rows, 1+dim), column 0 = sigmoid(networks[0](x)), then networks[1](x)."""
+    R = x.shape[0]
+    dev = x.device
+    a1 = torch.empty(2, R, h1, device=dev, dtype=torch.float32)
+    a2 = torch.empty(2, R, h2, device=dev, dtype=torch.float32)
+    out = torch.empty(R, 1 + dim, device=dev, dtype=torch.float32)
+    if R == 0:
+        return out
+    check(lib().wvn_double_mlp_forward_f32(dim, h1, h2, ptr(flat_params), ptr(x.contiguous()), R, ptr(a1), ptr(a2),
+                                           ptr(out), stream()))
     return out
 
 
@@ -711,6 +732,65 @@ class MlpTrainer(_TrainerHandle):
         check(lib().wvn_mlp_train_apply(*d, ptr(self.params), ptr(self.grads), ptr(self.exp_avg), ptr(self.exp_avg_sq),
                                         ptr(self.step_counter), n_total, byref(self.cfg), ptr(self.scalars), s))
         check(lib().wvn_mlp_train_read_metrics(ptr(self.scalars), ptr(self.metrics), s))
+        return self.conf[:R]
+
+
+class DoubleMlpTrainer(_TrainerHandle):
+    """The online train step of a DoubleMLP on its flat fp32 parameters (csrc/double_mlp_train.cu): forward of both
+    networks, TraversabilityLoss with the ConfidenceGenerator update, backward and Adam as one fixed launch sequence
+    without host synchronisation, bit-reproducible.  ``exp_avg`` / ``exp_avg_sq`` / ``step_counter`` are
+    torch.optim.Adam's state over the 12 parameter tensors, flattened in ``parameters()`` order.  Single-GPU."""
+
+    _DESTROY = "wvn_double_mlp_trainer_destroy"
+    _SET_CONFIDENCE = "wvn_double_mlp_trainer_set_confidence"
+    _COPY_CONFIDENCE = "wvn_double_mlp_trainer_copy_confidence"
+
+    def __init__(self, model, max_rows=4096, w_trav=0.03, w_reco=0.5, std_factor=0.5, anomaly_balanced=True, lr=1e-3,
+                 betas=(0.9, 0.999), eps=1e-8):
+        model.check_supported()
+        _C.require_device()
+        params = model.flat_params
+        dev = params.device
+        self.model = model
+        self.dim, (self.h1, self.h2) = model.input_size, model.hidden
+        self.n_params = lib().wvn_double_mlp_param_count(self.dim, self.h1, self.h2)
+        assert params.numel() == self.n_params and params.dtype == torch.float32
+        self.cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
+        self.grads = torch.zeros(self.n_params, device=dev)
+        self.exp_avg = torch.zeros(self.n_params, device=dev)
+        self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
+        self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
+        self.metrics = torch.zeros(6, device=dev)
+        self.cg_mean = torch.zeros(1, device=dev)
+        self.cg_std = torch.ones(1, device=dev)
+        self._h = None
+        self._conf = None
+        self._create(max_rows)
+
+    def _new_handle(self, max_rows):
+        h = c_void_p()
+        check(lib().wvn_double_mlp_trainer_create(self.dim, self.h1, self.h2, max_rows, byref(self.cfg), ptr(self.grads),
+                                                  byref(h)))
+        return h
+
+    def _create(self, max_rows):
+        super()._create(max_rows)
+        self.conf = torch.empty(self.max_rows, device=self.grads.device)
+
+    def step(self, x, y, y_valid, n_total=None):
+        """x [R,D] f32, y [R] f32, y_valid [R] bool.  Returns the confidence vector [R]; metrics stay on the device in
+        ``self.metrics`` (loss_total, loss_trav, loss_reco, loss_trav_conf, mean, std)."""
+        if n_total is not None and n_total != x.shape[0]:
+            raise ValueError("DoubleMlpTrainer: the step is single-GPU, n_total must be the batch's row count")
+        R = x.shape[0]
+        self._reserve(R)
+        x = x.contiguous().float()
+        y = y.contiguous().float()
+        yv = y_valid.contiguous().to(torch.uint8)
+        check(lib().wvn_double_mlp_train_step(self._h, ptr(self.model.flat_params), ptr(self.exp_avg),
+                                              ptr(self.exp_avg_sq), ptr(self.step_counter), ptr(x), R, ptr(y), ptr(yv),
+                                              ptr(self.cg_mean), ptr(self.cg_std), ptr(self.conf), ptr(self.metrics),
+                                              stream()))
         return self.conf[:R]
 
 

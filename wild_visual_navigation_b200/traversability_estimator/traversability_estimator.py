@@ -13,7 +13,8 @@ list and must already carry their per-segment features and supervision (``Missio
 (csrc/mlp_train.cu) with all scalars on the device; with a ``process_group`` the three confidence
 statistics and the flat gradient are all-reduced (NCCL over NVLink) for a global-batch step.
 In anomaly-detection mode the step is the LinearRnvp flow's (csrc/flow_train.cu: forward, NLL, confidence update,
-backward, Adam) on the labelled rows only; it is single-GPU.
+backward, Adam) on the labelled rows only; it is single-GPU.  With ``model.name == "DoubleMLP"`` the step is the
+DoubleMLP's (csrc/double_mlp_train.cu: the same TraversabilityLoss on two separate networks), also single-GPU.
 """
 from __future__ import annotations
 
@@ -34,6 +35,7 @@ def default_params(anomaly_detection: bool = False):
     return {
         "model": {"name": "LinearRnvp" if anomaly_detection else "SimpleMLP",
                   "simple_mlp_cfg": {"input_size": 384, "hidden_sizes": [256, 32, 1], "reconstruction": True},
+                  "double_mlp_cfg": {"input_size": 384, "hidden_sizes": [64, 32, 1]},
                   "linear_rnvp_cfg": {"input_size": 384, "coupling_topology": [200], "mask_type": "odds",
                                       "conditioning_size": 0, "use_permutation": True, "single_function": False}},
         "loss": {"anomaly_balanced": True, "w_trav": 0.03, "w_temp": 0.0, "w_reco": 0.5, "method": "latest_measurement",
@@ -105,6 +107,9 @@ class TraversabilityEstimator:
         if anomaly_detection != (_get(model_cfg, "name") == "LinearRnvp"):
             raise ValueError("anomaly_detection=True goes with model.name 'LinearRnvp' (and only with it), got "
                              f"{_get(model_cfg, 'name')!r}")
+        self._double = _get(model_cfg, "name") == "DoubleMLP"
+        if self._double and process_group is not None:
+            raise ValueError("DoubleMLP trains on one GPU: process_group is not supported")
         self._model = get_model(model_cfg).to(self._device)
         self._model.train()
         gp = _get(self._params, "general")
@@ -127,6 +132,12 @@ class TraversabilityEstimator:
         self._traversability_loss.to(self._device)
         m = self._model
         cg = self._traversability_loss._confidence_generator
+        if self._double:
+            self._trainer = ops.DoubleMlpTrainer(m, max_rows=max_rows, w_trav=lp["w_trav"], w_reco=lp["w_reco"],
+                                                 std_factor=cg.std_factor, anomaly_balanced=lp["anomaly_balanced"],
+                                                 lr=self._lr)
+            self._bind_confidence_state()
+            return
         self._trainer = ops.MlpTrainer(m.flat_params, m.input_size, m.hidden[0], m.hidden[1], max_rows=max_rows,
                                        w_trav=lp["w_trav"], w_reco=lp["w_reco"], std_factor=cg.std_factor,
                                        anomaly_balanced=lp["anomaly_balanced"], lr=self._lr, process_group=process_group)
@@ -201,6 +212,8 @@ class TraversabilityEstimator:
         number (what ``feat[mask]`` would give).  No host synchronisation (the gather happens inside the kernels)."""
         if self._anomaly_detection:
             raise ValueError("train_on_padded is the SimpleMLP step; in anomaly-detection mode use train_on_batch")
+        if self._double:
+            raise ValueError("train_on_padded is the SimpleMLP step; with a DoubleMLP use train_on_batch")
         with self._learning_lock:
             conf = self._trainer.step_padded(feat, n_rows, y, y_valid)
             self._last_confidence = conf
