@@ -48,7 +48,10 @@ int wvn_check_device(void);
  * 102: adds wvn_mlp_trainer_copy_confidence (no layout change).
  * 103: wvn_gemm_ex_args gained trailing `residual` / `ldr` (epi 6); adds the ResNet handle, the im2col / max-pool
  * primitives and wvn_segment_pool_pyramid.
- * 104: adds the LinearRnvp flow handles, their functions wvn_flow_* and the struct wvn_flow_buffers; no layout change. */
+ * 104: adds the LinearRnvp flow handles, their functions wvn_flow_* and the struct wvn_flow_buffers; no layout change.
+ * 106: adds the padded, phased and data-parallel DoubleMLP and flow steps (wvn_double_mlp_train_step_padded,
+ * wvn_double_mlp_trainer_init_comm, wvn_double_mlp_trainer_stats, wvn_flow_train_step_padded, wvn_flow_init_comm,
+ * wvn_flow_stats); no layout change. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -431,7 +434,8 @@ int wvn_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_trai
                            float* grads, wvn_mlp_trainer_t** out);
 void wvn_mlp_trainer_destroy(wvn_mlp_trainer_t* t);
 /* Library-owned NCCL communicator (libnccl.so.2 is resolved from the running process): rank 0 fills a 128-byte id with
- * wvn_comm_unique_id, the caller broadcasts it by any means, every rank calls wvn_mlp_trainer_init_comm. */
+ * wvn_comm_unique_id, the caller broadcasts it by any means, every rank calls wvn_mlp_trainer_init_comm (or
+ * wvn_double_mlp_trainer_init_comm / wvn_flow_init_comm: every trainer takes a communicator the same way). */
 int wvn_comm_unique_id(void* id128);
 int wvn_mlp_trainer_init_comm(wvn_mlp_trainer_t* t, const void* id128, int rank, int world);
 /* ConfidenceGenerator method of the fused step (utils/confidence_generator.py:49-76): 0 latest_measurement (default),
@@ -484,6 +488,25 @@ int wvn_double_mlp_train_step(wvn_double_mlp_trainer_t* t, float* params, float*
                               long long* step_counter, const float* x, int rows, const float* y,
                               const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
                               float* metrics_out, void* stream);
+/* The same step on rows padded per group, data-parallel.  x: [groups, rows_per_group, dim] fp32; n_rows: [groups] int32
+ * (device) live rows per group, or NULL when every row is live; y / y_valid / confidence_out are indexed by the
+ * COMPACTED row number (live rows of group 0, then group 1, ...).  Padding rows may hold anything (NaN included): they
+ * are never read.  groups * rows_per_group <= max_rows.  wvn_double_mlp_train_step is this step with one group.
+ * phase_mask: 7 = whole step; 1 = forward + the statistic sums, 2 = generator update + backward + weight gradients,
+ * 4 = metrics + Adam.  With a communicator (wvn_double_mlp_trainer_init_comm) the step all-reduces the statistics after
+ * phase 1 and the gradient after phase 2 itself; without one a data-parallel caller all-reduces, between the phases,
+ * the statistics block (wvn_double_mlp_trainer_stats) — doubles 0..5 with SUM, and for moving_average double 6 with MIN
+ * and 7 with MAX — after phase 1, and the gradient (n_params floats) and double 8 of the block with SUM after phase 2. */
+int wvn_double_mlp_train_step_padded(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                                     long long* step_counter, const float* x, int groups, int rows_per_group,
+                                     const int* n_rows, const float* y, const unsigned char* y_valid, float* cg_mean,
+                                     float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
+                                     void* stream);
+int wvn_double_mlp_trainer_init_comm(wvn_double_mlp_trainer_t* t, const void* id128, int rank, int world);
+/* The trainer's statistics block (device, 9 doubles): sum and sum of squares of loss_reco over the labelled rows, sum of
+ * (trav - y)^2, labelled and live row counts, 0, loss_reco's min and max, the confidence-weighted traversability error
+ * summed over the live rows.  Valid until the trainer is destroyed. */
+double* wvn_double_mlp_trainer_stats(wvn_double_mlp_trainer_t* t);
 
 /* ------------------------------------------------------------------------------------------
  * LinearRnvp anomaly-detection learner (model/linear_rnvp.py, fp32): LinearRnvp(dim, [hidden]) with flow_n = 2,
@@ -523,6 +546,22 @@ int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp
                         const wvn_flow_buffers* buffers, const float* x, int rows, const unsigned char* y_valid,
                         float* cg_mean, float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
                         void* stream);
+/* The same step on rows padded per group, data-parallel.  x: [groups, rows_per_group, dim] fp32; n_rows: [groups] int32
+ * (device) live rows per group, or NULL; y_valid (NULL: all) is indexed by the COMPACTED row number and selects the
+ * rows trained on; confidence_out: the selected rows in order.  Padding rows are never read.  phase_mask: 7 = whole step;
+ * 1 = forward + the NLL sums, 2 = generator update + metrics + confidence + backward, 4 = Adam (note: phase 1 here
+ * stops BEFORE the generator update, which needs the global sums).  With a communicator (wvn_flow_init_comm) the step
+ * all-reduces itself; without one a data-parallel caller all-reduces the statistics block (wvn_flow_stats) — doubles
+ * 0..5 with SUM, and for moving_average 6 with MIN and 7 with MAX — after phase 1 and the gradient after phase 2.
+ * The loss is the NLL's mean over the global labelled count; a rank with no labelled row still takes part. */
+int wvn_flow_train_step_padded(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                               const wvn_flow_buffers* buffers, const float* x, int groups, int rows_per_group,
+                               const int* n_rows, const unsigned char* y_valid, float* cg_mean, float* cg_std,
+                               float* confidence_out, float* metrics_out, int phase_mask, void* stream);
+int wvn_flow_init_comm(wvn_flow_t* h, const void* id128, int rank, int world);
+/* The handle's statistics block (device, 8 doubles): sum and sum of squares of the NLL over the labelled rows, their
+ * number, 0, 0, 0, the NLL's min and max.  Valid until the handle is destroyed. */
+double* wvn_flow_stats(wvn_flow_t* h);
 
 /* Inference handle (no backward workspaces, no gradient buffer).  max_rows: rows of wvn_flow_infer_rows per call;
  * chunk_pixels: pixels per wgmma chunk of wvn_flow_infer_pixels (0 = 8192). */

@@ -120,7 +120,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 105; }
+int wvn_version(void) { return 106; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -1340,11 +1340,11 @@ void wvn_mlp_trainer_destroy(wvn_mlp_trainer_t* t) {
   delete t;
 }
 
-int wvn_comm_unique_id(void* id128) { return fused_comm_unique_id(id128); }
+int wvn_comm_unique_id(void* id128) { return comm_unique_id(id128); }
 
 int wvn_mlp_trainer_init_comm(wvn_mlp_trainer_t* t, const void* id128, int rank, int world) {
   WVN_REQUIRE(t, "wvn_mlp_trainer_init_comm: null trainer");
-  return fused_trainer_init_comm(t->impl, id128, rank, world);
+  return trainer_comm_init(fused_trainer_comm(t->impl), id128, rank, world);
 }
 
 int wvn_mlp_trainer_set_confidence(wvn_mlp_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
@@ -1429,6 +1429,23 @@ int wvn_double_mlp_train_step(wvn_double_mlp_trainer_t* t, float* params, float*
                            confidence_out, metrics_out, S(stream));
 }
 
+int wvn_double_mlp_trainer_init_comm(wvn_double_mlp_trainer_t* t, const void* id128, int rank, int world) {
+  WVN_REQUIRE(t, "wvn_double_mlp_trainer_init_comm: null trainer");
+  return trainer_comm_init(double_trainer_comm(t->impl), id128, rank, world);
+}
+
+double* wvn_double_mlp_trainer_stats(wvn_double_mlp_trainer_t* t) { return t ? double_trainer_stats(t->impl) : nullptr; }
+
+int wvn_double_mlp_train_step_padded(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                                     long long* step_counter, const float* x, int groups, int rows_per_group,
+                                     const int* n_rows, const float* y, const unsigned char* y_valid, float* cg_mean,
+                                     float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
+                                     void* stream) {
+  WVN_REQUIRE(t, "wvn_double_mlp_train_step_padded: null trainer");
+  return double_train_step_padded(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows,
+                                  y, y_valid, cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
+}
+
 }  // extern "C"
 
 // ============================================================================================
@@ -1502,6 +1519,23 @@ int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp
   WVN_REQUIRE(h && buffers, "wvn_flow_train_step: null argument");
   return flow_train_step(h->impl, params, exp_avg, exp_avg_sq, step_counter, buffers_of(buffers), x, rows, y_valid,
                          cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
+}
+
+int wvn_flow_init_comm(wvn_flow_t* h, const void* id128, int rank, int world) {
+  WVN_REQUIRE(h, "wvn_flow_init_comm: null handle");
+  return trainer_comm_init(flow_trainer_comm(h->impl), id128, rank, world);
+}
+
+double* wvn_flow_stats(wvn_flow_t* h) { return h ? flow_trainer_stats(h->impl) : nullptr; }
+
+int wvn_flow_train_step_padded(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                               const wvn_flow_buffers* buffers, const float* x, int groups, int rows_per_group,
+                               const int* n_rows, const unsigned char* y_valid, float* cg_mean, float* cg_std,
+                               float* confidence_out, float* metrics_out, int phase_mask, void* stream) {
+  WVN_REQUIRE(h && buffers, "wvn_flow_train_step_padded: null argument");
+  return flow_train_step_padded(h->impl, params, exp_avg, exp_avg_sq, step_counter, buffers_of(buffers), x, groups,
+                                rows_per_group, n_rows, y_valid, cg_mean, cg_std, confidence_out, metrics_out,
+                                phase_mask, S(stream));
 }
 
 int wvn_flow_infer_create(int dim, int hidden, int max_rows, int chunk_pixels, wvn_flow_infer_t** out) {

@@ -4,15 +4,21 @@
 //
 // Two networks read the same rows: net 0 (dim -> h1 -> h2 -> 1, sigmoid) gives traversability, net 1 (dim -> h1 -> h2
 // -> dim) the reconstruction; out = [sigmoid(net0(x)) | net1(x)] has SimpleMLP's (rows, 1 + dim) layout, so the loss,
-// its gradient and the confidence are SimpleMLP's.  The step is one fixed sequence of 12 launches with every scalar on
-// the device (no host synchronisation):
-//   forward: 3 batched GEMMs of two problems each (one per net; bias + ReLU, then layer 3 writes column 0 through the
-//   sigmoid and columns 1..dim) -> per-row loss terms -> statistics + generator update (train_core.cuh) -> dLoss/dOut
-//   and per-row confidence -> 2 batched data-gradient GEMMs (ReLU backward) -> ONE six-problem launch of every weight
-//   and bias gradient -> loss metrics -> Adam (mlp_adam_step).
+// its gradient and the confidence are SimpleMLP's.  The step is one fixed sequence of 15 launches with every scalar on
+// the device (no host synchronisation), in three phases with a data-parallel exchange after the first two:
+//   1: compaction of the padded rows (train_core) -> gather of the live rows -> forward: 3 batched GEMMs of two problems
+//      each (one per net; bias + ReLU, then layer 3 writes column 0 through the sigmoid and columns 1..dim) -> per-row
+//      loss terms -> this rank's statistic sums and loss_reco's extrema      [SUM of the sums, MIN / MAX of the extrema]
+//   2: generator update (train_core.cuh) -> dLoss/dOut with the global row counts and per-row confidence -> 2 batched
+//      data-gradient GEMMs (ReLU backward) -> ONE six-problem launch of every weight and bias gradient -> this rank's
+//      confidence-weighted traversability error                             [SUM of the gradient and that error]
+//   4: loss metrics from the global sums -> Adam (mlp_adam_step).
+// Every launch after the compaction is bounded by the device count of live rows, so a padded batch and the same rows
+// compacted run the same arithmetic.
 // Training batches are small (~8 nodes x ~100 segments), so the step is latency-bound: the GEMMs are the training core's
 // fp32 CUDA-core tiles, every output element and every sum is formed by one thread (or one fixed reduction tree) in a
 // fixed order, with no atomics: two runs of the same step are bit-identical.
+#include <stddef.h>
 #include <string.h>
 
 #include <algorithm>
@@ -29,21 +35,38 @@ namespace {
 constexpr int kRowThreads = 256;    // one warp per row
 constexpr int kStatThreads = 256;   // the single-block reductions
 
-// The step's scalars.  The sums are the fused SimpleMLP step's (FusedScalars): over the labelled rows the sum of
-// loss_reco and of its square, over all rows the sum of (trav - y)^2, the two row counts and loss_reco's extrema.
+// The step's scalars.  The first kStatDoubles are the statistics block every trainer exchanges (train_core.h): over
+// the labelled rows the sum of loss_reco and of its square, over the live rows the sum of (trav - y)^2, the two row
+// counts, then loss_reco's extrema.  trav_w: the confidence-weighted traversability error summed over the live rows.
 struct DoubleScalars {
-  double sum_lr, sum_lr2, sum_raw, n_valid, n_rows, x_min, x_max;
+  double sum_lr, sum_lr2, sum_raw, n_valid, n_rows, reserved, x_min, x_max;
+  double trav_w;
   float lo, hi, cmin, cmax, g_reco, g_trav;   // the updated generator and the loss-gradient scales
   float mean, std;
 };
+static_assert(offsetof(DoubleScalars, x_min) == kStatSums * sizeof(double) &&
+              offsetof(DoubleScalars, trav_w) == kStatDoubles * sizeof(double), "statistics block layout");
+
+// xg[i] = x[comp[i]]: the live rows, compacted (one warp per row)
+__global__ void __launch_bounds__(kRowThreads)
+double_gather_kernel(const float* __restrict__ x, const int* __restrict__ comp, const int* __restrict__ n_live, int dim,
+                     float* __restrict__ xg) {
+  const int lane = threadIdx.x & 31;
+  const int r = (blockIdx.x * kRowThreads + threadIdx.x) >> 5;
+  if (r >= *n_live) return;
+  const float* src = x + static_cast<long long>(comp[r]) * dim;
+  float* dst = xg + static_cast<long long>(r) * dim;
+  for (int d = lane; d < dim; d += 32) dst[d] = src[d];
+}
 
 // loss_reco[r] = mean_d (out[r, 1 + d] - x[r, d])^2,  raw[r] = (out[r, 0] - y[r])^2
 __global__ void __launch_bounds__(kRowThreads)
 double_loss_rows_kernel(const float* __restrict__ out, const float* __restrict__ x, const float* __restrict__ y,
-                        float* __restrict__ loss_reco, float* __restrict__ raw, int rows, int dim) {
+                        float* __restrict__ loss_reco, float* __restrict__ raw, const int* __restrict__ n_live,
+                        int dim) {
   const int lane = threadIdx.x & 31;
   const int r = (blockIdx.x * kRowThreads + threadIdx.x) >> 5;
-  if (r >= rows) return;
+  if (r >= *n_live) return;
   const float* o = out + static_cast<long long>(r) * (dim + 1);
   const float* xr = x + static_cast<long long>(r) * dim;
   float acc = 0.f;
@@ -59,16 +82,16 @@ double_loss_rows_kernel(const float* __restrict__ out, const float* __restrict__
   }
 }
 
-// One block: the statistic sums in fp64 (fixed reduction order), then one thread updates the ConfidenceGenerator.
-// loss_reco's extrema (moving_average's clip) skip NaN rows (fminf / fmaxf).  The fused SimpleMLP step skips them too,
-// except that a 32-row tile whose every live row is NaN makes its x_max NaN (mlp_train_fused.cu, atomicMax on the bits).
+// One block: this rank's statistic sums in fp64 (fixed reduction order) and loss_reco's extrema.  The extrema skip NaN
+// rows (fminf / fmaxf).  The fused SimpleMLP step skips them too, except that a 32-row tile whose every live row is NaN
+// makes its x_max NaN (mlp_train_fused.cu, atomicMax on the bits).
 __global__ void __launch_bounds__(kStatThreads, 1)
 double_stats_kernel(const float* __restrict__ loss_reco, const float* __restrict__ raw,
-                    const unsigned char* __restrict__ y_valid, int rows, int dim, LossCfg cfg, ConfState cs,
-                    float* __restrict__ cg_mean, float* __restrict__ cg_std, DoubleScalars* __restrict__ sc) {
+                    const unsigned char* __restrict__ y_valid, const int* __restrict__ n_live,
+                    DoubleScalars* __restrict__ sc) {
   __shared__ double red[4][kStatThreads / 32];
   __shared__ float rmin[kStatThreads / 32], rmax[kStatThreads / 32];
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int rows = *n_live, t = threadIdx.x, lane = t & 31, warp = t >> 5;
   double s1 = 0.0, s2 = 0.0, sraw = 0.0, nv = 0.0;
   float mn = INFINITY, mx = 0.f;
   for (int i = t; i < rows; i += kStatThreads) {
@@ -96,13 +119,22 @@ double_stats_kernel(const float* __restrict__ loss_reco, const float* __restrict
     S1 += red[0][w]; S2 += red[1][w]; SR += red[2][w]; NV += red[3][w];
     MN = fminf(MN, rmin[w]); MX = fmaxf(MX, rmax[w]);
   }
-  const double NR = static_cast<double>(rows);
-  sc->sum_lr = S1; sc->sum_lr2 = S2; sc->sum_raw = SR; sc->n_valid = NV; sc->n_rows = NR;
+  sc->sum_lr = S1; sc->sum_lr2 = S2; sc->sum_raw = SR; sc->n_valid = NV; sc->n_rows = static_cast<double>(rows);
+  sc->reserved = 0.0;
   sc->x_min = MN; sc->x_max = MX;
-  const ConfUpdate u = conf_generator_update(cs, cfg.std_factor, NV, S1, S2, MN, MX, cg_mean);
+}
+
+// One thread: the ConfidenceGenerator update from the (all-reduced) sums, and the loss-gradient scales over the global
+// row counts.
+__global__ void double_conf_kernel(int dim, LossCfg cfg, ConfState cs, float* __restrict__ cg_mean,
+                                   float* __restrict__ cg_std, DoubleScalars* __restrict__ sc) {
+  if (threadIdx.x != 0) return;
+  const double NV = sc->n_valid;
+  const ConfUpdate u = conf_generator_update(cs, cfg.std_factor, NV, sc->sum_lr, sc->sum_lr2, sc->x_min, sc->x_max,
+                                             cg_mean);
   sc->lo = u.lo; sc->hi = u.hi; sc->cmin = u.cmin; sc->cmax = u.cmax;
   sc->g_reco = cfg.w_reco * 2.f / (static_cast<float>(NV) * static_cast<float>(dim));
-  sc->g_trav = cfg.w_trav * 2.f / static_cast<float>(NR);
+  sc->g_trav = cfg.w_trav * 2.f / static_cast<float>(sc->n_rows);
   sc->mean = u.mean;
   sc->std = u.std;
   if (cg_mean) *cg_mean = u.mean;
@@ -115,11 +147,11 @@ __global__ void __launch_bounds__(kRowThreads)
 double_dout_kernel(const float* __restrict__ out, const float* __restrict__ x, const float* __restrict__ y,
                    const unsigned char* __restrict__ y_valid, const float* __restrict__ loss_reco,
                    const float* __restrict__ raw, const DoubleScalars* __restrict__ sc, LossCfg cfg, int method,
-                   float* __restrict__ d_out, float* __restrict__ conf_out, float* __restrict__ wraw, int rows,
-                   int dim) {
+                   float* __restrict__ d_out, float* __restrict__ conf_out, float* __restrict__ wraw,
+                   const int* __restrict__ n_live, int dim) {
   const int lane = threadIdx.x & 31;
   const int r = (blockIdx.x * kRowThreads + threadIdx.x) >> 5;
-  if (r >= rows) return;
+  if (r >= *n_live) return;
   const float lo = sc->lo, hi = sc->hi, cmin = sc->cmin, cmax = sc->cmax, g_reco = sc->g_reco, g_trav = sc->g_trav;
   const bool v = y_valid[r] != 0;
   const float conf = row_confidence(method, loss_reco[r], lo, hi, cmin, cmax);
@@ -136,23 +168,28 @@ double_dout_kernel(const float* __restrict__ out, const float* __restrict__ x, c
   }
 }
 
-// Loss metrics (one block, fixed reduction order); leaves them in metrics[6] for the host.
+// This rank's confidence-weighted traversability error sum (one block, fixed reduction order).
 __global__ void __launch_bounds__(kStatThreads, 1)
-double_finish_kernel(const float* __restrict__ wraw, int rows, LossCfg cfg, const DoubleScalars* __restrict__ sc,
-                     float* __restrict__ metrics) {
+double_trav_w_kernel(const float* __restrict__ wraw, const int* __restrict__ n_live, DoubleScalars* __restrict__ sc) {
   __shared__ double red[kStatThreads / 32];
-  const int t = threadIdx.x;
+  const int rows = *n_live, t = threadIdx.x;
   double s = 0.0;
   for (int i = t; i < rows; i += kStatThreads) s += static_cast<double>(wraw[i]);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if ((t & 31) == 0) red[t >> 5] = s;
   __syncthreads();
-  if (t != 0 || metrics == nullptr) return;
+  if (t != 0) return;
   double S = 0.0;
   for (int w = 0; w < kStatThreads / 32; ++w) S += red[w];
+  sc->trav_w = S;
+}
+
+// Loss metrics from the global sums; leaves them in metrics[6] for the host.
+__global__ void double_finish_kernel(LossCfg cfg, const DoubleScalars* __restrict__ sc, float* __restrict__ metrics) {
+  if (threadIdx.x != 0) return;
   const float loss_reco = static_cast<float>(sc->sum_lr / sc->n_valid);
-  const float loss_trav_conf = static_cast<float>(S / sc->n_rows);
+  const float loss_trav_conf = static_cast<float>(sc->trav_w / sc->n_rows);
   metrics[0] = cfg.w_trav * loss_trav_conf + cfg.w_reco * loss_reco;
   metrics[1] = static_cast<float>(sc->sum_raw / sc->n_rows);
   metrics[2] = loss_reco;
@@ -192,27 +229,29 @@ int double_mlp_check_shape(const MlpShape& s, const char* who) {
 
 namespace {
 
-// The three forward launches; a1 / a2 hold net 0's block, then net 1's, `pitch` rows apart.
+// The three forward launches; a1 / a2 hold net 0's block, then net 1's, `pitch` rows apart.  n_live (device, may be
+// NULL): only the first *n_live of the `rows` rows are computed.
 int forward_gemms(const MlpShape& s, const DoubleOffsets& o, const float* params, const float* x, int rows, long long pitch,
-                  float* a1, float* a2, float* out, cudaStream_t stream) {
-  const int D = s.dim, h1 = s.h1, h2 = s.h2;
+                  float* a1, float* a2, float* out, const int* n_live, cudaStream_t stream) {
+  const int D = s.dim, h1 = s.h1, h2 = s.h2, live = n_live ? 1 : 0;
   GemmProblem ps[2];
   for (int k = 0; k < 2; ++k) {   // a1_k = ReLU(x W1_k^T + b1_k)
-    ps[k] = gemm_problem(x, D, 1, params + o.w1[k], 1, D, a1 + k * pitch * h1, h1, rows, h1, D);
+    ps[k] = gemm_problem(x, D, 1, params + o.w1[k], 1, D, a1 + k * pitch * h1, h1, rows, h1, D, live);
     ps[k].bias = params + o.b1[k]; ps[k].act = F32_RELU_FMAX;
   }
-  WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
+  WVN_PROPAGATE(launch_gemms(ps, 2, n_live, stream));
   for (int k = 0; k < 2; ++k) {   // a2_k = ReLU(a1_k W2_k^T + b2_k)
-    ps[k] = gemm_problem(a1 + k * pitch * h1, h1, 1, params + o.w2[k], 1, h1, a2 + k * pitch * h2, h2, rows, h2, h1);
+    ps[k] = gemm_problem(a1 + k * pitch * h1, h1, 1, params + o.w2[k], 1, h1, a2 + k * pitch * h2, h2, rows, h2, h1,
+                         live);
     ps[k].bias = params + o.b2[k]; ps[k].act = F32_RELU_FMAX;
   }
-  WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
+  WVN_PROPAGATE(launch_gemms(ps, 2, n_live, stream));
   // column 0 = sigmoid(a2_0 w3_0 + b3_0), columns 1..dim = a2_1 W3_1^T + b3_1
-  ps[0] = gemm_problem(a2, h2, 1, params + o.w3[0], 1, h2, out, D + 1, rows, 1, h2);
+  ps[0] = gemm_problem(a2, h2, 1, params + o.w3[0], 1, h2, out, D + 1, rows, 1, h2, live);
   ps[0].bias = params + o.b3[0]; ps[0].act = F32_SIGMOID_COL0;
-  ps[1] = gemm_problem(a2 + pitch * h2, h2, 1, params + o.w3[1], 1, h2, out + 1, D + 1, rows, D, h2);
+  ps[1] = gemm_problem(a2 + pitch * h2, h2, 1, params + o.w3[1], 1, h2, out + 1, D + 1, rows, D, h2, live);
   ps[1].bias = params + o.b3[1];
-  return launch_gemms(ps, 2, nullptr, stream);
+  return launch_gemms(ps, 2, n_live, stream);
 }
 
 }  // namespace
@@ -221,7 +260,7 @@ int double_mlp_forward_f32(const MlpShape& s, const float* params, const float* 
                            float* out, cudaStream_t stream) {
   WVN_PROPAGATE(double_mlp_check_shape(s, "double mlp forward"));
   WVN_REQUIRE(params && x && a1 && a2 && out && rows > 0, "double mlp forward: bad argument");
-  return forward_gemms(s, double_mlp_offsets(s), params, x, rows, rows, a1, a2, out, stream);
+  return forward_gemms(s, double_mlp_offsets(s), params, x, rows, rows, a1, a2, out, nullptr, stream);
 }
 
 struct DoubleTrainer {
@@ -232,9 +271,12 @@ struct DoubleTrainer {
   int max_rows = 0;
   void* arena = nullptr;
   DoubleScalars* sc = nullptr;
-  float *a1 = nullptr, *a2 = nullptr, *out = nullptr, *d_out = nullptr, *d2 = nullptr, *d1 = nullptr;
+  int* comp = nullptr;     // compacted -> padded row map
+  int* n_live = nullptr;   // this rank's live rows (device)
+  float *xg = nullptr, *a1 = nullptr, *a2 = nullptr, *out = nullptr, *d_out = nullptr, *d2 = nullptr, *d1 = nullptr;
   float *loss_reco = nullptr, *raw = nullptr, *wraw = nullptr, *grads = nullptr;
   TrainerConf conf;
+  TrainerComm comm;
 };
 
 int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, float* grads_ext,
@@ -245,9 +287,9 @@ int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, 
   t->s = s; t->o = double_mlp_offsets(s); t->loss = loss; t->adam = adam;
   t->max_rows = max_rows;
   const size_t R = max_rows, D = s.dim, h1 = s.h1, h2 = s.h2;
-  // a1 / d1 [2][R, h1], a2 / d2 [2][R, h2], out / d_out [R, 1 + D], loss_reco / raw / wraw [R], grads
-  const size_t floats = 2 * (2 * R * h1 + 2 * R * h2 + R * (D + 1)) + 3 * R + (grads_ext ? 0 : t->o.total);
-  const size_t head = 256;
+  // xg [R, D], a1 / d1 [2][R, h1], a2 / d2 [2][R, h2], out / d_out [R, 1 + D], loss_reco / raw / wraw [R], grads
+  const size_t floats = R * D + 2 * (2 * R * h1 + 2 * R * h2 + R * (D + 1)) + 3 * R + (grads_ext ? 0 : t->o.total);
+  const size_t head = 256 + (R * sizeof(int) + 255) / 256 * 256;   // scalars | n_live at 128 | comp at 256
   const size_t bytes = head + floats * sizeof(float);
   if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
     delete t;
@@ -265,10 +307,14 @@ int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, 
     delete t;
     return set_error(WVN_ERR_CUDA, "double mlp trainer: cudaMemset of %zu bytes failed", bytes);
   }
+  static_assert(sizeof(DoubleScalars) <= 128, "scalars overlap n_live");
   char* base = reinterpret_cast<char*>(t->arena);
   t->sc = reinterpret_cast<DoubleScalars*>(base);
+  t->n_live = reinterpret_cast<int*>(base + 128);
+  t->comp = reinterpret_cast<int*>(base + 256);
   float* f = reinterpret_cast<float*>(base + head);
   auto take = [&](size_t n) { float* p = f; f += n; return p; };
+  t->xg = take(R * D);
   t->a1 = take(2 * R * h1);
   t->d1 = take(2 * R * h1);
   t->a2 = take(2 * R * h2);
@@ -285,67 +331,96 @@ int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, 
 
 void double_trainer_destroy(DoubleTrainer* t) {
   if (!t) return;
+  trainer_comm_destroy(&t->comm);
   if (t->arena) cudaFree(t->arena);
   trainer_conf_destroy(&t->conf);
   delete t;
 }
 
 TrainerConf* double_trainer_conf(DoubleTrainer* t) { return &t->conf; }
+TrainerComm* double_trainer_comm(DoubleTrainer* t) { return &t->comm; }
+double* double_trainer_stats(DoubleTrainer* t) { return &t->sc->sum_lr; }
+
+int double_train_step_padded(DoubleTrainer* t, float* params, float* exp_avg, float* exp_avg_sq,
+                             long long* step_counter, const float* x, int groups, int rows_per_group,
+                             const int* n_rows, const float* y, const unsigned char* y_valid, float* cg_mean,
+                             float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream) {
+  WVN_REQUIRE(t && params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
+              "double mlp train step: null argument");
+  const long long cap = static_cast<long long>(groups) * rows_per_group;
+  WVN_REQUIRE(groups > 0 && rows_per_group > 0 && cap <= t->max_rows,
+              "double mlp train step: %d x %d rows outside (0, %d]", groups, rows_per_group, t->max_rows);
+  const MlpShape& s = t->s;
+  const DoubleOffsets& o = t->o;
+  const int D = s.dim, h1 = s.h1, h2 = s.h2, n3 = D + 1, rows = static_cast<int>(cap);
+  const long long R = t->max_rows;   // the per-net blocks of a1 / a2 / d1 / d2 are max_rows rows apart
+  const int row_blocks = (rows * 32 + kRowThreads - 1) / kRowThreads;
+  // every row loop, GEMM and reduction below is bounded by the device count *n_live: padding rows are never read
+  if (phase_mask & 1) {   // live rows -> forward -> per-row loss terms -> this rank's statistic sums (-> all-reduce)
+    WVN_PROPAGATE(compact_rows(groups, rows_per_group, n_rows, nullptr, t->comp, t->n_live, stream));
+    double_gather_kernel<<<row_blocks, kRowThreads, 0, stream>>>(x, t->comp, t->n_live, D, t->xg);
+    WVN_CHECK_LAUNCH("double_gather_kernel");
+    WVN_PROPAGATE(forward_gemms(s, o, params, t->xg, rows, R, t->a1, t->a2, t->out, t->n_live, stream));
+    double_loss_rows_kernel<<<row_blocks, kRowThreads, 0, stream>>>(t->out, t->xg, y, t->loss_reco, t->raw, t->n_live, D);
+    WVN_CHECK_LAUNCH("double_loss_rows_kernel");
+    double_stats_kernel<<<1, kStatThreads, 0, stream>>>(t->loss_reco, t->raw, y_valid, t->n_live, t->sc);
+    WVN_CHECK_LAUNCH("double_stats_kernel");
+    WVN_PROPAGATE(trainer_comm_stats(&t->comm, &t->sc->sum_lr, t->conf.cs.method == CONF_MOVING_AVERAGE, stream));
+  }
+  if (phase_mask & 2) {   // generator update -> dLoss/dOut + confidence -> backward -> gradients (-> all-reduce)
+    double_conf_kernel<<<1, 32, 0, stream>>>(D, t->loss, t->conf.cs, cg_mean, cg_std, t->sc);
+    WVN_CHECK_LAUNCH("double_conf_kernel");
+    double_dout_kernel<<<row_blocks, kRowThreads, 0, stream>>>(t->out, t->xg, y, y_valid, t->loss_reco, t->raw, t->sc,
+                                                               t->loss, t->conf.cs.method, t->d_out, conf_out, t->wraw,
+                                                               t->n_live, D);
+    WVN_CHECK_LAUNCH("double_dout_kernel");
+    // data gradients: d2_k = (dOut_k W3_k) * (a2_k > 0), d1_k = (d2_k W2_k) * (a1_k > 0)
+    GemmProblem ps[2];
+    ps[0] = gemm_problem(t->d_out, n3, 1, params + o.w3[0], h2, 1, t->d2, h2, rows, h2, 1, 1);
+    ps[1] = gemm_problem(t->d_out + 1, n3, 1, params + o.w3[1], h2, 1, t->d2 + R * h2, h2, rows, h2, D, 1);
+    for (int k = 0; k < 2; ++k) { ps[k].ref = t->a2 + k * R * h2; ps[k].ld_ref = h2; }
+    WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
+    for (int k = 0; k < 2; ++k) {
+      ps[k] = gemm_problem(t->d2 + k * R * h2, h2, 1, params + o.w2[k], h1, 1, t->d1 + k * R * h1, h1, rows, h1, h2, 1);
+      ps[k].ref = t->a1 + k * R * h1; ps[k].ld_ref = h1;
+    }
+    WVN_PROPAGATE(launch_gemms(ps, 2, t->n_live, stream));
+    // every weight gradient dW = dZ^T A and bias gradient db = column sums of dZ: one launch of six problems, the row
+    // reduction (K) bounded by *n_live (a rank without live rows contributes zeros)
+    GemmProblem wg[6];
+    wg[0] = gemm_problem(t->d_out, 1, n3, t->a2, h2, 1, t->grads + o.w3[0], h2, 1, h2, rows, 2);
+    wg[0].db = t->grads + o.b3[0];
+    wg[1] = gemm_problem(t->d_out + 1, 1, n3, t->a2 + R * h2, h2, 1, t->grads + o.w3[1], h2, D, h2, rows, 2);
+    wg[1].db = t->grads + o.b3[1];
+    for (int k = 0; k < 2; ++k) {
+      wg[2 + k] = gemm_problem(t->d2 + k * R * h2, 1, h2, t->a1 + k * R * h1, h1, 1, t->grads + o.w2[k], h1, h2, h1, rows,
+                               2);
+      wg[2 + k].db = t->grads + o.b2[k];
+      wg[4 + k] = gemm_problem(t->d1 + k * R * h1, 1, h1, t->xg, D, 1, t->grads + o.w1[k], D, h1, D, rows, 2);
+      wg[4 + k].db = t->grads + o.b1[k];
+    }
+    WVN_PROPAGATE(launch_gemms(wg, 6, t->n_live, stream));
+    double_trav_w_kernel<<<1, kStatThreads, 0, stream>>>(t->wraw, t->n_live, t->sc);
+    WVN_CHECK_LAUNCH("double_trav_w_kernel");
+    WVN_PROPAGATE(trainer_comm_sum(&t->comm, t->grads, o.total, false, stream));
+    WVN_PROPAGATE(trainer_comm_sum(&t->comm, &t->sc->trav_w, 1, true, stream));
+  }
+  if (phase_mask & 4) {   // loss metrics from the global sums, then Adam
+    if (metrics) {
+      double_finish_kernel<<<1, 32, 0, stream>>>(t->loss, t->sc, metrics);
+      WVN_CHECK_LAUNCH("double_finish_kernel");
+    }
+    WVN_PROPAGATE(mlp_adam_step(params, t->grads, exp_avg, exp_avg_sq, static_cast<long long>(o.total), t->adam,
+                                step_counter, stream));
+  }
+  return WVN_OK;
+}
 
 int double_train_step(DoubleTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                       const float* x, int rows, const float* y, const unsigned char* y_valid, float* cg_mean,
                       float* cg_std, float* conf_out, float* metrics, cudaStream_t stream) {
-  WVN_REQUIRE(t && params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
-              "double mlp train step: null argument");
-  WVN_REQUIRE(rows > 0 && rows <= t->max_rows, "double mlp train step: rows=%d outside (0, %d]", rows, t->max_rows);
-  const MlpShape& s = t->s;
-  const DoubleOffsets& o = t->o;
-  const int D = s.dim, h1 = s.h1, h2 = s.h2, n3 = D + 1;
-  const long long R = t->max_rows;   // the per-net blocks of a1 / a2 / d1 / d2 are max_rows rows apart
-  WVN_PROPAGATE(forward_gemms(s, o, params, x, rows, R, t->a1, t->a2, t->out, stream));
-  // ---- loss terms, statistics + generator update, dLoss/dOut + confidence
-  const int row_blocks = (rows * 32 + kRowThreads - 1) / kRowThreads;
-  double_loss_rows_kernel<<<row_blocks, kRowThreads, 0, stream>>>(t->out, x, y, t->loss_reco, t->raw, rows, D);
-  WVN_CHECK_LAUNCH("double_loss_rows_kernel");
-  double_stats_kernel<<<1, kStatThreads, 0, stream>>>(t->loss_reco, t->raw, y_valid, rows, D, t->loss, t->conf.cs,
-                                                      cg_mean, cg_std, t->sc);
-  WVN_CHECK_LAUNCH("double_stats_kernel");
-  double_dout_kernel<<<row_blocks, kRowThreads, 0, stream>>>(t->out, x, y, y_valid, t->loss_reco, t->raw, t->sc, t->loss,
-                                                             t->conf.cs.method, t->d_out, conf_out, t->wraw, rows, D);
-  WVN_CHECK_LAUNCH("double_dout_kernel");
-  // ---- data gradients: d2_k = (dOut_k W3_k) * (a2_k > 0), d1_k = (d2_k W2_k) * (a1_k > 0)
-  {
-    GemmProblem ps[2];
-    ps[0] = gemm_problem(t->d_out, n3, 1, params + o.w3[0], h2, 1, t->d2, h2, rows, h2, 1);
-    ps[1] = gemm_problem(t->d_out + 1, n3, 1, params + o.w3[1], h2, 1, t->d2 + R * h2, h2, rows, h2, D);
-    for (int k = 0; k < 2; ++k) { ps[k].ref = t->a2 + k * R * h2; ps[k].ld_ref = h2; }
-    WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
-    for (int k = 0; k < 2; ++k) {
-      ps[k] = gemm_problem(t->d2 + k * R * h2, h2, 1, params + o.w2[k], h1, 1, t->d1 + k * R * h1, h1, rows, h1, h2);
-      ps[k].ref = t->a1 + k * R * h1; ps[k].ld_ref = h1;
-    }
-    WVN_PROPAGATE(launch_gemms(ps, 2, nullptr, stream));
-  }
-  // ---- every weight gradient dW = dZ^T A and bias gradient db = column sums of dZ: one launch of six problems
-  {
-    GemmProblem wg[6];
-    wg[0] = gemm_problem(t->d_out, 1, n3, t->a2, h2, 1, t->grads + o.w3[0], h2, 1, h2, rows);
-    wg[0].db = t->grads + o.b3[0];
-    wg[1] = gemm_problem(t->d_out + 1, 1, n3, t->a2 + R * h2, h2, 1, t->grads + o.w3[1], h2, D, h2, rows);
-    wg[1].db = t->grads + o.b3[1];
-    for (int k = 0; k < 2; ++k) {
-      wg[2 + k] = gemm_problem(t->d2 + k * R * h2, 1, h2, t->a1 + k * R * h1, h1, 1, t->grads + o.w2[k], h1, h2, h1, rows);
-      wg[2 + k].db = t->grads + o.b2[k];
-      wg[4 + k] = gemm_problem(t->d1 + k * R * h1, 1, h1, x, D, 1, t->grads + o.w1[k], D, h1, D, rows);
-      wg[4 + k].db = t->grads + o.b1[k];
-    }
-    WVN_PROPAGATE(launch_gemms(wg, 6, nullptr, stream));
-  }
-  // ---- loss metrics, then Adam
-  double_finish_kernel<<<1, kStatThreads, 0, stream>>>(t->wraw, rows, t->loss, t->sc, metrics);
-  WVN_CHECK_LAUNCH("double_finish_kernel");
-  return mlp_adam_step(params, t->grads, exp_avg, exp_avg_sq, static_cast<long long>(o.total), t->adam, step_counter,
-                       stream);
+  return double_train_step_padded(t, params, exp_avg, exp_avg_sq, step_counter, x, 1, rows, nullptr, y, y_valid, cg_mean,
+                                  cg_std, conf_out, metrics, 7, stream);
 }
 
 }  // namespace wvn

@@ -7,10 +7,12 @@
 // Loss: NLL_r = -(sum_j log N(z_rj; 0, 1) + log_det_r), loss = mean_r NLL_r; the ConfidenceGenerator is updated with
 // x = x_positive = NLL over the (labelled) rows of the batch.
 //
-// The step is one fixed sequence of ~24 launches with every scalar on the device (no host synchronisation):
-//   compact (labelled rows from y_valid) -> gather -> per coupling 3 batched GEMMs (s | t) + the coupling kernel
-//   -> NLL statistics + confidence update (train_core.cuh) + per-row confidence -> per coupling (last first): dx / ds / dt, 2-3 batched
-//   data-gradient GEMMs, du -> one batched launch of all 12 weight-gradient products (+ bias gradients) -> Adam
+// The step is one fixed sequence of ~25 launches with every scalar on the device (no host synchronisation):
+//   compact (the live rows of padded groups whose y_valid is set, train_core) -> gather -> per coupling 3 batched GEMMs
+//   (s | t) + the coupling kernel -> NLL sums [data-parallel: all-reduced] -> confidence update (train_core.cuh) +
+//   per-row confidence -> per coupling (last first): dx / ds / dt, 2-3 batched
+//   data-gradient GEMMs, du -> one batched launch of all 12 weight-gradient products (+ bias gradients) [data-parallel:
+//   the gradient all-reduced] -> Adam
 //   (mlp_adam_step).  The GEMMs, Adam and the generator's state are the training core shared with the MLP trainers
 //   (train_core.h / train_core.cuh).
 // Training batches are small (~8 nodes x ~16 labelled segments), so the step is latency-bound: the GEMMs are plain
@@ -18,6 +20,7 @@
 // The weight-gradient columns that see masked-out inputs (mu = 0) and the last-layer rows that feed masked-out outputs
 // ((1 - m) = 0) come out as exact zeros, as in the reference, so Adam leaves those parameters bit-identical.
 #include <cuda_bf16.h>
+#include <stddef.h>
 #include <string.h>
 
 #include <algorithm>
@@ -35,39 +38,6 @@ namespace {
 constexpr float kLogSqrt2Pi = 0.91893853320467274178f;   // math.log(math.sqrt(2 * math.pi)), torch.distributions.Normal
 constexpr int kRowThreads = 128;
 constexpr int kStatThreads = 256;
-
-// ------------------------------------------------------------------------------------------------ row compaction
-// comp[i] = index of the i-th row with y_valid set (y_valid NULL: every row); *n_live = their number.  One block of 1024.
-__global__ void __launch_bounds__(1024)
-flow_compact_kernel(const unsigned char* __restrict__ y_valid, int rows, int* __restrict__ comp, int* __restrict__ n_live) {
-  __shared__ int wsum[32];
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const int per = (rows + 1023) / 1024, b = t * per, e = min(rows, b + per);
-  int c = 0;
-  for (int i = b; i < e; ++i) c += (y_valid == nullptr || y_valid[i] != 0) ? 1 : 0;
-  int v = c;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += u;
-  }
-  if (lane == 31) wsum[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    int w = wsum[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += u;
-    }
-    wsum[lane] = w;
-  }
-  __syncthreads();
-  int pos = v - c + (warp > 0 ? wsum[warp - 1] : 0);
-  for (int i = b; i < e; ++i)
-    if (y_valid == nullptr || y_valid[i] != 0) comp[pos++] = i;
-  if (t == 0) *n_live = wsum[31];
-}
 
 // u0 = x[comp], mu0 = u0 * mask
 __global__ void __launch_bounds__(kRowThreads)
@@ -153,18 +123,19 @@ flow_coupling_fwd_kernel(CouplingFwd c, int dim, const int* __restrict__ n_live)
 }
 
 // ------------------------------------------------------------------------------------------------ statistics + confidence
-// One block of kStatThreads: sums / extrema of the NLL over the live rows; then one thread updates the generator
-// (train_core.cuh) and writes the metrics and the loss gradient scale 1 / n for the backward kernels.
+// The first kStatDoubles are the statistics block every trainer exchanges (train_core.h): the sum of the NLL over the
+// labelled rows, the sum of its squares, their number, then the NLL's extrema.
 struct FlowScalars {
+  double s1, s2, n, reserved[3], x_min, x_max;
   float inv_n;
   float lo, hi, cmin, cmax;   // the updated generator, for the per-row confidence (train_core.cuh)
-  float pad[3];
 };
+static_assert(offsetof(FlowScalars, x_min) == kStatSums * sizeof(double) &&
+              offsetof(FlowScalars, inv_n) == kStatDoubles * sizeof(double), "statistics block layout");
 
+// One block of kStatThreads: this rank's sums / extrema of the NLL over its labelled rows.
 __global__ void __launch_bounds__(kStatThreads, 1)
-flow_stats_kernel(const float* __restrict__ nll, const int* __restrict__ n_live, ConfState cs, float std_factor,
-                  float* __restrict__ cg_mean, float* __restrict__ cg_std, float* __restrict__ metrics,
-                  FlowScalars* __restrict__ sc) {
+flow_sums_kernel(const float* __restrict__ nll, const int* __restrict__ n_live, FlowScalars* __restrict__ sc) {
   __shared__ double r1[kStatThreads / 32], r2[kStatThreads / 32];
   __shared__ float rmin[kStatThreads / 32], rmax[kStatThreads / 32];
   const int n = *n_live, t = threadIdx.x, lane = t & 31, warp = t >> 5;
@@ -187,24 +158,32 @@ flow_stats_kernel(const float* __restrict__ nll, const int* __restrict__ n_live,
   if (lane == 0) { r1[warp] = s1; r2[warp] = s2; rmin[warp] = mn; rmax[warp] = mx; }
   __syncthreads();
   if (t != 0) return;
-  {
-    double S1 = 0.0, S2 = 0.0;
-    float MN = INFINITY, MX = -INFINITY;
-    for (int w = 0; w < kStatThreads / 32; ++w) { S1 += r1[w]; S2 += r2[w]; MN = fminf(MN, rmin[w]); MX = fmaxf(MX, rmax[w]); }
-    const double dn = static_cast<double>(n);
-    const ConfUpdate u = conf_generator_update(cs, std_factor, dn, S1, S2, MN, MX, cg_mean);
-    if (cg_mean) *cg_mean = u.mean;
-    if (cg_std) *cg_std = u.std;
-    sc->lo = u.lo; sc->hi = u.hi; sc->cmin = u.cmin; sc->cmax = u.cmax;
-    sc->inv_n = 1.f / static_cast<float>(n);   // d mean / d NLL_r (n == 0: no row reads it)
-    if (metrics) {
-      metrics[0] = static_cast<float>(S1 / dn);   // loss = -mean(logprob.sum(1) + log_det); NaN for an empty batch
-      metrics[1] = 0.f;                            // AnomalyLoss reports loss_trav = loss_reco = 0
-      metrics[2] = 0.f;
-      metrics[3] = static_cast<float>(n);
-      metrics[4] = u.mean;
-      metrics[5] = u.std;
-    }
+  double S1 = 0.0, S2 = 0.0;
+  float MN = INFINITY, MX = -INFINITY;
+  for (int w = 0; w < kStatThreads / 32; ++w) { S1 += r1[w]; S2 += r2[w]; MN = fminf(MN, rmin[w]); MX = fmaxf(MX, rmax[w]); }
+  sc->s1 = S1; sc->s2 = S2; sc->n = static_cast<double>(n);
+  sc->reserved[0] = sc->reserved[1] = sc->reserved[2] = 0.0;
+  sc->x_min = MN; sc->x_max = MX;
+}
+
+// One thread: the generator update from the (all-reduced) sums, the metrics and the loss gradient scale 1 / n for the
+// backward kernels.
+__global__ void flow_conf_kernel(ConfState cs, float std_factor, float* __restrict__ cg_mean, float* __restrict__ cg_std,
+                                 float* __restrict__ metrics, FlowScalars* __restrict__ sc) {
+  if (threadIdx.x != 0) return;
+  const double S1 = sc->s1, dn = sc->n;
+  const ConfUpdate u = conf_generator_update(cs, std_factor, dn, S1, sc->s2, sc->x_min, sc->x_max, cg_mean);
+  if (cg_mean) *cg_mean = u.mean;
+  if (cg_std) *cg_std = u.std;
+  sc->lo = u.lo; sc->hi = u.hi; sc->cmin = u.cmin; sc->cmax = u.cmax;
+  sc->inv_n = 1.f / static_cast<float>(dn);   // d mean / d NLL_r (n == 0: no row reads it)
+  if (metrics) {
+    metrics[0] = static_cast<float>(S1 / dn);   // loss = -mean(logprob.sum(1) + log_det); NaN for an empty batch
+    metrics[1] = 0.f;                            // AnomalyLoss reports loss_trav = loss_reco = 0
+    metrics[2] = 0.f;
+    metrics[3] = static_cast<float>(dn);
+    metrics[4] = u.mean;
+    metrics[5] = u.std;
   }
 }
 
@@ -300,6 +279,7 @@ struct FlowTrainer {
         *dmu[2] = {nullptr, nullptr}, *du = nullptr;
   bool forward_only = false;   // inference: no backward workspaces, no gradient buffer
   TrainerConf conf;
+  TrainerComm comm;
 };
 
 int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, const AdamCfg& adam, float* grads_ext,
@@ -329,6 +309,7 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
   }
   cudaMemset(t->arena, 0, bytes);
   char* base = reinterpret_cast<char*>(t->arena);
+  static_assert(sizeof(FlowScalars) <= 128, "scalars overlap n_live");
   t->sc = reinterpret_cast<FlowScalars*>(base);
   t->n_live = reinterpret_cast<int*>(base + 128);
   t->comp = reinterpret_cast<int*>(base + 256);
@@ -363,22 +344,25 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
 
 void flow_trainer_destroy(FlowTrainer* t) {
   if (!t) return;
+  trainer_comm_destroy(&t->comm);
   if (t->arena) cudaFree(t->arena);
   trainer_conf_destroy(&t->conf);
   delete t;
 }
 
 TrainerConf* flow_trainer_conf(FlowTrainer* t) { return &t->conf; }
+TrainerComm* flow_trainer_comm(FlowTrainer* t) { return &t->comm; }
+double* flow_trainer_stats(FlowTrainer* t) { return &t->sc->s1; }
 
 namespace {
 
-// compaction + both couplings' forward; the last coupling writes z / logprob / log_det / nll / trav as given
-int flow_forward(FlowTrainer* t, const float* params, const FlowBuffers& b, const float* x, int rows,
-                 const unsigned char* y_valid, float* z, float* logprob, float* ld_out, float* trav, const float* cg_mean,
-                 const float* cg_std, float std_factor, cudaStream_t stream) {
-  const int D = t->s.dim, h = t->s.hidden;
-  flow_compact_kernel<<<1, 1024, 0, stream>>>(y_valid, rows, t->comp, t->n_live);
-  WVN_CHECK_LAUNCH("flow_compact_kernel");
+// compaction of the padded rows (train_core) + both couplings' forward on the kept rows, `rows` = groups * rpg of
+// them at most; the last coupling writes z / logprob / log_det / nll / trav as given
+int flow_forward(FlowTrainer* t, const float* params, const FlowBuffers& b, const float* x, int groups, int rpg,
+                 const int* n_rows, const unsigned char* y_valid, float* z, float* logprob, float* ld_out, float* trav,
+                 const float* cg_mean, const float* cg_std, float std_factor, cudaStream_t stream) {
+  const int D = t->s.dim, h = t->s.hidden, rows = groups * rpg;
+  WVN_PROPAGATE(compact_rows(groups, rpg, n_rows, y_valid, t->comp, t->n_live, stream));
   if (rows == 0) return WVN_OK;
   flow_gather_kernel<<<rows, kRowThreads, 0, stream>>>(x, t->comp, t->n_live, D, b.mask0, t->u[0], t->mu[0]);
   WVN_CHECK_LAUNCH("flow_gather_kernel");
@@ -441,27 +425,42 @@ int flow_forward_rows(FlowTrainer* t, const float* params, const FlowBuffers& b,
                       float* trav, cudaStream_t stream) {
   WVN_PROPAGATE(check_args(t, params, b, x, rows));
   WVN_REQUIRE(!trav || (cg_mean && cg_std), "flow rows: trav needs the generator's mean and std");
-  return flow_forward(t, params, b, x, rows, nullptr, z, logprob, log_det, trav, cg_mean, cg_std, std_factor, stream);
+  return flow_forward(t, params, b, x, 1, rows, nullptr, nullptr, z, logprob, log_det, trav, cg_mean, cg_std, std_factor,
+                      stream);
 }
 
-int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
-                    const FlowBuffers& b, const float* x, int rows, const unsigned char* y_valid, float* cg_mean,
-                    float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream) {
+namespace {
+
+// The stages of a step.  The compacted entry's phase 1 runs kFwd | kGen, the padded entry's phase 2 kGen | kBwd: the
+// statistics exchange sits between kFwd and kGen.
+enum : int { kFwd = 1, kBwd = 2, kAdam = 4, kGen = 8 };
+
+int flow_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+              const FlowBuffers& b, const float* x, int groups, int rpg, const int* n_rows, const unsigned char* y_valid,
+              float* cg_mean, float* cg_std, float* conf_out, float* metrics, int stages, cudaStream_t stream) {
+  WVN_REQUIRE(groups >= 0 && rpg >= 0, "flow train step: %d x %d rows", groups, rpg);
+  const long long cap = static_cast<long long>(groups) * rpg;
+  WVN_REQUIRE(cap <= t->max_rows, "flow: %lld rows exceed the handle's capacity %d", cap, t->max_rows);
+  const int rows = static_cast<int>(cap);
   WVN_PROPAGATE(check_args(t, params, b, x, rows));
   WVN_REQUIRE(exp_avg && exp_avg_sq && step_counter && conf_out, "flow train step: null argument");
   WVN_REQUIRE(!t->forward_only, "flow train step: the handle was created for inference only");
   const int D = t->s.dim, h = t->s.hidden;
   const int R = std::max(rows, 1);
-  if (phase_mask & 1) {
-    WVN_PROPAGATE(flow_forward(t, params, b, x, rows, y_valid, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f,
-                               stream));
-    flow_stats_kernel<<<1, kStatThreads, 0, stream>>>(t->nll, t->n_live, t->conf.cs, t->std_factor, cg_mean, cg_std, metrics,
-                                                      t->sc);
-    WVN_CHECK_LAUNCH("flow_stats_kernel");
+  if (stages & kFwd) {   // kept rows -> forward -> this rank's NLL sums (-> all-reduce)
+    WVN_PROPAGATE(flow_forward(t, params, b, x, groups, rpg, n_rows, y_valid, nullptr, nullptr, nullptr, nullptr, nullptr,
+                               nullptr, 0.f, stream));
+    flow_sums_kernel<<<1, kStatThreads, 0, stream>>>(t->nll, t->n_live, t->sc);
+    WVN_CHECK_LAUNCH("flow_sums_kernel");
+    WVN_PROPAGATE(trainer_comm_stats(&t->comm, &t->sc->s1, t->conf.cs.method == CONF_MOVING_AVERAGE, stream));
+  }
+  if (stages & kGen) {   // generator update from the global sums, metrics, per-row confidence
+    flow_conf_kernel<<<1, 32, 0, stream>>>(t->conf.cs, t->std_factor, cg_mean, cg_std, metrics, t->sc);
+    WVN_CHECK_LAUNCH("flow_conf_kernel");
     flow_conf_rows_kernel<<<(R + 255) / 256, 256, 0, stream>>>(t->nll, t->n_live, t->conf.cs.method, t->sc, conf_out);
     WVN_CHECK_LAUNCH("flow_conf_rows_kernel");
   }
-  if (phase_mask & 2) {
+  if (stages & kBwd) {   // the flat gradient, scaled by 1 / the global labelled count (-> all-reduce)
     // couplings in reverse; coupling 0 needs no input gradient
     for (int c = 1; c >= 0; --c) {
       const float* mask = c == 0 ? b.mask0 : b.mask1;
@@ -506,12 +505,32 @@ int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_av
       }
       WVN_PROPAGATE(launch_gemms(wg, 6, t->n_live, stream));
     }
+    WVN_PROPAGATE(trainer_comm_sum(&t->comm, t->grads, flow_param_count(t->s), false, stream));
   }
-  if (phase_mask & 4) {
+  if (stages & kAdam) {
     WVN_PROPAGATE(mlp_adam_step(params, t->grads, exp_avg, exp_avg_sq, static_cast<long long>(flow_param_count(t->s)),
                                 t->adam, step_counter, stream));
   }
   return WVN_OK;
+}
+
+}  // namespace
+
+int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                    const FlowBuffers& b, const float* x, int rows, const unsigned char* y_valid, float* cg_mean,
+                    float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream) {
+  const int stages = ((phase_mask & 1) ? kFwd | kGen : 0) | (phase_mask & (kBwd | kAdam));
+  return flow_step(t, params, exp_avg, exp_avg_sq, step_counter, b, x, 1, rows, nullptr, y_valid, cg_mean, cg_std,
+                   conf_out, metrics, stages, stream);
+}
+
+int flow_train_step_padded(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                           const FlowBuffers& b, const float* x, int groups, int rows_per_group, const int* n_rows,
+                           const unsigned char* y_valid, float* cg_mean, float* cg_std, float* conf_out, float* metrics,
+                           int phase_mask, cudaStream_t stream) {
+  const int stages = (phase_mask & 1) | ((phase_mask & 2) ? kGen | kBwd : 0) | (phase_mask & kAdam);
+  return flow_step(t, params, exp_avg, exp_avg_sq, step_counter, b, x, groups, rows_per_group, n_rows, y_valid, cg_mean,
+                   cg_std, conf_out, metrics, stages, stream);
 }
 
 // ================================================================================================ per-pixel inference

@@ -42,6 +42,11 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
 void flow_trainer_destroy(FlowTrainer* t);
 // The trainer's ConfidenceGenerator (bound and copied with trainer_conf_bind / trainer_conf_copy).
 TrainerConf* flow_trainer_conf(FlowTrainer* t);
+// The trainer's communicator (set up with trainer_comm_init; none: the exchanges are the caller's).
+TrainerComm* flow_trainer_comm(FlowTrainer* t);
+// The step's statistics block (device, the kStatDoubles of train_core.h): sum and sum of squares of the NLL over the
+// labelled rows, their number, 0, 0, 0, the NLL's min and max.
+double* flow_trainer_stats(FlowTrainer* t);
 
 // LinearRnvp.forward on rows x [rows, dim]: z / logprob [rows, dim], log_det [rows] (each may be NULL); with trav
 // non-NULL also ConfidenceGenerator.inference_without_update of the per-row NLL -(sum(logprob) + log_det) from the
@@ -57,6 +62,15 @@ int flow_forward_rows(FlowTrainer* t, const float* params, const FlowBuffers& b,
 int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                     const FlowBuffers& b, const float* x, int rows, const unsigned char* y_valid, float* cg_mean,
                     float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream);
+// The same step on rows padded per group, x [groups, rows_per_group, dim] with n_rows[g] (device int32; NULL: all) live
+// rows in group g, of which those whose y_valid (compacted numbering; NULL: all) is set are trained on.  Padding rows
+// are never read.  phase_mask splits the step around the data-parallel exchanges: 1 = forward + this rank's NLL sums
+// (+ their all-reduce); 2 = generator update from the global sums, metrics, per-row confidence, backward scaled by the
+// global labelled count (+ the gradient all-reduce); 4 = Adam; 7 = the whole step.
+int flow_train_step_padded(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                           const FlowBuffers& b, const float* x, int groups, int rows_per_group, const int* n_rows,
+                           const unsigned char* y_valid, float* cg_mean, float* cg_std, float* conf_out, float* metrics,
+                           int phase_mask, cudaStream_t stream);
 
 // Per-pixel anomaly map on wgmma: bf16 operands packed by set_params (re-pack after the parameters change), fp32
 // accumulation; the masks and permutations are read from b on every call.  tokens: [batch, gh * gw, dim] fp32; trav

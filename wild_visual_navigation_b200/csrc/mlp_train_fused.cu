@@ -16,9 +16,8 @@
 // Rows arrive PADDED, as the segment-pooling kernel leaves them: x [groups, rows_per_group, dim] with n_rows[g] live rows
 // per group (device memory).  The compaction the reference does with a boolean mask (`feat[seg_mask]`) happens inside
 // the kernels — labels y / y_valid are indexed by the compacted row number — so the step has no host synchronisation.
-// The communicator is NCCL, resolved at run time from the process (torch has loaded libnccl.so.2); the library owns it
-// (wvn_mlp_trainer_init_comm), so the collectives are issued from here on the caller's stream.
-#include <dlfcn.h>
+// The communicator is the training core's (train_core.h: NCCL, owned by the library, wvn_mlp_trainer_init_comm), so the
+// collectives are issued from here on the caller's stream.
 #include <string.h>
 
 #include <algorithm>
@@ -516,38 +515,6 @@ train_apply_kernel(float* __restrict__ p, const float* __restrict__ g, float* __
   adam_update(p, g, m, v, n, cfg, step_ptr);
 }
 
-// ------------------------------------------------------------------------------------------------ NCCL (dlopen)
-typedef struct { char internal[128]; } NcclUniqueId;
-typedef void* NcclComm;
-struct NcclApi {
-  int (*GetUniqueId)(NcclUniqueId*) = nullptr;
-  int (*CommInitRank)(NcclComm*, int, NcclUniqueId, int) = nullptr;
-  int (*CommDestroy)(NcclComm) = nullptr;
-  int (*AllReduce)(const void*, void*, size_t, int, int, NcclComm, cudaStream_t) = nullptr;
-  const char* (*GetErrorString)(int) = nullptr;
-  bool ok = false;
-};
-constexpr int kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2, kNcclMin = 3;  // ncclDataType_t / ncclRedOp_t values (nccl.h)
-
-NcclApi& nccl() {
-  static NcclApi api;
-  static bool tried = false;
-  if (tried) return api;
-  tried = true;
-  // the process (torch.distributed) has normally loaded libnccl.so.2 already; RTLD_NOLOAD-first keeps a single copy
-  void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD | RTLD_GLOBAL);
-  if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-  if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
-  if (!h) return api;
-  api.GetUniqueId = reinterpret_cast<decltype(api.GetUniqueId)>(dlsym(h, "ncclGetUniqueId"));
-  api.CommInitRank = reinterpret_cast<decltype(api.CommInitRank)>(dlsym(h, "ncclCommInitRank"));
-  api.CommDestroy = reinterpret_cast<decltype(api.CommDestroy)>(dlsym(h, "ncclCommDestroy"));
-  api.AllReduce = reinterpret_cast<decltype(api.AllReduce)>(dlsym(h, "ncclAllReduce"));
-  api.GetErrorString = reinterpret_cast<decltype(api.GetErrorString)>(dlsym(h, "ncclGetErrorString"));
-  api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllReduce && api.GetErrorString;
-  return api;
-}
-
 }  // namespace
 
 struct FusedTrainer {
@@ -560,8 +527,7 @@ struct FusedTrainer {
         *loss_reco = nullptr, *raw = nullptr, *grads = nullptr;
   FusedScalars* sc = nullptr;
   void* arena = nullptr;
-  NcclComm comm = nullptr;
-  int world = 1;
+  TrainerComm comm;        // the library's communicator of a data-parallel step (train_core.h)
   size_t smem_fwd = 0, smem_bwd = 0;
   TrainerConf conf;        // ConfidenceGenerator method + where its state lives
 };
@@ -621,7 +587,7 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
 
 void fused_trainer_destroy(FusedTrainer* t) {
   if (!t) return;
-  if (t->comm && nccl().ok) nccl().CommDestroy(t->comm);
+  trainer_comm_destroy(&t->comm);
   if (t->arena) cudaFree(t->arena);
   trainer_conf_destroy(&t->conf);
   delete t;
@@ -629,28 +595,7 @@ void fused_trainer_destroy(FusedTrainer* t) {
 
 TrainerConf* fused_trainer_conf(FusedTrainer* t) { return &t->conf; }
 
-int fused_comm_unique_id(void* id128) {
-  WVN_REQUIRE(id128, "comm: null id buffer");
-  NcclApi& api = nccl();
-  if (!api.ok) return set_error(WVN_ERR_STATE, "comm: libnccl.so.2 is not loadable in this process");
-  NcclUniqueId id;
-  const int rc = api.GetUniqueId(&id);
-  if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclGetUniqueId: %s", api.GetErrorString(rc));
-  memcpy(id128, &id, sizeof(id));
-  return WVN_OK;
-}
-
-int fused_trainer_init_comm(FusedTrainer* t, const void* id128, int rank, int world) {
-  WVN_REQUIRE(t && id128 && world >= 1 && rank >= 0 && rank < world, "comm: bad arguments");
-  NcclApi& api = nccl();
-  if (!api.ok) return set_error(WVN_ERR_STATE, "comm: libnccl.so.2 is not loadable in this process");
-  NcclUniqueId id;
-  memcpy(&id, id128, sizeof(id));
-  const int rc = api.CommInitRank(&t->comm, world, id, rank);
-  if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclCommInitRank: %s", api.GetErrorString(rc));
-  t->world = world;
-  return WVN_OK;
-}
+TrainerComm* fused_trainer_comm(FusedTrainer* t) { return &t->comm; }
 
 int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                      const float* x, int groups, int rpg, const int* n_rows, const float* y,
@@ -664,22 +609,13 @@ int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_
   const MlpShape& s = t->s;
   const int tiles = static_cast<int>((rows + TR - 1) / TR);
   const long long np = static_cast<long long>(t->o.total);
-  NcclApi& api = nccl();
   if (phase_mask & 1) {
     // no memsets: the statistic sums were left clean by the previous step's K4 (by create for the first step)
     train_fwd_rows_kernel<<<tiles, kThreads, t->smem_fwd, stream>>>(s, t->o, params, x, y, y_valid, n_rows, groups, rpg,
                                                                    t->h1, t->h2, t->out, t->loss_reco, t->raw, t->sc,
                                                                    t->grads + np);
     WVN_CHECK_LAUNCH("train_fwd_rows_kernel");
-    if (t->comm) {
-      const int rc = api.AllReduce(t->sc, t->sc, 6, kNcclFloat64, kNcclSum, t->comm, stream);
-      if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclAllReduce(stats): %s", api.GetErrorString(rc));
-      if (t->conf.cs.method == CONF_MOVING_AVERAGE) {
-        int r2 = api.AllReduce(&t->sc->x_min, &t->sc->x_min, 1, kNcclFloat64, kNcclMin, t->comm, stream);
-        if (r2 == 0) r2 = api.AllReduce(&t->sc->x_max, &t->sc->x_max, 1, kNcclFloat64, kNcclMax, t->comm, stream);
-        if (r2 != 0) return set_error(WVN_ERR_CUDA, "ncclAllReduce(extrema): %s", api.GetErrorString(r2));
-      }
-    }
+    WVN_PROPAGATE(trainer_comm_stats(&t->comm, &t->sc->sum_lr, t->conf.cs.method == CONF_MOVING_AVERAGE, stream));
   }
   if (phase_mask & 2) {
     if (t->conf.cs.method != CONF_LATEST) {   // generators with memory: one thread updates the state once
@@ -708,10 +644,7 @@ int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_
     }
     train_wgrad_kernel<<<blocks, 256, 0, stream>>>(w);
     WVN_CHECK_LAUNCH("train_wgrad_kernel");
-    if (t->comm) {
-      const int rc = api.AllReduce(t->grads, t->grads, static_cast<size_t>(np + 1), kNcclFloat32, kNcclSum, t->comm, stream);
-      if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclAllReduce(grads): %s", api.GetErrorString(rc));
-    }
+    WVN_PROPAGATE(trainer_comm_sum(&t->comm, t->grads, static_cast<size_t>(np + 1), false, stream));
   }
   if (phase_mask & 4) {
     int blocks = static_cast<int>((np + 255) / 256);

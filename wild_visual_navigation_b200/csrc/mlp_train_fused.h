@@ -34,8 +34,8 @@ struct FusedTrainer;
 int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, void* scalars_ext,
                          float* grads_ext, FusedTrainer** out);
 void fused_trainer_destroy(FusedTrainer* t);
-int fused_comm_unique_id(void* id128);
-int fused_trainer_init_comm(FusedTrainer* t, const void* id128, int rank, int world);
+// The trainer's communicator (set up with trainer_comm_init; none: the exchanges are the caller's).
+TrainerComm* fused_trainer_comm(FusedTrainer* t);
 // The trainer's ConfidenceGenerator (bound and copied with trainer_conf_bind / trainer_conf_copy).
 TrainerConf* fused_trainer_conf(FusedTrainer* t);
 // phase_mask: 1 = forward + statistics (+ their all-reduce), 2 = backward + weight gradients (+ gradient all-reduce),

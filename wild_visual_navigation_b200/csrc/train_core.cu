@@ -1,5 +1,7 @@
 // wvn-b200: the fp32 training core shared by the MLP and LinearRnvp trainers (train_core.h): the private
-// ConfidenceGenerator block, Adam, and the batched fp32 CUDA-core GEMM.
+// ConfidenceGenerator block, Adam, the batched fp32 CUDA-core GEMM, the compaction of padded rows and the NCCL
+// communicator of data-parallel steps.
+#include <dlfcn.h>
 #include <string.h>
 
 #include <algorithm>
@@ -208,6 +210,159 @@ int launch_gemms(const GemmProblem* ps, int count, const int* n_live, cudaStream
   else gemm_f32_kernel<false, false><<<grid, 256, 0, stream>>>(g);
   WVN_CHECK_LAUNCH("gemm_f32_kernel");
   return WVN_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ padded rows
+namespace {
+
+// Exclusive prefix sum of v over the block of 1024 threads; *total = the sum over the block.
+__device__ __forceinline__ int block_exclusive_scan(int v, int* wsum, int* total) {
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int u = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += u;
+  }
+  __syncthreads();   // wsum is free (a previous scan has been read)
+  if (lane == 31) wsum[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    int w = wsum[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += u;
+    }
+    wsum[lane] = w;
+  }
+  __syncthreads();
+  *total = wsum[31];
+  return inc - v + (warp > 0 ? wsum[warp - 1] : 0);
+}
+
+// One block of 1024: every thread walks a contiguous range of padded rows three times (live count, kept count, write).
+__global__ void __launch_bounds__(1024)
+compact_rows_kernel(int groups, int rpg, const int* __restrict__ n_rows, const unsigned char* __restrict__ y_valid,
+                    int* __restrict__ comp, int* __restrict__ n_live) {
+  __shared__ int wsum[32];
+  const long long rows = static_cast<long long>(groups) * rpg;
+  const long long per = (rows + 1023) / 1024, b = threadIdx.x * per, e = min(rows, b + per);
+  auto live = [&](long long r) {
+    if (n_rows == nullptr) return true;
+    const long long g = r / rpg;
+    return r - g * rpg < n_rows[g];
+  };
+  int c = 0;
+  for (long long r = b; r < e; ++r) c += live(r) ? 1 : 0;
+  int total;
+  const int ci0 = block_exclusive_scan(c, wsum, &total);   // compacted number of this range's first live row
+  int k = 0, ci = ci0;
+  for (long long r = b; r < e; ++r)
+    if (live(r)) k += (y_valid == nullptr || y_valid[ci++] != 0) ? 1 : 0;
+  int pos = block_exclusive_scan(k, wsum, &total);
+  ci = ci0;
+  for (long long r = b; r < e; ++r)
+    if (live(r) && (y_valid == nullptr || y_valid[ci++] != 0)) comp[pos++] = static_cast<int>(r);
+  if (threadIdx.x == 0) *n_live = total;
+}
+
+}  // namespace
+
+int compact_rows(int groups, int rows_per_group, const int* n_rows, const unsigned char* y_valid, int* comp, int* n_live,
+                 cudaStream_t stream) {
+  WVN_REQUIRE(groups >= 0 && rows_per_group >= 0 && comp && n_live, "compact rows: bad arguments");
+  compact_rows_kernel<<<1, 1024, 0, stream>>>(groups, rows_per_group, n_rows, y_valid, comp, n_live);
+  WVN_CHECK_LAUNCH("compact_rows_kernel");
+  return WVN_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ NCCL (dlopen)
+namespace {
+
+typedef struct { char internal[128]; } NcclUniqueId;
+typedef void* NcclComm;
+struct NcclApi {
+  int (*GetUniqueId)(NcclUniqueId*) = nullptr;
+  int (*CommInitRank)(NcclComm*, int, NcclUniqueId, int) = nullptr;
+  int (*CommDestroy)(NcclComm) = nullptr;
+  int (*AllReduce)(const void*, void*, size_t, int, int, NcclComm, cudaStream_t) = nullptr;
+  const char* (*GetErrorString)(int) = nullptr;
+  bool ok = false;
+};
+constexpr int kNcclFloat32 = 7, kNcclFloat64 = 8, kNcclSum = 0, kNcclMax = 2, kNcclMin = 3;  // ncclDataType_t / ncclRedOp_t values (nccl.h)
+
+NcclApi& nccl() {
+  static NcclApi api;
+  static bool tried = false;
+  if (tried) return api;
+  tried = true;
+  // the process (torch.distributed) has normally loaded libnccl.so.2 already; RTLD_NOLOAD-first keeps a single copy
+  void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD | RTLD_GLOBAL);
+  if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
+  if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
+  if (!h) return api;
+  api.GetUniqueId = reinterpret_cast<decltype(api.GetUniqueId)>(dlsym(h, "ncclGetUniqueId"));
+  api.CommInitRank = reinterpret_cast<decltype(api.CommInitRank)>(dlsym(h, "ncclCommInitRank"));
+  api.CommDestroy = reinterpret_cast<decltype(api.CommDestroy)>(dlsym(h, "ncclCommDestroy"));
+  api.AllReduce = reinterpret_cast<decltype(api.AllReduce)>(dlsym(h, "ncclAllReduce"));
+  api.GetErrorString = reinterpret_cast<decltype(api.GetErrorString)>(dlsym(h, "ncclGetErrorString"));
+  api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllReduce && api.GetErrorString;
+  return api;
+}
+
+int all_reduce(TrainerComm* c, void* buf, size_t n, int type, int op, const char* what, cudaStream_t stream) {
+  NcclApi& api = nccl();
+  const int rc = api.AllReduce(buf, buf, n, type, op, static_cast<NcclComm>(c->comm), stream);
+  if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclAllReduce(%s): %s", what, api.GetErrorString(rc));
+  return WVN_OK;
+}
+
+}  // namespace
+
+int comm_unique_id(void* id128) {
+  WVN_REQUIRE(id128, "comm: null id buffer");
+  NcclApi& api = nccl();
+  if (!api.ok) return set_error(WVN_ERR_STATE, "comm: libnccl.so.2 is not loadable in this process");
+  NcclUniqueId id;
+  const int rc = api.GetUniqueId(&id);
+  if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclGetUniqueId: %s", api.GetErrorString(rc));
+  memcpy(id128, &id, sizeof(id));
+  return WVN_OK;
+}
+
+int trainer_comm_init(TrainerComm* c, const void* id128, int rank, int world) {
+  WVN_REQUIRE(c && id128 && world >= 1 && rank >= 0 && rank < world, "comm: bad arguments");
+  NcclApi& api = nccl();
+  if (!api.ok) return set_error(WVN_ERR_STATE, "comm: libnccl.so.2 is not loadable in this process");
+  NcclUniqueId id;
+  memcpy(&id, id128, sizeof(id));
+  NcclComm comm = nullptr;
+  const int rc = api.CommInitRank(&comm, world, id, rank);
+  if (rc != 0) return set_error(WVN_ERR_CUDA, "ncclCommInitRank: %s", api.GetErrorString(rc));
+  trainer_comm_destroy(c);
+  c->comm = comm;
+  c->world = world;
+  return WVN_OK;
+}
+
+void trainer_comm_destroy(TrainerComm* c) {
+  if (c->comm && nccl().ok) nccl().CommDestroy(static_cast<NcclComm>(c->comm));
+  c->comm = nullptr;
+  c->world = 1;
+}
+
+int trainer_comm_stats(TrainerComm* c, double* stats, bool extrema, cudaStream_t stream) {
+  if (!c->comm) return WVN_OK;
+  WVN_PROPAGATE(all_reduce(c, stats, kStatSums, kNcclFloat64, kNcclSum, "stats", stream));
+  if (!extrema) return WVN_OK;
+  WVN_PROPAGATE(all_reduce(c, stats + kStatSums, 1, kNcclFloat64, kNcclMin, "extrema", stream));
+  return all_reduce(c, stats + kStatSums + 1, 1, kNcclFloat64, kNcclMax, "extrema", stream);
+}
+
+int trainer_comm_sum(TrainerComm* c, void* buf, size_t n, bool f64, cudaStream_t stream) {
+  if (!c->comm) return WVN_OK;
+  return all_reduce(c, buf, n, f64 ? kNcclFloat64 : kNcclFloat32, kNcclSum, "grads", stream);
 }
 
 }  // namespace wvn

@@ -1,8 +1,10 @@
 // wvn-b200: the fp32 training core shared by the MLP trainers (mlp_train.cu, mlp_train_fused.cu) and the LinearRnvp
-// trainer (flow_train.cu): the ConfidenceGenerator state a trainer keeps, Adam, and the batched fp32 tile GEMM.
+// trainer (flow_train.cu): the ConfidenceGenerator state a trainer keeps, Adam, the batched fp32 tile GEMM, the
+// compaction of padded rows and the data-parallel exchange.
 #pragma once
 
 #include <cuda_runtime.h>
+#include <stddef.h>
 
 namespace wvn {
 
@@ -70,5 +72,33 @@ GemmProblem gemm_problem(const float* a, long long a_rs, long long a_cs, const f
 // One launch for `count` problems.  splits > 1 (one problem, no live bound, no epilogue, no db): K is cut into up to
 // `splits` ranges of a multiple of 16 whose partial products are added into C with fp32 atomics (C zeroed by the caller).
 int launch_gemms(const GemmProblem* ps, int count, const int* n_live, cudaStream_t stream, int splits = 1);
+
+// ---- padded rows
+// Rows arrive padded per group, as the segment pooling leaves them: padded row r = g * rows_per_group + s is live when
+// s < n_rows[g] (n_rows NULL: every row).  Live rows are numbered group by group (the compacted numbering of
+// `feat[mask]`); y_valid (NULL: keep every live row) is indexed by that number and drops the rows it does not set.
+// comp[i] = padded index of the i-th kept row, *n_live = their number.  One launch; padding rows are never read.
+int compact_rows(int groups, int rows_per_group, const int* n_rows, const unsigned char* y_valid, int* comp, int* n_live,
+                 cudaStream_t stream);
+
+// ---- data-parallel exchange
+// Every trainer's statistics block begins with the same 8 doubles: six plain sums (all-reduced with SUM, one of them a
+// row count), then the extrema of the confidence input (MIN / MAX; moving_average's min-max normalisation).
+constexpr int kStatSums = 6;
+constexpr int kStatDoubles = 8;
+// The library's own NCCL communicator (libnccl.so.2 resolved from the running process): when a trainer has one, its step
+// issues the collectives itself, between its kernels on the caller's stream.  Without one, every exchange is a no-op and
+// a caller with another transport all-reduces the same buffers between the step's phases.
+struct TrainerComm {
+  void* comm = nullptr;
+  int world = 1;
+};
+int comm_unique_id(void* id128);
+int trainer_comm_init(TrainerComm* c, const void* id128, int rank, int world);
+void trainer_comm_destroy(TrainerComm* c);
+// stats[0, kStatSums) SUM; with `extrema` also stats[6] MIN and stats[7] MAX.
+int trainer_comm_stats(TrainerComm* c, double* stats, bool extrema, cudaStream_t stream);
+// SUM of n fp32 (f64 = false) or fp64 values in place.
+int trainer_comm_sum(TrainerComm* c, void* buf, size_t n, bool f64, cudaStream_t stream);
 
 }  // namespace wvn

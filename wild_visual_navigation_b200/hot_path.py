@@ -10,6 +10,10 @@ learning node (wvn_learning_node.py:651-656 + traversability_estimator.py:448-49
 ``bench.py`` times exactly ``HotPathStep.step`` and ``tests/test_bench_path_gpu.py`` holds it to the oracle, so the
 benchmarked configuration and the tested one are the same object.  The step has no host synchronisation: the pooled
 rows go to the trainer padded per frame with their device-side counts (csrc/mlp_train_fused.cu).
+
+``model`` / ``anomaly_detection`` pick the learner as the nodes' ``model.name`` does: SimpleMLP (the default),
+DoubleMLP, or with ``anomaly_detection=True`` the LinearRnvp flow; each is built with ``input_size`` = the backbone's
+feature dimension and trains on the same padded rows, data-parallel with ``process_group``.
 """
 from __future__ import annotations
 
@@ -23,21 +27,29 @@ from .traversability_estimator import TraversabilityEstimator
 class HotPathStep:
     def __init__(self, device: str, state_dict, head_state_dict, batch: int = 32, input_size: int = 448,
                  backbone_type: str = "vit_small", patch_size: int = 8, chunk: int = 32, flip_tta: bool = False,
-                 run_clustering: bool = True, n_image_clusters: int = 20, process_group=None, feature_type: str = "dino"):
+                 run_clustering: bool = True, n_image_clusters: int = 20, process_group=None, feature_type: str = "dino",
+                 model: str = "SimpleMLP", anomaly_detection: bool = False):
         self.device, self.batch, self.input_size = device, batch, input_size
         self.fe = FeatureExtractor(device, segmentation_type="stego", feature_type=feature_type, input_size=input_size,
                                    state_dict=state_dict, head_state_dict=head_state_dict, flip_tta=flip_tta,
                                    run_clustering=run_clustering, n_image_clusters=n_image_clusters, max_batch=batch,
                                    chunk=chunk, backbone_type=backbone_type, patch_size=patch_size)
         self.smax = self.fe.max_segments
+        if model not in ("SimpleMLP", "DoubleMLP"):
+            raise ValueError(f"HotPathStep: model must be 'SimpleMLP' or 'DoubleMLP', got {model!r}")
+        if anomaly_detection and model != "SimpleMLP":
+            raise ValueError("HotPathStep: anomaly_detection=True selects the LinearRnvp learner; leave model at its default")
         params = None
-        if self.fe.feature_dim != 384:
+        if self.fe.feature_dim != 384 or model != "SimpleMLP" or anomaly_detection:
             from .traversability_estimator.traversability_estimator import default_params
 
-            params = default_params()
-            params["model"]["simple_mlp_cfg"]["input_size"] = self.fe.feature_dim
+            params = default_params(anomaly_detection)
+            if model == "DoubleMLP":
+                params["model"]["name"] = "DoubleMLP"
+            cfg = {"SimpleMLP": "simple_mlp_cfg", "DoubleMLP": "double_mlp_cfg"}[model]
+            params["model"]["linear_rnvp_cfg" if anomaly_detection else cfg]["input_size"] = self.fe.feature_dim
         self.te = TraversabilityEstimator(params=params, device=device, process_group=process_group,
-                                          max_rows=batch * self.smax)
+                                          max_rows=batch * self.smax, anomaly_detection=anomaly_detection)
         self.cg = self.te._traversability_loss._confidence_generator
         self.ti = TraversabilityInference(self.fe._dino, self.te._model, self.cg)
 
@@ -45,7 +57,9 @@ class HotPathStep:
     def step(self, img: torch.Tensor, y: torch.Tensor, y_valid: torch.Tensor) -> dict:
         """img: (B,3,H,W) float in [0,1] or (B,H0,W0,3) uint8 camera frames; y / y_valid: supervision of the pooled
         rows in compacted order (frame 0's segments, then frame 1's, ...), at least B*smax entries.
-        Returns the extract_batch dict plus ``trav`` / ``conf`` (B,H,H) and ``confidence_rows``."""
+        Returns the extract_batch dict plus ``trav`` / ``conf`` (B,H,H) and ``confidence_rows``.  ``confidence_rows``
+        holds one confidence per live row in compacted order; for the LinearRnvp flow it holds the labelled rows'
+        (those ``y_valid`` sets), in order, and ``conf`` is None (the node publishes no confidence map there)."""
         r = self.fe.extract_batch(img)                                        # ViT + STEGO seg + pooling + graph
         trav, conf = self.ti.predict_from_tokens(r["tokens"], self.input_size)   # per-pixel MLP -> maps
         crow = self.te.train_on_padded(r["feat"], r["n_segments"], y, y_valid)  # fwd + loss + bwd + (all-reduce) + Adam

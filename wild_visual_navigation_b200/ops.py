@@ -536,12 +536,27 @@ def double_mlp_forward_f32(flat_params, x, dim, h1, h2):
     return out
 
 
+def _device_doubles(address, n, device):
+    """A float64 tensor over ``n`` doubles of device memory the library owns (no copy)."""
+    class _Block:
+        __cuda_array_interface__ = {"shape": (n,), "typestr": "<f8", "data": (int(address), False), "version": 2}
+
+    return torch.as_tensor(_Block(), device=device)
+
+
 class _TrainerHandle:
     """Owns a library trainer handle with workspaces for ``max_rows`` rows and replaces it by a larger one when a call
     needs more.  Remembers the ConfidenceGenerator binding, so the replacement keeps the generator where it was.
-    Subclasses name their ABI functions and make the handle in ``_new_handle``."""
+    Subclasses name their ABI functions and make the handle in ``_new_handle``.
 
-    _DESTROY = _SET_CONFIDENCE = _COPY_CONFIDENCE = None
+    Data-parallel steps (``process_group``) are run here for every trainer: with an NCCL group the handle gets the
+    library's own communicator and the step issues both all-reduces itself, between its kernels; with any other backend
+    (gloo in tests) the step runs as phase 1 / all-reduce of the statistics block / phase 2 / all-reduce of the gradient
+    / phase 4 through ``torch.distributed`` on the same buffers.  ``stats``: the handle's statistics block (6 sums, then
+    the extrema); ``_grad_exchange()``: the buffers summed after phase 2."""
+
+    _DESTROY = _SET_CONFIDENCE = _COPY_CONFIDENCE = _INIT_COMM = None
+    pg = None
 
     def _create(self, max_rows):
         h = self._new_handle(int(max_rows))
@@ -555,6 +570,42 @@ class _TrainerHandle:
         self.max_rows = int(max_rows)
         if self._conf is not None:
             self.set_confidence(*self._conf)
+        self._init_comm()
+
+    def _init_comm(self):
+        self._lib_comm = False
+        if self.pg is None:
+            return
+        import torch.distributed as dist
+
+        if dist.get_backend(self.pg) == "nccl":
+            # the library owns its communicator: rank 0 makes the id, torch.distributed only carries the 128 bytes
+            rank, world = dist.get_rank(self.pg), dist.get_world_size(self.pg)
+            buf = (ctypes.c_ubyte * 128)()
+            if rank == 0:
+                check(lib().wvn_comm_unique_id(buf))
+            idt = torch.tensor(list(buf), dtype=torch.uint8, device=self.exp_avg.device)
+            dist.broadcast(idt, src=dist.get_global_rank(self.pg, 0), group=self.pg)
+            raw = (ctypes.c_ubyte * 128)(*idt.cpu().tolist())
+            check(getattr(lib(), self._INIT_COMM)(self._h, raw, rank, world))
+            self._lib_comm = True
+
+    def _run_phases(self, phase):
+        """``phase(mask)`` enqueues those phases of one step on the current stream."""
+        if self.pg is None or self._lib_comm:
+            phase(7)
+            return
+        import torch.distributed as dist
+
+        phase(1)
+        dist.all_reduce(self.stats[:6], group=self.pg)
+        if self._conf is not None and self._conf[0] == 3:   # moving_average normalises by the global extrema
+            dist.all_reduce(self.stats[6:7], op=dist.ReduceOp.MIN, group=self.pg)
+            dist.all_reduce(self.stats[7:8], op=dist.ReduceOp.MAX, group=self.pg)
+        phase(2)
+        for t in self._grad_exchange():
+            dist.all_reduce(t, group=self.pg)
+        phase(4)
 
     def _reserve(self, rows):
         if rows > self.max_rows:
@@ -615,6 +666,7 @@ class MlpTrainer(_TrainerHandle):
             self._alloc_ws(max_rows)
             return
         self.scalars = torch.zeros((lib().wvn_mlp_trainer_scalars_bytes() + 7) // 8, device=dev, dtype=torch.float64)
+        self.stats = self.scalars
         self._create(max_rows)
 
     # ---- fused path ---------------------------------------------------------------------------
@@ -628,24 +680,14 @@ class MlpTrainer(_TrainerHandle):
                                            ptr(self.grads), byref(h)))
         return h
 
+    _INIT_COMM = "wvn_mlp_trainer_init_comm"
+
     def _create(self, max_rows):
         super()._create(max_rows)
         self.conf = torch.empty(self.max_rows + 32, device=self.params.device, dtype=torch.float32)
-        self._lib_comm = False
-        if self.pg is not None:
-            import torch.distributed as dist
 
-            if dist.get_backend(self.pg) == "nccl":
-                # the library owns its communicator: rank 0 makes the id, torch.distributed only carries the 128 bytes
-                rank, world = dist.get_rank(self.pg), dist.get_world_size(self.pg)
-                buf = (ctypes.c_ubyte * 128)()
-                if rank == 0:
-                    check(lib().wvn_comm_unique_id(buf))
-                idt = torch.tensor(list(buf), dtype=torch.uint8, device=self.params.device)
-                dist.broadcast(idt, src=dist.get_global_rank(self.pg, 0), group=self.pg)
-                raw = (ctypes.c_ubyte * 128)(*idt.cpu().tolist())
-                check(lib().wvn_mlp_trainer_init_comm(self._h, raw, rank, world))
-                self._lib_comm = True
+    def _grad_exchange(self):
+        return (self.grads,)   # the confidence-weighted error sum rides at its end
 
     def set_confidence(self, method=0, *args, **kwargs):
         assert not self.legacy or method == 0, "the round-1 kernels implement latest_measurement only"
@@ -663,19 +705,7 @@ class MlpTrainer(_TrainerHandle):
                                            ptr(self.step_counter), ptr(x), groups, rpg, ptr(n_rows), ptr(y), ptr(yv),
                                            ptr(self.cg_mean), ptr(self.cg_std), ptr(self.conf), ptr(self.metrics), mask, s))
 
-        if self.pg is None or self._lib_comm:
-            phase(7)
-        else:  # non-NCCL process group (tests): the same two exchanges through torch.distributed
-            import torch.distributed as dist
-
-            phase(1)
-            dist.all_reduce(self.scalars[:6], group=self.pg)
-            if self._conf is not None and self._conf[0] == 3:   # moving_average normalises by the global extrema
-                dist.all_reduce(self.scalars[6:7], op=dist.ReduceOp.MIN, group=self.pg)
-                dist.all_reduce(self.scalars[7:8], op=dist.ReduceOp.MAX, group=self.pg)
-            phase(2)
-            dist.all_reduce(self.grads, group=self.pg)
-            phase(4)
+        self._run_phases(phase)
 
     def step_padded(self, feat, n_rows, y, y_valid):
         """feat [G, S, D] f32 padded per group, n_rows [G] int32 (device): the first n_rows[g] rows of group g are live.
@@ -735,18 +765,29 @@ class MlpTrainer(_TrainerHandle):
         return self.conf[:R]
 
 
+def _check_padded(feat, n_rows, dim):
+    G, S, D = feat.shape
+    assert D == dim and feat.dtype == torch.float32, "step_padded: feat must be (G, S, dim) float32"
+    assert n_rows.dtype == torch.int32 and n_rows.shape == (G,), "step_padded: n_rows must be (G,) int32"
+    return G, S
+
+
 class DoubleMlpTrainer(_TrainerHandle):
     """The online train step of a DoubleMLP on its flat fp32 parameters (csrc/double_mlp_train.cu): forward of both
     networks, TraversabilityLoss with the ConfidenceGenerator update, backward and Adam as one fixed launch sequence
     without host synchronisation, bit-reproducible.  ``exp_avg`` / ``exp_avg_sq`` / ``step_counter`` are
-    torch.optim.Adam's state over the 12 parameter tensors, flattened in ``parameters()`` order.  Single-GPU."""
+    torch.optim.Adam's state over the 12 parameter tensors, flattened in ``parameters()`` order.  Rows may arrive padded
+    per frame (``step_padded``).  With ``process_group`` the step is global-batch exact (see ``_TrainerHandle``): the
+    statistic sums, row counts and extrema are all-reduced after the forward, the gradient and the confidence-weighted
+    error sum after the backward."""
 
     _DESTROY = "wvn_double_mlp_trainer_destroy"
     _SET_CONFIDENCE = "wvn_double_mlp_trainer_set_confidence"
     _COPY_CONFIDENCE = "wvn_double_mlp_trainer_copy_confidence"
+    _INIT_COMM = "wvn_double_mlp_trainer_init_comm"
 
     def __init__(self, model, max_rows=4096, w_trav=0.03, w_reco=0.5, std_factor=0.5, anomaly_balanced=True, lr=1e-3,
-                 betas=(0.9, 0.999), eps=1e-8):
+                 betas=(0.9, 0.999), eps=1e-8, process_group=None):
         model.check_supported()
         _C.require_device()
         params = model.flat_params
@@ -763,6 +804,7 @@ class DoubleMlpTrainer(_TrainerHandle):
         self.metrics = torch.zeros(6, device=dev)
         self.cg_mean = torch.zeros(1, device=dev)
         self.cg_std = torch.ones(1, device=dev)
+        self.pg = process_group
         self._h = None
         self._conf = None
         self._create(max_rows)
@@ -776,21 +818,42 @@ class DoubleMlpTrainer(_TrainerHandle):
     def _create(self, max_rows):
         super()._create(max_rows)
         self.conf = torch.empty(self.max_rows, device=self.grads.device)
+        self.stats = _device_doubles(lib().wvn_double_mlp_trainer_stats(self._h), 9, self.grads.device)
+
+    def _grad_exchange(self):
+        return (self.grads, self.stats[8:9])   # + the confidence-weighted error sum, kept in fp64
+
+    def _run(self, x, groups, rpg, n_rows, y, y_valid):
+        self._reserve(groups * rpg)
+        x = x.contiguous().float()
+        y = y.contiguous().float()
+        yv = y_valid.contiguous().to(torch.uint8)
+        s = stream()
+
+        def phase(mask):
+            check(lib().wvn_double_mlp_train_step_padded(
+                self._h, ptr(self.model.flat_params), ptr(self.exp_avg), ptr(self.exp_avg_sq), ptr(self.step_counter),
+                ptr(x), groups, rpg, ptr(n_rows), ptr(y), ptr(yv), ptr(self.cg_mean), ptr(self.cg_std), ptr(self.conf),
+                ptr(self.metrics), mask, s))
+
+        self._run_phases(phase)
+
+    def step_padded(self, feat, n_rows, y, y_valid):
+        """feat [G, S, D] f32 padded per group, n_rows [G] int32 (device): the first n_rows[g] rows of group g are live;
+        padding may hold anything.  y / y_valid are indexed by the compacted row number.  Returns the confidence buffer
+        (compacted order; the live prefix has sum(n_rows) entries — no host sync happens here)."""
+        G, S = _check_padded(feat, n_rows, self.dim)
+        self._run(feat, G, S, n_rows, y, y_valid)
+        return self.conf
 
     def step(self, x, y, y_valid, n_total=None):
         """x [R,D] f32, y [R] f32, y_valid [R] bool.  Returns the confidence vector [R]; metrics stay on the device in
         ``self.metrics`` (loss_total, loss_trav, loss_reco, loss_trav_conf, mean, std)."""
         if n_total is not None and n_total != x.shape[0]:
-            raise ValueError("DoubleMlpTrainer: the step is single-GPU, n_total must be the batch's row count")
+            raise ValueError("DoubleMlpTrainer: the global row count is all-reduced by the step, n_total must be the "
+                             "batch's row count")
         R = x.shape[0]
-        self._reserve(R)
-        x = x.contiguous().float()
-        y = y.contiguous().float()
-        yv = y_valid.contiguous().to(torch.uint8)
-        check(lib().wvn_double_mlp_train_step(self._h, ptr(self.model.flat_params), ptr(self.exp_avg),
-                                              ptr(self.exp_avg_sq), ptr(self.step_counter), ptr(x), R, ptr(y), ptr(yv),
-                                              ptr(self.cg_mean), ptr(self.cg_std), ptr(self.conf), ptr(self.metrics),
-                                              stream()))
+        self._run(x, 1, R, None, y, y_valid)
         return self.conf[:R]
 
 
@@ -887,13 +950,17 @@ class FlowTrainer(_TrainerHandle):
     """The anomaly-detection train step on a LinearRnvp's flat fp32 parameters (csrc/flow_train.cu): forward, loss
     ``-mean(logprob.sum(1) + log_det)`` over the labelled rows, ConfidenceGenerator update with the per-row NLL,
     backward and Adam as one fixed launch sequence without host synchronisation.  ``exp_avg`` / ``exp_avg_sq`` /
-    ``step_counter`` are torch.optim.Adam's state over the 24 parameter tensors, flattened in ``parameters()`` order."""
+    ``step_counter`` are torch.optim.Adam's state over the 24 parameter tensors, flattened in ``parameters()`` order.
+    Rows may arrive padded per frame (``step_padded``).  With ``process_group`` the step is global-batch exact (see
+    ``_TrainerHandle``): the NLL sums, the labelled-row count and the extrema are all-reduced after the forward, the
+    gradient after the backward; the loss is the mean over the global labelled count."""
 
     _DESTROY = "wvn_flow_destroy"
     _SET_CONFIDENCE = "wvn_flow_set_confidence"
     _COPY_CONFIDENCE = "wvn_flow_copy_confidence"
+    _INIT_COMM = "wvn_flow_init_comm"
 
-    def __init__(self, model, max_rows=4096, std_factor=0.5, lr=1e-3, betas=(0.9, 0.999), eps=1e-8):
+    def __init__(self, model, max_rows=4096, std_factor=0.5, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, process_group=None):
         _C.require_device()
         params = model.flat_params
         assert params.is_cuda and params.dtype == torch.float32
@@ -909,6 +976,7 @@ class FlowTrainer(_TrainerHandle):
         self.metrics = torch.zeros(6, device=dev)
         self.cg_mean = torch.zeros(1, device=dev)
         self.cg_std = torch.ones(1, device=dev)
+        self.pg = process_group
         self._h = None
         self._conf = None
         self._create(max_rows)
@@ -921,11 +989,42 @@ class FlowTrainer(_TrainerHandle):
     def _create(self, max_rows):
         super()._create(max_rows)
         self.conf = torch.empty(self.max_rows, device=self.grads.device)
+        self.stats = _device_doubles(lib().wvn_flow_stats(self._h), 8, self.grads.device)
+
+    def _grad_exchange(self):
+        return (self.grads,)
+
+    def _run(self, x, groups, rpg, n_rows, y_valid):
+        self._reserve(groups * rpg)
+        x = x.contiguous().float()
+        yv = None if y_valid is None else y_valid.contiguous().to(torch.uint8)
+        s = stream()
+
+        def phase(mask):
+            check(lib().wvn_flow_train_step_padded(
+                self._h, ptr(self.model.flat_params), ptr(self.exp_avg), ptr(self.exp_avg_sq), ptr(self.step_counter),
+                byref(flow_buffers(self.model)), ptr(x), groups, rpg, ptr(n_rows), ptr(yv), ptr(self.cg_mean),
+                ptr(self.cg_std), ptr(self.conf), ptr(self.metrics), mask, s))
+
+        self._run_phases(phase)
+
+    def step_padded(self, feat, n_rows, y, y_valid):
+        """feat [G, S, D] f32 padded per group, n_rows [G] int32 (device); y_valid (compacted numbering) selects the rows
+        the flow learns from; ``y`` is ignored (AnomalyLoss uses no labels).  Returns the confidence buffer: the selected
+        rows' confidences in order (the live prefix has metrics[3] entries — no host sync happens here)."""
+        G, S = _check_padded(feat, n_rows, self.dim)
+        self._run(feat, G, S, n_rows, y_valid)
+        return self.conf
 
     def step(self, x, y_valid=None, phase_mask=7):
         """x (R, D) fp32; y_valid (R,) bool or None (every row).  Returns the confidence of the labelled rows in
-        order (a view of length R whose first n entries are live; n is metrics[3])."""
+        order (a view of length R whose first n entries are live; n is metrics[3]).  phase_mask (single process only):
+        1 = forward + statistics + generator update, 2 = backward, 4 = Adam."""
         R = x.shape[0]
+        if self.pg is not None:
+            assert phase_mask == 7, "FlowTrainer.step: a data-parallel step runs whole"
+            self._run(x, 1, R, None, y_valid)
+            return self.conf[:R]
         self._reserve(R)
         x = x.contiguous().float()
         yv = None if y_valid is None else y_valid.contiguous().to(torch.uint8)

@@ -10,11 +10,13 @@ projection and visualisation are OUT OF SCOPE (SURVEY.md §2): mission nodes are
 list and must already carry their per-segment features and supervision (``MissionNode``).
 
 ``train()`` runs forward + loss + backward + Adam as one fixed sequence of fp32 CUDA kernels
-(csrc/mlp_train.cu) with all scalars on the device; with a ``process_group`` the three confidence
-statistics and the flat gradient are all-reduced (NCCL over NVLink) for a global-batch step.
+(csrc/mlp_train_fused.cu) with all scalars on the device.
 In anomaly-detection mode the step is the LinearRnvp flow's (csrc/flow_train.cu: forward, NLL, confidence update,
-backward, Adam) on the labelled rows only; it is single-GPU.  With ``model.name == "DoubleMLP"`` the step is the
-DoubleMLP's (csrc/double_mlp_train.cu: the same TraversabilityLoss on two separate networks), also single-GPU.
+backward, Adam) on the labelled rows only.  With ``model.name == "DoubleMLP"`` the step is the DoubleMLP's
+(csrc/double_mlp_train.cu: the same TraversabilityLoss on two separate networks).
+Every learner is data-parallel: with a ``process_group`` the confidence statistics (sums, row counts, extrema) and the
+flat gradient are all-reduced inside the step (NCCL over NVLink) for a global-batch step, and every learner takes rows
+still padded per frame (``train_on_padded``).
 """
 from __future__ import annotations
 
@@ -83,13 +85,30 @@ def _get(p, key):
     return p[key] if isinstance(p, dict) else getattr(p, key)
 
 
+def _check_padded_args(feat, n_rows, y, y_valid, dim, y_optional):
+    def bad(what):
+        raise ValueError(f"train_on_padded: {what}")
+
+    if not torch.is_tensor(feat) or feat.dim() != 3 or feat.dtype != torch.float32 or feat.shape[2] != dim:
+        bad(f"feat must be a (B, smax, {dim}) float32 tensor")
+    if not torch.is_tensor(n_rows) or n_rows.dtype != torch.int32 or tuple(n_rows.shape) != (feat.shape[0],):
+        bad(f"n_rows must be a ({feat.shape[0]},) int32 tensor")
+    if not (y is None and y_optional) and (not torch.is_tensor(y) or y.dim() != 1 or not y.is_floating_point()):
+        bad("y must be a 1-D floating-point tensor")
+    if not torch.is_tensor(y_valid) or y_valid.dim() != 1 or y_valid.dtype not in (torch.bool, torch.uint8):
+        bad("y_valid must be a 1-D bool or uint8 tensor")
+    for t in (n_rows, y, y_valid):
+        if t is not None and t.device != feat.device:
+            bad("feat, n_rows, y and y_valid must be on one device")
+
+
 class TraversabilityEstimator:
     def __init__(self, params=None, device: str = "cuda", max_distance: float = 3, image_distance_thr: float = None,
                  supervision_distance_thr: float = None, min_samples_for_training: int = 10, vis_node_index: int = 10,
                  mode=None, extraction_store_folder=None, anomaly_detection: bool = False, process_group=None,
                  max_rows: int = 4096):
-        if anomaly_detection and process_group is not None:
-            raise ValueError("anomaly_detection (LinearRnvp) trains on one GPU: process_group is not supported")
+        if process_group is not None and not isinstance(process_group, torch.distributed.ProcessGroup):
+            raise ValueError(f"process_group must be a torch.distributed.ProcessGroup, got {type(process_group).__name__}")
         self._device = device
         self._mode = mode
         self._extraction_store_folder = extraction_store_folder
@@ -108,8 +127,6 @@ class TraversabilityEstimator:
             raise ValueError("anomaly_detection=True goes with model.name 'LinearRnvp' (and only with it), got "
                              f"{_get(model_cfg, 'name')!r}")
         self._double = _get(model_cfg, "name") == "DoubleMLP"
-        if self._double and process_group is not None:
-            raise ValueError("DoubleMLP trains on one GPU: process_group is not supported")
         self._model = get_model(model_cfg).to(self._device)
         self._model.train()
         gp = _get(self._params, "general")
@@ -123,7 +140,8 @@ class TraversabilityEstimator:
                                                     log_folder=_get(gp, "model_path"))
             self._traversability_loss.to(self._device)
             cg = self._traversability_loss._confidence_generator
-            self._trainer = ops.FlowTrainer(self._model, max_rows=max_rows, std_factor=cg.std_factor, lr=self._lr)
+            self._trainer = ops.FlowTrainer(self._model, max_rows=max_rows, std_factor=cg.std_factor, lr=self._lr,
+                                            process_group=process_group)
             self._bind_confidence_state()
             return
         lp = dict(_get(self._params, "loss"))
@@ -135,7 +153,7 @@ class TraversabilityEstimator:
         if self._double:
             self._trainer = ops.DoubleMlpTrainer(m, max_rows=max_rows, w_trav=lp["w_trav"], w_reco=lp["w_reco"],
                                                  std_factor=cg.std_factor, anomaly_balanced=lp["anomaly_balanced"],
-                                                 lr=self._lr)
+                                                 lr=self._lr, process_group=process_group)
             self._bind_confidence_state()
             return
         self._trainer = ops.MlpTrainer(m.flat_params, m.input_size, m.hidden[0], m.hidden[1], max_rows=max_rows,
@@ -208,12 +226,11 @@ class TraversabilityEstimator:
 
     def train_on_padded(self, feat, n_rows, y, y_valid):
         """The same step on rows that are still padded per frame, as ``FeatureExtractor.extract_batch`` returns them:
-        ``feat`` (B, smax, D), ``n_rows`` (B,) int32 on the device; ``y`` / ``y_valid`` are indexed by the compacted row
-        number (what ``feat[mask]`` would give).  No host synchronisation (the gather happens inside the kernels)."""
-        if self._anomaly_detection:
-            raise ValueError("train_on_padded is the SimpleMLP step; in anomaly-detection mode use train_on_batch")
-        if self._double:
-            raise ValueError("train_on_padded is the SimpleMLP step; with a DoubleMLP use train_on_batch")
+        ``feat`` (B, smax, D) float32, ``n_rows`` (B,) int32 on the device; ``y`` (float) / ``y_valid`` (bool or uint8)
+        are 1-D and indexed by the compacted row number (what ``feat[mask]`` would give).  No host synchronisation (the
+        gather happens inside the kernels).  In anomaly-detection mode the flow learns from the rows ``y_valid`` sets
+        and ignores ``y`` (it may be None); the returned confidences are those rows', in order."""
+        _check_padded_args(feat, n_rows, y, y_valid, self._model.input_size, y_optional=self._anomaly_detection)
         with self._learning_lock:
             conf = self._trainer.step_padded(feat, n_rows, y, y_valid)
             self._last_confidence = conf
