@@ -1,12 +1,11 @@
 """The DoubleMLP learner on the GPU: row forward, train step, per-pixel / per-segment inference, checkpoints and the
 hand-off, each against float64 (oracle/double_mlp.py) or the reference's own fp32 run (tests/golden/double_mlp.pt).
+The train step's statistics, generator update, gradients and Adam are checked phase by phase against float64 under a
+derived bound in test_double_mlp_train_step_gpu.py.
 
-Bounds (u = 2^-24).  Row forward: every layer is one fp32 fma chain over K terms plus the bias, so
+Row forward bound (u = 2^-24): every layer is one fp32 fma chain over K terms plus the bias, so
 |z - z64| <= e_in |W|^T + (K + 2) u ((|a| + e_in) |W|^T + |b|); ReLU is 1-Lipschitz and the sigmoid 1/4-Lipschitz
-(+ 4 u for expf and the division).  Train step: the loss terms, statistics and generator state carry the forward's
-relative error (held to 2e-5); the confidence moves by at most the generator's Lipschitz constant times that; the
-gradients are held to 1e-4 of their own size plus 1e-5 of their tensor's largest element; Adam is checked on the
-kernel's own gradients, where it is a handful of fp32 operations per element (the bound is spelled out there).
+(+ 4 u for expf and the division).
 """
 import math
 import os
@@ -120,92 +119,6 @@ def _split(flat, sd):
         out[k] = flat[off : off + v.numel()].view(v.shape).double()
         off += v.numel()
     return out
-
-
-def _conf_lipschitz(method, mean, std, f=0.5):
-    if method == "kalman_filter":
-        return 0.61 / (std * f)
-    if method == "moving_average":
-        return None
-    return 1.0 / (2 * std)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("method,balanced", CASES)
-def test_train_step_phase_by_phase(method, balanced):
-    """Three steps of 300 / 340 / 380 rows at D = 384, [64, 32, 1]: metrics, generator, per-row confidence, every
-    gradient element, and Adam against float64."""
-    _phase_by_phase(method, balanced, 384, 64, 32)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("D,h1,h2", [(90, 20, 7), (1, 4, 1), (1024, 256, 32), (384, 128, 32), (2, 8, 3)])
-@pytest.mark.parametrize("method", ["latest_measurement", "moving_average"])
-def test_train_step_shapes(D, h1, h2, method):
-    """The same checks at an odd shape and at the bound's extremes (D = 1 / 1024, h1 = 4 / 256, h2 = 1)."""
-    _phase_by_phase(method, True, D, h1, h2)
-
-
-def _phase_by_phase(method, balanced, D, h1, h2):
-    m = _model(D, h1, h2)
-    tr = _trainer(m, method, balanced)
-    cg = ConfidenceState(0.5, method)
-    for s in range(3):
-        R = 300 + 40 * s
-        x, y, yv = _rows(R, D, 10 + s)
-        sd = _sd64(m)
-        ea, eas = tr.exp_avg.double().clone(), tr.exp_avg_sq.double().clone()
-        _, g_ref, loss, aux = odm.train_step(sd, {}, x.double(), y, yv, cg, anomaly_balanced=balanced)
-        conf = tr.step(x, y, yv).double()
-        met = tr.metrics.double()
-        torch.cuda.synchronize()
-        for i, k in enumerate(("loss_trav", "loss_reco", "loss_trav_confidence")):
-            assert abs(met[1 + i] - aux[k]) <= 2e-5 * abs(aux[k]) + 1e-7, (s, k)
-        assert abs(met[0] - loss) <= 2e-5 * abs(loss) + 1e-7
-        assert abs(met[4] - aux["mean"]) <= 2e-5 * abs(aux["mean"]) + 1e-7
-        assert abs(met[5] - aux["std"]) <= 2e-5 * abs(aux["std"]) + 2e-5 * abs(aux["mean"]) + 1e-7
-        L = _conf_lipschitz(method, abs(aux["mean"].item()), aux["std"].item())
-        if L is not None:
-            lr = ((odm.forward(sd, x.double())[:, 1:] - x.double()) ** 2).mean(1)
-            bound = L * 2e-5 * (lr.abs() + abs(aux["mean"].item()) + 2 * aux["std"].item()) + 1e-6
-            assert_within(conf, aux["confidence"].double(), bound, f"conf step {s}")
-        else:
-            assert (conf - aux["confidence"].double()).abs().max() <= 1e-3
-        grads = _split(tr.grads, sd)
-        for k, g in g_ref.items():
-            assert_within(grads[k], g, 1e-4 * g.abs() + 1e-5 * g.abs().max() + 1e-12, f"grad {k} step {s}")
-        # Adam on the kernel's own gradients
-        # with the hyper-parameters as the kernel holds them (fp32: 1 - fp32(0.999) is 1.3e-5 off 0.001)
-        gf = tr.grads.double()
-        t = s + 1
-        b1, b2, lr, eps = (float(torch.tensor(v, dtype=torch.float32)) for v in (0.9, 0.999, 1e-3, 1e-8))
-        mm = ea + (gf - ea) * (1 - b1)
-        vv = b2 * eas + (1 - b2) * gf * gf
-        denom = vv.sqrt() / math.sqrt(1 - b2**t) + eps
-        step_size = lr / (1 - b1**t)
-        p_ref = torch.cat([v.reshape(-1) for v in sd.values()]) - step_size * mm / denom
-        p_new = m.flat_params.double()
-        # m's lerp m + (g - m)(1 - b1) rounds relative to |m_old| + |g| (it may cancel); the division, sqrt and bias
-        # corrections add a few u of the update; the subtraction u |p|
-        bound = (8 * U * p_ref.abs() + step_size * (4 * U * (ea.abs() + gf.abs()) + 8 * U * mm.abs()) / denom
-                 + 64 * U * 1e-3)
-        assert_within(p_new, p_ref, bound, f"adam step {s}")
-        assert int(tr.step_counter.item()) == t
-
-
-@pytest.mark.gpu
-def test_train_step_negative_control():
-    """A bias gradient scaled by 1.01 fails the gradient check."""
-    m = _model(384, 64, 32)
-    tr = _trainer(m, "latest_measurement", True)
-    x, y, yv = _rows(300, 384, 3)
-    sd = _sd64(m)
-    _, g_ref, _, _ = odm.train_step(sd, {}, x.double(), y, yv, ConfidenceState(0.5))
-    tr.step(x, y, yv)
-    g = _split(tr.grads, sd)["networks.1.2.bias"] * 1.01
-    ref = g_ref["networks.1.2.bias"]
-    with pytest.raises(AssertionError):
-        assert_within(g, ref, 1e-4 * ref.abs() + 1e-5 * ref.abs().max() + 1e-12, "scaled")
 
 
 @pytest.mark.gpu
