@@ -51,7 +51,9 @@ int wvn_check_device(void);
  * 104: adds the LinearRnvp flow handles, their functions wvn_flow_* and the struct wvn_flow_buffers; no layout change.
  * 106: adds the padded, phased and data-parallel DoubleMLP and flow steps (wvn_double_mlp_train_step_padded,
  * wvn_double_mlp_trainer_init_comm, wvn_double_mlp_trainer_stats, wvn_flow_train_step_padded, wvn_flow_init_comm,
- * wvn_flow_stats); no layout change. */
+ * wvn_flow_stats); no layout change.
+ * 107: adds wvn_mission_propagate and wvn_mission_propagate_workspace_bytes (the mission graph's label propagation);
+ * no layout change. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -339,6 +341,28 @@ int wvn_slic(const float* img, int batch, int h, int w, int num_components, floa
 int wvn_project_and_render(const float* K, const float* pose_camera_in_world, const float* points, const float* colors,
                            int color_batched, int batch, int n_points, int h, int w, const float* traversability,
                            float* masks, float* projected, unsigned char* valid, float* supervision_inout, void* stream);
+
+/* Mission-graph label propagation — one supervision event into every in-range mission node
+ * (TraversabilityEstimator.add_supervision_node, traversability_estimator.py:257-289, then each node's
+ * MissionNode.update_supervision_signal, nodes.py:400-440), in one pass over each slot's h x w.  For list entry i and
+ * slot s = slots[i] (distinct slots; any order, e.g. a wrapped ring range):
+ *   mask[s] = fmin(restart[i] ? 0 : mask[s], render(points, K[s], pose_cam_in_world[s]) * traversability)
+ *   y[s][k] = nan_to_num(mean of mask[s] over the pixels of segment k that are not NaN), y_valid[s][k] = y[s][k] > 0,
+ *   slot_valid[s] = any(y_valid[s])
+ * The footprint is projected and rasterised exactly as wvn_project_and_render does it (shared device code) with colour 1;
+ * the mask has one channel (the reference's three are identical).  restart (nullable): per list entry, nonzero = the
+ * node's mask was dropped (clear_debug_data), so the event starts it from a zero mask as the reference does.
+ * slots [n_slots] int32, restart [n_slots] uint8, points [n_points,3] world frame, traversability: device scalar — all on
+ * the device.  Per slot: K [cap,4,4] SCALED camera matrices, pose_cam_in_world [cap,4,4], seg [cap,h,w] int32 (ids outside
+ * [0, smax) ignored), mask [cap,h,w] fp32 (NaN = unlabelled), y [cap,smax] fp32, y_valid [cap,smax] uint8, slot_valid
+ * [cap] int32 (nullable).  Slots not in the list are not touched.  1 <= smax <= 4096, 1 <= n_points <= 1024.
+ * workspace: wvn_mission_propagate_workspace_bytes(>= n_slots, smax) bytes that are zero before the first call; each call
+ * leaves them zero again.  No allocation, no host synchronisation: everything is enqueued on `stream`. */
+size_t wvn_mission_propagate_workspace_bytes(int max_slots, int smax);
+int wvn_mission_propagate(const int* slots, const unsigned char* restart, int n_slots, const float* K,
+                          const float* pose_cam_in_world, const float* points, int n_points, const float* traversability,
+                          const int* seg, float* mask, int h, int w, int smax, float* y, unsigned char* y_valid,
+                          int* slot_valid, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Traversability MLP inference over every pixel — replaces

@@ -104,6 +104,8 @@ SIGNATURES = {
     "wvn_slic_workspace_bytes": (_S, [_I, _I, _I, _I]),
     "wvn_slic": (_I, [_P, _I, _I, _I, _I, _F, _I, _P, _P, _P, _P, _P, _P]),
     "wvn_project_and_render": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "wvn_mission_propagate_workspace_bytes": (_S, [_I, _I]),
+    "wvn_mission_propagate": (_I, [_P, _P, _I, _P, _P, _P, _I, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
     "wvn_mlp_infer_create": (_I, [_I, _I, _I, _I, POINTER(_P)]),
     "wvn_mlp_infer_destroy": (None, [_P]),
     "wvn_mlp_infer_reserve": (_I, [_P, _I]),

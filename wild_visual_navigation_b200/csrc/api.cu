@@ -15,6 +15,7 @@
 #include "gemm.h"
 #include "host_common.h"
 #include "mlp_train.h"
+#include "mission_graph.h"
 #include "mlp_train_fused.h"
 #include "pixel_head.h"
 #include "resnet_kernels.h"
@@ -120,7 +121,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 106; }
+int wvn_version(void) { return 107; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -647,6 +648,22 @@ int wvn_project_and_render(const float* K, const float* pose_camera_in_world, co
   a.batch = batch; a.n_points = n_points; a.h = h; a.w = w; a.color_batched = color_batched;
   return footprint_render(a, K, pose_camera_in_world, points, colors, traversability, masks, projected, valid,
                           supervision_inout, S(stream));
+}
+
+size_t wvn_mission_propagate_workspace_bytes(int max_slots, int smax) {
+  return mission_propagate_workspace_bytes(max_slots, smax);
+}
+
+int wvn_mission_propagate(const int* slots, const unsigned char* restart, int n_slots, const float* K,
+                          const float* pose_cam_in_world, const float* points, int n_points, const float* traversability,
+                          const int* seg, float* mask, int h, int w, int smax, float* y, unsigned char* y_valid,
+                          int* slot_valid, void* workspace, void* stream) {
+  WVN_REQUIRE(slots && K && pose_cam_in_world && points && traversability && seg && mask && y && y_valid && workspace,
+              "wvn_mission_propagate: null argument");
+  MissionPropagateArgs a;
+  a.n_slots = n_slots; a.n_points = n_points; a.h = h; a.w = w; a.smax = smax;
+  return mission_propagate(a, slots, restart, K, pose_cam_in_world, points, traversability, seg, mask, y, y_valid,
+                           slot_valid, workspace, S(stream));
 }
 
 // ============================================================================================

@@ -10,51 +10,16 @@
 // read-modify-write when fused).
 #include "footprint_kernels.h"
 
+#include "footprint_common.cuh"
 #include "host_common.h"
 
 namespace wvn {
 namespace {
 
+using namespace footprint;
+
 constexpr int kRowsPerBlock = 16;
 constexpr int kThreads = 256;
-
-// General 4x4 inverse (the reference calls Tensor.inverse(), not an SE(3) shortcut) by cofactors in double.
-__device__ void invert4x4(const float* __restrict__ m, float* __restrict__ out) {
-  double a[16], inv[16];
-  for (int i = 0; i < 16; ++i) a[i] = m[i];
-  inv[0] = a[5] * a[10] * a[15] - a[5] * a[11] * a[14] - a[9] * a[6] * a[15] + a[9] * a[7] * a[14] + a[13] * a[6] * a[11] - a[13] * a[7] * a[10];
-  inv[4] = -a[4] * a[10] * a[15] + a[4] * a[11] * a[14] + a[8] * a[6] * a[15] - a[8] * a[7] * a[14] - a[12] * a[6] * a[11] + a[12] * a[7] * a[10];
-  inv[8] = a[4] * a[9] * a[15] - a[4] * a[11] * a[13] - a[8] * a[5] * a[15] + a[8] * a[7] * a[13] + a[12] * a[5] * a[11] - a[12] * a[7] * a[9];
-  inv[12] = -a[4] * a[9] * a[14] + a[4] * a[10] * a[13] + a[8] * a[5] * a[14] - a[8] * a[6] * a[13] - a[12] * a[5] * a[10] + a[12] * a[6] * a[9];
-  inv[1] = -a[1] * a[10] * a[15] + a[1] * a[11] * a[14] + a[9] * a[2] * a[15] - a[9] * a[3] * a[14] - a[13] * a[2] * a[11] + a[13] * a[3] * a[10];
-  inv[5] = a[0] * a[10] * a[15] - a[0] * a[11] * a[14] - a[8] * a[2] * a[15] + a[8] * a[3] * a[14] + a[12] * a[2] * a[11] - a[12] * a[3] * a[10];
-  inv[9] = -a[0] * a[9] * a[15] + a[0] * a[11] * a[13] + a[8] * a[1] * a[15] - a[8] * a[3] * a[13] - a[12] * a[1] * a[11] + a[12] * a[3] * a[9];
-  inv[13] = a[0] * a[9] * a[14] - a[0] * a[10] * a[13] - a[8] * a[1] * a[14] + a[8] * a[2] * a[13] + a[12] * a[1] * a[10] - a[12] * a[2] * a[9];
-  inv[2] = a[1] * a[6] * a[15] - a[1] * a[7] * a[14] - a[5] * a[2] * a[15] + a[5] * a[3] * a[14] + a[13] * a[2] * a[7] - a[13] * a[3] * a[6];
-  inv[6] = -a[0] * a[6] * a[15] + a[0] * a[7] * a[14] + a[4] * a[2] * a[15] - a[4] * a[3] * a[14] - a[12] * a[2] * a[7] + a[12] * a[3] * a[6];
-  inv[10] = a[0] * a[5] * a[15] - a[0] * a[7] * a[13] - a[4] * a[1] * a[15] + a[4] * a[3] * a[13] + a[12] * a[1] * a[7] - a[12] * a[3] * a[5];
-  inv[14] = -a[0] * a[5] * a[14] + a[0] * a[6] * a[13] + a[4] * a[1] * a[14] - a[4] * a[2] * a[13] - a[12] * a[1] * a[6] + a[12] * a[2] * a[5];
-  inv[3] = -a[1] * a[6] * a[11] + a[1] * a[7] * a[10] + a[5] * a[2] * a[11] - a[5] * a[3] * a[10] - a[9] * a[2] * a[7] + a[9] * a[3] * a[6];
-  inv[7] = a[0] * a[6] * a[11] - a[0] * a[7] * a[10] - a[4] * a[2] * a[11] + a[4] * a[3] * a[10] + a[8] * a[2] * a[7] - a[8] * a[3] * a[6];
-  inv[11] = -a[0] * a[5] * a[11] + a[0] * a[7] * a[9] + a[4] * a[1] * a[11] - a[4] * a[3] * a[9] - a[8] * a[1] * a[7] + a[8] * a[3] * a[5];
-  inv[15] = a[0] * a[5] * a[10] - a[0] * a[6] * a[9] - a[4] * a[1] * a[10] + a[4] * a[2] * a[9] + a[8] * a[1] * a[6] - a[8] * a[2] * a[5];
-  const double det = a[0] * inv[0] + a[1] * inv[4] + a[2] * inv[8] + a[3] * inv[12];
-  const double r = 1.0 / det;  // singular pose -> inf / NaN, like Tensor.inverse() failing loudly is not possible here
-  for (int i = 0; i < 16; ++i) out[i] = static_cast<float>(inv[i] * r);
-}
-
-// kornia convert_points_from_homogeneous: scale = 1 / (z + 1e-8) where |z| > 1e-8, else 1.
-__device__ __forceinline__ float hom_scale(float z) { return fabsf(z) > 1e-8f ? 1.0f / (z + 1e-8f) : 1.0f; }
-
-__device__ __forceinline__ void transform4(const float* __restrict__ T, float x, float y, float z, float& ox, float& oy,
-                                           float& oz) {
-  const float hx = T[0] * x + T[1] * y + T[2] * z + T[3];
-  const float hy = T[4] * x + T[5] * y + T[6] * z + T[7];
-  const float hz = T[8] * x + T[9] * y + T[10] * z + T[11];
-  const float hw = T[12] * x + T[13] * y + T[14] * z + T[15];
-  const float s = hom_scale(hw);
-  ox = s * hx; oy = s * hy; oz = s * hz;
-}
 
 // smem: px[n + 1] | py[n + 1] (polygon closed by repeating point 0; kornia appends it unless last == first, and a
 // repeated vertex only adds a zero-length edge that cannot change any span) | Tcw[16]
@@ -74,15 +39,9 @@ footprint_render_kernel(FootprintArgs a, const float* __restrict__ Kmat, const f
   __syncthreads();
   const float* Kb = Kmat + 16 * static_cast<size_t>(b);
   for (int i = t; i < n; i += kThreads) {
-    const float* p = points + (static_cast<size_t>(b) * n + i) * 3;
-    float cx, cy, cz, ix, iy, iz;
-    transform4(Tcw, p[0], p[1], p[2], cx, cy, cz);       // world -> camera
-    transform4(Kb, cx, cy, cz, ix, iy, iz);              // PinholeCamera.project with identity extrinsics ...
-    const float s = hom_scale(iz);                       // ... and its own homogeneous division
-    float u = s * ix, v = s * iy;
-    const bool vz = cz >= 0.f;
-    const bool ok = vz && u >= 0.f && u <= static_cast<float>(a.w) && v >= 0.f && v <= static_cast<float>(a.h);
-    if (!vz) u = v = nanf("");
+    float u, v;
+    bool ok;
+    project_point(Tcw, Kb, points + (static_cast<size_t>(b) * n + i) * 3, a.w, a.h, u, v, ok);
     px[i] = u; py[i] = v;
     if (blockIdx.x == 0) {
       if (projected) { projected[(static_cast<size_t>(b) * n + i) * 2] = u; projected[(static_cast<size_t>(b) * n + i) * 2 + 1] = v; }
@@ -104,25 +63,8 @@ footprint_render_kernel(FootprintArgs a, const float* __restrict__ Kmat, const f
     const int y = blockIdx.x * kRowsPerBlock + ry;
     if (y >= a.h) break;
     const float yf = static_cast<float>(y);
-    float xl = wf, xr = -1.f;
-    for (int e = lane; e < n; e += 32) {
-      const float xs = px[e], ys = py[e], xe = px[e + 1], ye = py[e + 1];
-      const bool act = (ys <= yf && yf <= ye) || (ys >= yf && yf >= ye);   // false for NaN vertices
-      if (act) {
-        // same operation order as the reference's tensor expression (no fused multiply-add)
-        float dx = __fdiv_rn(__fsub_rn(xe, xs), __fadd_rn(__fsub_rn(ye, ys), 1e-12f));
-        dx = fminf(fmaxf(dx, -wf), wf);
-        const float x = __fadd_rn(__fmul_rn(__fsub_rn(yf, ys), dx), xs);
-        // torch.min / max propagate NaN; x can only be NaN for inf vertices, which the clamp removes except inf * 0
-        xl = (x != x || xl != xl) ? nanf("") : fminf(xl, x);
-        xr = (x != x || xr != xr) ? nanf("") : fmaxf(xr, x);
-      }
-    }
-    for (int o = 16; o; o >>= 1) {
-      const float ol = __shfl_xor_sync(0xffffffffu, xl, o), orr = __shfl_xor_sync(0xffffffffu, xr, o);
-      xl = (ol != ol || xl != xl) ? nanf("") : fminf(xl, ol);
-      xr = (orr != orr || xr != xr) ? nanf("") : fmaxf(xr, orr);
-    }
+    float xl, xr;
+    row_span(px, py, n, yf, wf, lane, xl, xr);
     const size_t row = static_cast<size_t>(b) * 3 * plane + static_cast<size_t>(y) * a.w;
     for (int x = lane; x < a.w; x += 32) {
       const float xf = static_cast<float>(x);

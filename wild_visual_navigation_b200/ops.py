@@ -196,6 +196,27 @@ def project_and_render(sK, pose_camera_in_world, points, colors, h, w, render=Tr
     return masks, proj, valid.bool()
 
 
+def mission_propagate_workspace(max_slots, smax, device):
+    """The zeroed workspace wvn_mission_propagate needs for up to ``max_slots`` list entries (every call leaves it zero)."""
+    return torch.zeros(max(int(lib().wvn_mission_propagate_workspace_bytes(max_slots, smax)), 1), device=device,
+                       dtype=torch.uint8)
+
+
+def mission_propagate(slots, restart, K, pose, points, traversability, seg, mask, y, y_valid, slot_valid, workspace):
+    """One supervision event into the listed mission-graph slots (see include/wvn_b200.h): slots [n] int32, restart [n]
+    uint8 or None, points [N,3] and traversability [1] fp32, all on the device; per slot K / pose [cap,4,4], seg [cap,H,W]
+    int32, mask [cap,H,W] fp32 (updated in place), y [cap,smax] fp32, y_valid [cap,smax] uint8, slot_valid [cap] int32 or
+    None.  Enqueued on the current stream; nothing is allocated and nothing waits for the device."""
+    n, smax = slots.numel(), y.shape[1]
+    H, W = mask.shape[1], mask.shape[2]
+    assert slots.dtype == torch.int32 and seg.dtype == torch.int32 and mask.dtype == torch.float32
+    assert seg.shape == mask.shape and y_valid.shape == y.shape and y_valid.dtype == torch.uint8
+    assert workspace.numel() >= lib().wvn_mission_propagate_workspace_bytes(n, smax)
+    check(lib().wvn_mission_propagate(ptr(slots), ptr(restart), n, ptr(K), ptr(pose), ptr(points), points.shape[0],
+                                      ptr(traversability), ptr(seg), ptr(mask), H, W, smax, ptr(y), ptr(y_valid),
+                                      ptr(slot_valid), ptr(workspace), stream()))
+
+
 def flip_average(head, batch, npad, grid):
     """STEGO flip-TTA merge of the head output [2*batch*npad, C] in place (see include/wvn_b200.h)."""
     assert head.is_contiguous() and head.shape[0] == 2 * batch * npad and head.dtype == torch.float32

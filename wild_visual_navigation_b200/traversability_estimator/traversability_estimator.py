@@ -5,9 +5,12 @@ On the hot path and implemented: ``__init__`` (seed 42, SimpleMLP + Traversabili
 ``anomaly_detection=True`` LinearRnvp + AnomalyLoss, Adam — :78-105), ``make_batch`` (:431-446), ``train`` (:448-497, same return dict), ``save_checkpoint`` /
 ``load_checkpoint`` (:377-429, same file format incl. a torch.optim.Adam-compatible
 ``optimizer_state_dict``), ``pause_learning`` / ``step`` / ``loss``.
-The mission / supervision graphs (networkx + liegroups, nodes.py / graphs.py), footprint
-projection and visualisation are OUT OF SCOPE (SURVEY.md §2): mission nodes are kept in a plain
-list and must already carry their per-segment features and supervision (``MissionNode``).
+Mission nodes that carry camera data (the reference's own ``MissionNode`` objects, or whole
+``FeatureExtractor.extract_batch`` results through ``add_mission_frames``) go into a device-resident
+mission graph (mission_graph.py), and ``add_supervision_node`` propagates each footprint into every
+in-range node's labels on the GPU; ``train()`` then samples labelled nodes from that graph as the
+reference does.  Nodes without camera data are kept in a plain list and must already carry their
+per-segment features and supervision (``MissionNode`` below), as before.  Visualisation is out of scope.
 
 ``train()`` runs forward + loss + backward + Adam as one fixed sequence of fp32 CUDA kernels
 (csrc/mlp_train_fused.cu) with all scalars on the device.
@@ -29,6 +32,7 @@ import torch
 from .. import ops
 from ..model import get_model
 from ..utils import AnomalyLoss, Batch, Data, TraversabilityLoss
+from .mission_graph import DistanceWindowGraph, MissionGraph, footprint_between
 
 
 def default_params(anomaly_detection: bool = False):
@@ -106,7 +110,7 @@ class TraversabilityEstimator:
     def __init__(self, params=None, device: str = "cuda", max_distance: float = 3, image_distance_thr: float = None,
                  supervision_distance_thr: float = None, min_samples_for_training: int = 10, vis_node_index: int = 10,
                  mode=None, extraction_store_folder=None, anomaly_detection: bool = False, process_group=None,
-                 max_rows: int = 4096):
+                 max_rows: int = 4096, mission_graph_capacity: int = 256, mission_graph_smax: int = None):
         if process_group is not None and not isinstance(process_group, torch.distributed.ProcessGroup):
             raise ValueError(f"process_group must be a torch.distributed.ProcessGroup, got {type(process_group).__name__}")
         self._device = device
@@ -117,6 +121,11 @@ class TraversabilityEstimator:
         self._params = params if params is not None else default_params(anomaly_detection)
         self._anomaly_detection = anomaly_detection
         self._mission_nodes = []
+        # the device mission graph is made by the first node that carries camera data (its image size fixes the slots)
+        self._mission_graph = None
+        self._mission_graph_capacity, self._mission_graph_smax = mission_graph_capacity, mission_graph_smax
+        self._image_distance_thr, self._max_distance = image_distance_thr, max_distance
+        self._supervision_graph = DistanceWindowGraph(edge_distance=supervision_distance_thr, max_distance=max_distance)
         self._learning_lock = Lock()
         self._pause_training = False
 
@@ -195,14 +204,86 @@ class TraversabilityEstimator:
             raise RuntimeError("device changes after construction are not supported (buffers are device-bound)")
 
     # ---- nodes -----------------------------------------------------------------------------
-    def add_mission_node(self, node: MissionNode, verbose: bool = False):
-        self._mission_nodes.append(node)
+    def add_mission_node(self, node, verbose: bool = False):
+        """A node with camera data (``features``, ``feature_segments``, ``pose_cam_in_world``, ``image_projector`` or
+        ``K``, ``timestamp``; the reference's ``MissionNode`` has them) goes into the device mission graph, gated by
+        ``image_distance_thr`` (traversability_estimator.py:166-196): returns True when it was added for training.
+        Any other node (``MissionNode`` above, labels already pooled) is appended to the plain list, as before."""
+        if getattr(node, "feature_segments", None) is None or getattr(node, "pose_cam_in_world", None) is None:
+            self._mission_nodes.append(node)
+            return True
+        seg, feat = node.feature_segments, node.features
+        K = getattr(node, "K", None)
+        if K is None:
+            K = node.image_projector.camera.intrinsics
+        K = K.reshape(-1, 4, 4)[0]
+        g = self._graph_for(seg.shape[-2], seg.shape[-1], feat.shape[0])
+        train = bool(getattr(node, "use_for_training", True))
+        added = g.add(feat, seg, K, node.pose_cam_in_world, float(node.timestamp),
+                      getattr(node, "pose_base_in_world", node.pose_cam_in_world), has_mask=train)
+        if added is not None and train and verbose:
+            print(f"adding node [{added}], total nodes [{g.get_num_nodes()}]")
+        return added is not None and train
+
+    def add_mission_frames(self, r, poses, K, timestamps, pose_cam_in_base=None):
+        """Adds a batch of frames straight from ``FeatureExtractor.extract_batch`` (``r``: seg [B,H,W], feat [B,S,D],
+        n_segments [B] on the device) to the device mission graph, device to device, each gated by
+        ``image_distance_thr`` like ``add_mission_node``.  ``poses``: [B,4,4] base poses in the world (host);
+        ``pose_cam_in_base``: [4,4] or [B,4,4] (default identity); ``K``: the scaled [4,4] or [B,4,4] camera matrices
+        of the H x W segmentation; ``timestamps``: B floats.  Returns the number of frames added."""
+        if r.get("n_segments") is None:
+            raise ValueError("add_mission_frames needs per-segment features (extract_batch with a segmentation)")
+        poses = torch.as_tensor(poses, dtype=torch.float32).cpu()
+        cam = poses if pose_cam_in_base is None else poses @ torch.as_tensor(pose_cam_in_base, dtype=torch.float32).cpu()
+        seg, feat = r["seg"], r["feat"]
+        g = self._graph_for(seg.shape[-2], seg.shape[-1], feat.shape[1])
+        return len(g.add_frames(feat, r["n_segments"], seg, K, cam, [float(t) for t in timestamps], poses))
+
+    def _graph_for(self, h, w, rows):
+        g = self._mission_graph
+        if g is None:
+            smax = self._mission_graph_smax or max(256, (int(rows) + 63) // 64 * 64)
+            g = MissionGraph(self._mission_graph_capacity, int(h), int(w), smax, self._model.input_size,
+                             device=self._device, edge_distance=self._image_distance_thr, max_distance=self._max_distance)
+            self._mission_graph = g
+        return g
+
+    def add_supervision_node(self, pnode):
+        """One footprint event (traversability_estimator.py:199-300): the supervision graph's edge gate (a node that is
+        too close only lowers the last node's traversability, pessimistically), the footprint between this node and the
+        last one, the 30 s mask sweep, the range query along the mission graph, then one ``wvn_mission_propagate`` launch
+        that renders, fmin-s and re-pools every in-range node's labels.  Host math on a few points, no device-to-host
+        copy.  Returns True when labels were propagated."""
+        if not pnode.is_valid():
+            return False
+        last_pnode = self._supervision_graph.get_last_node()
+        if not self._supervision_graph.add_node(pnode):
+            if last_pnode is not None:
+                last_pnode.update_traversability(pnode.traversability, pnode.traversability_var)
+            return False
+        if last_pnode is None or not last_pnode.is_valid():
+            return False
+        footprint = footprint_between(pnode, last_pnode)
+        g = self._mission_graph
+        last = g.get_last_node() if g is not None else None
+        if last is None or not last.has_mask:
+            return False
+        g.sweep(last.timestamp)
+        nodes = g.get_nodes_within_radius_range(self._supervision_graph.max_distance)
+        if len(nodes) < 1:
+            return False
+        g.propagate(nodes, footprint, pnode.traversability)
         return True
 
     def get_mission_nodes(self):
-        return self._mission_nodes
+        return self._mission_graph.get_nodes() if self._mission_graph is not None else self._mission_nodes
+
+    def get_supervision_nodes(self):
+        return self._supervision_graph.get_nodes()
 
     def get_num_valid_nodes(self):
+        if self._mission_graph is not None:
+            return self._mission_graph.get_num_valid_nodes()
         return sum(1 for n in self._mission_nodes if n.is_valid())
 
     def make_batch(self, batch_size: int = 8):
@@ -238,16 +319,26 @@ class TraversabilityEstimator:
         return conf
 
     def train(self):
-        """One step of the training loop; same gating and return dict as the reference (:448-497)."""
+        """One step of the training loop; same gating and return dict as the reference (:448-497).  With a device
+        mission graph the batch is sampled from it (sorted valid nodes, ``random.shuffle``, the first ``batch_size``)
+        and trained in the padded layout; reading the valid flags and row counts is one small device-to-host copy."""
         if self._pause_training:
             return {}
         num_valid_nodes = self.get_num_valid_nodes()
         return_dict = {"mission_graph_num_valid_node": num_valid_nodes}
         if num_valid_nodes > self._min_samples_for_training:
-            graph = self.make_batch(_get(_get(self._params, "ablation_data_module"), "batch_size"))
+            bs = _get(_get(self._params, "ablation_data_module"), "batch_size")
+            if self._mission_graph is not None:
+                g = self._mission_graph
+                self.last_sampled_nodes = g.get_n_random_valid_nodes(n=bs)
+                self.train_on_padded(*g.gather(self.last_sampled_nodes))
+                graph = True
+            else:
+                graph = self.make_batch(bs)
+                if graph is not None:
+                    self.train_on_batch(graph)
             if graph is not None:
-                log_step = (self._step % 20) == 0
-                self.train_on_batch(graph)
+                log_step = ((self._step - 1) % 20) == 0
                 m = self._trainer.metrics.tolist()  # the reference's three .item() calls, as one D2H copy
                 self._loss = torch.tensor(m[0])
                 if log_step:
