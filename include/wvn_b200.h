@@ -53,7 +53,9 @@ int wvn_check_device(void);
  * wvn_double_mlp_trainer_init_comm, wvn_double_mlp_trainer_stats, wvn_flow_train_step_padded, wvn_flow_init_comm,
  * wvn_flow_stats); no layout change.
  * 107: adds wvn_mission_propagate and wvn_mission_propagate_workspace_bytes (the mission graph's label propagation);
- * no layout change. */
+ * no layout change.  The SimpleGCN learner's functions (wvn_gcn_*) were added later under the same version number:
+ * they add symbols only.  A caller that binds every declared symbol at load (the Python package does) needs a library
+ * that exports them. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -531,6 +533,55 @@ int wvn_double_mlp_trainer_init_comm(wvn_double_mlp_trainer_t* t, const void* id
  * (trav - y)^2, labelled and live row counts, 0, loss_reco's min and max, the confidence-weighted traversability error
  * summed over the live rows.  Valid until the trainer is destroyed. */
 double* wvn_double_mlp_trainer_stats(wvn_double_mlp_trainer_t* t);
+
+/* ------------------------------------------------------------------------------------------
+ * SimpleGCN learner (model/simple_gcn.py, fp32): SimpleGCN(dim, True, [h1, h2, 1]) — GCNConv(dim, h1) ReLU
+ * GCNConv(h1, h2) ReLU GCNConv(h2, 1 + dim), sigmoid on column 0; output [rows, 1 + dim], SimpleMLP's layout.  Each
+ * GCNConv is torch_geometric 2.x's with its defaults: Z = D^-1/2 (A + I) D^-1/2 X W^T + b, A[i, j] the number of edges
+ * j -> i once the input's self-loops are dropped, D = 1 + the in-degree.  Edges are directed as given (not symmetrised).
+ * Bounds: 1 <= dim <= 1024, 1 <= h1, h2 <= 512.  params / exp_avg / exp_avg_sq: flat fp32 buffers of
+ * wvn_gcn_param_count floats in parameters() order (layers.{0,1,2}: bias, then lin.weight [out, in]).
+ * Rows come padded per frame: x [groups, rows_per_group, dim] fp32 with n_rows [groups] int32 (device; NULL: all) live
+ * rows per frame, and the frame's graph as edges [groups, edges_per_group, 2] int64 (source, target) local row ids of
+ * which the first n_edges[g] (device int32) are read.  Edges with an endpoint outside the frame's live rows are dropped.
+ * The handle owns the workspaces for max_rows padded rows and max_edges padded edges (groups * edges_per_group).
+ * ---------------------------------------------------------------------------------------- */
+typedef struct wvn_gcn_trainer wvn_gcn_trainer_t;
+size_t wvn_gcn_param_count(int dim, int h1, int h2);
+/* cfg: the loss weights, anomaly_balanced, the generator's std_factor and Adam's lr / betas / eps; grads: optional
+ * caller-owned device buffer of wvn_gcn_param_count floats (NULL: the trainer allocates it). */
+int wvn_gcn_trainer_create(int dim, int h1, int h2, int max_rows, int max_edges, const wvn_train_config* cfg,
+                           float* grads, wvn_gcn_trainer_t** out);
+void wvn_gcn_trainer_destroy(wvn_gcn_trainer_t* t);
+/* The ConfidenceGenerator method and state of the train step, as wvn_mlp_trainer_set_confidence. */
+int wvn_gcn_trainer_set_confidence(wvn_gcn_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
+                                   double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov);
+/* As wvn_mlp_trainer_copy_confidence: a larger trainer takes over the generator state src keeps itself. */
+int wvn_gcn_trainer_copy_confidence(wvn_gcn_trainer_t* dst, const wvn_gcn_trainer_t* src, void* stream);
+/* One step of TraversabilityEstimator.train() with TraversabilityLoss on the padded frames and their graphs: graph
+ * build, forward, loss, the ConfidenceGenerator update, backward, Adam; no host synchronisation, bit-reproducible.
+ * y / y_valid / confidence_out are indexed by the COMPACTED row number (live rows of frame 0, then frame 1, ...).
+ * metrics_out (device, 7 floats, may be NULL): loss_total, loss_trav, loss_reco, loss_trav_confidence, cg_mean, cg_std,
+ * and 1 when some n_edges[g] was negative (the segment reducer's overflow flag; that frame's edges are not read), else 0.
+ * phase_mask and the data-parallel exchange as wvn_double_mlp_train_step_padded (statistics block:
+ * wvn_gcn_trainer_stats, the same 9 doubles; double 5 carries the overflow flag, so its SUM tells every rank). */
+int wvn_gcn_train_step_padded(wvn_gcn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                              long long* step_counter, const float* x, int groups, int rows_per_group,
+                              const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
+                              const float* y, const unsigned char* y_valid, float* cg_mean, float* cg_std,
+                              float* confidence_out, float* metrics_out, int phase_mask, void* stream);
+int wvn_gcn_trainer_init_comm(wvn_gcn_trainer_t* t, const void* id128, int rank, int world);
+/* The trainer's statistics block (device, 9 doubles), laid out as wvn_double_mlp_trainer_stats. */
+double* wvn_gcn_trainer_stats(wvn_gcn_trainer_t* t);
+/* SimpleGCN.forward on the same padded input (a negative n_edges[g]: no edges for that frame), then per live row
+ * traversability = out[:, 0] and the confidence of its reconstruction loss under the generator (mean / std device
+ * scalars, std_factor; ConfidenceGenerator.inference_without_update).  out (may be NULL): [groups * rows_per_group,
+ * 1 + dim], the live rows first in compacted order.  trav / confidence (may be NULL): [groups * rows_per_group] in
+ * PADDED order; padding rows are not written. */
+int wvn_gcn_infer_rows(wvn_gcn_trainer_t* t, const float* params, const float* x, int groups, int rows_per_group,
+                       const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
+                       const float* cg_mean, const float* cg_std, float std_factor, float* out, float* trav,
+                       float* confidence, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * LinearRnvp anomaly-detection learner (model/linear_rnvp.py, fp32): LinearRnvp(dim, [hidden]) with flow_n = 2,

@@ -140,6 +140,16 @@ SIGNATURES = {
     "wvn_double_mlp_train_step_padded": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
     "wvn_double_mlp_trainer_init_comm": (_I, [_P, _P, _I, _I]),
     "wvn_double_mlp_trainer_stats": (_P, [_P]),
+    "wvn_gcn_param_count": (_S, [_I, _I, _I]),
+    "wvn_gcn_trainer_create": (_I, [_I, _I, _I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
+    "wvn_gcn_trainer_destroy": (None, [_P]),
+    "wvn_gcn_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
+    "wvn_gcn_trainer_copy_confidence": (_I, [_P, _P, _P]),
+    "wvn_gcn_trainer_init_comm": (_I, [_P, _P, _I, _I]),
+    "wvn_gcn_trainer_stats": (_P, [_P]),
+    "wvn_gcn_train_step_padded": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I,
+                                       _P]),
+    "wvn_gcn_infer_rows": (_I, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _F, _P, _P, _P, _P]),
     "wvn_flow_param_count": (_S, [_I, _I]),
     "wvn_flow_create": (_I, [_I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
     "wvn_flow_destroy": (None, [_P]),

@@ -2,7 +2,7 @@
 
 Keeps the reference's class surface for the per-frame path (SURVEY.md §8b):
 ``FeatureExtractor`` / ``DinoInterface`` / ``TorchVisionInterface`` / ``StegoInterface`` / ``SegmentExtractor`` /
-``SimpleMLP`` / ``DoubleMLP`` / ``LinearRnvp`` / ``get_model`` / ``Data`` / ``Batch`` / ``ConfidenceGenerator`` /
+``SimpleMLP`` / ``DoubleMLP`` / ``SimpleGCN`` / ``LinearRnvp`` / ``get_model`` / ``Data`` / ``Batch`` / ``ConfidenceGenerator`` /
 ``TraversabilityLoss`` / ``AnomalyLoss`` / ``TraversabilityEstimator`` — implemented on hand-written CUDA
 kernels behind the C ABI in ``include/wvn_b200.h``.  No CPU fallback.
 """
@@ -11,7 +11,7 @@ import os
 WVN_ROOT_DIR = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 from .utils import Data, Batch, ConfidenceGenerator, TraversabilityLoss, AnomalyLoss  # noqa: E402,F401
-from .model import SimpleMLP, DoubleMLP, LinearRnvp, get_model  # noqa: E402,F401
+from .model import SimpleMLP, DoubleMLP, SimpleGCN, LinearRnvp, get_model  # noqa: E402,F401
 from .feature_extractor import (  # noqa: E402,F401
     DinoInterface,
     StegoInterface,

@@ -12,6 +12,7 @@
 #include "attention.h"
 #include "dense_kernels.h"
 #include "double_mlp_train.h"
+#include "gcn_train.h"
 #include "gemm.h"
 #include "host_common.h"
 #include "mlp_train.h"
@@ -1461,6 +1462,78 @@ int wvn_double_mlp_train_step_padded(wvn_double_mlp_trainer_t* t, float* params,
   WVN_REQUIRE(t, "wvn_double_mlp_train_step_padded: null trainer");
   return double_train_step_padded(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows,
                                   y, y_valid, cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
+}
+
+}  // extern "C"
+
+// ============================================================================================
+// SimpleGCN learner: graph build, row forward and online train step (gcn_train.cu)
+// ============================================================================================
+struct wvn_gcn_trainer {
+  GcnTrainer* impl = nullptr;
+};
+
+extern "C" {
+
+size_t wvn_gcn_param_count(int dim, int h1, int h2) { return gcn_param_count(shape_of(dim, h1, h2)); }
+
+int wvn_gcn_trainer_create(int dim, int h1, int h2, int max_rows, int max_edges, const wvn_train_config* cfg,
+                           float* grads, wvn_gcn_trainer_t** out) {
+  WVN_REQUIRE(cfg && out, "wvn_gcn_trainer_create: null argument");
+  WVN_PROPAGATE(wvn_check_device());
+  AdamCfg a;
+  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
+  GcnTrainer* impl = nullptr;
+  WVN_PROPAGATE(gcn_trainer_create(shape_of(dim, h1, h2), max_rows, max_edges, loss_of(cfg), a, grads, &impl));
+  wvn_gcn_trainer* t = new wvn_gcn_trainer();
+  t->impl = impl;
+  *out = t;
+  return WVN_OK;
+}
+
+void wvn_gcn_trainer_destroy(wvn_gcn_trainer_t* t) {
+  if (!t) return;
+  gcn_trainer_destroy(t->impl);
+  delete t;
+}
+
+int wvn_gcn_trainer_set_confidence(wvn_gcn_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
+                                   double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
+  WVN_REQUIRE(t, "wvn_gcn_trainer_set_confidence: null trainer");
+  return trainer_conf_bind(gcn_trainer_conf(t->impl), method, var, running_n, running_sum, running_sum_of_squares,
+                           kf_proc_cov, kf_meas_cov);
+}
+
+int wvn_gcn_trainer_copy_confidence(wvn_gcn_trainer_t* dst, const wvn_gcn_trainer_t* src, void* stream) {
+  WVN_REQUIRE(dst && src, "wvn_gcn_trainer_copy_confidence: null trainer");
+  return trainer_conf_copy(gcn_trainer_conf(dst->impl), gcn_trainer_conf(src->impl), S(stream));
+}
+
+int wvn_gcn_trainer_init_comm(wvn_gcn_trainer_t* t, const void* id128, int rank, int world) {
+  WVN_REQUIRE(t, "wvn_gcn_trainer_init_comm: null trainer");
+  return trainer_comm_init(gcn_trainer_comm(t->impl), id128, rank, world);
+}
+
+double* wvn_gcn_trainer_stats(wvn_gcn_trainer_t* t) { return t ? gcn_trainer_stats(t->impl) : nullptr; }
+
+int wvn_gcn_train_step_padded(wvn_gcn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                              long long* step_counter, const float* x, int groups, int rows_per_group,
+                              const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
+                              const float* y, const unsigned char* y_valid, float* cg_mean, float* cg_std,
+                              float* confidence_out, float* metrics_out, int phase_mask, void* stream) {
+  WVN_REQUIRE(t, "wvn_gcn_train_step_padded: null trainer");
+  return gcn_train_step_padded(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows,
+                               edges, edges_per_group, n_edges, y, y_valid, cg_mean, cg_std, confidence_out,
+                               metrics_out, phase_mask, S(stream));
+}
+
+int wvn_gcn_infer_rows(wvn_gcn_trainer_t* t, const float* params, const float* x, int groups, int rows_per_group,
+                       const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
+                       const float* cg_mean, const float* cg_std, float std_factor, float* out, float* trav,
+                       float* confidence, void* stream) {
+  WVN_REQUIRE(t, "wvn_gcn_infer_rows: null trainer");
+  return gcn_infer_rows(t->impl, params, x, groups, rows_per_group, n_rows, edges, edges_per_group, n_edges, cg_mean,
+                        cg_std, std_factor, out, trav, confidence, S(stream));
 }
 
 }  // extern "C"

@@ -12,8 +12,10 @@ benchmarked configuration and the tested one are the same object.  The step has 
 rows go to the trainer padded per frame with their device-side counts (csrc/mlp_train_fused.cu).
 
 ``model`` / ``anomaly_detection`` pick the learner as the nodes' ``model.name`` does: SimpleMLP (the default),
-DoubleMLP, or with ``anomaly_detection=True`` the LinearRnvp flow; each is built with ``input_size`` = the backbone's
-feature dimension and trains on the same padded rows, data-parallel with ``process_group``.
+DoubleMLP, SimpleGCN, or with ``anomaly_detection=True`` the LinearRnvp flow; each is built with ``input_size`` = the
+backbone's feature dimension and trains on the same padded rows, data-parallel with ``process_group``.  The SimpleGCN
+also reads each frame's segment adjacency (``edges`` / ``n_edges``), and its maps are segment-wise: the per-segment
+traversability and confidence on the frame's graph, scattered through ``seg`` on the device.
 """
 from __future__ import annotations
 
@@ -35,8 +37,9 @@ class HotPathStep:
                                    run_clustering=run_clustering, n_image_clusters=n_image_clusters, max_batch=batch,
                                    chunk=chunk, backbone_type=backbone_type, patch_size=patch_size)
         self.smax = self.fe.max_segments
-        if model not in ("SimpleMLP", "DoubleMLP"):
-            raise ValueError(f"HotPathStep: model must be 'SimpleMLP' or 'DoubleMLP', got {model!r}")
+        if model not in ("SimpleMLP", "DoubleMLP", "SimpleGCN"):
+            raise ValueError(f"HotPathStep: model must be 'SimpleMLP', 'DoubleMLP' or 'SimpleGCN', got {model!r}")
+        self.gcn = model == "SimpleGCN"
         if anomaly_detection and model != "SimpleMLP":
             raise ValueError("HotPathStep: anomaly_detection=True selects the LinearRnvp learner; leave model at its default")
         params = None
@@ -44,9 +47,9 @@ class HotPathStep:
             from .traversability_estimator.traversability_estimator import default_params
 
             params = default_params(anomaly_detection)
-            if model == "DoubleMLP":
-                params["model"]["name"] = "DoubleMLP"
-            cfg = {"SimpleMLP": "simple_mlp_cfg", "DoubleMLP": "double_mlp_cfg"}[model]
+            if model != "SimpleMLP":
+                params["model"]["name"] = model
+            cfg = {"SimpleMLP": "simple_mlp_cfg", "DoubleMLP": "double_mlp_cfg", "SimpleGCN": "simple_gcn_cfg"}[model]
             params["model"]["linear_rnvp_cfg" if anomaly_detection else cfg]["input_size"] = self.fe.feature_dim
         self.te = TraversabilityEstimator(params=params, device=device, process_group=process_group,
                                           max_rows=batch * self.smax, anomaly_detection=anomaly_detection)
@@ -61,6 +64,12 @@ class HotPathStep:
         holds one confidence per live row in compacted order; for the LinearRnvp flow it holds the labelled rows'
         (those ``y_valid`` sets), in order, and ``conf`` is None (the node publishes no confidence map there)."""
         r = self.fe.extract_batch(img)                                        # ViT + STEGO seg + pooling + graph
+        if self.gcn:   # segment-wise maps on each frame's graph; the step trains on the same rows and edges
+            trav, conf = self.ti.predict_frames(r["feat"], r["n_segments"], r["edges"], r["n_edges"], r["seg"])
+            crow = self.te.train_on_padded(r["feat"], r["n_segments"], y, y_valid, edges=r["edges"],
+                                           n_edges=r["n_edges"])
+            r["trav"], r["conf"], r["confidence_rows"] = trav, conf, crow
+            return r
         trav, conf = self.ti.predict_from_tokens(r["tokens"], self.input_size)   # per-pixel MLP -> maps
         crow = self.te.train_on_padded(r["feat"], r["n_segments"], y, y_valid)  # fwd + loss + bwd + (all-reduce) + Adam
         self.ti.refresh_weights()                                              # inference sees the updated MLP

@@ -21,6 +21,10 @@ DoubleMLP instantiation (csrc/pixel_head.cu: G of both networks interpolated, la
 other shapes, and ``predict_segments``, run the two networks packed as one block-structured MLP (layer 1 both nets'
 rows, layer 2 block-diagonal, layer 3 the traversability row on net 0's half and the reconstruction rows on net 1's)
 through the unfused GEMM chain.
+
+A ``SimpleGCN`` predicts segment-wise only (``predict_segments`` with the frame's segment adjacency, csrc/gcn_train.cu):
+there is no graph over pixels, so ``predict`` / ``predict_from_tokens`` raise ``ValueError`` (the reference's node
+builds ``Data(x=...)`` without ``edge_index`` and cannot run a GCN either).
 """
 from __future__ import annotations
 
@@ -28,12 +32,20 @@ import torch
 
 from . import ops
 from .model.linear_rnvp import LinearRnvp
+from .model.simple_gcn import SimpleGCN
 from .model.simple_mlp import DoubleMLP, SimpleMLP
 from .utils.confidence_generator import ConfidenceGenerator
 
 
 class TraversabilityInference:
     def __init__(self, dino, model: SimpleMLP, confidence_generator: ConfidenceGenerator, chunk_rows: int = 0):
+        self._gcn = isinstance(model, SimpleGCN)
+        if self._gcn:
+            model.check_supported()
+            self._dino, self._model, self._cg = dino, model, confidence_generator
+            self._gcn_infer = ops.GcnInference(model)
+            self._flow = self._double = False
+            return
         self._flow = isinstance(model, LinearRnvp)
         if self._flow:
             if model.flat_params is None or not model.flat_params.is_cuda:
@@ -60,7 +72,10 @@ class TraversabilityInference:
     def refresh_weights(self):
         """Re-pack the bf16 GEMM operands after the MLP parameters changed (the node's ``load_model``,
         wvn_feature_extractor_node.py:407-450, runs at <= 1 Hz).  For a LinearRnvp the bf16 operands of the per-pixel
-        path are re-packed; masks and permutations are read from the module's buffers on every call."""
+        path are re-packed; masks and permutations are read from the module's buffers on every call.  A SimpleGCN's
+        kernels read its fp32 parameters on every call: nothing to re-pack."""
+        if self._gcn:
+            return
         if self._flow:
             self._flow_infer.set_params(self._model.flat_params)
             return
@@ -79,11 +94,13 @@ class TraversabilityInference:
     @torch.no_grad()
     def predict(self, img: torch.Tensor):
         """img (B,3,H,W) in [0,1] -> (trav (B,H,H), conf (B,H,H)) fp32 on the device."""
+        self._no_pixels_for_gcn()
         tokens = self._dino.inference_tokens(img)
         return self.predict_from_tokens(tokens, img.shape[2])
 
     @torch.no_grad()
     def predict_from_tokens(self, tokens: torch.Tensor, out_size: int):
+        self._no_pixels_for_gcn()
         g = self._dino.grid
         if self._flow:   # anomaly mode: (trav, None) — the node publishes no confidence map here
             return self._flow_infer.pixels(self._model, tokens, (g, g), (out_size, out_size), self._cg.mean.data,
@@ -98,10 +115,35 @@ class TraversabilityInference:
         return self._mlp.pixels(tokens, (g, g), (out_size, out_size), self._cg.mean.data, self._cg.std.data,
                                 self._cg.std_factor)
 
+    def _no_pixels_for_gcn(self):
+        if self._gcn:
+            raise ValueError("SimpleGCN predicts per segment only (there is no graph over pixels): use predict_segments "
+                             "with the frame's edges")
+
     @torch.no_grad()
-    def predict_segments(self, feat: torch.Tensor, seg: torch.Tensor):
+    def predict_frames(self, feat, n_rows, edges, n_edges, seg):
+        """SimpleGCN, segment-wise on a batch as ``extract_batch`` leaves it: feat [B, smax, D], n_rows [B], edges
+        [B, E, 2] / n_edges [B] on the device, seg [B, H, W] -> (trav, conf) [B, H, W], each pixel its segment's value.
+        Device ops only (no host synchronisation)."""
+        if not self._gcn:
+            raise ValueError("predict_frames is the SimpleGCN's segment-wise path")
+        trav, conf = self._gcn_infer.rows_padded(feat, n_rows, edges, n_edges, self._cg.mean.data, self._cg.std.data,
+                                                 self._cg.std_factor)
+        B = seg.shape[0]
+        idx = seg.reshape(B, -1).long()
+        return trav.gather(1, idx).view_as(seg), conf.gather(1, idx).view_as(seg)
+
+    @torch.no_grad()
+    def predict_segments(self, feat: torch.Tensor, seg: torch.Tensor, edges: torch.Tensor = None):
         """Segment-wise mode (``prediction_per_pixel=False``, node :324-327): MLP on the S pooled rows,
-        scattered back through ``seg``.  For a LinearRnvp: (trav[seg], None), trav the confidence of each row's NLL."""
+        scattered back through ``seg``.  For a LinearRnvp: (trav[seg], None), trav the confidence of each row's NLL.
+        A SimpleGCN runs on the frame's graph ``edges`` (2, E) (source, target segment ids, as ``extract`` returns
+        them), which it requires; the other learners ignore it."""
+        if self._gcn:
+            if edges is None:
+                raise ValueError("predict_segments: a SimpleGCN needs the frame's edges (2, E)")
+            trav, conf = self._gcn_infer.rows(feat, edges, self._cg.mean.data, self._cg.std.data, self._cg.std_factor)
+            return trav[seg], conf[seg]
         if self._flow:
             return self._flow_infer.trav(self._model, feat, self._cg.mean.data, self._cg.std.data,
                                          self._cg.std_factor)[seg], None

@@ -1,11 +1,12 @@
 """Name -> model registry (reference: wild_visual_navigation/model/network_register.py:44-55)."""
 from .linear_rnvp import LinearRnvp
+from .simple_gcn import SimpleGCN
 from .simple_mlp import DoubleMLP, SimpleMLP
 
 
 def get_model(model_cfg):
-    """model_cfg: mapping / attribute bag with ``name`` and ``simple_mlp_cfg`` / ``double_mlp_cfg`` / ``linear_rnvp_cfg`` like
-    ``ExperimentParams.model`` (cfg/experiment_params.py:104-140)."""
+    """model_cfg: mapping / attribute bag with ``name`` and ``simple_mlp_cfg`` / ``double_mlp_cfg`` / ``simple_gcn_cfg`` /
+    ``linear_rnvp_cfg`` like ``ExperimentParams.model`` (cfg/experiment_params.py:104-140)."""
     get = (lambda k: model_cfg[k]) if isinstance(model_cfg, dict) else (lambda k: getattr(model_cfg, k))
     name = get("name")
     if name == "SimpleMLP":
@@ -16,6 +17,10 @@ def get_model(model_cfg):
         cfg = get("double_mlp_cfg")
         cfg = dict(cfg) if isinstance(cfg, dict) else dict(vars(cfg))
         return DoubleMLP(**cfg)
+    if name == "SimpleGCN":
+        cfg = get("simple_gcn_cfg")
+        cfg = dict(cfg) if isinstance(cfg, dict) else dict(vars(cfg))
+        return SimpleGCN(**cfg)
     if name == "LinearRnvp":
         cfg = get("linear_rnvp_cfg")
         cfg = dict(cfg) if isinstance(cfg, dict) else dict(vars(cfg))

@@ -879,6 +879,220 @@ class DoubleMlpTrainer(_TrainerHandle):
 
 
 # --------------------------------------------------------------------------------------------
+# SimpleGCN learner: graph convolutions over each frame's segment adjacency
+# --------------------------------------------------------------------------------------------
+def _check_edges(edges, n_edges, groups):
+    """edges [G, E, 2] integer (source, target local row ids), n_edges [G] int32 on the device -> (int64 edges, E)."""
+    if not torch.is_tensor(edges) or edges.dim() != 3 or edges.shape[0] != groups or edges.shape[2] != 2 \
+            or edges.is_floating_point():
+        raise ValueError(f"edges must be a ({groups}, E, 2) integer tensor")
+    if not torch.is_tensor(n_edges) or n_edges.dtype != torch.int32 or tuple(n_edges.shape) != (groups,):
+        raise ValueError(f"n_edges must be a ({groups},) int32 tensor")
+    return edges.contiguous().long(), int(edges.shape[1])
+
+
+def _graph_as_padded(x, edge_index):
+    """A batched graph (rows x [N, D], edge_index [2, E]) as one frame of the padded layout, without host sync."""
+    if edge_index is None or not torch.is_tensor(edge_index) or edge_index.dim() != 2 or edge_index.shape[0] != 2:
+        raise ValueError("SimpleGCN needs the graph's edge_index, a (2, E) integer tensor")
+    E = edge_index.shape[1]
+    edges = edge_index.to(x.device, torch.int64).t().contiguous().reshape(1, E, 2)
+    return edges, torch.full((1,), E, device=x.device, dtype=torch.int32)
+
+
+def _batch_as_frames(x, edge_index, ptr):
+    """A ``Batch.from_data_list`` graph split back into its nodes (``ptr`` [G + 1], host): feat [G, S, D] padded,
+    n_rows [G], each node's edges in local ids [G, E, 2] (stably grouped by the source's node) and n_edges [G].  The
+    per-frame graph build then scans each node's edges only, and the step is bit-identical to the one-frame form
+    (same compacted rows, same in-edge order per row).  Device ops only, no device-to-host copy."""
+    _graph_as_padded(x, edge_index)   # argument checks
+    ptr = [int(v) for v in ptr]
+    G, dev = len(ptr) - 1, x.device
+    sizes = [ptr[i + 1] - ptr[i] for i in range(G)]
+    S = max(max(sizes), 1)
+    idx = torch.tensor([g * S + r for g in range(G) for r in range(sizes[g])], dtype=torch.long)
+    feat = torch.zeros(G * S, x.shape[1], device=dev, dtype=torch.float32)
+    feat.index_copy_(0, idx.to(dev, non_blocking=True), x.float())
+    n_rows = torch.tensor(sizes, dtype=torch.int32).to(dev, non_blocking=True)
+    ei = edge_index.to(dev, torch.int64)
+    E = ei.shape[1]
+    ptr_d = torch.tensor(ptr, dtype=torch.int64).to(dev, non_blocking=True)
+    frame = (torch.searchsorted(ptr_d, ei[0].contiguous(), right=True) - 1).clamp(0, G - 1)
+    frame, order = torch.sort(frame, stable=True)
+    ei = ei[:, order]
+    counts = torch.zeros(G, device=dev, dtype=torch.int64).index_add_(0, frame, torch.ones_like(frame))
+    pos = torch.arange(E, device=dev) - (torch.cumsum(counts, 0) - counts)[frame]
+    edges = torch.full((G, max(E, 1), 2), -1, device=dev, dtype=torch.int64)
+    edges[frame, pos] = (ei - ptr_d[frame]).t()
+    return feat.view(G, S, -1), n_rows, edges, counts.to(torch.int32)
+
+
+class GcnTrainer(_TrainerHandle):
+    """The online train step of a SimpleGCN on its flat fp32 parameters (csrc/gcn_train.cu): graph build, the three
+    graph convolutions, TraversabilityLoss with the ConfidenceGenerator update, backward and Adam as one fixed launch
+    sequence without host synchronisation, bit-reproducible.  ``exp_avg`` / ``exp_avg_sq`` / ``step_counter`` are
+    torch.optim.Adam's state over the 6 parameter tensors in ``parameters()`` order.  Rows arrive padded per frame with
+    each frame's edges (``step_padded``) or as one batched graph (``step``).  With ``process_group`` the step is
+    global-batch exact (see ``_TrainerHandle``); no edge crosses frames, so sharding frames loses nothing.
+    ``metrics[6]`` is 1 after a step that met a negative edge count (the segment reducer's overflow flag)."""
+
+    _DESTROY = "wvn_gcn_trainer_destroy"
+    _SET_CONFIDENCE = "wvn_gcn_trainer_set_confidence"
+    _COPY_CONFIDENCE = "wvn_gcn_trainer_copy_confidence"
+    _INIT_COMM = "wvn_gcn_trainer_init_comm"
+
+    def __init__(self, model, max_rows=4096, max_edges=16384, w_trav=0.03, w_reco=0.5, std_factor=0.5,
+                 anomaly_balanced=True, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, process_group=None):
+        model.check_supported()
+        _C.require_device()
+        params = model.flat_params
+        dev = params.device
+        self.model = model
+        self.dim, (self.h1, self.h2) = model.input_size, model.hidden
+        self.n_params = lib().wvn_gcn_param_count(self.dim, self.h1, self.h2)
+        assert params.numel() == self.n_params and params.dtype == torch.float32
+        self.cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
+        self.grads = torch.zeros(self.n_params, device=dev)
+        self.exp_avg = torch.zeros(self.n_params, device=dev)
+        self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
+        self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
+        self.metrics = torch.zeros(7, device=dev)
+        self.cg_mean = torch.zeros(1, device=dev)
+        self.cg_std = torch.ones(1, device=dev)
+        self.pg = process_group
+        self.max_edges = int(max_edges)
+        self._h = None
+        self._conf = None
+        self._create(max_rows)
+
+    def _new_handle(self, max_rows):
+        h = c_void_p()
+        check(lib().wvn_gcn_trainer_create(self.dim, self.h1, self.h2, max_rows, self.max_edges, byref(self.cfg),
+                                           ptr(self.grads), byref(h)))
+        return h
+
+    def _create(self, max_rows):
+        super()._create(max_rows)
+        self.conf = torch.empty(self.max_rows, device=self.grads.device)
+        self.stats = _device_doubles(lib().wvn_gcn_trainer_stats(self._h), 9, self.grads.device)
+
+    def _reserve_edges(self, rows, edges):
+        if edges > self.max_edges:
+            self.max_edges = int(edges * 1.5)
+            self._create(max(self.max_rows, int(rows)))
+        else:
+            self._reserve(rows)
+
+    def _grad_exchange(self):
+        return (self.grads, self.stats[8:9])   # + the confidence-weighted error sum, kept in fp64
+
+    def _run(self, x, groups, rpg, n_rows, edges, epg, n_edges, y, y_valid):
+        self._reserve_edges(groups * rpg, groups * epg)
+        x = x.contiguous().float()
+        y = y.contiguous().float()
+        yv = y_valid.contiguous().to(torch.uint8)
+        s = stream()
+
+        def phase(mask):
+            check(lib().wvn_gcn_train_step_padded(
+                self._h, ptr(self.model.flat_params), ptr(self.exp_avg), ptr(self.exp_avg_sq), ptr(self.step_counter),
+                ptr(x), groups, rpg, ptr(n_rows), ptr(edges), epg, ptr(n_edges), ptr(y), ptr(yv), ptr(self.cg_mean),
+                ptr(self.cg_std), ptr(self.conf), ptr(self.metrics), mask, s))
+
+        self._run_phases(phase)
+
+    def step_padded(self, feat, n_rows, edges, n_edges, y, y_valid):
+        """feat [G, S, D] f32 padded per frame, n_rows [G] int32 (device); edges [G, E, 2] (source, target) local row
+        ids with n_edges [G] int32 (device) valid rows.  y / y_valid are indexed by the compacted row number.  Returns
+        the confidence buffer (compacted order; the live prefix has sum(n_rows) entries — no host sync happens here)."""
+        G, S = _check_padded(feat, n_rows, self.dim)
+        edges, E = _check_edges(edges, n_edges, G)
+        self._run(feat, G, S, n_rows, edges, E, n_edges, y, y_valid)
+        return self.conf
+
+    def step(self, x, edge_index, y, y_valid, ptr=None):
+        """x [R, D] f32 with the batched graph edge_index [2, E] (Batch.from_data_list offsets), y [R] f32, y_valid [R]
+        bool.  ``ptr`` (host, the batch's node boundaries): each node becomes a frame of its own, so the graph build
+        scans each node's edges rather than the whole batch's; the result is the same bit for bit.  Returns the
+        confidence vector [R]; metrics stay on the device in ``self.metrics``."""
+        R = x.shape[0]
+        if ptr is not None and len(ptr) > 2:
+            feat, n_rows, edges, n_edges = _batch_as_frames(x, edge_index, ptr)
+            self._run(feat, feat.shape[0], feat.shape[1], n_rows, edges, edges.shape[1], n_edges, y, y_valid)
+            return self.conf[:R]
+        edges, n_edges = _graph_as_padded(x, edge_index)
+        self._run(x, 1, R, None, edges, edges.shape[1], n_edges, y, y_valid)
+        return self.conf[:R]
+
+
+class GcnInference:
+    """SimpleGCN forward and per-row traversability / confidence on rows with their graph (csrc/gcn_train.cu, the
+    trainer's forward kernels on a handle of its own).  Reads the model's flat parameters on every call."""
+
+    def __init__(self, model, max_rows=1024, max_edges=8192):
+        model.check_supported()
+        _C.require_device()
+        self.model = model
+        self.dim, (self.h1, self.h2) = model.input_size, model.hidden
+        self.cfg = TrainConfig(0.0, 0.0, 0.5, 0, 0.0, 0.9, 0.999, 1e-8)
+        self._h = None
+        self.max_rows, self.max_edges = 0, 0
+        self._create(max_rows, max_edges)
+
+    def _create(self, rows, edges):
+        h = c_void_p()
+        rows, edges = max(int(rows), self.max_rows), max(int(edges), self.max_edges)
+        check(lib().wvn_gcn_trainer_create(self.dim, self.h1, self.h2, rows, edges, byref(self.cfg), None, byref(h)))
+        if self._h is not None:
+            lib().wvn_gcn_trainer_destroy(self._h)
+        self._h, self.max_rows, self.max_edges = h, rows, edges
+
+    def _run(self, x, groups, rpg, n_rows, edges, epg, n_edges, cg_mean=None, cg_std=None, std_factor=0.5,
+             want_out=False, want_rows=True):
+        if groups * rpg > self.max_rows or groups * epg > self.max_edges:
+            self._create(max(self.max_rows, int(groups * rpg * 1.5)), max(self.max_edges, int(groups * epg * 1.5)))
+        x = x.contiguous().float()
+        dev = x.device
+        out = torch.empty(groups * rpg, self.dim + 1, device=dev) if want_out else None
+        trav = torch.full((2, groups * rpg), float("nan"), device=dev) if want_rows else None
+        trav, conf = (trav[0], trav[1]) if want_rows else (None, None)
+        check(lib().wvn_gcn_infer_rows(self._h, ptr(self.model.flat_params), ptr(x), groups, rpg, ptr(n_rows), ptr(edges),
+                                       epg, ptr(n_edges), ptr(cg_mean), ptr(cg_std), float(std_factor), ptr(out),
+                                       ptr(trav), ptr(conf), stream()))
+        return out, trav, conf
+
+    def forward_graph(self, x, edge_index):
+        """SimpleGCN.forward: x [N, D] with edge_index [2, E] -> (N, 1 + D)."""
+        N = x.shape[0]
+        edges, n_edges = _graph_as_padded(x, edge_index)
+        out, _, _ = self._run(x, 1, N, None, edges, edges.shape[1], n_edges, want_out=True, want_rows=False)
+        return out
+
+    def rows(self, x, edge_index, cg_mean, cg_std, std_factor):
+        """x [N, D] with its graph edge_index [2, E] -> (trav [N], conf [N]) fp32."""
+        N = x.shape[0]
+        edges, n_edges = _graph_as_padded(x, edge_index)
+        _, trav, conf = self._run(x, 1, N, None, edges, edges.shape[1], n_edges, cg_mean, cg_std, std_factor)
+        return trav, conf
+
+    def rows_padded(self, feat, n_rows, edges, n_edges, cg_mean, cg_std, std_factor):
+        """feat [G, S, D] with n_rows [G] and the frames' edges [G, E, 2] / n_edges [G] -> (trav [G, S], conf [G, S]),
+        padding rows NaN."""
+        G, S = _check_padded(feat, n_rows, self.dim)
+        edges, E = _check_edges(edges, n_edges, G)
+        _, trav, conf = self._run(feat, G, S, n_rows, edges, E, n_edges, cg_mean, cg_std, std_factor)
+        return trav.view(G, S), conf.view(G, S)
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().wvn_gcn_trainer_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+# --------------------------------------------------------------------------------------------
 # LinearRnvp flow (anomaly-detection learner): fp32 row forward and online train step
 # --------------------------------------------------------------------------------------------
 def flow_buffers(model):

@@ -227,11 +227,12 @@ def range_query(timestamps, edges, max_distance):
 class MissionGraphNode:
     """A view of one node of a ``MissionGraph``: host bookkeeping plus its slot in the device buffers."""
 
-    __slots__ = ("graph", "slot", "serial", "timestamp", "pose_base_in_world", "has_mask")
+    __slots__ = ("graph", "slot", "serial", "timestamp", "pose_base_in_world", "has_mask", "has_edges")
 
     def __init__(self, graph, slot, serial, timestamp, pose_base_in_world, has_mask):
         self.graph, self.slot, self.serial = graph, slot, serial
         self.timestamp, self.pose_base_in_world, self.has_mask = timestamp, pose_base_in_world, has_mask
+        self.has_edges = False
 
     def __lt__(self, other):
         return self.timestamp < other.timestamp
@@ -275,10 +276,13 @@ class MissionGraph:
 
     Device buffers (``capacity`` slots): ``features`` [cap, smax, D] fp32, ``meta`` [2, cap] int32 (row 0 = n_rows,
     row 1 = valid flag written by each propagation), ``seg`` [cap, H, W] int32, ``mask`` [cap, H, W] fp32 (NaN =
-    unlabelled), ``y`` [cap, smax] fp32, ``y_valid`` [cap, smax] uint8, ``K`` / ``pose_cam_in_world`` [cap, 4, 4] fp32."""
+    unlabelled), ``y`` [cap, smax] fp32, ``y_valid`` [cap, smax] uint8, ``K`` / ``pose_cam_in_world`` [cap, 4, 4] fp32.
+    With ``emax > 0`` (a learner that reads the segment adjacency) also ``edges`` [cap, emax, 2] int32 (source, target
+    segment ids) and ``n_edges`` [cap] int32; a frame with more than ``emax`` edges is stored with the segment reducer's
+    overflow flag (a negative count), which the train step reports."""
 
     def __init__(self, capacity: int, height: int, width: int, smax: int, dim: int, device="cuda",
-                 edge_distance: float = None, max_distance: float = float("inf")):
+                 edge_distance: float = None, max_distance: float = float("inf"), emax: int = 0):
         if capacity < 1 or smax < 1 or smax > 4096 or height < 1 or width < 1:
             raise ValueError(f"MissionGraph: bad geometry (capacity {capacity}, {height}x{width}, smax {smax})")
         dev = torch.device(device)
@@ -293,6 +297,9 @@ class MissionGraph:
         self.y_valid = torch.zeros(capacity, smax, device=dev, dtype=torch.uint8)
         self.K = torch.eye(4, device=dev).repeat(capacity, 1, 1)
         self.pose_cam_in_world = torch.eye(4, device=dev).repeat(capacity, 1, 1)
+        self.emax = int(emax)
+        self.edges = torch.zeros(capacity, emax, 2, device=dev, dtype=torch.int32) if emax > 0 else None
+        self.n_edges = torch.zeros(capacity, device=dev, dtype=torch.int32) if emax > 0 else None
         self._ws = ops.mission_propagate_workspace(capacity, smax, dev)
         self._nodes = []          # live nodes, oldest first
         self._edges = []          # _edges[k]: distance between _nodes[k] and _nodes[k + 1]
@@ -385,10 +392,12 @@ class MissionGraph:
         self.slot_valid.index_fill_(0, slots_t, 0)
         self._meta_host = None
 
-    def add(self, features, seg, K, pose_cam_in_world, timestamp, pose_base_in_world, has_mask=True):
+    def add(self, features, seg, K, pose_cam_in_world, timestamp, pose_base_in_world, has_mask=True, edges=None):
         """One node: features [S, D] (S <= smax), seg [H, W] (any integer dtype), K the scaled 4x4 camera matrix of the
-        H x W image, poses 4x4.  Returns the node, or None when the edge gate refuses it.  A node without a mask
-        (``has_mask=False``, the reference's ``use_for_training=False``) starts from a zero mask at its first event."""
+        H x W image, poses 4x4, and with edge storage its adjacency ``edges`` (2, E) (the reference's
+        ``feature_edges``; None: the node has none).  Returns the node, or None when the edge gate refuses it.  A node
+        without a mask (``has_mask=False``, the reference's ``use_for_training=False``) starts from a zero mask at its
+        first event."""
         S = features.shape[0]
         if S > self.smax or features.shape[1] != self.dim or tuple(seg.shape) != (self.height, self.width):
             raise ValueError(f"MissionGraph.add: features {tuple(features.shape)} / segmentation {tuple(seg.shape)} do "
@@ -406,12 +415,20 @@ class MissionGraph:
         self.features[slot, :S].copy_(features.to(self.device, torch.float32))
         self.seg[slot].copy_(seg.to(self.device))
         self._reset_slots(dev[132:136].view(torch.int32).long())
-        return self._commit(slot, timestamp, pose_base_in_world, has_mask)
+        node = self._commit(slot, timestamp, pose_base_in_world, has_mask)
+        if self.edges is not None and edges is not None:
+            E = edges.shape[1]
+            if E <= self.emax:
+                self.edges[slot, :E].copy_(edges.t().to(self.device, torch.int32))
+            self.n_edges[slot].fill_(E if E <= self.emax else -1)
+            node.has_edges = True
+        return node
 
-    def add_frames(self, feat, n_rows, seg, K, poses_cam_in_world, timestamps, poses_base_in_world):
+    def add_frames(self, feat, n_rows, seg, K, poses_cam_in_world, timestamps, poses_base_in_world, edges=None,
+                   n_edges=None):
         """A batch of frames as ``FeatureExtractor.extract_batch`` leaves them (feat [B, S, D], n_rows [B] int32 and
-        seg [B, H, W] on the device), copied device to device.  K / poses: [B, 4, 4] host tensors (K may be one 4x4).
-        Returns the nodes that passed the edge gate."""
+        seg [B, H, W] on the device, and with edge storage its ``edges`` [B, E, 2] / ``n_edges`` [B]), copied device to
+        device.  K / poses: [B, 4, 4] host tensors (K may be one 4x4).  Returns the nodes that passed the edge gate."""
         B, S, D = feat.shape
         if S > self.smax or D != self.dim or tuple(seg.shape[1:]) != (self.height, self.width):
             raise ValueError(f"MissionGraph.add_frames: feat {tuple(feat.shape)} / seg {tuple(seg.shape)} do not fit "
@@ -442,6 +459,13 @@ class MissionGraph:
         self.n_rows.index_copy_(0, slots_t, n_rows.to(torch.int32).index_select(0, frames_t))
         self.seg.index_copy_(0, slots_t, seg.index_select(0, frames_t).to(torch.int32))
         self._reset_slots(slots_t)
+        if self.edges is not None and edges is not None and n_edges is not None:
+            E = min(edges.shape[1], self.emax)
+            self.edges[:, :E].index_copy_(0, slots_t, edges[:, :E].index_select(0, frames_t).to(torch.int32))
+            ne = n_edges.to(torch.int32).index_select(0, frames_t)
+            self.n_edges.index_copy_(0, slots_t, torch.where(ne > self.emax, torch.full_like(ne, -1), ne))
+            for nd in self._nodes[-n:]:
+                nd.has_edges = True
         return self._nodes[-n:]
 
     # ---- one supervision event (add_supervision_node, traversability_estimator.py:233-289) ------------------------
@@ -487,3 +511,13 @@ class MissionGraph:
         y = torch.cat([self.y[nd.slot, : int(nr[nd.slot])] for nd in nodes])
         y_valid = torch.cat([self.y_valid[nd.slot, : int(nr[nd.slot])] for nd in nodes])
         return feat, n_rows, y, y_valid
+
+    def gather_edges(self, nodes):
+        """The sampled nodes' adjacency in the padded layout: edges [B, emax, 2] int64 (local segment ids) and n_edges
+        [B] int32.  Raises ValueError when the graph keeps no edges or a node came without them."""
+        if self.edges is None:
+            raise ValueError("MissionGraph: this graph keeps no segment adjacency (emax = 0)")
+        if any(not nd.has_edges for nd in nodes):
+            raise ValueError("SimpleGCN: a sampled mission node has no feature_edges (the segment adjacency)")
+        slots = torch.tensor([nd.slot for nd in nodes], dtype=torch.long).to(self.device, non_blocking=True)
+        return self.edges.index_select(0, slots).long(), self.n_edges.index_select(0, slots)

@@ -16,7 +16,9 @@ per-segment features and supervision (``MissionNode`` below), as before.  Visual
 (csrc/mlp_train_fused.cu) with all scalars on the device.
 In anomaly-detection mode the step is the LinearRnvp flow's (csrc/flow_train.cu: forward, NLL, confidence update,
 backward, Adam) on the labelled rows only.  With ``model.name == "DoubleMLP"`` the step is the DoubleMLP's
-(csrc/double_mlp_train.cu: the same TraversabilityLoss on two separate networks).
+(csrc/double_mlp_train.cu: the same TraversabilityLoss on two separate networks).  With ``model.name == "SimpleGCN"``
+it is the SimpleGCN's (csrc/gcn_train.cu: three graph convolutions over each node's segment adjacency,
+``MissionNode.feature_edges``), which needs every trained node to carry its edges.
 Every learner is data-parallel: with a ``process_group`` the confidence statistics (sums, row counts, extrema) and the
 flat gradient are all-reduced inside the step (NCCL over NVLink) for a global-batch step, and every learner takes rows
 still padded per frame (``train_on_padded``).
@@ -42,6 +44,7 @@ def default_params(anomaly_detection: bool = False):
         "model": {"name": "LinearRnvp" if anomaly_detection else "SimpleMLP",
                   "simple_mlp_cfg": {"input_size": 384, "hidden_sizes": [256, 32, 1], "reconstruction": True},
                   "double_mlp_cfg": {"input_size": 384, "hidden_sizes": [64, 32, 1]},
+                  "simple_gcn_cfg": {"input_size": 384, "reconstruction": True, "hidden_sizes": [256, 128, 1]},
                   "linear_rnvp_cfg": {"input_size": 384, "coupling_topology": [200], "mask_type": "odds",
                                       "conditioning_size": 0, "use_permutation": True, "single_function": False}},
         "loss": {"anomaly_balanced": True, "w_trav": 0.03, "w_temp": 0.0, "w_reco": 0.5, "method": "latest_measurement",
@@ -55,14 +58,16 @@ def default_params(anomaly_detection: bool = False):
 
 class MissionNode:
     """What ``MissionNode.as_pyg_data`` hands to the learner (nodes.py:199-241): per-segment
-    features ``x (S,D)``, supervision ``y (S,)`` in [0,1] and ``y_valid (S,)`` bool."""
+    features ``x (S,D)``, supervision ``y (S,)`` in [0,1] and ``y_valid (S,)`` bool, and the segment adjacency
+    ``feature_edges (2, E)`` (source, target) when the learner is a SimpleGCN."""
 
     def __init__(self, features: torch.Tensor, supervision_signal: torch.Tensor, supervision_signal_valid: torch.Tensor,
-                 timestamp: float = 0.0):
+                 timestamp: float = 0.0, feature_edges: torch.Tensor = None):
         self.features = features
         self.supervision_signal = supervision_signal
         self.supervision_signal_valid = supervision_signal_valid
         self.timestamp = timestamp
+        self.feature_edges = feature_edges
 
     def is_valid(self):
         return self.features is not None and self.supervision_signal is not None
@@ -81,8 +86,9 @@ class MissionNode:
     def as_pyg_data(self, anomaly_detection: bool = False):
         if anomaly_detection:   # the flow learns from the labelled rows only (nodes.py:207-214)
             v = self.supervision_signal_valid
-            return Data(x=self.features[v], y=self.supervision_signal[v], y_valid=v[v])
-        return Data(x=self.features, y=self.supervision_signal, y_valid=self.supervision_signal_valid)
+            return Data(x=self.features[v], y=self.supervision_signal[v], y_valid=v[v], edge_index=self.feature_edges)
+        return Data(x=self.features, y=self.supervision_signal, y_valid=self.supervision_signal_valid,
+                    edge_index=self.feature_edges)
 
 
 def _get(p, key):
@@ -110,7 +116,8 @@ class TraversabilityEstimator:
     def __init__(self, params=None, device: str = "cuda", max_distance: float = 3, image_distance_thr: float = None,
                  supervision_distance_thr: float = None, min_samples_for_training: int = 10, vis_node_index: int = 10,
                  mode=None, extraction_store_folder=None, anomaly_detection: bool = False, process_group=None,
-                 max_rows: int = 4096, mission_graph_capacity: int = 256, mission_graph_smax: int = None):
+                 max_rows: int = 4096, mission_graph_capacity: int = 256, mission_graph_smax: int = None,
+                 mission_graph_emax: int = None):
         if process_group is not None and not isinstance(process_group, torch.distributed.ProcessGroup):
             raise ValueError(f"process_group must be a torch.distributed.ProcessGroup, got {type(process_group).__name__}")
         self._device = device
@@ -124,6 +131,7 @@ class TraversabilityEstimator:
         # the device mission graph is made by the first node that carries camera data (its image size fixes the slots)
         self._mission_graph = None
         self._mission_graph_capacity, self._mission_graph_smax = mission_graph_capacity, mission_graph_smax
+        self._mission_graph_emax = mission_graph_emax
         self._image_distance_thr, self._max_distance = image_distance_thr, max_distance
         self._supervision_graph = DistanceWindowGraph(edge_distance=supervision_distance_thr, max_distance=max_distance)
         self._learning_lock = Lock()
@@ -136,6 +144,7 @@ class TraversabilityEstimator:
             raise ValueError("anomaly_detection=True goes with model.name 'LinearRnvp' (and only with it), got "
                              f"{_get(model_cfg, 'name')!r}")
         self._double = _get(model_cfg, "name") == "DoubleMLP"
+        self._gcn = _get(model_cfg, "name") == "SimpleGCN"
         self._model = get_model(model_cfg).to(self._device)
         self._model.train()
         gp = _get(self._params, "general")
@@ -159,6 +168,12 @@ class TraversabilityEstimator:
         self._traversability_loss.to(self._device)
         m = self._model
         cg = self._traversability_loss._confidence_generator
+        if self._gcn:
+            self._trainer = ops.GcnTrainer(m, max_rows=max_rows, w_trav=lp["w_trav"], w_reco=lp["w_reco"],
+                                           std_factor=cg.std_factor, anomaly_balanced=lp["anomaly_balanced"], lr=self._lr,
+                                           process_group=process_group)
+            self._bind_confidence_state()
+            return
         if self._double:
             self._trainer = ops.DoubleMlpTrainer(m, max_rows=max_rows, w_trav=lp["w_trav"], w_reco=lp["w_reco"],
                                                  std_factor=cg.std_factor, anomaly_balanced=lp["anomaly_balanced"],
@@ -220,7 +235,8 @@ class TraversabilityEstimator:
         g = self._graph_for(seg.shape[-2], seg.shape[-1], feat.shape[0])
         train = bool(getattr(node, "use_for_training", True))
         added = g.add(feat, seg, K, node.pose_cam_in_world, float(node.timestamp),
-                      getattr(node, "pose_base_in_world", node.pose_cam_in_world), has_mask=train)
+                      getattr(node, "pose_base_in_world", node.pose_cam_in_world), has_mask=train,
+                      edges=getattr(node, "feature_edges", None))
         if added is not None and train and verbose:
             print(f"adding node [{added}], total nodes [{g.get_num_nodes()}]")
         return added is not None and train
@@ -237,14 +253,19 @@ class TraversabilityEstimator:
         cam = poses if pose_cam_in_base is None else poses @ torch.as_tensor(pose_cam_in_base, dtype=torch.float32).cpu()
         seg, feat = r["seg"], r["feat"]
         g = self._graph_for(seg.shape[-2], seg.shape[-1], feat.shape[1])
-        return len(g.add_frames(feat, r["n_segments"], seg, K, cam, [float(t) for t in timestamps], poses))
+        return len(g.add_frames(feat, r["n_segments"], seg, K, cam, [float(t) for t in timestamps], poses,
+                                edges=r.get("edges"), n_edges=r.get("n_edges")))
 
     def _graph_for(self, h, w, rows):
         g = self._mission_graph
         if g is None:
             smax = self._mission_graph_smax or max(256, (int(rows) + 63) // 64 * 64)
+            # the SimpleGCN reads each node's segment adjacency: the slots keep up to emax edges (default 16 per
+            # segment, about 4x the density of the reference's STEGO graph); a frame with more is reported as overflowed
+            emax = (self._mission_graph_emax or 16 * smax) if self._gcn else 0
             g = MissionGraph(self._mission_graph_capacity, int(h), int(w), smax, self._model.input_size,
-                             device=self._device, edge_distance=self._image_distance_thr, max_distance=self._max_distance)
+                             device=self._device, edge_distance=self._image_distance_thr, max_distance=self._max_distance,
+                             emax=emax)
             self._mission_graph = g
         return g
 
@@ -290,7 +311,10 @@ class TraversabilityEstimator:
         """Samples ``batch_size`` random valid nodes (graphs.py:137-143) and concatenates them (utils/data.py:22-58)."""
         nodes = [n for n in self._mission_nodes if n.is_valid()]
         random.shuffle(nodes)
-        return Batch.from_data_list([n.as_pyg_data(self._anomaly_detection) for n in nodes[:batch_size]])
+        nodes = nodes[:batch_size]
+        if self._gcn and any(getattr(n, "feature_edges", None) is None for n in nodes):
+            raise ValueError("SimpleGCN: a sampled mission node has no feature_edges (the segment adjacency)")
+        return Batch.from_data_list([n.as_pyg_data(self._anomaly_detection) for n in nodes])
 
     # ---- the train step ----------------------------------------------------------------------
     def train_on_batch(self, graph, n_total=None):
@@ -299,24 +323,44 @@ class TraversabilityEstimator:
         with self._learning_lock:
             if self._anomaly_detection:   # AnomalyLoss: the flow's step on the labelled rows of the batch
                 conf = self._trainer.step(graph.x, graph.y_valid)
+            elif self._gcn:
+                if getattr(graph, "edge_index", None) is None:
+                    raise ValueError("SimpleGCN: the batch has no edge_index")
+                if n_total is not None and n_total != graph.x.shape[0]:
+                    raise ValueError("SimpleGCN: the global row count is all-reduced by the step, n_total must be the "
+                                     "batch's row count")
+                conf = self._trainer.step(graph.x, graph.edge_index, graph.y, graph.y_valid, ptr=getattr(graph, "ptr", None))
             else:
                 conf = self._trainer.step(graph.x, graph.y, graph.y_valid, n_total=n_total)
             self._last_confidence = conf
         self._step += 1
         return conf
 
-    def train_on_padded(self, feat, n_rows, y, y_valid):
+    def train_on_padded(self, feat, n_rows, y, y_valid, edges=None, n_edges=None):
         """The same step on rows that are still padded per frame, as ``FeatureExtractor.extract_batch`` returns them:
         ``feat`` (B, smax, D) float32, ``n_rows`` (B,) int32 on the device; ``y`` (float) / ``y_valid`` (bool or uint8)
         are 1-D and indexed by the compacted row number (what ``feat[mask]`` would give).  No host synchronisation (the
         gather happens inside the kernels).  In anomaly-detection mode the flow learns from the rows ``y_valid`` sets
-        and ignores ``y`` (it may be None); the returned confidences are those rows', in order."""
+        and ignores ``y`` (it may be None); the returned confidences are those rows', in order.  A SimpleGCN also needs
+        each frame's graph, ``edges`` (B, E, 2) (source, target) local segment ids with ``n_edges`` (B,) int32 valid rows
+        (``extract_batch``'s ``edges`` / ``n_edges``); the other learners ignore them.  A negative ``n_edges`` (the
+        segment reducer's overflow flag) trains that frame without its edges and sets ``metrics[6]``, which the next
+        ``train()`` raises on (``overflowed()`` reads it here, with one device-to-host copy)."""
         _check_padded_args(feat, n_rows, y, y_valid, self._model.input_size, y_optional=self._anomaly_detection)
+        if self._gcn and (edges is None or n_edges is None):
+            raise ValueError("train_on_padded: a SimpleGCN needs edges and n_edges")
         with self._learning_lock:
-            conf = self._trainer.step_padded(feat, n_rows, y, y_valid)
+            if self._gcn:
+                conf = self._trainer.step_padded(feat, n_rows, edges, n_edges, y, y_valid)
+            else:
+                conf = self._trainer.step_padded(feat, n_rows, y, y_valid)
             self._last_confidence = conf
         self._step += 1
         return conf
+
+    def overflowed(self) -> bool:
+        """True when the last SimpleGCN step met an overflowed segment adjacency on any rank (one device-to-host copy)."""
+        return self._gcn and bool(self._trainer.metrics[6].item() != 0)
 
     def train(self):
         """One step of the training loop; same gating and return dict as the reference (:448-497).  With a device
@@ -331,7 +375,11 @@ class TraversabilityEstimator:
             if self._mission_graph is not None:
                 g = self._mission_graph
                 self.last_sampled_nodes = g.get_n_random_valid_nodes(n=bs)
-                self.train_on_padded(*g.gather(self.last_sampled_nodes))
+                if self._gcn:
+                    edges, n_edges = g.gather_edges(self.last_sampled_nodes)
+                    self.train_on_padded(*g.gather(self.last_sampled_nodes), edges=edges, n_edges=n_edges)
+                else:
+                    self.train_on_padded(*g.gather(self.last_sampled_nodes))
                 graph = True
             else:
                 graph = self.make_batch(bs)
@@ -340,6 +388,9 @@ class TraversabilityEstimator:
             if graph is not None:
                 log_step = ((self._step - 1) % 20) == 0
                 m = self._trainer.metrics.tolist()  # the reference's three .item() calls, as one D2H copy
+                if self._gcn and m[6] != 0:
+                    raise ValueError("SimpleGCN: a frame's segment adjacency overflowed (negative n_edges); its edges "
+                                     "were not used")
                 self._loss = torch.tensor(m[0])
                 if log_step:
                     print(f"step: {self._step - 1} | loss: {m[0]:5f} | loss_trav: {m[1]:5f} | loss_reco: {m[2]:5f}")
