@@ -45,7 +45,7 @@ const char* wvn_last_error(void);
 int wvn_check_device(void);
 /* ABI version.  101: wvn_vit_config and wvn_gemm_ex_args gained a trailing `int registers` (0 = the layout of 100), so
  * callers that fill these structs by layout (ctypes mirrors, code compiled against an older header) must add the field.
- * 102: adds wvn_mlp_trainer_copy_confidence (no layout change).
+ * 102: adds wvn_mlp_trainer_copy_confidence; no layout change.
  * 103: wvn_gemm_ex_args gained trailing `residual` / `ldr` (epi 6); adds the ResNet handle, the im2col / max-pool
  * primitives and wvn_segment_pool_pyramid.
  * 104: adds the LinearRnvp flow handles, their functions wvn_flow_* and the struct wvn_flow_buffers; no layout change.
@@ -55,7 +55,11 @@ int wvn_check_device(void);
  * 107: adds wvn_mission_propagate and wvn_mission_propagate_workspace_bytes (the mission graph's label propagation);
  * no layout change.  The SimpleGCN learner's functions (wvn_gcn_*) were added later under the same version number:
  * they add symbols only.  A caller that binds every declared symbol at load (the Python package does) needs a library
- * that exports them. */
+ * that exports them.
+ * 108: the four learners' trainers share one handle type, wvn_trainer_t, and five entry points (wvn_trainer_destroy,
+ * wvn_trainer_set_confidence, wvn_trainer_copy_confidence, wvn_trainer_init_comm, wvn_trainer_stats) in place of
+ * each learner's own; wvn_flow_create is renamed wvn_flow_trainer_create and wvn_double_mlp_train_step is removed (its
+ * padded form with one group is the same step).  A learner's entry point refuses another learner's handle. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -440,6 +444,42 @@ int wvn_mlp_forward_f32(int dim, int h1, int h2, const float* params, const floa
                         float* h2_buf, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Trainers.  Every learner's train step (SimpleMLP, DoubleMLP, SimpleGCN, LinearRnvp) runs on a wvn_trainer_t made by
+ * that learner's create function; the functions below work on any of them.  A learner's own entry points return
+ * WVN_STATUS_INVALID, before they enqueue anything, when given another learner's handle.
+ *
+ * Data-parallel steps: each step has three phases (phase_mask 1, 2, 4; 7 = the whole step) with an exchange after the
+ * first two.  With a communicator (wvn_trainer_init_comm) the step issues both all-reduces itself, between its kernels
+ * on the caller's stream.  Without one, a data-parallel caller all-reduces, between the phases, the statistics block
+ * (wvn_trainer_stats) — doubles 0..5 with SUM, and for moving_average double 6 with MIN and 7 with MAX — after phase 1,
+ * and after phase 2 the gradient with SUM and, when the block has a ninth double, that double with SUM.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct wvn_trainer wvn_trainer_t;
+void wvn_trainer_destroy(wvn_trainer_t* t);
+/* ConfidenceGenerator method of the step (utils/confidence_generator.py:49-76): 0 latest_measurement (default),
+ * 1 running_mean (:94-115), 2 kalman_filter (:131-145 with utils/kalman_filter.py:78-111, D = 1, F = H = 1; kf_proc_cov /
+ * kf_meas_cov = its Q / R), 3 moving_average (:117-129, window of 5 steps kept inside the trainer).  The state the
+ * reference keeps in module parameters is read and updated in place through these device pointers — var (1,1) fp32;
+ * running_n / running_sum / running_sum_of_squares (1,) fp64 — each may be NULL (the trainer then keeps a private copy). */
+int wvn_trainer_set_confidence(wvn_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
+                               double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov);
+/* Copies the confidence state src keeps itself (moving_average's window of 5 steps; var / running sums given as NULL to
+ * set_confidence) into dst, ordered on `stream`.  For replacing a trainer by a larger one: create the new one, copy,
+ * then destroy the old one; the generator continues as if nothing had changed.  Both must be the same learner's. */
+int wvn_trainer_copy_confidence(wvn_trainer_t* dst, const wvn_trainer_t* src, void* stream);
+/* Library-owned NCCL communicator (libnccl.so.2 is resolved from the running process): rank 0 fills a 128-byte id with
+ * wvn_comm_unique_id, the caller broadcasts it by any means, every rank calls wvn_trainer_init_comm. */
+int wvn_comm_unique_id(void* id128);
+int wvn_trainer_init_comm(wvn_trainer_t* t, const void* id128, int rank, int world);
+/* The trainer's statistics block (device doubles; *n_doubles receives their number, 8 or 9): sum and sum of squares of
+ * the confidence input (loss_reco, or the NLL for LinearRnvp) over the labelled rows, sum of (trav - y)^2 (0 for
+ * LinearRnvp), labelled and live row counts (LinearRnvp: labelled, then 0), a sixth sum (SimpleGCN: the overflow flag,
+ * so its SUM tells every rank; else 0), the input's min and max; DoubleMLP and SimpleGCN add a ninth double, the
+ * confidence-weighted traversability error summed over the live rows, written by phase 2.  For SimpleMLP the block is
+ * the first 8 doubles of the trainer's scalars.  Valid until the trainer is destroyed. */
+double* wvn_trainer_stats(wvn_trainer_t* t, int* n_doubles);
+
+/* ------------------------------------------------------------------------------------------
  * Fused online train step — the same arithmetic as the three-phase entry points above in FOUR kernels, with the
  * row compaction (`feat[seg_mask]`, wvn_feature_extractor_node.py:324-327 / nodes.py:199-241) and, for data-parallel
  * runs, the two all-reduces inside the library (SURVEY.md §8b "wvn_mlp_train_step(..., ncclComm_t or NULL, ...)",
@@ -449,33 +489,15 @@ int wvn_mlp_forward_f32(int dim, int h1, int h2, const float* params, const floa
  *   number (live rows of group 0, then group 1, ...);  metrics_out (device, 6 floats, may be NULL): loss_total,
  *   loss_trav, loss_reco, loss_trav_confidence, cg_mean, cg_std.  params / exp_avg / exp_avg_sq: flat fp32 buffers in
  *   state_dict order (torch.optim.Adam state), step_counter: device int64.
- * phase_mask: 7 = whole step; 1 / 2 / 4 = forward+stats / backward+weight-gradients / metrics+Adam separately (a caller
- * without a library communicator all-reduces `scalars` (6 doubles) after phase 1 and `grads` (n_params + 1) after 2).
+ * phase_mask: 7 = whole step; 1 / 2 / 4 = forward+stats / backward+weight-gradients / metrics+Adam separately; the
+ * gradient a caller without a communicator all-reduces has n_params + 1 floats.
  * ---------------------------------------------------------------------------------------- */
-typedef struct wvn_mlp_trainer wvn_mlp_trainer_t;
 /* scalars: optional caller-owned device buffer of wvn_mlp_trainer_scalars_bytes(); grads: optional caller-owned device
  * buffer of n_params + 1 floats (NULL: the trainer allocates them with its workspace). */
 size_t wvn_mlp_trainer_scalars_bytes(void);
 int wvn_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_train_config* cfg, void* scalars,
-                           float* grads, wvn_mlp_trainer_t** out);
-void wvn_mlp_trainer_destroy(wvn_mlp_trainer_t* t);
-/* Library-owned NCCL communicator (libnccl.so.2 is resolved from the running process): rank 0 fills a 128-byte id with
- * wvn_comm_unique_id, the caller broadcasts it by any means, every rank calls wvn_mlp_trainer_init_comm (or
- * wvn_double_mlp_trainer_init_comm / wvn_flow_init_comm: every trainer takes a communicator the same way). */
-int wvn_comm_unique_id(void* id128);
-int wvn_mlp_trainer_init_comm(wvn_mlp_trainer_t* t, const void* id128, int rank, int world);
-/* ConfidenceGenerator method of the fused step (utils/confidence_generator.py:49-76): 0 latest_measurement (default),
- * 1 running_mean (:94-115), 2 kalman_filter (:131-145 with utils/kalman_filter.py:78-111, D = 1, F = H = 1; kf_proc_cov /
- * kf_meas_cov = its Q / R), 3 moving_average (:117-129, window of 5 steps kept inside the trainer).  The state the
- * reference keeps in module parameters is read and updated in place through these device pointers — var (1,1) fp32;
- * running_n / running_sum / running_sum_of_squares (1,) fp64 — each may be NULL (the trainer then keeps a private copy). */
-int wvn_mlp_trainer_set_confidence(wvn_mlp_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
-                                   double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov);
-/* Copies the confidence state src keeps itself (moving_average's window of 5 steps; var / running sums given as NULL to
- * set_confidence) into dst, ordered on `stream`.  For replacing a trainer by a larger one: create the new one, copy,
- * then destroy the old one; the generator continues as if nothing had changed. */
-int wvn_mlp_trainer_copy_confidence(wvn_mlp_trainer_t* dst, const wvn_mlp_trainer_t* src, void* stream);
-int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+                           float* grads, wvn_trainer_t** out);
+int wvn_mlp_train_step(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                        const float* x, int groups, int rows_per_group, const int* n_rows, const float* y,
                        const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
                        float* metrics_out, int phase_mask, void* stream);
@@ -488,7 +510,6 @@ int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, floa
  * fp32 buffers of wvn_double_mlp_param_count floats in parameters() order (networks.0.{0,2,4}.{weight,bias}, then
  * networks.1's), i.e. torch.optim.Adam's state.  The trainer owns the workspaces for max_rows rows.
  * ---------------------------------------------------------------------------------------- */
-typedef struct wvn_double_mlp_trainer wvn_double_mlp_trainer_t;
 size_t wvn_double_mlp_param_count(int dim, int h1, int h2);
 /* DoubleMLP.forward on x [rows, dim] fp32: a1_buf [2, rows, h1], a2_buf [2, rows, h2] (net 0, then net 1) receive the
  * hidden activations, out [rows, 1 + dim] the output. */
@@ -497,42 +518,20 @@ int wvn_double_mlp_forward_f32(int dim, int h1, int h2, const float* params, con
 /* cfg: the loss weights, anomaly_balanced, the generator's std_factor and Adam's lr / betas / eps; grads: optional
  * caller-owned device buffer of wvn_double_mlp_param_count floats (NULL: the trainer allocates it). */
 int wvn_double_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_train_config* cfg, float* grads,
-                                  wvn_double_mlp_trainer_t** out);
-void wvn_double_mlp_trainer_destroy(wvn_double_mlp_trainer_t* t);
-/* The ConfidenceGenerator method and state of the train step, as wvn_mlp_trainer_set_confidence. */
-int wvn_double_mlp_trainer_set_confidence(wvn_double_mlp_trainer_t* t, int method, float* var, double* running_n,
-                                          double* running_sum, double* running_sum_of_squares, float kf_proc_cov,
-                                          float kf_meas_cov);
-/* As wvn_mlp_trainer_copy_confidence: a larger trainer takes over the generator state src keeps itself. */
-int wvn_double_mlp_trainer_copy_confidence(wvn_double_mlp_trainer_t* dst, const wvn_double_mlp_trainer_t* src,
-                                           void* stream);
-/* One step of TraversabilityEstimator.train() with TraversabilityLoss on x [rows, dim] fp32, y [rows] fp32, y_valid
- * [rows] uint8 (0 < rows <= max_rows): forward, loss, the ConfidenceGenerator update, backward, Adam; one fixed
- * sequence of launches, no host synchronisation, bit-reproducible.  confidence_out [rows]; metrics_out (device,
- * 6 floats, may be NULL): loss_total, loss_trav, loss_reco, loss_trav_confidence, cg_mean, cg_std. */
-int wvn_double_mlp_train_step(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
-                              long long* step_counter, const float* x, int rows, const float* y,
-                              const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
-                              float* metrics_out, void* stream);
-/* The same step on rows padded per group, data-parallel.  x: [groups, rows_per_group, dim] fp32; n_rows: [groups] int32
- * (device) live rows per group, or NULL when every row is live; y / y_valid / confidence_out are indexed by the
- * COMPACTED row number (live rows of group 0, then group 1, ...).  Padding rows may hold anything (NaN included): they
- * are never read.  groups * rows_per_group <= max_rows.  wvn_double_mlp_train_step is this step with one group.
- * phase_mask: 7 = whole step; 1 = forward + the statistic sums, 2 = generator update + backward + weight gradients,
- * 4 = metrics + Adam.  With a communicator (wvn_double_mlp_trainer_init_comm) the step all-reduces the statistics after
- * phase 1 and the gradient after phase 2 itself; without one a data-parallel caller all-reduces, between the phases,
- * the statistics block (wvn_double_mlp_trainer_stats) — doubles 0..5 with SUM, and for moving_average double 6 with MIN
- * and 7 with MAX — after phase 1, and the gradient (n_params floats) and double 8 of the block with SUM after phase 2. */
-int wvn_double_mlp_train_step_padded(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                                  wvn_trainer_t** out);
+/* One step of TraversabilityEstimator.train() with TraversabilityLoss on rows padded per group: forward, loss, the
+ * ConfidenceGenerator update, backward, Adam; one fixed sequence of launches, no host synchronisation,
+ * bit-reproducible.  x: [groups, rows_per_group, dim] fp32; n_rows: [groups] int32 (device) live rows per group, or NULL
+ * when every row is live; y [fp32] / y_valid [uint8] / confidence_out are indexed by the COMPACTED row number (live rows
+ * of group 0, then group 1, ...).  Padding rows may hold anything (NaN included): they are never read.
+ * groups * rows_per_group <= max_rows.  metrics_out (device, 6 floats, may be NULL): loss_total, loss_trav, loss_reco,
+ * loss_trav_confidence, cg_mean, cg_std.  phase_mask: 7 = whole step; 1 = forward + the statistic sums, 2 = generator
+ * update + backward + weight gradients, 4 = metrics + Adam. */
+int wvn_double_mlp_train_step_padded(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
                                      long long* step_counter, const float* x, int groups, int rows_per_group,
                                      const int* n_rows, const float* y, const unsigned char* y_valid, float* cg_mean,
                                      float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
                                      void* stream);
-int wvn_double_mlp_trainer_init_comm(wvn_double_mlp_trainer_t* t, const void* id128, int rank, int world);
-/* The trainer's statistics block (device, 9 doubles): sum and sum of squares of loss_reco over the labelled rows, sum of
- * (trav - y)^2, labelled and live row counts, 0, loss_reco's min and max, the confidence-weighted traversability error
- * summed over the live rows.  Valid until the trainer is destroyed. */
-double* wvn_double_mlp_trainer_stats(wvn_double_mlp_trainer_t* t);
 
 /* ------------------------------------------------------------------------------------------
  * SimpleGCN learner (model/simple_gcn.py, fp32): SimpleGCN(dim, True, [h1, h2, 1]) — GCNConv(dim, h1) ReLU
@@ -546,39 +545,28 @@ double* wvn_double_mlp_trainer_stats(wvn_double_mlp_trainer_t* t);
  * which the first n_edges[g] (device int32) are read.  Edges with an endpoint outside the frame's live rows are dropped.
  * The handle owns the workspaces for max_rows padded rows and max_edges padded edges (groups * edges_per_group).
  * ---------------------------------------------------------------------------------------- */
-typedef struct wvn_gcn_trainer wvn_gcn_trainer_t;
 size_t wvn_gcn_param_count(int dim, int h1, int h2);
 /* cfg: the loss weights, anomaly_balanced, the generator's std_factor and Adam's lr / betas / eps; grads: optional
  * caller-owned device buffer of wvn_gcn_param_count floats (NULL: the trainer allocates it). */
 int wvn_gcn_trainer_create(int dim, int h1, int h2, int max_rows, int max_edges, const wvn_train_config* cfg,
-                           float* grads, wvn_gcn_trainer_t** out);
-void wvn_gcn_trainer_destroy(wvn_gcn_trainer_t* t);
-/* The ConfidenceGenerator method and state of the train step, as wvn_mlp_trainer_set_confidence. */
-int wvn_gcn_trainer_set_confidence(wvn_gcn_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
-                                   double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov);
-/* As wvn_mlp_trainer_copy_confidence: a larger trainer takes over the generator state src keeps itself. */
-int wvn_gcn_trainer_copy_confidence(wvn_gcn_trainer_t* dst, const wvn_gcn_trainer_t* src, void* stream);
+                           float* grads, wvn_trainer_t** out);
 /* One step of TraversabilityEstimator.train() with TraversabilityLoss on the padded frames and their graphs: graph
  * build, forward, loss, the ConfidenceGenerator update, backward, Adam; no host synchronisation, bit-reproducible.
  * y / y_valid / confidence_out are indexed by the COMPACTED row number (live rows of frame 0, then frame 1, ...).
  * metrics_out (device, 7 floats, may be NULL): loss_total, loss_trav, loss_reco, loss_trav_confidence, cg_mean, cg_std,
  * and 1 when some n_edges[g] was negative (the segment reducer's overflow flag; that frame's edges are not read), else 0.
- * phase_mask and the data-parallel exchange as wvn_double_mlp_train_step_padded (statistics block:
- * wvn_gcn_trainer_stats, the same 9 doubles; double 5 carries the overflow flag, so its SUM tells every rank). */
-int wvn_gcn_train_step_padded(wvn_gcn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+ * phase_mask as wvn_double_mlp_train_step_padded. */
+int wvn_gcn_train_step_padded(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
                               long long* step_counter, const float* x, int groups, int rows_per_group,
                               const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
                               const float* y, const unsigned char* y_valid, float* cg_mean, float* cg_std,
                               float* confidence_out, float* metrics_out, int phase_mask, void* stream);
-int wvn_gcn_trainer_init_comm(wvn_gcn_trainer_t* t, const void* id128, int rank, int world);
-/* The trainer's statistics block (device, 9 doubles), laid out as wvn_double_mlp_trainer_stats. */
-double* wvn_gcn_trainer_stats(wvn_gcn_trainer_t* t);
 /* SimpleGCN.forward on the same padded input (a negative n_edges[g]: no edges for that frame), then per live row
  * traversability = out[:, 0] and the confidence of its reconstruction loss under the generator (mean / std device
  * scalars, std_factor; ConfidenceGenerator.inference_without_update).  out (may be NULL): [groups * rows_per_group,
  * 1 + dim], the live rows first in compacted order.  trav / confidence (may be NULL): [groups * rows_per_group] in
  * PADDED order; padding rows are not written. */
-int wvn_gcn_infer_rows(wvn_gcn_trainer_t* t, const float* params, const float* x, int groups, int rows_per_group,
+int wvn_gcn_infer_rows(wvn_trainer_t* t, const float* params, const float* x, int groups, int rows_per_group,
                        const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
                        const float* cg_mean, const float* cg_std, float std_factor, float* out, float* trav,
                        float* confidence, void* stream);
@@ -593,7 +581,6 @@ int wvn_gcn_infer_rows(wvn_gcn_trainer_t* t, const float* params, const float* x
  * buffers on every call, so "odds" and "half" masks and a loaded permutation cost nothing.
  * The handle owns the workspaces for max_rows rows (allocated at create, nothing per call).
  * ---------------------------------------------------------------------------------------- */
-typedef struct wvn_flow wvn_flow_t;
 typedef struct {
   const float* mask0;       /* flows.0.mask [dim] fp32 */
   const float* mask1;       /* flows.2.mask [dim] fp32 */
@@ -605,19 +592,14 @@ typedef struct {
 size_t wvn_flow_param_count(int dim, int hidden);
 /* cfg: std_factor (the ConfidenceGenerator's) and Adam's lr / betas / eps are used; grads: optional caller-owned device
  * buffer of wvn_flow_param_count floats (NULL: the handle allocates it). */
-int wvn_flow_create(int dim, int hidden, int max_rows, const wvn_train_config* cfg, float* grads, wvn_flow_t** out);
-void wvn_flow_destroy(wvn_flow_t* h);
-/* The ConfidenceGenerator method and state of the train step, as wvn_mlp_trainer_set_confidence. */
-int wvn_flow_set_confidence(wvn_flow_t* h, int method, float* var, double* running_n, double* running_sum,
-                            double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov);
-/* As wvn_mlp_trainer_copy_confidence: a larger handle takes over the generator state src keeps itself. */
-int wvn_flow_copy_confidence(wvn_flow_t* dst, const wvn_flow_t* src, void* stream);
+int wvn_flow_trainer_create(int dim, int hidden, int max_rows, const wvn_train_config* cfg, float* grads,
+                            wvn_trainer_t** out);
 /* One step of TraversabilityEstimator.train() with AnomalyLoss on the rows of x [rows, dim] whose y_valid [rows] uint8
  * is set (NULL: every row): forward, loss -mean(sum(logprob) + log_det), the ConfidenceGenerator update with the
  * per-row NLL, backward, Adam.  No host synchronisation.  confidence_out [rows]: the labelled rows in order;
  * metrics_out (device, 6 floats, may be NULL): loss_total, loss_trav (0), loss_reco (0), labelled rows, cg_mean, cg_std.
  * phase_mask: 7 = whole step; 1 = forward + statistics + generator update, 2 = backward (gradient), 4 = Adam. */
-int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int wvn_flow_train_step(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                         const wvn_flow_buffers* buffers, const float* x, int rows, const unsigned char* y_valid,
                         float* cg_mean, float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
                         void* stream);
@@ -625,18 +607,12 @@ int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp
  * (device) live rows per group, or NULL; y_valid (NULL: all) is indexed by the COMPACTED row number and selects the
  * rows trained on; confidence_out: the selected rows in order.  Padding rows are never read.  phase_mask: 7 = whole step;
  * 1 = forward + the NLL sums, 2 = generator update + metrics + confidence + backward, 4 = Adam (note: phase 1 here
- * stops BEFORE the generator update, which needs the global sums).  With a communicator (wvn_flow_init_comm) the step
- * all-reduces itself; without one a data-parallel caller all-reduces the statistics block (wvn_flow_stats) — doubles
- * 0..5 with SUM, and for moving_average 6 with MIN and 7 with MAX — after phase 1 and the gradient after phase 2.
- * The loss is the NLL's mean over the global labelled count; a rank with no labelled row still takes part. */
-int wvn_flow_train_step_padded(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
-                               const wvn_flow_buffers* buffers, const float* x, int groups, int rows_per_group,
-                               const int* n_rows, const unsigned char* y_valid, float* cg_mean, float* cg_std,
-                               float* confidence_out, float* metrics_out, int phase_mask, void* stream);
-int wvn_flow_init_comm(wvn_flow_t* h, const void* id128, int rank, int world);
-/* The handle's statistics block (device, 8 doubles): sum and sum of squares of the NLL over the labelled rows, their
- * number, 0, 0, 0, the NLL's min and max.  Valid until the handle is destroyed. */
-double* wvn_flow_stats(wvn_flow_t* h);
+ * stops BEFORE the generator update, which needs the global sums).  The loss is the NLL's mean over the global labelled
+ * count; a rank with no labelled row still takes part. */
+int wvn_flow_train_step_padded(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                               long long* step_counter, const wvn_flow_buffers* buffers, const float* x, int groups,
+                               int rows_per_group, const int* n_rows, const unsigned char* y_valid, float* cg_mean,
+                               float* cg_std, float* confidence_out, float* metrics_out, int phase_mask, void* stream);
 
 /* Inference handle (no backward workspaces, no gradient buffer).  max_rows: rows of wvn_flow_infer_rows per call;
  * chunk_pixels: pixels per wgmma chunk of wvn_flow_infer_pixels (0 = 8192). */

@@ -13,11 +13,14 @@ output its SHA-256 plus a strided sample (every 101st element, as float32):
   * DinoInterface tokens of ViT-S/16 @448 at B = 8 (the patch-16 loader and patch-embed GEMM);
   * ops.mlp_forward_f32 of that SimpleMLP at R = 4096 and 65536 rows;
   * FlowInference.rows (z, log_det, logprob) of a seeded LinearRnvp(384, [200]) at R = 4096;
-  * after three FlowTrainer steps at R = 1024, per confidence method: the parameters, Adam's moments, the confidence
-    vector, the metrics and the generator's mean / std / var / running sums.
+  * after three train steps of each learner (MlpTrainer, DoubleMlpTrainer, GcnTrainer, FlowTrainer) created for
+    1024 rows, at R = 1024, 800 and 1500 (the last one replaces the handle by a larger one and copies its generator
+    over), per confidence method: the parameters, Adam's moments, the confidence vector, the metrics and the
+    generator's mean / std / var / running sums.
 `compare` reports, per output, whether the two builds agree bit for bit and, where not, the largest difference in
-the samples.  Every output here is deterministic for a given build (no atomics race in them), so any difference is
-the build's.
+the samples.  Every output here except the SimpleMLP train record is deterministic for a given build (no atomics race
+in them), so any difference there is the build's.  The fused SimpleMLP step adds its per-row and per-tile sums with
+atomics, so its record (mlp_train_*) can differ in the last bits between two runs of the same build.
 """
 import hashlib
 import json
@@ -117,7 +120,6 @@ def write(out_dir):
         _record(out_dir, f"mlp_forward_f32_{R}", ops.mlp_forward_f32(model.flat_params, x, 384, 256, 32), index)
 
     from wild_visual_navigation_b200 import LinearRnvp
-    from wild_visual_navigation_b200.utils import AnomalyLoss
 
     torch.manual_seed(42)
     flow = LinearRnvp(384, [200], use_permutation=True).to(dev)
@@ -125,27 +127,54 @@ def write(out_dir):
     rows = ops.FlowInference(384, 200, max_rows=4096).rows(flow, x)
     for k in ("z", "log_det", "logprob"):
         _record(out_dir, f"flow_rows_{k}", rows[k], index)
-    for method in ("latest_measurement", "running_mean", "kalman_filter", "moving_average"):
+
+    # ---- the four learners' train steps, with a regrowth in the last step
+    from wild_visual_navigation_b200 import DoubleMLP, SimpleGCN
+
+    def learner(kind):
         torch.manual_seed(42)
-        flow = LinearRnvp(384, [200], use_permutation=True).to(dev)
-        cg = AnomalyLoss(0.5, method).to(dev)._confidence_generator
-        tr = ops.FlowTrainer(flow, max_rows=1024)
-        tr.cg_mean, tr.cg_std = cg.mean.data, cg.std.data
-        kf = getattr(cg, "_kalman_filter", None)
-        tr.set_confidence(cg.method_id, cg.var.data, getattr(cg, "running_n", None), getattr(cg, "running_sum", None),
-                          getattr(cg, "running_sum_of_squares", None),
-                          kf_proc_cov=float(kf.proc_cov.item()) if kf is not None else 0.2,
-                          kf_meas_cov=float(kf.meas_cov.item()) if kf is not None else 1.0)
-        gs = torch.Generator(device=dev).manual_seed(14)
-        for _ in range(3):
-            conf = tr.step(torch.randn(1024, 384, device=dev, generator=gs) * 0.5)
-        out = {"params": flow.flat_params, "exp_avg": tr.exp_avg, "exp_avg_sq": tr.exp_avg_sq, "conf": conf,
-               "metrics": tr.metrics, "cg_mean": cg.mean, "cg_std": cg.std, "cg_var": cg.var}
-        for k in ("running_n", "running_sum", "running_sum_of_squares"):
-            if hasattr(cg, k):
-                out["cg_" + k] = getattr(cg, k)
-        for k, t in out.items():
-            _record(out_dir, f"flow_train_{method}_{k}", t, index)
+        if kind == "mlp":
+            m = SimpleMLP(384, [256, 32, 1], True).to(dev)
+            return m, ops.MlpTrainer(m.flat_params, 384, 256, 32, max_rows=1024)
+        if kind == "double_mlp":
+            m = DoubleMLP(384, [64, 32, 1]).to(dev)
+            return m, ops.DoubleMlpTrainer(m, max_rows=1024)
+        if kind == "gcn":
+            m = SimpleGCN(384, True, [256, 128, 1]).to(dev)
+            return m, ops.GcnTrainer(m, max_rows=1024, max_edges=4096)
+        m = LinearRnvp(384, [200], use_permutation=True).to(dev)
+        return m, ops.FlowTrainer(m, max_rows=1024)
+
+    for kind in ("mlp", "double_mlp", "gcn", "flow"):
+        for method in ("latest_measurement", "running_mean", "kalman_filter", "moving_average"):
+            m, tr = learner(kind)
+            cg = ConfidenceGenerator(std_factor=0.5, method=method).to(dev)
+            tr.cg_mean, tr.cg_std = cg.mean.data, cg.std.data
+            kf = getattr(cg, "_kalman_filter", None)
+            tr.set_confidence(cg.method_id, cg.var.data, getattr(cg, "running_n", None),
+                              getattr(cg, "running_sum", None), getattr(cg, "running_sum_of_squares", None),
+                              kf_proc_cov=float(kf.proc_cov.item()) if kf is not None else 0.2,
+                              kf_meas_cov=float(kf.meas_cov.item()) if kf is not None else 1.0)
+            gs = torch.Generator(device=dev).manual_seed(14)
+            for R in (1024, 800, 1500):
+                x = torch.randn(R, 384, device=dev, generator=gs) * 0.5
+                y = torch.rand(R, device=dev, generator=gs)
+                yv = torch.rand(R, device=dev, generator=gs) < 0.4
+                if kind == "gcn":
+                    ei = torch.randint(0, R, (2, 3 * R), device=dev, generator=gs)
+                    conf = tr.step(x, ei, y, yv)
+                elif kind == "flow":
+                    conf = tr.step(x)   # every row labelled: the whole confidence vector is live
+                else:
+                    conf = tr.step(x, y, yv)
+            assert tr.max_rows > 1024
+            out = {"params": m.flat_params, "exp_avg": tr.exp_avg, "exp_avg_sq": tr.exp_avg_sq, "conf": conf,
+                   "metrics": tr.metrics, "cg_mean": cg.mean, "cg_std": cg.std, "cg_var": cg.var}
+            for k in ("running_n", "running_sum", "running_sum_of_squares"):
+                if hasattr(cg, k):
+                    out["cg_" + k] = getattr(cg, k)
+            for k, t in out.items():
+                _record(out_dir, f"{kind}_train_{method}_{k}", t, index)
     torch.cuda.synchronize()
 
     with open(os.path.join(out_dir, "index.json"), "w") as f:

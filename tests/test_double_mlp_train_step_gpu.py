@@ -588,7 +588,7 @@ def test_flow_padded_step_equals_compacted_step(geometry, mask):
 
 # ------------------------------------------------------------------------------------------------ GPU: workspace, growth
 @pytest.mark.gpu
-def test_stale_workspace_rows_are_not_read():
+def test_stale_workspace_rows_are_never_read():
     """A 3000-row step with features x8 leaves large activations and gradients in the workspaces; a following
     500-row padded step must be bit-identical to the same step on a fresh trainer (new, zeroed workspaces) given the
     first trainer's params, moments, step counter and generator state."""
@@ -605,7 +605,7 @@ def test_stale_workspace_rows_are_not_read():
         getattr(B.tr, name).copy_(getattr(A.tr, name))
     B.var.copy_(A.var)
     B.running.copy_(A.running)
-    ccheck(lib().wvn_double_mlp_trainer_copy_confidence(B.tr._h, A.tr._h, stream()))   # the handle's private state
+    ccheck(lib().wvn_trainer_copy_confidence(B.tr._h, A.tr._h, stream()))   # the handle's private state
     g = torch.Generator().manual_seed(32)
     counts = torch.randint(0, 51, (10,), generator=g)
     counts[3] = 50

@@ -88,7 +88,7 @@ def test_library_graph_logic_matches_oracle(golden):
     assert mg.range_query(ts[:4], [1.0, 1.0, 1.0], 2.0) == (3, [1, 2])
 
 
-def test_abi_exports_mission_propagate():
+def test_abi_version_and_mission_propagate_exports():
     import __graft_entry__ as g
 
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -97,6 +97,6 @@ def test_abi_exports_mission_propagate():
     from wild_visual_navigation_b200 import _C
 
     l = _C.lib()
-    assert l.wvn_version() == 107
+    assert l.wvn_version() == 108
     assert hasattr(l, "wvn_mission_propagate") and hasattr(l, "wvn_mission_propagate_workspace_bytes")
     assert l.wvn_mission_propagate_workspace_bytes(3, 10) == 3 * (2 * 10 * 4 + 4)

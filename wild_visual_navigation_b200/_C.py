@@ -122,39 +122,26 @@ SIGNATURES = {
     "wvn_mlp_train_apply": (_I, [_I, _I, _I, _P, _P, _P, _P, _P, _L, POINTER(TrainConfig), _P, _P]),
     "wvn_mlp_train_read_metrics": (_I, [_P, _P, _P]),
     "wvn_mlp_forward_f32": (_I, [_I, _I, _I, _P, _P, _I, _P, _P, _P, _P]),
+    "wvn_trainer_destroy": (None, [_P]),
+    "wvn_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
+    "wvn_trainer_copy_confidence": (_I, [_P, _P, _P]),
+    "wvn_trainer_init_comm": (_I, [_P, _P, _I, _I]),
+    "wvn_trainer_stats": (_P, [_P, POINTER(_I)]),
     "wvn_mlp_trainer_scalars_bytes": (_S, []),
     "wvn_mlp_trainer_create": (_I, [_I, _I, _I, _I, POINTER(TrainConfig), _P, _P, POINTER(_P)]),
-    "wvn_mlp_trainer_destroy": (None, [_P]),
     "wvn_comm_unique_id": (_I, [_P]),
-    "wvn_mlp_trainer_init_comm": (_I, [_P, _P, _I, _I]),
-    "wvn_mlp_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
-    "wvn_mlp_trainer_copy_confidence": (_I, [_P, _P, _P]),
     "wvn_mlp_train_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
     "wvn_double_mlp_param_count": (_S, [_I, _I, _I]),
     "wvn_double_mlp_forward_f32": (_I, [_I, _I, _I, _P, _P, _I, _P, _P, _P, _P]),
     "wvn_double_mlp_trainer_create": (_I, [_I, _I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
-    "wvn_double_mlp_trainer_destroy": (None, [_P]),
-    "wvn_double_mlp_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
-    "wvn_double_mlp_trainer_copy_confidence": (_I, [_P, _P, _P]),
-    "wvn_double_mlp_train_step": (_I, [_P, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P]),
     "wvn_double_mlp_train_step_padded": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _P]),
-    "wvn_double_mlp_trainer_init_comm": (_I, [_P, _P, _I, _I]),
-    "wvn_double_mlp_trainer_stats": (_P, [_P]),
     "wvn_gcn_param_count": (_S, [_I, _I, _I]),
     "wvn_gcn_trainer_create": (_I, [_I, _I, _I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
-    "wvn_gcn_trainer_destroy": (None, [_P]),
-    "wvn_gcn_trainer_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
-    "wvn_gcn_trainer_copy_confidence": (_I, [_P, _P, _P]),
-    "wvn_gcn_trainer_init_comm": (_I, [_P, _P, _I, _I]),
-    "wvn_gcn_trainer_stats": (_P, [_P]),
     "wvn_gcn_train_step_padded": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _I,
                                        _P]),
     "wvn_gcn_infer_rows": (_I, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _F, _P, _P, _P, _P]),
     "wvn_flow_param_count": (_S, [_I, _I]),
-    "wvn_flow_create": (_I, [_I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
-    "wvn_flow_destroy": (None, [_P]),
-    "wvn_flow_set_confidence": (_I, [_P, _I, _P, _P, _P, _P, _F, _F]),
-    "wvn_flow_copy_confidence": (_I, [_P, _P, _P]),
+    "wvn_flow_trainer_create": (_I, [_I, _I, _I, POINTER(TrainConfig), _P, POINTER(_P)]),
     "wvn_flow_infer_create": (_I, [_I, _I, _I, _I, POINTER(_P)]),
     "wvn_flow_infer_destroy": (None, [_P]),
     "wvn_flow_infer_set_params": (_I, [_P, _P, _P]),
@@ -163,8 +150,6 @@ SIGNATURES = {
     "wvn_flow_train_step": (_I, [_P, _P, _P, _P, _P, POINTER(FlowBuffers), _P, _I, _P, _P, _P, _P, _P, _I, _P]),
     "wvn_flow_train_step_padded": (_I, [_P, _P, _P, _P, _P, POINTER(FlowBuffers), _P, _I, _I, _P, _P, _P, _P, _P, _P, _I,
                                         _P]),
-    "wvn_flow_init_comm": (_I, [_P, _P, _I, _I]),
-    "wvn_flow_stats": (_P, [_P]),
 }
 
 

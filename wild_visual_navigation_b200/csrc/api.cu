@@ -122,7 +122,7 @@ struct wvn_vit {
 extern "C" {
 
 const char* wvn_last_error(void) { return last_error(); }
-int wvn_version(void) { return 107; }
+int wvn_version(void) { return 108; }
 
 int wvn_check_device(void) {
   int n = 0;
@@ -1274,6 +1274,11 @@ static LossCfg loss_of(const wvn_train_config* c) {
   l.w_trav = c->w_trav; l.w_reco = c->w_reco; l.std_factor = c->std_factor; l.anomaly_balanced = c->anomaly_balanced;
   return l;
 }
+static AdamCfg adam_of(const wvn_train_config* c) {
+  AdamCfg a;
+  a.lr = c->lr; a.beta1 = c->beta1; a.beta2 = c->beta2; a.eps = c->eps;
+  return a;
+}
 
 size_t wvn_mlp_param_count(int dim, int h1, int h2) { return mlp_param_count(shape_of(dim, h1, h2)); }
 size_t wvn_mlp_train_workspace_bytes(int dim, int h1, int h2, int max_rows) {
@@ -1307,9 +1312,7 @@ int wvn_mlp_train_apply(int dim, int h1, int h2, float* params, const float* gra
               "wvn_mlp_train_apply: null argument");
   const long long n = static_cast<long long>(mlp_param_count(shape_of(dim, h1, h2)));
   WVN_PROPAGATE(mlp_train_finalize(reinterpret_cast<TrainScalars*>(scalars), grads, n, n_total, loss_of(cfg), S(stream)));
-  AdamCfg a;
-  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
-  return mlp_adam_step(params, grads, exp_avg, exp_avg_sq, n, a, step_counter, S(stream));
+  return mlp_adam_step(params, grads, exp_avg, exp_avg_sq, n, adam_of(cfg), step_counter, S(stream));
 }
 
 __global__ void read_metrics_kernel(const TrainScalars* sc, float* out) {
@@ -1331,59 +1334,58 @@ int wvn_mlp_forward_f32(int dim, int h1, int h2, const float* params, const floa
 }
 
 
-// -------------------------------------------------------------------------------- fused train step
-struct wvn_mlp_trainer {
-  FusedTrainer* impl = nullptr;
-};
+// -------------------------------------------------------------------------------- trainers
+// A wvn_trainer_t is the address of the learner's Trainer base (train_core.h).
+static Trainer* impl(wvn_trainer_t* h) { return reinterpret_cast<Trainer*>(h); }
+static wvn_trainer_t* handle_of(Trainer* t) { return reinterpret_cast<wvn_trainer_t*>(t); }
 
-size_t wvn_mlp_trainer_scalars_bytes(void) { return sizeof(FusedScalars); }
+void wvn_trainer_destroy(wvn_trainer_t* t) { delete impl(t); }
 
-int wvn_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_train_config* cfg, void* scalars, float* grads,
-                           wvn_mlp_trainer_t** out) {
-  WVN_REQUIRE(cfg && out, "wvn_mlp_trainer_create: null argument");
-  WVN_PROPAGATE(wvn_check_device());
-  AdamCfg a;
-  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
-  FusedTrainer* impl = nullptr;
-  WVN_PROPAGATE(fused_trainer_create(shape_of(dim, h1, h2), max_rows, loss_of(cfg), a, scalars, grads, &impl));
-  wvn_mlp_trainer* t = new wvn_mlp_trainer();
-  t->impl = impl;
-  *out = t;
-  return WVN_OK;
+int wvn_trainer_set_confidence(wvn_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
+                               double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
+  WVN_REQUIRE(t, "wvn_trainer_set_confidence: null trainer");
+  return trainer_conf_bind(&impl(t)->conf, method, var, running_n, running_sum, running_sum_of_squares, kf_proc_cov,
+                           kf_meas_cov);
 }
 
-void wvn_mlp_trainer_destroy(wvn_mlp_trainer_t* t) {
-  if (!t) return;
-  fused_trainer_destroy(t->impl);
-  delete t;
+int wvn_trainer_copy_confidence(wvn_trainer_t* dst, const wvn_trainer_t* src, void* stream) {
+  WVN_REQUIRE(dst && src, "wvn_trainer_copy_confidence: null trainer");
+  const Trainer* from = reinterpret_cast<const Trainer*>(src);
+  WVN_PROPAGATE(trainer_check(from, impl(dst)->kind, "wvn_trainer_copy_confidence"));
+  return trainer_conf_copy(&impl(dst)->conf, &from->conf, S(stream));
 }
 
 int wvn_comm_unique_id(void* id128) { return comm_unique_id(id128); }
 
-int wvn_mlp_trainer_init_comm(wvn_mlp_trainer_t* t, const void* id128, int rank, int world) {
-  WVN_REQUIRE(t, "wvn_mlp_trainer_init_comm: null trainer");
-  return trainer_comm_init(fused_trainer_comm(t->impl), id128, rank, world);
+int wvn_trainer_init_comm(wvn_trainer_t* t, const void* id128, int rank, int world) {
+  WVN_REQUIRE(t, "wvn_trainer_init_comm: null trainer");
+  return trainer_comm_init(&impl(t)->comm, id128, rank, world);
 }
 
-int wvn_mlp_trainer_set_confidence(wvn_mlp_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
-                                   double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
-  WVN_REQUIRE(t, "wvn_mlp_trainer_set_confidence: null trainer");
-  return trainer_conf_bind(fused_trainer_conf(t->impl), method, var, running_n, running_sum, running_sum_of_squares,
-                           kf_proc_cov, kf_meas_cov);
+double* wvn_trainer_stats(wvn_trainer_t* t, int* n_doubles) {
+  if (n_doubles) *n_doubles = t ? impl(t)->n_stats : 0;
+  return t ? impl(t)->stats : nullptr;
 }
 
-int wvn_mlp_trainer_copy_confidence(wvn_mlp_trainer_t* dst, const wvn_mlp_trainer_t* src, void* stream) {
-  WVN_REQUIRE(dst && src, "wvn_mlp_trainer_copy_confidence: null trainer");
-  return trainer_conf_copy(fused_trainer_conf(dst->impl), fused_trainer_conf(src->impl), S(stream));
+// -------------------------------------------------------------------------------- fused train step
+size_t wvn_mlp_trainer_scalars_bytes(void) { return sizeof(FusedScalars); }
+
+int wvn_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_train_config* cfg, void* scalars, float* grads,
+                           wvn_trainer_t** out) {
+  WVN_REQUIRE(cfg && out, "wvn_mlp_trainer_create: null argument");
+  WVN_PROPAGATE(wvn_check_device());
+  Trainer* t = nullptr;
+  WVN_PROPAGATE(fused_trainer_create(shape_of(dim, h1, h2), max_rows, loss_of(cfg), adam_of(cfg), scalars, grads, &t));
+  *out = handle_of(t);
+  return WVN_OK;
 }
 
-int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int wvn_mlp_train_step(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                        const float* x, int groups, int rows_per_group, const int* n_rows, const float* y,
                        const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
                        float* metrics_out, int phase_mask, void* stream) {
-  WVN_REQUIRE(t, "wvn_mlp_train_step: null trainer");
-  return fused_train_step(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows, y, y_valid,
-                          cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
+  return fused_train_step(impl(t), params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows, y,
+                          y_valid, cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
 }
 
 }  // extern "C"
@@ -1391,10 +1393,6 @@ int wvn_mlp_train_step(wvn_mlp_trainer_t* t, float* params, float* exp_avg, floa
 // ============================================================================================
 // DoubleMLP learner: fp32 row forward and online train step (double_mlp_train.cu)
 // ============================================================================================
-struct wvn_double_mlp_trainer {
-  DoubleTrainer* impl = nullptr;
-};
-
 extern "C" {
 
 size_t wvn_double_mlp_param_count(int dim, int h1, int h2) { return double_mlp_param_count(shape_of(dim, h1, h2)); }
@@ -1405,62 +1403,21 @@ int wvn_double_mlp_forward_f32(int dim, int h1, int h2, const float* params, con
 }
 
 int wvn_double_mlp_trainer_create(int dim, int h1, int h2, int max_rows, const wvn_train_config* cfg, float* grads,
-                                  wvn_double_mlp_trainer_t** out) {
+                                  wvn_trainer_t** out) {
   WVN_REQUIRE(cfg && out, "wvn_double_mlp_trainer_create: null argument");
   WVN_PROPAGATE(wvn_check_device());
-  AdamCfg a;
-  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
-  DoubleTrainer* impl = nullptr;
-  WVN_PROPAGATE(double_trainer_create(shape_of(dim, h1, h2), max_rows, loss_of(cfg), a, grads, &impl));
-  wvn_double_mlp_trainer* t = new wvn_double_mlp_trainer();
-  t->impl = impl;
-  *out = t;
+  Trainer* t = nullptr;
+  WVN_PROPAGATE(double_trainer_create(shape_of(dim, h1, h2), max_rows, loss_of(cfg), adam_of(cfg), grads, &t));
+  *out = handle_of(t);
   return WVN_OK;
 }
 
-void wvn_double_mlp_trainer_destroy(wvn_double_mlp_trainer_t* t) {
-  if (!t) return;
-  double_trainer_destroy(t->impl);
-  delete t;
-}
-
-int wvn_double_mlp_trainer_set_confidence(wvn_double_mlp_trainer_t* t, int method, float* var, double* running_n,
-                                          double* running_sum, double* running_sum_of_squares, float kf_proc_cov,
-                                          float kf_meas_cov) {
-  WVN_REQUIRE(t, "wvn_double_mlp_trainer_set_confidence: null trainer");
-  return trainer_conf_bind(double_trainer_conf(t->impl), method, var, running_n, running_sum, running_sum_of_squares,
-                           kf_proc_cov, kf_meas_cov);
-}
-
-int wvn_double_mlp_trainer_copy_confidence(wvn_double_mlp_trainer_t* dst, const wvn_double_mlp_trainer_t* src,
-                                           void* stream) {
-  WVN_REQUIRE(dst && src, "wvn_double_mlp_trainer_copy_confidence: null trainer");
-  return trainer_conf_copy(double_trainer_conf(dst->impl), double_trainer_conf(src->impl), S(stream));
-}
-
-int wvn_double_mlp_train_step(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
-                              long long* step_counter, const float* x, int rows, const float* y,
-                              const unsigned char* y_valid, float* cg_mean, float* cg_std, float* confidence_out,
-                              float* metrics_out, void* stream) {
-  WVN_REQUIRE(t, "wvn_double_mlp_train_step: null trainer");
-  return double_train_step(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, rows, y, y_valid, cg_mean, cg_std,
-                           confidence_out, metrics_out, S(stream));
-}
-
-int wvn_double_mlp_trainer_init_comm(wvn_double_mlp_trainer_t* t, const void* id128, int rank, int world) {
-  WVN_REQUIRE(t, "wvn_double_mlp_trainer_init_comm: null trainer");
-  return trainer_comm_init(double_trainer_comm(t->impl), id128, rank, world);
-}
-
-double* wvn_double_mlp_trainer_stats(wvn_double_mlp_trainer_t* t) { return t ? double_trainer_stats(t->impl) : nullptr; }
-
-int wvn_double_mlp_train_step_padded(wvn_double_mlp_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+int wvn_double_mlp_train_step_padded(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
                                      long long* step_counter, const float* x, int groups, int rows_per_group,
                                      const int* n_rows, const float* y, const unsigned char* y_valid, float* cg_mean,
                                      float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
                                      void* stream) {
-  WVN_REQUIRE(t, "wvn_double_mlp_train_step_padded: null trainer");
-  return double_train_step_padded(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows,
+  return double_train_step_padded(impl(t), params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows,
                                   y, y_valid, cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
 }
 
@@ -1469,70 +1426,35 @@ int wvn_double_mlp_train_step_padded(wvn_double_mlp_trainer_t* t, float* params,
 // ============================================================================================
 // SimpleGCN learner: graph build, row forward and online train step (gcn_train.cu)
 // ============================================================================================
-struct wvn_gcn_trainer {
-  GcnTrainer* impl = nullptr;
-};
-
 extern "C" {
 
 size_t wvn_gcn_param_count(int dim, int h1, int h2) { return gcn_param_count(shape_of(dim, h1, h2)); }
 
 int wvn_gcn_trainer_create(int dim, int h1, int h2, int max_rows, int max_edges, const wvn_train_config* cfg,
-                           float* grads, wvn_gcn_trainer_t** out) {
+                           float* grads, wvn_trainer_t** out) {
   WVN_REQUIRE(cfg && out, "wvn_gcn_trainer_create: null argument");
   WVN_PROPAGATE(wvn_check_device());
-  AdamCfg a;
-  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
-  GcnTrainer* impl = nullptr;
-  WVN_PROPAGATE(gcn_trainer_create(shape_of(dim, h1, h2), max_rows, max_edges, loss_of(cfg), a, grads, &impl));
-  wvn_gcn_trainer* t = new wvn_gcn_trainer();
-  t->impl = impl;
-  *out = t;
+  Trainer* t = nullptr;
+  WVN_PROPAGATE(gcn_trainer_create(shape_of(dim, h1, h2), max_rows, max_edges, loss_of(cfg), adam_of(cfg), grads, &t));
+  *out = handle_of(t);
   return WVN_OK;
 }
 
-void wvn_gcn_trainer_destroy(wvn_gcn_trainer_t* t) {
-  if (!t) return;
-  gcn_trainer_destroy(t->impl);
-  delete t;
-}
-
-int wvn_gcn_trainer_set_confidence(wvn_gcn_trainer_t* t, int method, float* var, double* running_n, double* running_sum,
-                                   double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
-  WVN_REQUIRE(t, "wvn_gcn_trainer_set_confidence: null trainer");
-  return trainer_conf_bind(gcn_trainer_conf(t->impl), method, var, running_n, running_sum, running_sum_of_squares,
-                           kf_proc_cov, kf_meas_cov);
-}
-
-int wvn_gcn_trainer_copy_confidence(wvn_gcn_trainer_t* dst, const wvn_gcn_trainer_t* src, void* stream) {
-  WVN_REQUIRE(dst && src, "wvn_gcn_trainer_copy_confidence: null trainer");
-  return trainer_conf_copy(gcn_trainer_conf(dst->impl), gcn_trainer_conf(src->impl), S(stream));
-}
-
-int wvn_gcn_trainer_init_comm(wvn_gcn_trainer_t* t, const void* id128, int rank, int world) {
-  WVN_REQUIRE(t, "wvn_gcn_trainer_init_comm: null trainer");
-  return trainer_comm_init(gcn_trainer_comm(t->impl), id128, rank, world);
-}
-
-double* wvn_gcn_trainer_stats(wvn_gcn_trainer_t* t) { return t ? gcn_trainer_stats(t->impl) : nullptr; }
-
-int wvn_gcn_train_step_padded(wvn_gcn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+int wvn_gcn_train_step_padded(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
                               long long* step_counter, const float* x, int groups, int rows_per_group,
                               const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
                               const float* y, const unsigned char* y_valid, float* cg_mean, float* cg_std,
                               float* confidence_out, float* metrics_out, int phase_mask, void* stream) {
-  WVN_REQUIRE(t, "wvn_gcn_train_step_padded: null trainer");
-  return gcn_train_step_padded(t->impl, params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows,
+  return gcn_train_step_padded(impl(t), params, exp_avg, exp_avg_sq, step_counter, x, groups, rows_per_group, n_rows,
                                edges, edges_per_group, n_edges, y, y_valid, cg_mean, cg_std, confidence_out,
                                metrics_out, phase_mask, S(stream));
 }
 
-int wvn_gcn_infer_rows(wvn_gcn_trainer_t* t, const float* params, const float* x, int groups, int rows_per_group,
+int wvn_gcn_infer_rows(wvn_trainer_t* t, const float* params, const float* x, int groups, int rows_per_group,
                        const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
                        const float* cg_mean, const float* cg_std, float std_factor, float* out, float* trav,
                        float* confidence, void* stream) {
-  WVN_REQUIRE(t, "wvn_gcn_infer_rows: null trainer");
-  return gcn_infer_rows(t->impl, params, x, groups, rows_per_group, n_rows, edges, edges_per_group, n_edges, cg_mean,
+  return gcn_infer_rows(impl(t), params, x, groups, rows_per_group, n_rows, edges, edges_per_group, n_edges, cg_mean,
                         cg_std, std_factor, out, trav, confidence, S(stream));
 }
 
@@ -1541,13 +1463,9 @@ int wvn_gcn_infer_rows(wvn_gcn_trainer_t* t, const float* params, const float* x
 // ============================================================================================
 // LinearRnvp flow: fp32 row forward and online train step (flow_train.cu)
 // ============================================================================================
-struct wvn_flow {
-  FlowTrainer* impl = nullptr;
-};
-
 // inference only: the fp32 row forward (forward workspaces only) and the per-pixel wgmma path
 struct wvn_flow_infer {
-  FlowTrainer* rows = nullptr;
+  Trainer* rows = nullptr;
   FlowPixels* pix = nullptr;
 };
 
@@ -1569,61 +1487,33 @@ size_t wvn_flow_param_count(int dim, int hidden) {
   return flow_param_count(s);
 }
 
-int wvn_flow_create(int dim, int hidden, int max_rows, const wvn_train_config* cfg, float* grads, wvn_flow_t** out) {
-  WVN_REQUIRE(cfg && out, "wvn_flow_create: null argument");
+int wvn_flow_trainer_create(int dim, int hidden, int max_rows, const wvn_train_config* cfg, float* grads,
+                            wvn_trainer_t** out) {
+  WVN_REQUIRE(cfg && out, "wvn_flow_trainer_create: null argument");
   WVN_PROPAGATE(wvn_check_device());
   FlowShape s;
   s.dim = dim; s.hidden = hidden;
-  AdamCfg a;
-  a.lr = cfg->lr; a.beta1 = cfg->beta1; a.beta2 = cfg->beta2; a.eps = cfg->eps;
-  FlowTrainer* impl = nullptr;
-  WVN_PROPAGATE(flow_trainer_create(s, max_rows, cfg->std_factor, a, grads, false, &impl));
-  wvn_flow* h = new wvn_flow();
-  h->impl = impl;
-  *out = h;
+  Trainer* t = nullptr;
+  WVN_PROPAGATE(flow_trainer_create(s, max_rows, cfg->std_factor, adam_of(cfg), grads, false, &t));
+  *out = handle_of(t);
   return WVN_OK;
 }
 
-void wvn_flow_destroy(wvn_flow_t* h) {
-  if (!h) return;
-  flow_trainer_destroy(h->impl);
-  delete h;
-}
-
-int wvn_flow_set_confidence(wvn_flow_t* h, int method, float* var, double* running_n, double* running_sum,
-                            double* running_sum_of_squares, float kf_proc_cov, float kf_meas_cov) {
-  WVN_REQUIRE(h, "wvn_flow_set_confidence: null handle");
-  return trainer_conf_bind(flow_trainer_conf(h->impl), method, var, running_n, running_sum, running_sum_of_squares,
-                           kf_proc_cov, kf_meas_cov);
-}
-
-int wvn_flow_copy_confidence(wvn_flow_t* dst, const wvn_flow_t* src, void* stream) {
-  WVN_REQUIRE(dst && src, "wvn_flow_copy_confidence: null handle");
-  return trainer_conf_copy(flow_trainer_conf(dst->impl), flow_trainer_conf(src->impl), S(stream));
-}
-
-int wvn_flow_train_step(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int wvn_flow_train_step(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                         const wvn_flow_buffers* buffers, const float* x, int rows, const unsigned char* y_valid,
                         float* cg_mean, float* cg_std, float* confidence_out, float* metrics_out, int phase_mask,
                         void* stream) {
-  WVN_REQUIRE(h && buffers, "wvn_flow_train_step: null argument");
-  return flow_train_step(h->impl, params, exp_avg, exp_avg_sq, step_counter, buffers_of(buffers), x, rows, y_valid,
+  WVN_REQUIRE(buffers, "wvn_flow_train_step: null argument");
+  return flow_train_step(impl(t), params, exp_avg, exp_avg_sq, step_counter, buffers_of(buffers), x, rows, y_valid,
                          cg_mean, cg_std, confidence_out, metrics_out, phase_mask, S(stream));
 }
 
-int wvn_flow_init_comm(wvn_flow_t* h, const void* id128, int rank, int world) {
-  WVN_REQUIRE(h, "wvn_flow_init_comm: null handle");
-  return trainer_comm_init(flow_trainer_comm(h->impl), id128, rank, world);
-}
-
-double* wvn_flow_stats(wvn_flow_t* h) { return h ? flow_trainer_stats(h->impl) : nullptr; }
-
-int wvn_flow_train_step_padded(wvn_flow_t* h, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
-                               const wvn_flow_buffers* buffers, const float* x, int groups, int rows_per_group,
-                               const int* n_rows, const unsigned char* y_valid, float* cg_mean, float* cg_std,
-                               float* confidence_out, float* metrics_out, int phase_mask, void* stream) {
-  WVN_REQUIRE(h && buffers, "wvn_flow_train_step_padded: null argument");
-  return flow_train_step_padded(h->impl, params, exp_avg, exp_avg_sq, step_counter, buffers_of(buffers), x, groups,
+int wvn_flow_train_step_padded(wvn_trainer_t* t, float* params, float* exp_avg, float* exp_avg_sq,
+                               long long* step_counter, const wvn_flow_buffers* buffers, const float* x, int groups,
+                               int rows_per_group, const int* n_rows, const unsigned char* y_valid, float* cg_mean,
+                               float* cg_std, float* confidence_out, float* metrics_out, int phase_mask, void* stream) {
+  WVN_REQUIRE(buffers, "wvn_flow_train_step_padded: null argument");
+  return flow_train_step_padded(impl(t), params, exp_avg, exp_avg_sq, step_counter, buffers_of(buffers), x, groups,
                                 rows_per_group, n_rows, y_valid, cg_mean, cg_std, confidence_out, metrics_out,
                                 phase_mask, S(stream));
 }
@@ -1646,7 +1536,7 @@ int wvn_flow_infer_create(int dim, int hidden, int max_rows, int chunk_pixels, w
 
 void wvn_flow_infer_destroy(wvn_flow_infer_t* h) {
   if (!h) return;
-  flow_trainer_destroy(h->rows);
+  delete h->rows;
   flow_pixels_destroy(h->pix);
   delete h;
 }

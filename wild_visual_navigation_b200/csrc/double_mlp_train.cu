@@ -94,24 +94,19 @@ int double_mlp_forward_f32(const MlpShape& s, const float* params, const float* 
   return forward_gemms(s, double_mlp_offsets(s), params, x, rows, rows, a1, a2, out, nullptr, stream);
 }
 
-struct DoubleTrainer {
+struct DoubleTrainer : Trainer {
+  DoubleTrainer() : Trainer(TRAINER_DOUBLE_MLP) {}
   MlpShape s;
   DoubleOffsets o;
-  LossCfg loss;
-  AdamCfg adam;
-  int max_rows = 0;
-  void* arena = nullptr;
   DoubleScalars* sc = nullptr;
   int* comp = nullptr;     // compacted -> padded row map
   int* n_live = nullptr;   // this rank's live rows (device)
   float *xg = nullptr, *a1 = nullptr, *a2 = nullptr, *out = nullptr, *d_out = nullptr, *d2 = nullptr, *d1 = nullptr;
-  float *loss_reco = nullptr, *raw = nullptr, *wraw = nullptr, *grads = nullptr;
-  TrainerConf conf;
-  TrainerComm comm;
+  float *loss_reco = nullptr, *raw = nullptr, *wraw = nullptr;
 };
 
 int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, float* grads_ext,
-                          DoubleTrainer** out) {
+                          Trainer** out) {
   WVN_REQUIRE(out && max_rows > 0, "double mlp trainer: bad arguments");
   WVN_PROPAGATE(double_mlp_check_shape(s, "double mlp trainer"));
   DoubleTrainer* t = new DoubleTrainer();
@@ -122,25 +117,16 @@ int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, 
   const size_t floats = R * D + 2 * (2 * R * h1 + 2 * R * h2 + R * (D + 1)) + 3 * R + (grads_ext ? 0 : t->o.total);
   const size_t head = 256 + (R * sizeof(int) + 255) / 256 * 256;   // scalars | n_live at 128 | comp at 256
   const size_t bytes = head + floats * sizeof(float);
-  if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
-    delete t;
-    return set_error(WVN_ERR_CUDA, "double mlp trainer: cudaMalloc of %zu bytes failed", bytes);
-  }
-  const int rc = trainer_conf_create(&t->conf);
+  const int rc = trainer_alloc(t, bytes, "double mlp trainer");
   if (rc != WVN_OK) {
-    cudaFree(t->arena);
     delete t;
     return rc;
-  }
-  if (cudaMemset(t->arena, 0, bytes) != cudaSuccess) {
-    trainer_conf_destroy(&t->conf);
-    cudaFree(t->arena);
-    delete t;
-    return set_error(WVN_ERR_CUDA, "double mlp trainer: cudaMemset of %zu bytes failed", bytes);
   }
   static_assert(sizeof(DoubleScalars) <= 128, "scalars overlap n_live");
   char* base = reinterpret_cast<char*>(t->arena);
   t->sc = reinterpret_cast<DoubleScalars*>(base);
+  t->stats = &t->sc->sum_lr;
+  t->n_stats = kStatDoubles + 1;
   t->n_live = reinterpret_cast<int*>(base + 128);
   t->comp = reinterpret_cast<int*>(base + 256);
   float* f = reinterpret_cast<float*>(base + head);
@@ -160,23 +146,13 @@ int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, 
   return WVN_OK;
 }
 
-void double_trainer_destroy(DoubleTrainer* t) {
-  if (!t) return;
-  trainer_comm_destroy(&t->comm);
-  if (t->arena) cudaFree(t->arena);
-  trainer_conf_destroy(&t->conf);
-  delete t;
-}
-
-TrainerConf* double_trainer_conf(DoubleTrainer* t) { return &t->conf; }
-TrainerComm* double_trainer_comm(DoubleTrainer* t) { return &t->comm; }
-double* double_trainer_stats(DoubleTrainer* t) { return &t->sc->sum_lr; }
-
-int double_train_step_padded(DoubleTrainer* t, float* params, float* exp_avg, float* exp_avg_sq,
+int double_train_step_padded(Trainer* base, float* params, float* exp_avg, float* exp_avg_sq,
                              long long* step_counter, const float* x, int groups, int rows_per_group,
                              const int* n_rows, const float* y, const unsigned char* y_valid, float* cg_mean,
                              float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream) {
-  WVN_REQUIRE(t && params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
+  WVN_PROPAGATE(trainer_check(base, TRAINER_DOUBLE_MLP, "double mlp train step"));
+  DoubleTrainer* t = static_cast<DoubleTrainer*>(base);
+  WVN_REQUIRE(params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
               "double mlp train step: null argument");
   const long long cap = static_cast<long long>(groups) * rows_per_group;
   WVN_REQUIRE(groups > 0 && rows_per_group > 0 && cap <= t->max_rows,
@@ -245,13 +221,6 @@ int double_train_step_padded(DoubleTrainer* t, float* params, float* exp_avg, fl
                                 step_counter, stream));
   }
   return WVN_OK;
-}
-
-int double_train_step(DoubleTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
-                      const float* x, int rows, const float* y, const unsigned char* y_valid, float* cg_mean,
-                      float* cg_std, float* conf_out, float* metrics, cudaStream_t stream) {
-  return double_train_step_padded(t, params, exp_avg, exp_avg_sq, step_counter, x, 1, rows, nullptr, y, y_valid, cg_mean,
-                                  cg_std, conf_out, metrics, 7, stream);
 }
 
 }  // namespace wvn

@@ -28,19 +28,12 @@ int double_mlp_check_shape(const MlpShape& s, const char* who);
 int double_mlp_forward_f32(const MlpShape& s, const float* params, const float* x, int rows, float* a1, float* a2,
                            float* out, cudaStream_t stream);
 
-struct DoubleTrainer;
 // grads_ext: caller-owned device buffer of double_mlp_param_count floats, or NULL (the trainer allocates it).
-int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, float* grads_ext,
-                          DoubleTrainer** out);
-void double_trainer_destroy(DoubleTrainer* t);
-// The trainer's ConfidenceGenerator (bound and copied with trainer_conf_bind / trainer_conf_copy).
-TrainerConf* double_trainer_conf(DoubleTrainer* t);
-// The trainer's communicator (set up with trainer_comm_init; none: the exchanges are the caller's).
-TrainerComm* double_trainer_comm(DoubleTrainer* t);
-// The step's statistics block (device, 9 doubles): the kStatDoubles of train_core.h (sum and sum of squares of loss_reco
-// over the labelled rows, sum of (trav - y)^2, labelled and live row counts, 0, loss_reco's min and max), then the
+// The statistics block has 9 doubles: the kStatDoubles of train_core.h (sum and sum of squares of loss_reco over the
+// labelled rows, sum of (trav - y)^2, labelled and live row counts, 0, loss_reco's min and max), then the
 // confidence-weighted traversability error summed over the live rows (written by phase 2, all-reduced with the gradient).
-double* double_trainer_stats(DoubleTrainer* t);
+int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, float* grads_ext,
+                          Trainer** out);
 // One TraversabilityEstimator.train() body on rows padded per group: x [groups, rows_per_group, dim] with n_rows[g]
 // (device int32; NULL: all) live rows in group g; y / y_valid (uint8) / conf_out are indexed by the compacted row number.
 // The live rows are gathered first, and every later launch is bounded by their device count, so padding (NaN included)
@@ -48,13 +41,9 @@ double* double_trainer_stats(DoubleTrainer* t);
 // from the global sums, dLoss/dOut with the global row counts, backward, weight gradients (+ the gradient all-reduce);
 // 4 = loss metrics from the global sums + Adam; 7 = the whole step.  metrics [6] (may be NULL): loss_total, loss_trav,
 // loss_reco, loss_trav_conf, cg_mean, cg_std.
-int double_train_step_padded(DoubleTrainer* t, float* params, float* exp_avg, float* exp_avg_sq,
+int double_train_step_padded(Trainer* t, float* params, float* exp_avg, float* exp_avg_sq,
                              long long* step_counter, const float* x, int groups, int rows_per_group,
                              const int* n_rows, const float* y, const unsigned char* y_valid, float* cg_mean,
                              float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream);
-// The same step on compacted rows x [rows, dim]: one group, every row live, phase_mask 7.
-int double_train_step(DoubleTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
-                      const float* x, int rows, const float* y, const unsigned char* y_valid, float* cg_mean,
-                      float* cg_std, float* conf_out, float* metrics, cudaStream_t stream);
 
 }  // namespace wvn

@@ -261,16 +261,12 @@ NetOffsets net_offsets(const FlowShape& s, int coupling, int net) {
 }
 }  // namespace
 
-struct FlowTrainer {
+struct FlowTrainer : Trainer {
+  FlowTrainer() : Trainer(TRAINER_FLOW) {}
   FlowShape s;
-  AdamCfg adam;
-  float std_factor = 0.5f;
-  int max_rows = 0;
-  void* arena = nullptr;
   int* comp = nullptr;
   int* n_live = nullptr;
   FlowScalars* sc = nullptr;
-  float* grads = nullptr;
   // activations (rows x width)
   float *u[2], *mu[2], *s1[2][2], *s2[2][2], *so[2][2];   // [coupling][net]; so[c][0] holds s = tanh after the forward
   float *z, *ld, *nll;
@@ -278,18 +274,16 @@ struct FlowTrainer {
   float *dx = nullptr, *dso[2] = {nullptr, nullptr}, *d2[2] = {nullptr, nullptr}, *d1[2] = {nullptr, nullptr},
         *dmu[2] = {nullptr, nullptr}, *du = nullptr;
   bool forward_only = false;   // inference: no backward workspaces, no gradient buffer
-  TrainerConf conf;
-  TrainerComm comm;
 };
 
 int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, const AdamCfg& adam, float* grads_ext,
-                        bool forward_only, FlowTrainer** out) {
+                        bool forward_only, Trainer** out) {
   WVN_REQUIRE(out && max_rows > 0, "flow trainer: bad arguments");
   WVN_REQUIRE(s.dim >= 2 && s.dim <= 4096 && s.hidden >= 8 && s.hidden <= 512 && s.hidden % 8 == 0,
               "flow trainer: LinearRnvp(%d, [%d]) outside the kernels' range (2 <= dim <= 4096, hidden <= 512 and a "
               "multiple of 8)", s.dim, s.hidden);
   FlowTrainer* t = new FlowTrainer();
-  t->s = s; t->adam = adam; t->std_factor = std_factor; t->forward_only = forward_only;
+  t->s = s; t->adam = adam; t->loss.std_factor = std_factor; t->forward_only = forward_only;
   t->max_rows = (max_rows + 63) / 64 * 64;   // whole 64-row GEMM tiles
   const size_t R = t->max_rows, D = s.dim, h = s.hidden, np = flow_param_count(s);
   const size_t floats = R * D * 4 + R * h * 8 + R * D * 4 + R * D + 2 * R       // forward
@@ -297,20 +291,15 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
                                                + (grads_ext ? 0 : np));
   const size_t head = 256 + ((R + 1) * sizeof(int) + 255) / 256 * 256;
   const size_t bytes = head + floats * sizeof(float);
-  if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
-    delete t;
-    return set_error(WVN_ERR_CUDA, "flow trainer: cudaMalloc of %zu bytes failed", bytes);
-  }
-  const int rc = trainer_conf_create(&t->conf);
+  const int rc = trainer_alloc(t, bytes, "flow trainer");
   if (rc != WVN_OK) {
-    cudaFree(t->arena);
     delete t;
     return rc;
   }
-  cudaMemset(t->arena, 0, bytes);
   char* base = reinterpret_cast<char*>(t->arena);
   static_assert(sizeof(FlowScalars) <= 128, "scalars overlap n_live");
   t->sc = reinterpret_cast<FlowScalars*>(base);
+  t->stats = &t->sc->s1;
   t->n_live = reinterpret_cast<int*>(base + 128);
   t->comp = reinterpret_cast<int*>(base + 256);
   float* f = reinterpret_cast<float*>(base + head);
@@ -341,18 +330,6 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
   *out = t;
   return WVN_OK;
 }
-
-void flow_trainer_destroy(FlowTrainer* t) {
-  if (!t) return;
-  trainer_comm_destroy(&t->comm);
-  if (t->arena) cudaFree(t->arena);
-  trainer_conf_destroy(&t->conf);
-  delete t;
-}
-
-TrainerConf* flow_trainer_conf(FlowTrainer* t) { return &t->conf; }
-TrainerComm* flow_trainer_comm(FlowTrainer* t) { return &t->comm; }
-double* flow_trainer_stats(FlowTrainer* t) { return &t->sc->s1; }
 
 namespace {
 
@@ -411,7 +388,7 @@ int flow_forward(FlowTrainer* t, const float* params, const FlowBuffers& b, cons
 }
 
 int check_args(FlowTrainer* t, const float* params, const FlowBuffers& b, const float* x, int rows) {
-  WVN_REQUIRE(t && params && b.mask0 && b.mask1 && b.p1 && b.invp1 && b.p3 && b.invp3, "flow: null argument");
+  WVN_REQUIRE(params && b.mask0 && b.mask1 && b.p1 && b.invp1 && b.p3 && b.invp3, "flow: null argument");
   WVN_REQUIRE(rows >= 0 && rows <= t->max_rows, "flow: %d rows exceed the handle's capacity %d", rows, t->max_rows);
   WVN_REQUIRE(rows == 0 || x, "flow: null rows");
   WVN_REQUIRE(static_cast<size_t>(t->s.dim) * sizeof(float) <= 48 * 1024, "flow: dim too large");
@@ -420,9 +397,11 @@ int check_args(FlowTrainer* t, const float* params, const FlowBuffers& b, const 
 
 }  // namespace
 
-int flow_forward_rows(FlowTrainer* t, const float* params, const FlowBuffers& b, const float* x, int rows, float* z,
+int flow_forward_rows(Trainer* base, const float* params, const FlowBuffers& b, const float* x, int rows, float* z,
                       float* log_det, float* logprob, const float* cg_mean, const float* cg_std, float std_factor,
                       float* trav, cudaStream_t stream) {
+  WVN_PROPAGATE(trainer_check(base, TRAINER_FLOW, "flow rows"));
+  FlowTrainer* t = static_cast<FlowTrainer*>(base);
   WVN_PROPAGATE(check_args(t, params, b, x, rows));
   WVN_REQUIRE(!trav || (cg_mean && cg_std), "flow rows: trav needs the generator's mean and std");
   return flow_forward(t, params, b, x, 1, rows, nullptr, nullptr, z, logprob, log_det, trav, cg_mean, cg_std, std_factor,
@@ -435,9 +414,11 @@ namespace {
 // statistics exchange sits between kFwd and kGen.
 enum : int { kFwd = 1, kBwd = 2, kAdam = 4, kGen = 8 };
 
-int flow_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int flow_step(Trainer* base, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
               const FlowBuffers& b, const float* x, int groups, int rpg, const int* n_rows, const unsigned char* y_valid,
               float* cg_mean, float* cg_std, float* conf_out, float* metrics, int stages, cudaStream_t stream) {
+  WVN_PROPAGATE(trainer_check(base, TRAINER_FLOW, "flow train step"));
+  FlowTrainer* t = static_cast<FlowTrainer*>(base);
   WVN_REQUIRE(groups >= 0 && rpg >= 0, "flow train step: %d x %d rows", groups, rpg);
   const long long cap = static_cast<long long>(groups) * rpg;
   WVN_REQUIRE(cap <= t->max_rows, "flow: %lld rows exceed the handle's capacity %d", cap, t->max_rows);
@@ -455,7 +436,7 @@ int flow_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, 
     WVN_PROPAGATE(trainer_comm_stats(&t->comm, &t->sc->s1, t->conf.cs.method == CONF_MOVING_AVERAGE, stream));
   }
   if (stages & kGen) {   // generator update from the global sums, metrics, per-row confidence
-    flow_conf_kernel<<<1, 32, 0, stream>>>(t->conf.cs, t->std_factor, cg_mean, cg_std, metrics, t->sc);
+    flow_conf_kernel<<<1, 32, 0, stream>>>(t->conf.cs, t->loss.std_factor, cg_mean, cg_std, metrics, t->sc);
     WVN_CHECK_LAUNCH("flow_conf_kernel");
     flow_conf_rows_kernel<<<(R + 255) / 256, 256, 0, stream>>>(t->nll, t->n_live, t->conf.cs.method, t->sc, conf_out);
     WVN_CHECK_LAUNCH("flow_conf_rows_kernel");
@@ -516,7 +497,7 @@ int flow_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, 
 
 }  // namespace
 
-int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int flow_train_step(Trainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                     const FlowBuffers& b, const float* x, int rows, const unsigned char* y_valid, float* cg_mean,
                     float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream) {
   const int stages = ((phase_mask & 1) ? kFwd | kGen : 0) | (phase_mask & (kBwd | kAdam));
@@ -524,7 +505,7 @@ int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_av
                    conf_out, metrics, stages, stream);
 }
 
-int flow_train_step_padded(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int flow_train_step_padded(Trainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                            const FlowBuffers& b, const float* x, int groups, int rows_per_group, const int* n_rows,
                            const unsigned char* y_valid, float* cg_mean, float* cg_std, float* conf_out, float* metrics,
                            int phase_mask, cudaStream_t stream) {

@@ -33,25 +33,17 @@ struct FlowBuffers {
   const long long* invp3 = nullptr;
 };
 
-struct FlowTrainer;
-
 // grads_ext: caller-owned device buffer of flow_param_count floats, or NULL (the trainer allocates it).
 // forward_only: allocate only what flow_forward_rows needs (no backward workspaces, no gradient buffer).
+// The statistics block is the kStatDoubles of train_core.h: sum and sum of squares of the NLL over the labelled rows,
+// their number, 0, 0, 0, the NLL's min and max.
 int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, const AdamCfg& adam, float* grads_ext,
-                        bool forward_only, FlowTrainer** out);
-void flow_trainer_destroy(FlowTrainer* t);
-// The trainer's ConfidenceGenerator (bound and copied with trainer_conf_bind / trainer_conf_copy).
-TrainerConf* flow_trainer_conf(FlowTrainer* t);
-// The trainer's communicator (set up with trainer_comm_init; none: the exchanges are the caller's).
-TrainerComm* flow_trainer_comm(FlowTrainer* t);
-// The step's statistics block (device, the kStatDoubles of train_core.h): sum and sum of squares of the NLL over the
-// labelled rows, their number, 0, 0, 0, the NLL's min and max.
-double* flow_trainer_stats(FlowTrainer* t);
+                        bool forward_only, Trainer** out);
 
 // LinearRnvp.forward on rows x [rows, dim]: z / logprob [rows, dim], log_det [rows] (each may be NULL); with trav
 // non-NULL also ConfidenceGenerator.inference_without_update of the per-row NLL -(sum(logprob) + log_det) from the
 // generator state at cg_mean / cg_std.
-int flow_forward_rows(FlowTrainer* t, const float* params, const FlowBuffers& b, const float* x, int rows, float* z,
+int flow_forward_rows(Trainer* t, const float* params, const FlowBuffers& b, const float* x, int rows, float* z,
                       float* log_det, float* logprob, const float* cg_mean, const float* cg_std, float std_factor,
                       float* trav, cudaStream_t stream);
 
@@ -59,7 +51,7 @@ int flow_forward_rows(FlowTrainer* t, const float* params, const FlowBuffers& b,
 // (y_valid NULL: every row).  phase_mask: 1 = forward, NLL statistics, confidence update; 2 = backward (the flat
 // gradient); 4 = Adam (bumps step_counter); 7 = the whole step.  conf_out [rows] is in compacted order (the labelled
 // rows in their order); metrics [6]: loss_total, loss_trav (0), loss_reco (0), number of rows, cg_mean, cg_std.
-int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int flow_train_step(Trainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                     const FlowBuffers& b, const float* x, int rows, const unsigned char* y_valid, float* cg_mean,
                     float* cg_std, float* conf_out, float* metrics, int phase_mask, cudaStream_t stream);
 // The same step on rows padded per group, x [groups, rows_per_group, dim] with n_rows[g] (device int32; NULL: all) live
@@ -67,7 +59,7 @@ int flow_train_step(FlowTrainer* t, float* params, float* exp_avg, float* exp_av
 // are never read.  phase_mask splits the step around the data-parallel exchanges: 1 = forward + this rank's NLL sums
 // (+ their all-reduce); 2 = generator update from the global sums, metrics, per-row confidence, backward scaled by the
 // global labelled count (+ the gradient all-reduce); 4 = Adam; 7 = the whole step.
-int flow_train_step_padded(FlowTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int flow_train_step_padded(Trainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                            const FlowBuffers& b, const float* x, int groups, int rows_per_group, const int* n_rows,
                            const unsigned char* y_valid, float* cg_mean, float* cg_std, float* conf_out, float* metrics,
                            int phase_mask, cudaStream_t stream);

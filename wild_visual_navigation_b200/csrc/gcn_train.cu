@@ -242,13 +242,11 @@ int gcn_check_shape(const MlpShape& s, const char* who) {
   return WVN_OK;
 }
 
-struct GcnTrainer {
+struct GcnTrainer : Trainer {
+  GcnTrainer() : Trainer(TRAINER_GCN) {}
   MlpShape s;
   GcnOffsets o;
-  LossCfg loss;
-  AdamCfg adam;
-  int max_rows = 0, max_edges = 0;
-  void* arena = nullptr;
+  int max_edges = 0;
   DoubleScalars* sc = nullptr;
   int* n_live = nullptr;
   double* overflow = nullptr;   // this rank's overflow flag, copied into the statistics block's sixth sum
@@ -259,13 +257,11 @@ struct GcnTrainer {
   // y_l = X_l W_l^T (forward), then Â^T dZ_l (backward); a_l = ReLU(Z_l); dz_l: dLoss/dZ_l (dz3 = d_out)
   float *xg = nullptr, *y1 = nullptr, *a1 = nullptr, *dz1 = nullptr, *y2 = nullptr, *a2 = nullptr, *dz2 = nullptr,
         *y3 = nullptr, *out = nullptr, *d_out = nullptr;
-  float *loss_reco = nullptr, *raw = nullptr, *wraw = nullptr, *grads = nullptr;
-  TrainerConf conf;
-  TrainerComm comm;
+  float *loss_reco = nullptr, *raw = nullptr, *wraw = nullptr;
 };
 
 int gcn_trainer_create(const MlpShape& s, int max_rows, int max_edges, const LossCfg& loss, const AdamCfg& adam,
-                       float* grads_ext, GcnTrainer** out) {
+                       float* grads_ext, Trainer** out) {
   WVN_REQUIRE(out && max_rows > 0 && max_edges >= 0, "gcn trainer: bad arguments");
   WVN_PROPAGATE(gcn_check_shape(s, "gcn trainer"));
   GcnTrainer* t = new GcnTrainer();
@@ -279,25 +275,16 @@ int gcn_trainer_create(const MlpShape& s, int max_rows, int max_edges, const Los
   const size_t head = 256;   // scalars | n_live at 128 | overflow at 136
   const size_t ints_bytes = (ints * sizeof(int) + 255) / 256 * 256;
   const size_t bytes = head + ints_bytes + floats * sizeof(float);
-  if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
-    delete t;
-    return set_error(WVN_ERR_CUDA, "gcn trainer: cudaMalloc of %zu bytes failed", bytes);
-  }
-  const int rc = trainer_conf_create(&t->conf);
+  const int rc = trainer_alloc(t, bytes, "gcn trainer");
   if (rc != WVN_OK) {
-    cudaFree(t->arena);
     delete t;
     return rc;
-  }
-  if (cudaMemset(t->arena, 0, bytes) != cudaSuccess) {
-    trainer_conf_destroy(&t->conf);
-    cudaFree(t->arena);
-    delete t;
-    return set_error(WVN_ERR_CUDA, "gcn trainer: cudaMemset of %zu bytes failed", bytes);
   }
   static_assert(sizeof(DoubleScalars) <= 128, "scalars overlap n_live");
   char* base = reinterpret_cast<char*>(t->arena);
   t->sc = reinterpret_cast<DoubleScalars*>(base);
+  t->stats = &t->sc->sum_lr;
+  t->n_stats = kStatDoubles + 1;
   t->n_live = reinterpret_cast<int*>(base + 128);
   t->overflow = reinterpret_cast<double*>(base + 136);
   int* ip = reinterpret_cast<int*>(base + head);
@@ -318,18 +305,6 @@ int gcn_trainer_create(const MlpShape& s, int max_rows, int max_edges, const Los
   *out = t;
   return WVN_OK;
 }
-
-void gcn_trainer_destroy(GcnTrainer* t) {
-  if (!t) return;
-  trainer_comm_destroy(&t->comm);
-  if (t->arena) cudaFree(t->arena);
-  trainer_conf_destroy(&t->conf);
-  delete t;
-}
-
-TrainerConf* gcn_trainer_conf(GcnTrainer* t) { return &t->conf; }
-TrainerComm* gcn_trainer_comm(GcnTrainer* t) { return &t->comm; }
-double* gcn_trainer_stats(GcnTrainer* t) { return &t->sc->sum_lr; }
 
 namespace {
 
@@ -376,12 +351,14 @@ int forward(GcnTrainer* t, const float* params, const float* x, int groups, int 
 
 }  // namespace
 
-int gcn_train_step_padded(GcnTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int gcn_train_step_padded(Trainer* base, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                           const float* x, int groups, int rows_per_group, const int* n_rows, const long long* edges,
                           int edges_per_group, const int* n_edges, const float* y, const unsigned char* y_valid,
                           float* cg_mean, float* cg_std, float* conf_out, float* metrics, int phase_mask,
                           cudaStream_t stream) {
-  WVN_REQUIRE(t && params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
+  WVN_PROPAGATE(trainer_check(base, TRAINER_GCN, "gcn train step"));
+  GcnTrainer* t = static_cast<GcnTrainer*>(base);
+  WVN_REQUIRE(params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
               "gcn train step: null argument");
   WVN_PROPAGATE(check_geometry(t, groups, rows_per_group, edges, edges_per_group, n_edges, "gcn train step"));
   const MlpShape& s = t->s;
@@ -447,11 +424,13 @@ int gcn_train_step_padded(GcnTrainer* t, float* params, float* exp_avg, float* e
   return WVN_OK;
 }
 
-int gcn_infer_rows(GcnTrainer* t, const float* params, const float* x, int groups, int rows_per_group,
+int gcn_infer_rows(Trainer* base, const float* params, const float* x, int groups, int rows_per_group,
                    const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
                    const float* cg_mean, const float* cg_std, float std_factor, float* out, float* trav, float* conf,
                    cudaStream_t stream) {
-  WVN_REQUIRE(t && params && x && (!conf || (cg_mean && cg_std)), "gcn infer rows: null argument");
+  WVN_PROPAGATE(trainer_check(base, TRAINER_GCN, "gcn infer rows"));
+  GcnTrainer* t = static_cast<GcnTrainer*>(base);
+  WVN_REQUIRE(params && x && (!conf || (cg_mean && cg_std)), "gcn infer rows: null argument");
   WVN_PROPAGATE(check_geometry(t, groups, rows_per_group, edges, edges_per_group, n_edges, "gcn infer rows"));
   const int D = t->s.dim, rows = groups * rows_per_group;
   WVN_PROPAGATE(forward(t, params, x, groups, rows_per_group, n_rows, edges, edges_per_group, n_edges, stream));

@@ -23,16 +23,11 @@ size_t gcn_param_count(const MlpShape& s);
 // The shapes the kernels take: 1 <= dim <= 1024, 1 <= h1, h2 <= 512 (WVN_ERR_INVALID else).
 int gcn_check_shape(const MlpShape& s, const char* who);
 
-struct GcnTrainer;
 // Workspaces for max_rows padded rows and max_edges padded edges (groups * edges_per_group).  grads_ext: caller-owned
-// device buffer of gcn_param_count floats, or NULL (the trainer allocates it).
+// device buffer of gcn_param_count floats, or NULL (the trainer allocates it).  The statistics block has 9 doubles,
+// laid out as the DoubleMLP trainer's (double_mlp_train.h).
 int gcn_trainer_create(const MlpShape& s, int max_rows, int max_edges, const LossCfg& loss, const AdamCfg& adam,
-                       float* grads_ext, GcnTrainer** out);
-void gcn_trainer_destroy(GcnTrainer* t);
-TrainerConf* gcn_trainer_conf(GcnTrainer* t);
-TrainerComm* gcn_trainer_comm(GcnTrainer* t);
-// The step's statistics block (device, 9 doubles), laid out as the DoubleMLP trainer's (double_mlp_train.h).
-double* gcn_trainer_stats(GcnTrainer* t);
+                       float* grads_ext, Trainer** out);
 
 // One TraversabilityEstimator.train() body on a batch of frames: x [groups, rows_per_group, dim] with n_rows[g] (device
 // int32; NULL: all) live rows in frame g; edges [groups, edges_per_group, 2] int64 (source, target) local row ids of
@@ -43,7 +38,7 @@ double* gcn_trainer_stats(GcnTrainer* t);
 // losses, the statistic sums (+ their all-reduce); 2 = generator update, dLoss/dOut, backward, gradients (+ the gradient
 // all-reduce); 4 = loss metrics + Adam; 7 = the whole step.  metrics [7] (may be NULL): loss_total, loss_trav,
 // loss_reco, loss_trav_conf, cg_mean, cg_std, the overflow flag.
-int gcn_train_step_padded(GcnTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int gcn_train_step_padded(Trainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                           const float* x, int groups, int rows_per_group, const int* n_rows, const long long* edges,
                           int edges_per_group, const int* n_edges, const float* y, const unsigned char* y_valid,
                           float* cg_mean, float* cg_std, float* conf_out, float* metrics, int phase_mask,
@@ -53,7 +48,7 @@ int gcn_train_step_padded(GcnTrainer* t, float* params, float* exp_avg, float* e
 // traversability = out[:, 0] and the confidence of loss_reco under the generator (inference_without_update).
 // out (may be NULL): [groups * rows_per_group, 1 + dim], the first live-count rows in compacted order.  trav / conf
 // (may be NULL): [groups * rows_per_group] in PADDED order; padding rows are not written.
-int gcn_infer_rows(GcnTrainer* t, const float* params, const float* x, int groups, int rows_per_group,
+int gcn_infer_rows(Trainer* t, const float* params, const float* x, int groups, int rows_per_group,
                    const int* n_rows, const long long* edges, int edges_per_group, const int* n_edges,
                    const float* cg_mean, const float* cg_std, float std_factor, float* out, float* trav, float* conf,
                    cudaStream_t stream);

@@ -16,7 +16,7 @@
 // Rows arrive PADDED, as the segment-pooling kernel leaves them: x [groups, rows_per_group, dim] with n_rows[g] live rows
 // per group (device memory).  The compaction the reference does with a boolean mask (`feat[seg_mask]`) happens inside
 // the kernels — labels y / y_valid are indexed by the compacted row number — so the step has no host synchronisation.
-// The communicator is the training core's (train_core.h: NCCL, owned by the library, wvn_mlp_trainer_init_comm), so the
+// The communicator is the training core's (train_core.h: NCCL, owned by the library, wvn_trainer_init_comm), so the
 // collectives are issued from here on the caller's stream.
 #include <string.h>
 
@@ -517,23 +517,18 @@ train_apply_kernel(float* __restrict__ p, const float* __restrict__ g, float* __
 
 }  // namespace
 
-struct FusedTrainer {
+struct FusedTrainer : Trainer {
+  FusedTrainer() : Trainer(TRAINER_MLP) {}
   MlpShape s;
   MlpOffsets o;
-  LossCfg loss;
-  AdamCfg adam;
-  int max_rows = 0;
   float *h1 = nullptr, *h2 = nullptr, *out = nullptr, *d_out = nullptr, *d_h2 = nullptr, *d_h1 = nullptr,
-        *loss_reco = nullptr, *raw = nullptr, *grads = nullptr;
+        *loss_reco = nullptr, *raw = nullptr;
   FusedScalars* sc = nullptr;
-  void* arena = nullptr;
-  TrainerComm comm;        // the library's communicator of a data-parallel step (train_core.h)
   size_t smem_fwd = 0, smem_bwd = 0;
-  TrainerConf conf;        // ConfidenceGenerator method + where its state lives
 };
 
 int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, void* scalars_ext,
-                         float* grads_ext, FusedTrainer** out) {
+                         float* grads_ext, Trainer** out) {
   WVN_REQUIRE(out && max_rows > 0, "trainer: bad arguments");
   WVN_REQUIRE(s.dim > 0 && s.dim <= 1024 && s.h1 > 0 && s.h1 <= 256 && s.h1 % 4 == 0 && s.h2 > 0 && s.h2 <= 32,
               "trainer: shape %d-%d-%d outside the fused kernels' range (dim <= 1024, h1 <= 256 and a multiple of 4, "
@@ -544,23 +539,18 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
   const size_t R = t->max_rows, n3 = s.dim + 1;
   const size_t floats = R * s.h1 * 2 + R * s.h2 * 2 + R * n3 * 2 + R * 2 + (t->o.total + 1);
   const size_t bytes = floats * sizeof(float) + 256;
-  if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
+  const int rc = trainer_alloc(t, bytes, "trainer");
+  if (rc != WVN_OK) {
     delete t;
-    return set_error(WVN_ERR_CUDA, "trainer: cudaMalloc of %zu bytes failed", bytes);
+    return rc;
   }
-  cudaMemset(t->arena, 0, bytes);
   t->sc = scalars_ext ? reinterpret_cast<FusedScalars*>(scalars_ext) : reinterpret_cast<FusedScalars*>(t->arena);
+  t->stats = &t->sc->sum_lr;
   {
     FusedScalars init;
     memset(&init, 0, sizeof(init));
     init.x_min = INFINITY;
     cudaMemcpy(t->sc, &init, sizeof(init), cudaMemcpyHostToDevice);
-  }
-  const int rc = trainer_conf_create(&t->conf);
-  if (rc != WVN_OK) {
-    cudaFree(t->arena);
-    delete t;
-    return rc;
   }
   float* f = reinterpret_cast<float*>(reinterpret_cast<char*>(t->arena) + 256);
   t->h1 = f; f += R * s.h1;
@@ -576,7 +566,7 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
                                  s.h2 * TR + TR + TR);
   t->smem_bwd = sizeof(float) * (((n3 * TRP + 3) & ~size_t(3)) + s.h2 * TR + TR + 8);
   if (t->smem_fwd > 227 * 1024 || t->smem_bwd > 227 * 1024) {
-    fused_trainer_destroy(t);
+    delete t;
     return set_error(WVN_ERR_INVALID, "trainer: shared memory need exceeds 227 KB");
   }
   cudaFuncSetAttribute(train_fwd_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(t->smem_fwd));
@@ -585,23 +575,13 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
   return WVN_OK;
 }
 
-void fused_trainer_destroy(FusedTrainer* t) {
-  if (!t) return;
-  trainer_comm_destroy(&t->comm);
-  if (t->arena) cudaFree(t->arena);
-  trainer_conf_destroy(&t->conf);
-  delete t;
-}
-
-TrainerConf* fused_trainer_conf(FusedTrainer* t) { return &t->conf; }
-
-TrainerComm* fused_trainer_comm(FusedTrainer* t) { return &t->comm; }
-
-int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int fused_train_step(Trainer* base, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                      const float* x, int groups, int rpg, const int* n_rows, const float* y,
                      const unsigned char* y_valid, float* cg_mean, float* cg_std, float* conf_out, float* metrics,
                      int phase_mask, cudaStream_t stream) {
-  WVN_REQUIRE(t && params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
+  WVN_PROPAGATE(trainer_check(base, TRAINER_MLP, "train step"));
+  FusedTrainer* t = static_cast<FusedTrainer*>(base);
+  WVN_REQUIRE(params && exp_avg && exp_avg_sq && step_counter && x && y && y_valid && conf_out,
               "train step: null argument");
   const long long rows = static_cast<long long>(groups) * rpg;
   WVN_REQUIRE(groups > 0 && rpg > 0 && rows <= t->max_rows, "train step: %d x %d rows exceed the trainer's capacity %d",

@@ -27,20 +27,14 @@ struct FusedScalars {
   float lo, hi, cmin, cmax, g_reco, g_trav;
 };
 
-struct FusedTrainer;
-
 // scalars_ext (sizeof(FusedScalars) bytes) / grads_ext (n_params + 1 floats): caller-owned device buffers, or NULL to
 // let the trainer allocate them with the rest of its workspace (everything is allocated here, nothing per step).
+// The statistics block is the scalars' first kStatDoubles.
 int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, const AdamCfg& adam, void* scalars_ext,
-                         float* grads_ext, FusedTrainer** out);
-void fused_trainer_destroy(FusedTrainer* t);
-// The trainer's communicator (set up with trainer_comm_init; none: the exchanges are the caller's).
-TrainerComm* fused_trainer_comm(FusedTrainer* t);
-// The trainer's ConfidenceGenerator (bound and copied with trainer_conf_bind / trainer_conf_copy).
-TrainerConf* fused_trainer_conf(FusedTrainer* t);
+                         float* grads_ext, Trainer** out);
 // phase_mask: 1 = forward + statistics (+ their all-reduce), 2 = backward + weight gradients (+ gradient all-reduce),
 // 4 = loss metrics + Adam; 7 = the whole step.
-int fused_train_step(FusedTrainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
+int fused_train_step(Trainer* t, float* params, float* exp_avg, float* exp_avg_sq, long long* step_counter,
                      const float* x, int groups, int rows_per_group, const int* n_rows, const float* y,
                      const unsigned char* y_valid, float* cg_mean, float* cg_std, float* conf_out, float* metrics,
                      int phase_mask, cudaStream_t stream);

@@ -1,6 +1,6 @@
-// wvn-b200: the fp32 training core shared by the MLP and LinearRnvp trainers (train_core.h): the private
-// ConfidenceGenerator block, Adam, the batched fp32 CUDA-core GEMM, the compaction of padded rows and the NCCL
-// communicator of data-parallel steps.
+// wvn-b200: the fp32 training core shared by the learners' trainers (train_core.h): the private ConfidenceGenerator
+// block, Adam, the batched fp32 CUDA-core GEMM, the compaction of padded rows, the NCCL communicator of data-parallel
+// steps and the trainer base's allocation and release.
 #include <dlfcn.h>
 #include <string.h>
 
@@ -363,6 +363,31 @@ int trainer_comm_stats(TrainerComm* c, double* stats, bool extrema, cudaStream_t
 int trainer_comm_sum(TrainerComm* c, void* buf, size_t n, bool f64, cudaStream_t stream) {
   if (!c->comm) return WVN_OK;
   return all_reduce(c, buf, n, f64 ? kNcclFloat64 : kNcclFloat32, kNcclSum, "grads", stream);
+}
+
+// ------------------------------------------------------------------------------------------------ trainer
+Trainer::~Trainer() {
+  trainer_comm_destroy(&comm);
+  if (arena) cudaFree(arena);
+  trainer_conf_destroy(&conf);
+}
+
+int trainer_alloc(Trainer* t, size_t bytes, const char* who) {
+  if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
+    t->arena = nullptr;
+    return set_error(WVN_ERR_CUDA, "%s: cudaMalloc of %zu bytes failed", who, bytes);
+  }
+  if (cudaMemset(t->arena, 0, bytes) != cudaSuccess)
+    return set_error(WVN_ERR_CUDA, "%s: cudaMemset of %zu bytes failed", who, bytes);
+  return trainer_conf_create(&t->conf);
+}
+
+int trainer_check(const Trainer* t, TrainerKind kind, const char* who) {
+  static const char* const names[] = {"SimpleMLP", "DoubleMLP", "SimpleGCN", "LinearRnvp"};
+  WVN_REQUIRE(t, "%s: null trainer", who);
+  WVN_REQUIRE(t->kind == kind, "%s: expected a %s trainer, got a %s trainer's handle", who, names[kind],
+              names[t->kind]);
+  return WVN_OK;
 }
 
 }  // namespace wvn

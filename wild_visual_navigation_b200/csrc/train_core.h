@@ -1,10 +1,12 @@
-// wvn-b200: the fp32 training core shared by the MLP trainers (mlp_train.cu, mlp_train_fused.cu) and the LinearRnvp
-// trainer (flow_train.cu): the ConfidenceGenerator state a trainer keeps, Adam, the batched fp32 tile GEMM, the
-// compaction of padded rows and the data-parallel exchange.
+// wvn-b200: the fp32 training core shared by the learners (mlp_train.cu, mlp_train_fused.cu, double_mlp_train.cu,
+// gcn_train.cu, flow_train.cu): the ConfidenceGenerator state a trainer keeps, Adam, the batched fp32 tile GEMM, the
+// compaction of padded rows, the data-parallel exchange and the trainer base every learner derives from.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stddef.h>
+
+#include "mlp_train.h"
 
 namespace wvn {
 
@@ -100,5 +102,32 @@ void trainer_comm_destroy(TrainerComm* c);
 int trainer_comm_stats(TrainerComm* c, double* stats, bool extrema, cudaStream_t stream);
 // SUM of n fp32 (f64 = false) or fp64 values in place.
 int trainer_comm_sum(TrainerComm* c, void* buf, size_t n, bool f64, cudaStream_t stream);
+
+// ---- the trainer every learner derives from
+enum TrainerKind : int { TRAINER_MLP = 0, TRAINER_DOUBLE_MLP = 1, TRAINER_GCN = 2, TRAINER_FLOW = 3 };
+
+// The state every learner's trainer (FusedTrainer, DoubleTrainer, GcnTrainer, FlowTrainer) keeps; the C ABI's
+// wvn_trainer_t is a pointer to it.  Deleting a trainer destroys its communicator, frees its arena and destroys its
+// generator block.
+struct Trainer {
+  explicit Trainer(TrainerKind k) : kind(k) {}
+  virtual ~Trainer();
+  const TrainerKind kind;
+  LossCfg loss;
+  AdamCfg adam;
+  int max_rows = 0;
+  void* arena = nullptr;   // every device workspace of the learner, one allocation
+  TrainerConf conf;        // ConfidenceGenerator method + where its state lives
+  TrainerComm comm;        // the library's communicator of a data-parallel step
+  double* stats = nullptr; // the statistics block: kStatDoubles, then the learner's own exchanged doubles
+  int n_stats = kStatDoubles;
+  float* grads = nullptr;
+};
+// Allocates t's arena of `bytes`, zeroed, and its generator block.  On failure the caller deletes t, which releases
+// whatever was allocated.
+int trainer_alloc(Trainer* t, size_t bytes, const char* who);
+// WVN_ERR_INVALID unless t is a trainer of `kind`: every entry point of a learner checks its handle on the host,
+// before it enqueues anything.
+int trainer_check(const Trainer* t, TrainerKind kind, const char* who);
 
 }  // namespace wvn

@@ -566,18 +566,32 @@ def _device_doubles(address, n, device):
 
 
 class _TrainerHandle:
-    """Owns a library trainer handle with workspaces for ``max_rows`` rows and replaces it by a larger one when a call
-    needs more.  Remembers the ConfidenceGenerator binding, so the replacement keeps the generator where it was.
-    Subclasses name their ABI functions and make the handle in ``_new_handle``.
+    """Owns a library trainer handle (``wvn_trainer_t``) with workspaces for ``max_rows`` rows and replaces it by a
+    larger one when a call needs more.  Remembers the ConfidenceGenerator binding, so the replacement keeps the generator
+    where it was.  Allocates the state every learner's step reads and updates: ``grads`` (``n_grads`` floats),
+    Adam's ``exp_avg`` / ``exp_avg_sq`` / ``step_counter``, ``metrics`` (``n_metrics`` floats) and the generator's
+    ``cg_mean`` / ``cg_std``.  Subclasses make the handle in ``_new_handle``.
 
     Data-parallel steps (``process_group``) are run here for every trainer: with an NCCL group the handle gets the
     library's own communicator and the step issues both all-reduces itself, between its kernels; with any other backend
     (gloo in tests) the step runs as phase 1 / all-reduce of the statistics block / phase 2 / all-reduce of the gradient
-    / phase 4 through ``torch.distributed`` on the same buffers.  ``stats``: the handle's statistics block (6 sums, then
-    the extrema); ``_grad_exchange()``: the buffers summed after phase 2."""
+    / phase 4 through ``torch.distributed`` on the same buffers.  ``stats``: the handle's statistics block (6 sums, the
+    extrema, and for some learners a ninth double exchanged with the gradient); ``_grad_exchange()``: the buffers
+    summed after phase 2."""
 
-    _DESTROY = _SET_CONFIDENCE = _COPY_CONFIDENCE = _INIT_COMM = None
-    pg = None
+    def __init__(self, device, n_params, cfg, max_rows, process_group, n_metrics=6, n_grads=None):
+        self.n_params, self.cfg, self.pg = n_params, cfg, process_group
+        self.grads = torch.zeros(n_params if n_grads is None else n_grads, device=device)
+        self.exp_avg = torch.zeros(n_params, device=device)
+        self.exp_avg_sq = torch.zeros(n_params, device=device)
+        self.step_counter = torch.zeros(1, device=device, dtype=torch.int64)
+        self.metrics = torch.zeros(n_metrics, device=device)
+        self.cg_mean = torch.zeros(1, device=device)
+        self.cg_std = torch.ones(1, device=device)
+        self._conf = None     # (method id, var, running_n, running_sum, running_sum_of_squares, kf_proc_cov, kf_meas_cov)
+        self._h = None
+        self._lib_comm = False
+        self._create(max_rows)
 
     def _create(self, max_rows):
         h = self._new_handle(int(max_rows))
@@ -585,10 +599,13 @@ class _TrainerHandle:
             # both handles' workspaces are alive until the old one is destroyed: peak memory briefly doubles here.
             # The confidence state the old handle kept itself (moving_average's window, var and running sums not bound
             # to caller tensors) moves over, so the generator does not restart
-            check(getattr(lib(), self._COPY_CONFIDENCE)(h, self._h, stream()))
-            getattr(lib(), self._DESTROY)(self._h)
+            check(lib().wvn_trainer_copy_confidence(h, self._h, stream()))
+            lib().wvn_trainer_destroy(self._h)
         self._h = h
         self.max_rows = int(max_rows)
+        self.conf = torch.empty(self.max_rows, device=self.grads.device)
+        n = ctypes.c_int()
+        self.stats = _device_doubles(lib().wvn_trainer_stats(h, byref(n)), n.value, self.grads.device)
         if self._conf is not None:
             self.set_confidence(*self._conf)
         self._init_comm()
@@ -608,7 +625,7 @@ class _TrainerHandle:
             idt = torch.tensor(list(buf), dtype=torch.uint8, device=self.exp_avg.device)
             dist.broadcast(idt, src=dist.get_global_rank(self.pg, 0), group=self.pg)
             raw = (ctypes.c_ubyte * 128)(*idt.cpu().tolist())
-            check(getattr(lib(), self._INIT_COMM)(self._h, raw, rank, world))
+            check(lib().wvn_trainer_init_comm(self._h, raw, rank, world))
             self._lib_comm = True
 
     def _run_phases(self, phase):
@@ -638,14 +655,18 @@ class _TrainerHandle:
         moving_average) and the device tensors holding its state (updated in place by the step; None = private)."""
         self._conf = (int(method), var, running_n, running_sum, running_sum_of_squares, float(kf_proc_cov), float(kf_meas_cov))
         if self._h is not None:
-            check(getattr(lib(), self._SET_CONFIDENCE)(self._h, int(method), ptr(var), ptr(running_n), ptr(running_sum),
-                                                       ptr(running_sum_of_squares), float(kf_proc_cov),
-                                                       float(kf_meas_cov)))
+            check(lib().wvn_trainer_set_confidence(self._h, int(method), ptr(var), ptr(running_n), ptr(running_sum),
+                                                   ptr(running_sum_of_squares), float(kf_proc_cov), float(kf_meas_cov)))
+
+    def _grad_exchange(self):
+        # the gradient, and the ninth double of the statistics block when the learner has one (DoubleMLP, SimpleGCN: the
+        # confidence-weighted error sum, kept in fp64)
+        return (self.grads, self.stats[8:9]) if self.stats.numel() > 8 else (self.grads,)
 
     def __del__(self):
         try:
             if getattr(self, "_h", None):
-                getattr(lib(), self._DESTROY)(self._h)
+                lib().wvn_trainer_destroy(self._h)
                 self._h = None
         except Exception:
             pass
@@ -665,50 +686,29 @@ class MlpTrainer(_TrainerHandle):
                  anomaly_balanced=True, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, process_group=None, legacy=False):
         _C.require_device()
         self.dim, self.h1, self.h2 = dim, h1, h2
-        self.n_params = lib().wvn_mlp_param_count(dim, h1, h2)
-        assert params.numel() == self.n_params and params.is_cuda and params.dtype == torch.float32
-        dev = params.device
+        n_params = lib().wvn_mlp_param_count(dim, h1, h2)
+        assert params.numel() == n_params and params.is_cuda and params.dtype == torch.float32
         self.params = params
-        self.grads = torch.zeros(self.n_params + 1, device=dev)
-        self.exp_avg = torch.zeros(self.n_params, device=dev)
-        self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
-        self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
-        self.cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
-        self.metrics = torch.zeros(6, device=dev)
-        self.cg_mean = torch.zeros(1, device=dev)
-        self.cg_std = torch.ones(1, device=dev)
-        self.pg = process_group
         self.legacy = legacy
-        self._conf = None     # (method id, var, running_n, running_sum, running_sum_of_squares, kf_proc_cov, kf_meas_cov)
-        self._h = None
-        self._lib_comm = False
-        if legacy:
-            self.scalars = torch.zeros(lib().wvn_mlp_train_scalars_bytes() // 8, device=dev, dtype=torch.float64)
-            self._alloc_ws(max_rows)
-            return
-        self.scalars = torch.zeros((lib().wvn_mlp_trainer_scalars_bytes() + 7) // 8, device=dev, dtype=torch.float64)
-        self.stats = self.scalars
-        self._create(max_rows)
+        nbytes = lib().wvn_mlp_train_scalars_bytes() if legacy else lib().wvn_mlp_trainer_scalars_bytes()
+        self.scalars = torch.zeros((nbytes + 7) // 8, device=params.device, dtype=torch.float64)
+        cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
+        # the gradient's extra float: the confidence-weighted error sum, exchanged with it
+        super().__init__(params.device, n_params, cfg, max_rows, process_group, n_grads=n_params + 1)
 
     # ---- fused path ---------------------------------------------------------------------------
-    _DESTROY = "wvn_mlp_trainer_destroy"
-    _SET_CONFIDENCE = "wvn_mlp_trainer_set_confidence"
-    _COPY_CONFIDENCE = "wvn_mlp_trainer_copy_confidence"
-
     def _new_handle(self, max_rows):
         h = c_void_p()
         check(lib().wvn_mlp_trainer_create(self.dim, self.h1, self.h2, max_rows, byref(self.cfg), ptr(self.scalars),
                                            ptr(self.grads), byref(h)))
         return h
 
-    _INIT_COMM = "wvn_mlp_trainer_init_comm"
-
     def _create(self, max_rows):
+        if self.legacy:
+            self._alloc_ws(max_rows)
+            return
         super()._create(max_rows)
         self.conf = torch.empty(self.max_rows + 32, device=self.params.device, dtype=torch.float32)
-
-    def _grad_exchange(self):
-        return (self.grads,)   # the confidence-weighted error sum rides at its end
 
     def set_confidence(self, method=0, *args, **kwargs):
         assert not self.legacy or method == 0, "the round-1 kernels implement latest_measurement only"
@@ -802,47 +802,23 @@ class DoubleMlpTrainer(_TrainerHandle):
     statistic sums, row counts and extrema are all-reduced after the forward, the gradient and the confidence-weighted
     error sum after the backward."""
 
-    _DESTROY = "wvn_double_mlp_trainer_destroy"
-    _SET_CONFIDENCE = "wvn_double_mlp_trainer_set_confidence"
-    _COPY_CONFIDENCE = "wvn_double_mlp_trainer_copy_confidence"
-    _INIT_COMM = "wvn_double_mlp_trainer_init_comm"
-
     def __init__(self, model, max_rows=4096, w_trav=0.03, w_reco=0.5, std_factor=0.5, anomaly_balanced=True, lr=1e-3,
                  betas=(0.9, 0.999), eps=1e-8, process_group=None):
         model.check_supported()
         _C.require_device()
         params = model.flat_params
-        dev = params.device
         self.model = model
         self.dim, (self.h1, self.h2) = model.input_size, model.hidden
-        self.n_params = lib().wvn_double_mlp_param_count(self.dim, self.h1, self.h2)
-        assert params.numel() == self.n_params and params.dtype == torch.float32
-        self.cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
-        self.grads = torch.zeros(self.n_params, device=dev)
-        self.exp_avg = torch.zeros(self.n_params, device=dev)
-        self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
-        self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
-        self.metrics = torch.zeros(6, device=dev)
-        self.cg_mean = torch.zeros(1, device=dev)
-        self.cg_std = torch.ones(1, device=dev)
-        self.pg = process_group
-        self._h = None
-        self._conf = None
-        self._create(max_rows)
+        n_params = lib().wvn_double_mlp_param_count(self.dim, self.h1, self.h2)
+        assert params.numel() == n_params and params.dtype == torch.float32
+        cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
+        super().__init__(params.device, n_params, cfg, max_rows, process_group)
 
     def _new_handle(self, max_rows):
         h = c_void_p()
         check(lib().wvn_double_mlp_trainer_create(self.dim, self.h1, self.h2, max_rows, byref(self.cfg), ptr(self.grads),
                                                   byref(h)))
         return h
-
-    def _create(self, max_rows):
-        super()._create(max_rows)
-        self.conf = torch.empty(self.max_rows, device=self.grads.device)
-        self.stats = _device_doubles(lib().wvn_double_mlp_trainer_stats(self._h), 9, self.grads.device)
-
-    def _grad_exchange(self):
-        return (self.grads, self.stats[8:9])   # + the confidence-weighted error sum, kept in fp64
 
     def _run(self, x, groups, rpg, n_rows, y, y_valid):
         self._reserve(groups * rpg)
@@ -936,34 +912,18 @@ class GcnTrainer(_TrainerHandle):
     global-batch exact (see ``_TrainerHandle``); no edge crosses frames, so sharding frames loses nothing.
     ``metrics[6]`` is 1 after a step that met a negative edge count (the segment reducer's overflow flag)."""
 
-    _DESTROY = "wvn_gcn_trainer_destroy"
-    _SET_CONFIDENCE = "wvn_gcn_trainer_set_confidence"
-    _COPY_CONFIDENCE = "wvn_gcn_trainer_copy_confidence"
-    _INIT_COMM = "wvn_gcn_trainer_init_comm"
-
     def __init__(self, model, max_rows=4096, max_edges=16384, w_trav=0.03, w_reco=0.5, std_factor=0.5,
                  anomaly_balanced=True, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, process_group=None):
         model.check_supported()
         _C.require_device()
         params = model.flat_params
-        dev = params.device
         self.model = model
         self.dim, (self.h1, self.h2) = model.input_size, model.hidden
-        self.n_params = lib().wvn_gcn_param_count(self.dim, self.h1, self.h2)
-        assert params.numel() == self.n_params and params.dtype == torch.float32
-        self.cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
-        self.grads = torch.zeros(self.n_params, device=dev)
-        self.exp_avg = torch.zeros(self.n_params, device=dev)
-        self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
-        self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
-        self.metrics = torch.zeros(7, device=dev)
-        self.cg_mean = torch.zeros(1, device=dev)
-        self.cg_std = torch.ones(1, device=dev)
-        self.pg = process_group
+        n_params = lib().wvn_gcn_param_count(self.dim, self.h1, self.h2)
+        assert params.numel() == n_params and params.dtype == torch.float32
         self.max_edges = int(max_edges)
-        self._h = None
-        self._conf = None
-        self._create(max_rows)
+        cfg = TrainConfig(w_trav, w_reco, std_factor, int(anomaly_balanced), lr, betas[0], betas[1], eps)
+        super().__init__(params.device, n_params, cfg, max_rows, process_group, n_metrics=7)
 
     def _new_handle(self, max_rows):
         h = c_void_p()
@@ -971,20 +931,12 @@ class GcnTrainer(_TrainerHandle):
                                            ptr(self.grads), byref(h)))
         return h
 
-    def _create(self, max_rows):
-        super()._create(max_rows)
-        self.conf = torch.empty(self.max_rows, device=self.grads.device)
-        self.stats = _device_doubles(lib().wvn_gcn_trainer_stats(self._h), 9, self.grads.device)
-
     def _reserve_edges(self, rows, edges):
         if edges > self.max_edges:
             self.max_edges = int(edges * 1.5)
             self._create(max(self.max_rows, int(rows)))
         else:
             self._reserve(rows)
-
-    def _grad_exchange(self):
-        return (self.grads, self.stats[8:9])   # + the confidence-weighted error sum, kept in fp64
 
     def _run(self, x, groups, rpg, n_rows, edges, epg, n_edges, y, y_valid):
         self._reserve_edges(groups * rpg, groups * epg)
@@ -1044,7 +996,7 @@ class GcnInference:
         rows, edges = max(int(rows), self.max_rows), max(int(edges), self.max_edges)
         check(lib().wvn_gcn_trainer_create(self.dim, self.h1, self.h2, rows, edges, byref(self.cfg), None, byref(h)))
         if self._h is not None:
-            lib().wvn_gcn_trainer_destroy(self._h)
+            lib().wvn_trainer_destroy(self._h)
         self._h, self.max_rows, self.max_edges = h, rows, edges
 
     def _run(self, x, groups, rpg, n_rows, edges, epg, n_edges, cg_mean=None, cg_std=None, std_factor=0.5,
@@ -1086,7 +1038,7 @@ class GcnInference:
     def __del__(self):
         try:
             if getattr(self, "_h", None):
-                lib().wvn_gcn_trainer_destroy(self._h)
+                lib().wvn_trainer_destroy(self._h)
                 self._h = None
         except Exception:
             pass
@@ -1190,44 +1142,20 @@ class FlowTrainer(_TrainerHandle):
     ``_TrainerHandle``): the NLL sums, the labelled-row count and the extrema are all-reduced after the forward, the
     gradient after the backward; the loss is the mean over the global labelled count."""
 
-    _DESTROY = "wvn_flow_destroy"
-    _SET_CONFIDENCE = "wvn_flow_set_confidence"
-    _COPY_CONFIDENCE = "wvn_flow_copy_confidence"
-    _INIT_COMM = "wvn_flow_init_comm"
-
     def __init__(self, model, max_rows=4096, std_factor=0.5, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, process_group=None):
         _C.require_device()
         params = model.flat_params
         assert params.is_cuda and params.dtype == torch.float32
-        dev = params.device
         self.model = model
         self.dim, self.hidden = model.input_size, model.hidden
-        self.cfg = TrainConfig(0.0, 0.0, float(std_factor), 0, float(lr), betas[0], betas[1], float(eps))
-        self.n_params = lib().wvn_flow_param_count(self.dim, self.hidden)
-        self.grads = torch.zeros(self.n_params, device=dev)
-        self.exp_avg = torch.zeros(self.n_params, device=dev)
-        self.exp_avg_sq = torch.zeros(self.n_params, device=dev)
-        self.step_counter = torch.zeros(1, device=dev, dtype=torch.int64)
-        self.metrics = torch.zeros(6, device=dev)
-        self.cg_mean = torch.zeros(1, device=dev)
-        self.cg_std = torch.ones(1, device=dev)
-        self.pg = process_group
-        self._h = None
-        self._conf = None
-        self._create(max_rows)
+        cfg = TrainConfig(0.0, 0.0, float(std_factor), 0, float(lr), betas[0], betas[1], float(eps))
+        super().__init__(params.device, lib().wvn_flow_param_count(self.dim, self.hidden), cfg, max_rows, process_group)
 
     def _new_handle(self, max_rows):
         h = c_void_p()
-        check(lib().wvn_flow_create(self.dim, self.hidden, max_rows, byref(self.cfg), ptr(self.grads), byref(h)))
+        check(lib().wvn_flow_trainer_create(self.dim, self.hidden, max_rows, byref(self.cfg), ptr(self.grads),
+                                            byref(h)))
         return h
-
-    def _create(self, max_rows):
-        super()._create(max_rows)
-        self.conf = torch.empty(self.max_rows, device=self.grads.device)
-        self.stats = _device_doubles(lib().wvn_flow_stats(self._h), 8, self.grads.device)
-
-    def _grad_exchange(self):
-        return (self.grads,)
 
     def _run(self, x, groups, rpg, n_rows, y_valid):
         self._reserve(groups * rpg)
