@@ -286,6 +286,37 @@ int wvn_stego_kmeans(float* rows, long long ld, int batch, int npad, int patches
                      int k, int iters, float* centroids_out, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * STEGO's dense CRF (run_crf=True; [EXTERNAL-RECALLED] stego crf.py dense_crf on pydensecrf, restated in
+ * oracle/dense_crf.py): DenseCRF2D with a Gaussian (sxy 1, Potts weight 3) and a bilateral (sxy 67, srgb 3, weight 4)
+ * kernel on permutohedral lattices, symmetric normalisation, `iterations` mean-field updates from
+ * U = -log(clip(softmax(logits), 1e-5, 1)).  The handle owns every workspace, sized at create for the worst case of
+ * `chunk` frames of size x size pixels; a run allocates nothing and never synchronises with the host.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct wvn_crf wvn_crf_t;
+/* size: side S of the transformed (square) image; max_classes in [1, 64]; chunk: frames refined together. */
+int wvn_crf_create(int size, int max_classes, int chunk, int iterations, wvn_crf_t** out);
+void wvn_crf_destroy(wvn_crf_t* h);
+size_t wvn_crf_workspace_bytes(const wvn_crf_t* h);
+/* img: the frames the patch loader read ([batch, 3, in_h, in_w] fp32 in [0, 1], or u8_hwc [batch, in_h, in_w, 3] uint8
+ * RGB), resized (nearest) to resized_h x resized_w and center-cropped to S x S as in wvn_vit_forward.
+ * head: the STEGO head output [batch*npad, ld] fp32 (patch p of frame b at row b*npad + 1 + p, grid x grid patches).
+ * Logits: columns [col0, col0+classes) upsampled bilinearly (align_corners=False) to S x S; with code_dim > 0 they are
+ * divided by the norm of the upsampled code (columns [code_col, code_col+code_dim)) and multiplied by logit_scale (the
+ * cluster probe: logit_scale 2).  labels: [batch, S, S] int64 argmax of Q; q_out (optional): [batch, S*S, classes]. */
+int wvn_crf_run(wvn_crf_t* h, const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
+                const float* head, long long ld, int npad, int grid, int col0, int classes, int code_col, int code_dim,
+                float logit_scale, long long* labels, float* q_out, void* stream);
+/* Testing.  wvn_crf_build: the two lattices (0: spatial, 1: bilateral) of frames [0, batch <= chunk).
+ * wvn_crf_filter: values [batch*S*S, v] through lattice `which`, unnormalised (splat, blur, slice) -> out.
+ * wvn_crf_export: vertex keys (packed as in oracle/dense_crf.py, ascending) and pixel counts, each pixel's d+1 vertex
+ * indices and barycentric weights ([batch*S*S, d+1]) and the vertex count m (device int). */
+int wvn_crf_build(wvn_crf_t* h, const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
+                  void* stream);
+int wvn_crf_filter(wvn_crf_t* h, int which, const float* values, int v, float* out, void* stream);
+int wvn_crf_export(wvn_crf_t* h, int which, unsigned long long* keys, int* counts, int* offsets, float* bary, int* m,
+                   void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Segment reductions — replace SegmentExtractor.adjacency_list / .centers
  * (feature_extractor/segment_extractor.py:40-92), FeatureExtractor.sparsify_features
  * (feature_extractor.py:389-396) and the relabel loop of segment_stego (:245-246).

@@ -95,6 +95,13 @@ SIGNATURES = {
     "wvn_flip_average": (_I, [_P, _I, _I, _I, _L, _P]),
     "wvn_stego_kmeans_workspace_bytes": (_S, [_I, _I, _I]),
     "wvn_stego_kmeans": (_I, [_P, _L, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
+    "wvn_crf_create": (_I, [_I, _I, _I, _I, POINTER(_P)]),
+    "wvn_crf_destroy": (None, [_P]),
+    "wvn_crf_workspace_bytes": (_S, [_P]),
+    "wvn_crf_run": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _L, _I, _I, _I, _I, _I, _I, _F, _P, _P, _P]),
+    "wvn_crf_build": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "wvn_crf_filter": (_I, [_P, _I, _P, _I, _P, _P]),
+    "wvn_crf_export": (_I, [_P, _I, _P, _P, _P, _P, _P, _P]),
     "wvn_segment_workspace_bytes": (_S, [_I, _I, _I, _I]),
     "wvn_segment_reduce": (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P]),
     "wvn_segment_relabel": (_I, [_P, _I, _L, _I, _P, _P, _P]),

@@ -10,6 +10,7 @@
 
 #include "../../include/wvn_b200.h"
 #include "attention.h"
+#include "dense_crf.h"
 #include "dense_kernels.h"
 #include "double_mlp_train.h"
 #include "gcn_train.h"
@@ -627,6 +628,61 @@ int wvn_slic_geometry(int h, int w, int num_components, int* grid_interval, int*
   WVN_REQUIRE(h > 0 && w > 0 && num_components > 0 && grid_interval && nx && ny, "wvn_slic_geometry: bad argument");
   slic_geometry(h, w, num_components, grid_interval, nx, ny);
   return WVN_OK;
+}
+
+struct wvn_crf {
+  DenseCrf* crf = nullptr;
+};
+
+int wvn_crf_create(int size, int max_classes, int chunk, int iterations, wvn_crf_t** out) {
+  WVN_REQUIRE(out, "wvn_crf_create: null argument");
+  WVN_PROPAGATE(wvn_check_device());
+  DenseCrf* c = nullptr;
+  WVN_PROPAGATE(crf_create(size, max_classes, chunk, iterations, &c));
+  *out = new wvn_crf{c};
+  return WVN_OK;
+}
+
+void wvn_crf_destroy(wvn_crf_t* h) {
+  if (!h) return;
+  crf_destroy(h->crf);
+  delete h;
+}
+
+size_t wvn_crf_workspace_bytes(const wvn_crf_t* h) { return h ? crf_workspace_bytes(h->crf) : 0; }
+
+static CrfInput crf_input(const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w) {
+  CrfInput in;
+  in.img = img; in.u8_hwc = u8_hwc; in.batch = batch; in.in_h = in_h; in.in_w = in_w;
+  in.resized_h = resized_h; in.resized_w = resized_w;
+  return in;
+}
+
+int wvn_crf_run(wvn_crf_t* h, const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
+                const float* head, long long ld, int npad, int grid, int col0, int classes, int code_col, int code_dim,
+                float logit_scale, long long* labels, float* q_out, void* stream) {
+  WVN_REQUIRE(h, "wvn_crf_run: null handle");
+  CrfInput in = crf_input(img, u8_hwc, batch, in_h, in_w, resized_h, resized_w);
+  in.head = head; in.ld = ld; in.npad = npad; in.grid = grid; in.col0 = col0; in.classes = classes;
+  in.code_col = code_col; in.code_dim = code_dim; in.logit_scale = logit_scale;
+  return crf_run(h->crf, in, labels, q_out, S(stream));
+}
+
+int wvn_crf_build(wvn_crf_t* h, const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
+                  void* stream) {
+  WVN_REQUIRE(h, "wvn_crf_build: null handle");
+  return crf_build(h->crf, crf_input(img, u8_hwc, batch, in_h, in_w, resized_h, resized_w), S(stream));
+}
+
+int wvn_crf_filter(wvn_crf_t* h, int which, const float* values, int v, float* out, void* stream) {
+  WVN_REQUIRE(h, "wvn_crf_filter: null handle");
+  return crf_filter(h->crf, which, values, v, out, S(stream));
+}
+
+int wvn_crf_export(wvn_crf_t* h, int which, unsigned long long* keys, int* counts, int* offsets, float* bary, int* m,
+                   void* stream) {
+  WVN_REQUIRE(h, "wvn_crf_export: null handle");
+  return crf_export(h->crf, which, keys, counts, offsets, bary, m, S(stream));
 }
 
 size_t wvn_slic_workspace_bytes(int batch, int h, int w, int num_components) {

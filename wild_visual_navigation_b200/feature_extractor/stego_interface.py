@@ -8,8 +8,11 @@ bilinear(align_corners=False) upsampling + argmax per pixel — algebraically th
 ``postprocess`` (upsample the 90-d code, then probe every pixel) without the 448x448x90 tensor.
 ``run_clustering=True`` (WVN's default through ``FeatureExtractor``): the cluster prediction comes from a per-image
 k-means of the code with ``n_image_clusters`` clusters (csrc/stego_kmeans.cu — one launch per batch of frames; the
-nearest-centroid scores replace the cluster-probe logits before the same upsample+argmax kernel).  CRF is out of scope
-(``run_crf`` must be False; the reference's own default for WVN, feature_extractor.py:52).
+nearest-centroid scores replace the cluster-probe logits before the same upsample+argmax kernel).
+``run_crf=True`` (the reference StegoInterface's default, off in WVN's FeatureExtractor): the cluster and linear
+predictions are the argmax of STEGO's dense CRF (csrc/dense_crf.cu, definition oracle/dense_crf.py) over the upsampled
+probe log-probabilities and the transformed image, instead of the plain argmax.  It cannot be combined with
+``run_clustering=True``.
 """
 from __future__ import annotations
 
@@ -27,9 +30,9 @@ class StegoInterface:
                  max_batch: int = 32, chunk: int = 0, code_dim: int = 90, kmeans_iters: int = 10):
         self._cfg = _Cfg(cfg) if cfg else _Cfg(model_path=model_path, input_size=input_size, run_crf=run_crf,
                                                run_clustering=run_clustering, n_image_clusters=n_image_clusters)
-        if self._cfg.run_crf:
-            raise ValueError("run_crf (pydensecrf on the CPU) is outside the H100 hot path; WVN itself runs with "
-                             "run_crf=False (feature_extractor.py:52)")
+        if self._cfg.run_crf and self._cfg.run_clustering:
+            raise ValueError("run_crf=True with run_clustering=True is not supported: what upstream feeds the CRF after "
+                             "its per-image k-means cannot be pinned; pass run_clustering=False")
         self._kmeans_iters = kmeans_iters
         self._device = device
         self._flip_tta = flip_tta
@@ -57,7 +60,10 @@ class StegoInterface:
                                    max_batch=max_batch * (2 if flip_tta else 1), chunk=chunk,
                                    state_dict=backbone_state_dict, head_weights=fold_stego_head(head_state_dict))
         self._code = self._cluster_pred = self._linear_pred = self._head_out = self._cl64 = self._li64 = self._code_tok = None
-        self._tokens = None
+        self._tokens = self._img = None
+        # the CRF's workspaces are sized once, for max_batch frames of input_size x input_size
+        self._crf = (ops.DenseCrf(input_size, max(self._n_clusters, self._n_classes), chunk=min(2, max_batch))
+                     if self._cfg.run_crf else None)
 
     def change_device(self, device):
         self._dino.change_device(device)
@@ -104,6 +110,13 @@ class StegoInterface:
                              self._kmeans_iters)
         self._head_out, self._geom = head, (B, H, npad, g, S)
         self._code_tok = self._code = self._cluster_pred = self._linear_pred = self._li64 = None
+        if self._crf is not None:
+            self._img = img
+            self._cl64 = self._to_image_size(self._crf_labels(HEAD_CLUSTER_COL, self._n_clusters, cluster=True))
+            if want_linear:
+                self._li64 = self._to_image_size(self._crf_labels(HEAD_LINEAR_COL, self._n_classes, cluster=False))
+            self._img_hw = (H, W)
+            return
         if want_linear:
             cl, li = ops.logits_argmax(head, HEAD_CLUSTER_COL, n_cluster_logits, B, npad, g, g, S, S,
                                        col0_b=HEAD_LINEAR_COL, classes_b=self._n_classes)
@@ -112,6 +125,13 @@ class StegoInterface:
             cl = ops.logits_argmax(head, HEAD_CLUSTER_COL, n_cluster_logits, B, npad, g, g, S, S)
         self._cl64 = self._to_image_size(cl)   # (B, H, H) int64 cluster ids
         self._img_hw = (H, W)
+
+    def _crf_labels(self, col0, classes, cluster):
+        """Dense-CRF labels (B, S, S) of the cluster probe (2 <normalize(code), normalize(c_k)>) or the linear probe."""
+        B, H, npad, g, S = self._geom
+        if cluster:
+            return self._crf.run(self._img, self._head_out, npad, g, col0, classes, HEAD_CODE_COL, self._code_dim, 2.0)
+        return self._crf.run(self._img, self._head_out, npad, g, col0, classes)
 
     def _to_image_size(self, pred):
         B, H, npad, g, S = self._geom
@@ -135,6 +155,8 @@ class StegoInterface:
     @property
     def linear_segments(self):
         if self._linear_pred is None and self._head_out is not None:
+            if self._li64 is None and self._crf is not None:
+                self._li64 = self._to_image_size(self._crf_labels(HEAD_LINEAR_COL, self._n_classes, cluster=False))
             if self._li64 is None:
                 B, H, npad, g, S = self._geom
                 self._li64 = self._to_image_size(ops.logits_argmax(self._head_out, HEAD_LINEAR_COL, self._n_classes, B, npad,

@@ -467,6 +467,78 @@ class ResNetBackbone:
             pass
 
 
+class DenseCrf:
+    """Owns a ``wvn_crf_t``: STEGO's dense CRF (oracle/dense_crf.py) for ``size`` x ``size`` frames with up to
+    ``max_classes`` labels, refined ``chunk`` frames at a time.  Every workspace is allocated here, for the worst case;
+    ``workspace_bytes`` says how much."""
+
+    def __init__(self, size, max_classes, chunk=2, iterations=10):
+        _C.require_device()
+        self.size, self.max_classes, self.chunk, self.iterations = size, max_classes, chunk, iterations
+        h = c_void_p()
+        check(lib().wvn_crf_create(size, max_classes, chunk, iterations, byref(h)))
+        self._h = h
+        self.workspace_bytes = lib().wvn_crf_workspace_bytes(h)
+
+    def _image_args(self, img, resized_hw):
+        img = img.contiguous()
+        if img.dtype == torch.uint8:
+            B, H, W, C = img.shape
+        else:
+            assert img.dtype == torch.float32
+            B, C, H, W = img.shape
+        assert C == 3
+        rh, rw = resized_hw or _resized_size(H, W, self.size)
+        return img, (c_void_p(img.data_ptr()), int(img.dtype == torch.uint8), B, H, W, rh, rw)
+
+    def run(self, img, head, npad, grid, col0, classes, code_col=0, code_dim=0, logit_scale=1.0, resized_hw=None,
+            want_q=False):
+        """img: the frames the backbone read ((B,3,H,W) fp32 or (B,H,W,3) uint8); head: STEGO head output
+        [B*npad, ld] fp32.  -> labels (B, S, S) int64, and with ``want_q`` also Q (B, S*S, classes) fp32."""
+        img, args = self._image_args(img, resized_hw)
+        B = args[2]
+        labels = torch.empty(B, self.size, self.size, device=head.device, dtype=torch.int64)
+        q = torch.empty(B, self.size * self.size, classes, device=head.device, dtype=torch.float32) if want_q else None
+        check(lib().wvn_crf_run(self._h, *args, ptr(head), head.stride(0), npad, grid, col0, classes, code_col, code_dim,
+                                logit_scale, ptr(labels), ptr(q), stream()))
+        return (labels, q) if want_q else labels
+
+    def build(self, img, resized_hw=None):
+        """Testing: build the two lattices of the frames of ``img`` (at most ``chunk``)."""
+        img, args = self._image_args(img, resized_hw)
+        check(lib().wvn_crf_build(self._h, *args, stream()))
+        self._built = args[2]
+
+    def filter(self, which, values):
+        """Testing: values [B*S*S, v] through lattice ``which`` (0 spatial, 1 bilateral) without normalisation."""
+        values = values.contiguous()
+        out = torch.empty_like(values)
+        check(lib().wvn_crf_filter(self._h, which, ptr(values), values.shape[1], ptr(out), stream()))
+        return out
+
+    def lattice(self, which):
+        """Testing: dict(keys (M,) packed int64 view, counts (M,), offsets (N, d+1), bary (N, d+1)) of lattice ``which``."""
+        d = 2 if which == 0 else 5
+        n = self._built * self.size * self.size
+        dev = "cuda"
+        keys = torch.empty(n * (d + 1), device=dev, dtype=torch.int64)
+        counts = torch.empty(n * (d + 1), device=dev, dtype=torch.int32)
+        offsets = torch.empty(n, d + 1, device=dev, dtype=torch.int32)
+        bary = torch.empty(n, d + 1, device=dev, dtype=torch.float32)
+        m = torch.empty(1, device=dev, dtype=torch.int32)
+        check(lib().wvn_crf_export(self._h, which, ptr(keys), ptr(counts), ptr(offsets), ptr(bary), ptr(m), stream()))
+        M = int(m.item())
+        return dict(keys=keys[:M], counts=counts[:M], offsets=offsets, bary=bary)
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().wvn_crf_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
 def _resized_size(h, w, size):
     # torchvision Resize(size:int): smaller edge -> size
     if h <= w:
