@@ -59,7 +59,9 @@ int wvn_check_device(void);
  * 108: the four learners' trainers share one handle type, wvn_trainer_t, and five entry points (wvn_trainer_destroy,
  * wvn_trainer_set_confidence, wvn_trainer_copy_confidence, wvn_trainer_init_comm, wvn_trainer_stats) in place of
  * each learner's own; wvn_flow_create is renamed wvn_flow_trainer_create and wvn_double_mlp_train_step is removed (its
- * padded form with one group is the same step).  A learner's entry point refuses another learner's handle. */
+ * padded form with one group is the same step).  A learner's entry point refuses another learner's handle.
+ * Later additions under 108 add symbols only: the dense CRF (wvn_crf_*), the EfficientNet-B0 handle (wvn_effnet_*)
+ * with its primitives, GEMM activation 3 (SiLU) and wvn_segment_pool_levels. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -75,7 +77,7 @@ int wvn_profile_collect(float* host_ms, long long* host_launches);
  * Primitive: bf16 tensor-core GEMM  C = A[M,K] * W[N,K]^T  (wgmma, fp32 accumulate)
  * Replaces every nn.Linear / 1x1-conv call of the path (cuBLAS in the reference).
  * out_kind: 0 = bf16 out[M,ldo] = act(acc + bias); 1 = fp32 out = acc + bias;
- *           2 = fp32 out += acc + bias (residual).   act: 0 none, 1 ReLU, 2 GELU(erf).
+ *           2 = fp32 out += acc + bias (residual).   act: 0 none, 1 ReLU, 2 GELU(erf), 3 SiLU (out_kind 0 only).
  * Any K >= 1: lda >= K and a multiple of 8, and W's rows are round_up(K, 8) elements apart (== K whenever K % 8 == 0);
  * columns past K of either operand are never read (the last 64-wide k-block is zero-filled past K).
  * N % block_n == 0, block_n in {0 (auto), 64, 128, 192, 224, 256}.
@@ -256,6 +258,57 @@ int wvn_im2col_image(const float* img, int batch, int h, int w, int k, int strid
 int wvn_maxpool3s2_bf16_nhwc(const void* in, int batch, int h, int w, int c, void* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * EfficientNet-B0 backbone handle — replaces TorchVisionInterface's model for model_type "efficientnet_b0"
+ * (torchvision efficientnet_b0 in eval mode behind create_feature_extractor).  NHWC bf16 activations at channel
+ * pitches rounded up to 64 (the pad channels are zero throughout), fp32 accumulation.  The stem (3 x 3 / 2, after an
+ * im2col pass of K = 27), every expand and project 1 x 1 conv and the head are wgmma GEMMs with batch norm folded in,
+ * SiLU or the residual add in the epilogue; each MBConv block's depthwise conv (+ batch norm + SiLU) is a SIMT kernel
+ * that also emits the squeeze-excitation's pool sums, then one kernel per frame computes the gates and one pass
+ * multiplies them in.  Nothing is allocated after create and forward never synchronises with the host.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct wvn_effnet wvn_effnet_t;
+
+typedef struct {
+  int image_size;   /* side of the square input, a multiple of 32 (e.g. 448) */
+  int max_batch;    /* largest batch a forward call may carry; the workspaces are sized for it at create */
+} wvn_effnet_config;
+
+int wvn_effnet_create(const wvn_effnet_config* cfg, wvn_effnet_t** out);
+void wvn_effnet_destroy(wvn_effnet_t* h);
+/* Bytes of activation, im2col, pool-sum and gate workspace the handle allocated at create. */
+size_t wvn_effnet_workspace_bytes(const wvn_effnet_t* h);
+/* Weights are named after torchvision's modules, batch norm folded in (as for wvn_resnet_set_weight), fp32, host or
+ * device, zero-padded to the channel pitches P(c) = round_up(c, 64):
+ *   features.0.{weight [64, 27] (out, ky, kx, in), bias [64]}                                  the stem
+ *   features.{s}.{i}.block.{j}.{weight [P(out), P(in)], bias [P(out)]}                         expand / project 1 x 1
+ *   features.{s}.{i}.block.{j}.{weight [k, k, P(c)] (channel fastest), bias [P(c)]}           depthwise k x k
+ *   features.{s}.{i}.block.{j}.fc1.{weight [sq, P(c)], bias [sq]}, .fc2.{weight [P(c), sq], bias [P(c)]}
+ *                                                                                            squeeze-excitation
+ *   features.8.{weight [1280, 320], bias [1280]}                                               the head
+ * with j counted as torchvision does (stage 1 has no expand conv: its depthwise is block.0). */
+int wvn_effnet_set_weight(wvn_effnet_t* h, const char* name, const float* data, long long numel);
+/* img: [batch, 3, image_size, image_size] fp32 in [0, 1] (ImageNet Normalize in the stem's loader).  taps: host array
+ * of five device pointers, each an NHWC bf16 map [batch, h_l, w_l, P(c_l)] (channels [c_l, P(c_l)) come out zero):
+ *   features.2.0.block.0  96 @ S/2,  features.3.0.block.0 144 @ S/4,  features.4.0.block.0 240 @ S/8,
+ *   features.6.0.block.0 672 @ S/16, features.8 1280 @ S/32. */
+int wvn_effnet_forward(wvn_effnet_t* h, const float* img, int batch, void* const* taps, void* stream);
+
+/* The EfficientNet path's primitives, exposed for testing.  NHWC bf16 maps at a channel pitch that is a multiple of 8.
+ * wvn_depthwise_silu_bf16_nhwc: out [batch, ho, wo, pitch] = bf16(SiLU(depthwise k x k conv (k 3 or 5, stride 1 or 2,
+ *   zero padding (k-1)/2) + bias)), weight [k, k, pitch] fp32, bias [pitch]; partial
+ *   [batch, wvn_depthwise_pool_blocks(ho, wo), pitch] fp32 receives the per-channel sums of the bf16-ROUNDED outputs
+ *   over consecutive blocks of 64 output pixels, each added in a fixed order (no atomics).
+ * wvn_se_gates: gates [batch, pitch] = sigmoid(fc2(SiLU(fc1(mean)))), mean = (sum of the frame's partial rows in row
+ *   order) / hw; fc1 [squeeze, pitch], fc2 [pitch, squeeze]; channels [channels, pitch) get gate 0.
+ * wvn_channel_scale_bf16_nhwc: in place x[b, p, c] = bf16(x[b, p, c] * gates[b, c]), x [batch, hw, pitch]. */
+int wvn_depthwise_silu_bf16_nhwc(const void* in, int batch, int h, int w, int pitch, int k, int stride,
+                                 const float* weight, const float* bias, void* out, float* partial, void* stream);
+int wvn_depthwise_pool_blocks(int ho, int wo);
+int wvn_se_gates(const float* partial, int batch, int nblk, int hw, int channels, int pitch, const float* fc1_w,
+                 const float* fc1_b, int squeeze, const float* fc2_w, const float* fc2_b, float* gates, void* stream);
+int wvn_channel_scale_bf16_nhwc(void* x, int batch, long long hw, int pitch, const float* gates, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Token grid -> image resolution
  * ---------------------------------------------------------------------------------------- */
 /* F.interpolate(features, (out,out), "bilinear", align_corners=True) (dino_interface.py:87-90).
@@ -340,6 +393,12 @@ int wvn_segment_reduce(const long long* seg, int batch, int h, int w, int smax, 
 int wvn_segment_pool_pyramid(const long long* seg, int batch, int h, int w, int smax, const float* centers,
                              void* const* taps, const int* tap_h, const int* tap_w, const int* tap_c, float* out,
                              void* stream);
+/* The same pooling over 1 to 5 levels whose maps are [batch, tap_h[l], tap_w[l], tap_pitch[l]] with the first tap_c[l]
+ * channels pooled (tap_pitch[l] >= tap_c[l]); out [batch, smax, sum(tap_c)].  wvn_segment_pool_pyramid is this call
+ * with four levels and tap_pitch = tap_c. */
+int wvn_segment_pool_levels(const long long* seg, int batch, int h, int w, int smax, const float* centers, int levels,
+                            void* const* taps, const int* tap_h, const int* tap_w, const int* tap_c, const int* tap_pitch,
+                            float* out, void* stream);
 /* In-place relabel of each frame to 0..S-1; scratch: [batch*num_labels] int32; counts: [batch] int32. */
 int wvn_segment_relabel(long long* seg, int batch, long long pix_per_frame, int num_labels, int* scratch, int* counts,
                         void* stream);

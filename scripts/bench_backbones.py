@@ -1,5 +1,5 @@
 """Backbone forward throughput: DINO ViT-S/8, DINOv2 ViT-S/14 / ViT-B/14 and their register variants (4 register
-tokens), and the torchvision ResNet-18 / ResNet-50 feature pyramids, at 448 x 448, B = 32 frames per call,
+tokens), and the torchvision ResNet-18 / ResNet-50 and EfficientNet-B0 feature pyramids, at 448 x 448, B = 32 frames per call,
 seeded weights.  `python scripts/bench_backbones.py [--steps 20] [--warmup 3] [--repeats 5] [--batch 32]
 [--backbones NAME ...]`.
 
@@ -14,7 +14,10 @@ patch embed 2 P (3 p^2) D; per block 2 n (3 D^2 + D^2 + 2 D M) for QKV / out-pro
 Q K^T and P V.  For a ResNet it is 2 Cout Cin k^2 Ho Wo summed over the convs up to the last tap (the whole trunk for
 both depths); the row also gives the library's workspace (activations and im2col rows) for the batch, and, in the same
 run, the frames/s of the fp32 oracle (oracle/resnet.py) run eagerly on the GPU and of the same ops in bf16,
-channels-last, with batch norm folded (cuDNN) as a baseline."""
+channels-last, with batch norm folded (cuDNN) as a baseline.  EfficientNet-B0's row is built the same way
+(oracle/efficientnet.py); its GFLOP/frame is 2 Cout (Cin / groups) k^2 Ho Wo over every conv (stem, expand, depthwise,
+project, head) plus the squeeze-excitations' two small matrix-vector products; the gate multiply and the residual adds
+are not counted."""
 import argparse
 import json
 import os
@@ -57,6 +60,19 @@ def resnet_gflop_per_frame(depth, image_size):
         out = side if (depth == 50 and conv.endswith("conv1")) else side // block_stride
         flop += 2 * cout * cin * k * k * out * out
     return flop / 1e9
+
+
+def effnet_gflop_per_frame(image_size):
+    from wild_visual_navigation_b200.feature_extractor.weights import efficientnet_b0_blocks
+
+    side = image_size // 2
+    flop = 2 * 32 * 3 * 9 * side * side  # the stem
+    for _, cin, cexp, cout, k, stride, sq in efficientnet_b0_blocks():
+        if cexp != cin:
+            flop += 2 * cexp * cin * side * side
+        side //= stride
+        flop += 2 * cexp * k * k * side * side + 2 * 2 * cexp * sq + 2 * cout * cexp * side * side
+    return (flop + 2 * 1280 * 320 * side * side) / 1e9
 
 
 def time_calls(fn, warmup, repeats, steps, batch):
@@ -152,6 +168,40 @@ def main():
                           "stem_im2col_gb": round(stem_col / 1e9, 3),
                           "oracle_fp32_eager_frames_per_s": round(fps_fp32, 1),
                           "cudnn_bf16_channels_last_frames_per_s": round(fps_cudnn, 1), **info}), flush=True)
+    if not args.backbones or "efficientnet_b0" in args.backbones:
+        from oracle import efficientnet as E
+        from wild_visual_navigation_b200.feature_extractor import TorchVisionInterface
+        from wild_visual_navigation_b200.feature_extractor.weights import (fold_efficientnet_bn,
+                                                                           synthetic_efficientnet_b0_state_dict)
+
+        sd = synthetic_efficientnet_b0_state_dict()
+        ti = TorchVisionInterface("cuda", "efficientnet_b0", S, state_dict=sd, max_batch=B)
+        fps, rates = time_calls(lambda: ti.inference_taps(img), args.warmup, args.repeats, args.steps, B)
+        gf = effnet_gflop_per_frame(S)
+        ws = ti._model.workspace_bytes
+        del ti
+        torch.cuda.empty_cache()
+        torch.backends.cudnn.allow_tf32 = False
+        torch.backends.cuda.matmul.allow_tf32 = False
+        sdc = {k: v.cuda() for k, v in sd.items()}
+        with torch.no_grad():
+            fps_fp32, _ = time_calls(lambda: E.efficientnet_pyramid(img, sdc), 1, 3, max(1, args.steps // 4), B)
+            folded = {}
+            for m, (w, b) in fold_efficientnet_bn(sd).items():
+                w = w.cuda().bfloat16()
+                folded[m + ".weight"] = w.to(memory_format=torch.channels_last) if w.dim() == 4 else w
+                folded[m + ".bias"] = b.cuda().bfloat16()
+            img16 = img.bfloat16().to(memory_format=torch.channels_last)
+            fps_cudnn, _ = time_calls(lambda: E.efficientnet_pyramid(img16, folded, folded=True), args.warmup,
+                                      args.repeats, args.steps, B)
+        del sdc, folded
+        torch.cuda.empty_cache()
+        print(json.dumps({"backbone": "efficientnet_b0", "image_size": S, "batch": B, "frames_per_s": round(fps, 1),
+                          "frames_per_s_runs": [round(r, 1) for r in rates], "gflop_per_frame": round(gf, 2),
+                          "tflop_per_s": round(fps * gf / 1e3, 1), "workspace_gb": round(ws / 1e9, 3),
+                          "oracle_fp32_eager_frames_per_s": round(fps_fp32, 1),
+                          "cudnn_bf16_channels_last_frames_per_s": round(fps_cudnn, 1), **info}), flush=True)
+
 
 if __name__ == "__main__":
     main()

@@ -45,6 +45,10 @@ class ResnetConfig(Structure):
     _fields_ = [("image_size", c_int), ("depth", c_int), ("max_batch", c_int)]
 
 
+class EffnetConfig(Structure):
+    _fields_ = [("image_size", c_int), ("max_batch", c_int)]
+
+
 class TrainConfig(Structure):
     _fields_ = [
         ("w_trav", c_float), ("w_reco", c_float), ("std_factor", c_float), ("anomaly_balanced", c_int),
@@ -90,6 +94,16 @@ SIGNATURES = {
     "wvn_im2col_image": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
     "wvn_maxpool3s2_bf16_nhwc": (_I, [_P, _I, _I, _I, _I, _P, _P]),
     "wvn_segment_pool_pyramid": (_I, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "wvn_segment_pool_levels": (_I, [_P, _I, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "wvn_effnet_create": (_I, [POINTER(EffnetConfig), POINTER(_P)]),
+    "wvn_effnet_destroy": (None, [_P]),
+    "wvn_effnet_workspace_bytes": (_S, [_P]),
+    "wvn_effnet_set_weight": (_I, [_P, c_char_p, _P, _L]),
+    "wvn_effnet_forward": (_I, [_P, _P, _I, _P, _P]),
+    "wvn_depthwise_silu_bf16_nhwc": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "wvn_depthwise_pool_blocks": (_I, [_I, _I]),
+    "wvn_se_gates": (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P]),
+    "wvn_channel_scale_bf16_nhwc": (_I, [_P, _I, _L, _I, _P, _P]),
     "wvn_upsample_dense": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "wvn_logits_argmax": (_I, [_P, _L, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "wvn_flip_average": (_I, [_P, _I, _I, _I, _L, _P]),

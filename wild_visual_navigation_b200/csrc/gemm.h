@@ -17,7 +17,7 @@ enum GemmEpilogue : int {
   EPI_BF16_RESID = 6, // out(bf16)[row, col]  = act(acc + bias + residual(bf16)[row, col])  (a residual block's last conv)
 };
 
-enum GemmAct : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2 };
+enum GemmAct : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SILU = 3 /* EPI_BF16 only */ };
 
 struct GemmArgs {
   int M = 0, N = 0, K = 0;

@@ -113,17 +113,17 @@ segment_pool_pyramid_kernel(const long long* __restrict__ seg, const float* __re
   const int s = blockIdx.x, b = blockIdx.y;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int D = 0;
-  for (int l = 0; l < 4; ++l) D += a.tc[l];
+  for (int l = 0; l < a.levels; ++l) D += a.tc[l];
   float* orow = out + (static_cast<long long>(b) * a.smax + s) * D;
   const long long* segb = seg + static_cast<long long>(b) * a.h * a.w;
   const float cx = centers[(static_cast<long long>(b) * a.smax + s) * 2 + 0];
   const float cy = centers[(static_cast<long long>(b) * a.smax + s) * 2 + 1];
   int off = 0;
-  for (int l = 0; l < 4; ++l) {
-    const int th = a.th[l], tw = a.tw[l], C = a.tc[l];
+  for (int l = 0; l < a.levels; ++l) {
+    const int th = a.th[l], tw = a.tw[l], C = a.tc[l], P = a.tp[l];
     const int sy = a.h / th, sx = a.w / tw;  // seg_l[i, j] = seg[i * H / h_l, j * W / w_l]
     const int cells = th * tw;
-    const __nv_bfloat16* map = reinterpret_cast<const __nv_bfloat16*>(a.taps[l]) + static_cast<long long>(b) * cells * C;
+    const __nv_bfloat16* map = reinterpret_cast<const __nv_bfloat16*>(a.taps[l]) + static_cast<long long>(b) * cells * P;
     float acc[kPoolMaxChannelsPerThread];
 #pragma unroll
     for (int j = 0; j < kPoolMaxChannelsPerThread; ++j) acc[j] = 0.f;
@@ -147,7 +147,7 @@ segment_pool_pyramid_kernel(const long long* __restrict__ seg, const float* __re
       if (m) list[pos + __popc(bal & ((1u << lane) - 1u))] = cell;
       __syncthreads();
       for (int q = 0; q < n; ++q) {
-        const __nv_bfloat16* src = map + static_cast<long long>(list[q]) * C;
+        const __nv_bfloat16* src = map + static_cast<long long>(list[q]) * P;
 #pragma unroll
         for (int j = 0; j < kPoolMaxChannelsPerThread; ++j) {
           const int c = tid + j * kPoolThreads;
@@ -170,7 +170,7 @@ segment_pool_pyramid_kernel(const long long* __restrict__ seg, const float* __re
       const bool empty = !(cx == cx) || !(cy == cy);
       const int i = empty ? 0 : min(max(static_cast<int>(floorf(cy / static_cast<float>(sy))), 0), th - 1);
       const int j = empty ? 0 : min(max(static_cast<int>(floorf(cx / static_cast<float>(sx))), 0), tw - 1);
-      const __nv_bfloat16* src = map + (static_cast<long long>(i) * tw + j) * C;
+      const __nv_bfloat16* src = map + (static_cast<long long>(i) * tw + j) * P;
       for (int c = tid; c < C; c += kPoolThreads) orow[off + c] = empty ? __int_as_float(0x7fc00000) : __bfloat162float(src[c]);
     }
     off += C;
@@ -224,13 +224,16 @@ int segment_pool_pyramid(const long long* seg, const float* centers, const Pyram
   WVN_REQUIRE(seg && centers && out && a.batch > 0 && a.h > 0 && a.w > 0 && a.smax > 0,
               "segment_pool_pyramid: bad arguments (batch=%d h=%d w=%d smax=%d)", a.batch, a.h, a.w, a.smax);
   WVN_REQUIRE(a.batch <= 65535, "segment_pool_pyramid: batch %d", a.batch);
-  for (int l = 0; l < 4; ++l) {
+  WVN_REQUIRE(a.levels >= 1 && a.levels <= kPyramidMaxLevels, "segment_pool_pyramid: %d levels (1 .. %d)", a.levels,
+              kPyramidMaxLevels);
+  for (int l = 0; l < a.levels; ++l) {
     WVN_REQUIRE(a.taps[l] && a.th[l] > 0 && a.tw[l] > 0 && a.h % a.th[l] == 0 && a.w % a.tw[l] == 0,
                 "segment_pool_pyramid: level %d is %dx%d, which must divide the %dx%d segmentation", l, a.th[l], a.tw[l],
                 a.h, a.w);
     WVN_REQUIRE(a.tc[l] > 0 && a.tc[l] <= kPoolThreads * kPoolMaxChannelsPerThread,
                 "segment_pool_pyramid: level %d has %d channels (1 .. %d)", l, a.tc[l],
                 kPoolThreads * kPoolMaxChannelsPerThread);
+    WVN_REQUIRE(a.tp[l] >= a.tc[l], "segment_pool_pyramid: level %d has pitch %d < %d channels", l, a.tp[l], a.tc[l]);
   }
   segment_pool_pyramid_kernel<<<dim3(a.smax, a.batch), kPoolThreads, 0, stream>>>(seg, centers, a, out);
   WVN_CHECK_LAUNCH("segment_pool_pyramid_kernel");

@@ -17,10 +17,13 @@ int im2col_image(const float* img, int batch, int h, int w, int k, int stride, i
 // 3 x 3 / stride 2 / pad 1 max-pool of an NHWC bf16 map [batch, h, w, c] (c % 8 == 0); padding is -inf.
 int maxpool3s2_nhwc(const void* in, int batch, int h, int w, int c, void* out, cudaStream_t stream);
 
+constexpr int kPyramidMaxLevels = 5;
+
 struct PyramidArgs {
   int batch = 0, h = 0, w = 0, smax = 0;
-  const void* taps[4] = {};     // NHWC bf16 [batch, th, tw, tc]
-  int th[4] = {}, tw[4] = {}, tc[4] = {};
+  int levels = 0;                             // 1 .. kPyramidMaxLevels
+  const void* taps[kPyramidMaxLevels] = {};  // NHWC bf16 [batch, th, tw, tp]; channels [tc, tp) are not read
+  int th[kPyramidMaxLevels] = {}, tw[kPyramidMaxLevels] = {}, tc[kPyramidMaxLevels] = {}, tp[kPyramidMaxLevels] = {};
 };
 // out [batch, smax, sum(tc)] fp32: per segment, the mean of each level's cells whose nearest-downsampled id is the
 // segment, levels concatenated; a segment without a cell at a level takes the cell under its full-resolution centroid

@@ -9,8 +9,9 @@
   * when segmentation and features are both "stego"/"dino" on the same backbone, one ViT forward
     serves both (the reference runs two backbones); with "dinov2" / "dinov2_reg" features, STEGO's DINO backbone
     segments and a second, DINOv2 handle gives the features;
-  * "torchvision" features (``model_type`` resnet18 / resnet50 / resnet50_dino) are a feature pyramid pooled per
-    segment level by level (csrc/resnet_kernels.cu), as sparsify_features' dict branch does.  Where a segment has no
+  * "torchvision" features (``model_type`` resnet18 / resnet50 / resnet50_dino / efficientnet_b0) are a feature
+    pyramid (four levels, five for EfficientNet-B0) pooled per segment level by level (csrc/resnet_kernels.cu), as
+    sparsify_features' dict branch does.  Where a segment has no
     cell at a coarse level the reference raises AttributeError; here it takes the cell under its centroid.  "random" and
     "none" segmentation crash in the reference with a pyramid and raise ValueError here.
 Supported: segmentation_type in {"slic" (the constructor default), "stego", "grid", "random", "none"/None},
@@ -26,7 +27,7 @@ from .. import ops
 from .dino_interface import DinoInterface
 from .segment_extractor import SegmentExtractor
 from .stego_interface import StegoInterface
-from .torchvision_interface import PYRAMID_KEYS, TorchVisionInterface
+from .torchvision_interface import MODEL_TYPES, TorchVisionInterface
 
 
 class FeatureExtractor:
@@ -53,7 +54,7 @@ class FeatureExtractor:
                 # the reference indexes / returns the pyramid dict as a tensor there and crashes
                 raise ValueError(f"segmentation_type [{segmentation_type}] does not work with torchvision features")
             if "model_type" not in kwargs:
-                raise ValueError("feature_type 'torchvision' needs model_type (resnet18, resnet50, resnet50_dino)")
+                raise ValueError(f"feature_type 'torchvision' needs model_type ({', '.join(MODEL_TYPES)})")
         elif "dino" in feature_type:
             # the reference hard-codes 384 for every dino variant (feature_extractor.py:56)
             self._feature_dim = 384 if common["backbone_type"] == "vit_small" else 768
@@ -78,7 +79,7 @@ class FeatureExtractor:
             # with segmentation_type="stego", STEGO segments on its own DINO backbone (`stego_state_dict`)
             self._dino = None
             self._tv = TorchVisionInterface(device, kwargs["model_type"], input_size, max_batch=common["max_batch"],
-                                            state_dict=kwargs.get("state_dict"),
+                                            pretrained=kwargs.get("pretrained", True), state_dict=kwargs.get("state_dict"),
                                             pretrained_weights=kwargs.get("pretrained_weights"))
             self._extractor = self._tv
             # the reference never sets it for torchvision (reading it raises); the pooled row width
@@ -219,7 +220,7 @@ class FeatureExtractor:
             out = {"seg": seg, "feat": feat, "centers": r["centers"], "edges": r["edges"], "n_edges": r["n_edges"],
                    "n_segments": counts, "tokens": None, "dense": None}
             if kwargs.get("return_dense_features", False):
-                out["dense"] = {k: t.permute(0, 3, 1, 2).float().contiguous() for k, t in zip(PYRAMID_KEYS, taps)}
+                out["dense"] = self._tv.dense(taps)
             return out
         if tokens is None:
             if self._feature_type == "stego":

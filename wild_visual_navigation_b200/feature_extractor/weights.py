@@ -12,6 +12,8 @@ LayerScale gammas ``blocks.N.ls{1,2}.gamma`` and an unused ``mask_token``; DINOv
 (``backbone="dinov2_reg"``, ``dinov2_vit{s,b}14_reg4_pretrain.pth``) adds ``register_tokens`` (1, R, D).
 The torchvision ResNets (``TorchVisionInterface``) take torchvision-layout state dicts (``resnet18`` / ``resnet50``
 ImageNet checkpoints, or DINO's ``dino_resnet50_pretrain.pth`` for ``resnet50_dino``); ``fc.*`` is not needed.
+EfficientNet-B0 (``efficientnet_b0``) takes torchvision-layout ``efficientnet_b0`` state dicts; ``classifier.*`` is not
+needed.
 """
 from __future__ import annotations
 
@@ -331,4 +333,186 @@ def fold_resnet_bn(sd: dict, depth: int) -> dict:
         gamma, beta, mean, var = (sd[bn + "." + k].to(dt) for k in ("weight", "bias", "running_mean", "running_var"))
         scale = gamma / torch.sqrt(var + RESNET_BN_EPS)
         out[conv.replace("downsample.0", "downsample")] = (w.to(dt) * scale[:, None, None, None], beta - mean * scale)
+    return out
+
+
+# --------------------------------------------------------------------------------------------
+# torchvision EfficientNet-B0
+# --------------------------------------------------------------------------------------------
+EFFNET_MODELS = ("efficientnet_b0",)
+# (expand ratio, kernel, stride, output channels, blocks) of the seven stages
+EFFNET_B0_STAGES = ((1, 3, 1, 16, 1), (6, 3, 2, 24, 2), (6, 5, 2, 40, 2), (6, 3, 2, 80, 3), (6, 5, 1, 112, 3),
+                    (6, 5, 2, 192, 4), (6, 3, 1, 320, 1))
+EFFNET_BN_EPS = 1e-5
+EFFNET_RESIDUAL_GAMMA = 0.2
+
+
+def efficientnet_b0_blocks():
+    """(prefix, in, expanded, out, kernel, stride, squeeze) of every MBConv block, prefix ``features.{s}.{i}.block.``."""
+    blocks, cin = [], 32
+    for s, (ratio, k, stride, cout, n) in enumerate(EFFNET_B0_STAGES, start=1):
+        for i in range(n):
+            blocks.append((f"features.{s}.{i}.block.", cin, cin * ratio, cout, k, stride if i == 0 else 1,
+                           max(1, cin // 4)))
+            cin = cout
+    return blocks
+
+
+def efficientnet_b0_layers():
+    """Every parameterised layer of the B0 trunk in forward order: ("conv", module, out, in per group, kernel) for a
+    conv + batch norm pair (conv ``{module}.0``, batch norm ``{module}.1``; depthwise convs have 1 input per group) and
+    ("se", module, expanded, squeeze) for a squeeze-excitation (``{module}.fc1``, ``{module}.fc2``)."""
+    layers = [("conv", "features.0", 32, 3, 3)]
+    for p, cin, cexp, cout, k, _, sq in efficientnet_b0_blocks():
+        j = 0
+        if cexp != cin:
+            layers.append(("conv", p + "0", cexp, cin, 1))
+            j = 1
+        layers += [("conv", p + str(j), cexp, 1, k), ("se", p + str(j + 1), cexp, sq),
+                   ("conv", p + str(j + 2), cout, cexp, 1)]
+    layers.append(("conv", "features.8", 1280, 320, 1))
+    return layers
+
+
+def _effnet_forward(sd: dict, x: torch.Tensor, calibrate: bool):
+    """The B0 trunk on a normalised image in eval-mode batch norm, or with ``calibrate`` in training-mode batch norm,
+    each batch norm's batch statistics stored as its running statistics (the layers before it already calibrated)."""
+    import torch.nn.functional as F
+
+    def cbn(x, m, stride=1, groups=1, act=True):
+        w = sd[m + ".0.weight"]
+        x = F.conv2d(x, w, stride=stride, padding=(w.shape[-1] - 1) // 2, groups=groups)
+        bn = m + ".1."
+        if calibrate:
+            sd[bn + "running_mean"], sd[bn + "running_var"] = x.mean((0, 2, 3)), x.var((0, 2, 3), unbiased=False)
+        x = F.batch_norm(x, sd[bn + "running_mean"], sd[bn + "running_var"], sd[bn + "weight"], sd[bn + "bias"], False,
+                         0.0, EFFNET_BN_EPS)
+        return F.silu(x) if act else x
+
+    x = cbn(x, "features.0", stride=2)
+    for p, cin, cexp, cout, k, stride, _ in efficientnet_b0_blocks():
+        j = 0
+        y = x
+        if cexp != cin:
+            y = cbn(y, p + "0")
+            j = 1
+        y = cbn(y, p + str(j), stride=stride, groups=cexp)
+        se = p + str(j + 1)
+        g = F.silu(F.conv2d(y.mean((2, 3), keepdim=True), sd[se + ".fc1.weight"], sd[se + ".fc1.bias"]))
+        y = y * torch.sigmoid(F.conv2d(g, sd[se + ".fc2.weight"], sd[se + ".fc2.bias"]))
+        y = cbn(y, p + str(j + 2), act=False)
+        x = x + y if stride == 1 and cin == cout else y
+    return cbn(x, "features.8")
+
+
+def synthetic_efficientnet_b0_state_dict(seed: int = 1):
+    """Seeded torchvision-layout EfficientNet-B0 weights (no ``classifier``).  Convs are Kaiming-normal (fan_out, as
+    torchvision initialises them), batch-norm affine parameters are drawn around (1, 0) (around (0.2, 0) for the
+    project conv of a residual block, so that each such block adds a correction to its input, see
+    RESNET_RESIDUAL_GAMMA), the squeeze-excitation's biases around 0, and the running statistics are calibrated on four
+    seeded 128 x 128 images, so that every tap keeps an RMS of order 1 through the 16 blocks."""
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    residual = {p + str(2 if cexp == cin else 3) for p, cin, cexp, cout, _, stride, _ in efficientnet_b0_blocks()
+                if stride == 1 and cin == cout}
+    with torch.no_grad():
+        for kind, m, cout, cin, *rest in efficientnet_b0_layers():
+            if kind == "se":
+                sq = cin
+                sd[m + ".fc1.weight"] = torch.randn(sq, cout, 1, 1, generator=g) * math.sqrt(2.0 / sq)
+                sd[m + ".fc1.bias"] = 0.2 * torch.randn(sq, generator=g)
+                sd[m + ".fc2.weight"] = torch.randn(cout, sq, 1, 1, generator=g) * math.sqrt(2.0 / cout)
+                sd[m + ".fc2.bias"] = 0.2 * torch.randn(cout, generator=g)
+                continue
+            k = rest[0]
+            fan_out = cout * k * k if cin > 1 or m == "features.0" else k * k
+            sd[m + ".0.weight"] = torch.randn(cout, cin, k, k, generator=g) * math.sqrt(2.0 / fan_out)
+            gamma = EFFNET_RESIDUAL_GAMMA if m in residual else 1.0
+            sd[m + ".1.weight"] = gamma * (1.0 + 0.2 * torch.randn(cout, generator=g))
+            sd[m + ".1.bias"] = 0.2 * torch.randn(cout, generator=g)
+            sd[m + ".1.running_mean"] = torch.zeros(cout)
+            sd[m + ".1.running_var"] = torch.ones(cout)
+            sd[m + ".1.num_batches_tracked"] = torch.tensor(0)
+        img = torch.rand(4, 3, 128, 128, generator=g)
+        x = (img - torch.tensor([0.485, 0.456, 0.406])[:, None, None]) / torch.tensor([0.229, 0.224, 0.225])[:, None, None]
+        _effnet_forward(sd, x, calibrate=True)
+    return sd
+
+
+def _effnet_param_shapes():
+    shapes = {}
+    for kind, m, cout, cin, *rest in efficientnet_b0_layers():
+        if kind == "se":
+            sq = cin
+            shapes.update({m + ".fc1.weight": (sq, cout, 1, 1), m + ".fc1.bias": (sq,), m + ".fc2.weight": (cout, sq, 1, 1),
+                           m + ".fc2.bias": (cout,)})
+        else:
+            shapes[m + ".0.weight"] = (cout, cin, rest[0], rest[0])
+            shapes.update({m + ".1." + leaf: (cout,) for leaf in ("weight", "bias", "running_mean", "running_var")})
+    return shapes
+
+
+def check_efficientnet_family(sd: dict, model_type: str) -> dict:
+    """Checks that a torchvision-layout state dict is an EfficientNet-B0 and returns the trunk's tensors
+    (``classifier.*`` and ``num_batches_tracked`` are dropped).  Raises ValueError naming what it got instead."""
+    if model_type not in EFFNET_MODELS:
+        raise ValueError(f"model_type '{model_type}' is not supported (efficientnet_b0)")
+    sd = {k.replace("module.", ""): v for k, v in sd.items()}
+    shapes = _effnet_param_shapes()
+    missing = [k for k in shapes if k not in sd]
+    bad = [f"{k} {tuple(sd[k].shape)} != {shapes[k]}" for k in shapes if k in sd and tuple(sd[k].shape) != shapes[k]]
+    if missing or bad:
+        if "conv1.weight" in sd and "features.0.0.weight" not in sd:
+            got = "a ResNet state dict"
+        elif "features.0.0.weight" in sd and tuple(sd["features.0.0.weight"].shape) != shapes["features.0.0.weight"]:
+            stem = sd["features.0.0.weight"].shape[0]
+            got = {48: "an EfficientNet-B4 state dict", 64: "an EfficientNet-B7 state dict"}.get(
+                stem, f"an EfficientNet with a {stem}-channel stem")
+        else:
+            got = "another"
+        detail = "; ".join((bad + [f"missing {m}" for m in missing])[:3])
+        raise ValueError(f"model_type '{model_type}' needs a torchvision EfficientNet-B0 state dict; got {got} ({detail})")
+    return {k: sd[k] for k in shapes}
+
+
+def load_efficientnet_state_dict(model_type: str, pretrained_weights=None, pretrained: bool = True, seed: int = 1):
+    """EfficientNet-B0 weights from ``pretrained_weights`` / ``$WVN_EFFICIENTNET_WEIGHTS`` (a torchvision
+    ``efficientnet_b0`` checkpoint, checked by check_efficientnet_family).  Without a checkpoint, ``pretrained=False``
+    gives seeded weights (synthetic_efficientnet_b0_state_dict, with a warning), as torchvision's ``pretrained=False``
+    gives random ones; ``pretrained=True`` asks for torchvision's ImageNet weights, which are only ever read from a
+    checkpoint here, so it raises ValueError instead of quietly running random weights."""
+    if model_type not in EFFNET_MODELS:
+        raise ValueError(f"model_type '{model_type}' is not supported (efficientnet_b0)")
+    path = pretrained_weights or os.environ.get("WVN_EFFICIENTNET_WEIGHTS")
+    if path:
+        sd = torch.load(path, map_location="cpu", weights_only=False)
+        if "state_dict" in sd:
+            sd = sd["state_dict"]
+        return check_efficientnet_family(sd, model_type)
+    if pretrained:
+        raise ValueError(f"model_type '{model_type}' with pretrained=True needs torchvision's ImageNet checkpoint "
+                         f"(state_dict, pretrained_weights or $WVN_EFFICIENTNET_WEIGHTS): downloading it is outside the "
+                         f"H100 hot path; pass pretrained=False for seeded weights")
+    warnings.warn(f"no {model_type} checkpoint given and pretrained=False: using seeded random weights with calibrated "
+                  f"batch-norm statistics — fine for parity and throughput work, not for real traversability")
+    return synthetic_efficientnet_b0_state_dict(seed)
+
+
+def fold_efficientnet_bn(sd: dict) -> dict:
+    """Eval-mode batch norm folded into the conv before it, in at least fp32 (fp64 stays fp64), as fold_resnet_bn.
+    Returns {module: (w', b')} for every conv + batch norm pair (stem ``features.0``, head ``features.8``) and
+    {``{module}.fc1`` / ``{module}.fc2``: (w [out, in], b)} for the squeeze-excitations."""
+    out = {}
+    for kind, m, *_ in efficientnet_b0_layers():
+        if kind == "se":
+            for fc in ("fc1", "fc2"):
+                w = sd[f"{m}.{fc}.weight"]
+                dt = torch.promote_types(w.dtype, torch.float32)
+                out[f"{m}.{fc}"] = (w.to(dt)[:, :, 0, 0], sd[f"{m}.{fc}.bias"].to(dt))
+            continue
+        w = sd[m + ".0.weight"]
+        dt = torch.promote_types(w.dtype, torch.float32)
+        gamma, beta, mean, var = (sd[m + ".1." + k].to(dt) for k in ("weight", "bias", "running_mean", "running_var"))
+        scale = gamma / torch.sqrt(var + EFFNET_BN_EPS)
+        out[m] = (w.to(dt) * scale[:, None, None, None], beta - mean * scale)
     return out

@@ -14,10 +14,10 @@ import torch
 import torch.nn.functional as F
 
 from . import _C
-from ._C import FlowBuffers, ResnetConfig, TrainConfig, VitConfig, check, lib, ptr, stream
+from ._C import EffnetConfig, FlowBuffers, ResnetConfig, TrainConfig, VitConfig, check, lib, ptr, stream
 
 OUT_BF16, OUT_F32, OUT_RESID_F32 = 0, 1, 2
-ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
+ACT_NONE, ACT_RELU, ACT_GELU, ACT_SILU = 0, 1, 2, 3
 
 
 # --------------------------------------------------------------------------------------------
@@ -418,16 +418,22 @@ def maxpool3s2_nhwc(x):
 
 
 def segment_pool_pyramid(seg, smax, taps, centers):
-    """Multiscale segment pooling (sparsify_features' pyramid branch).  seg [B,H,W] int64, taps: four NHWC bf16 maps
-    [B,h_l,w_l,c_l], centers [B,smax,2] fp32 (col, row) -> feat [B,smax,sum c_l] fp32 (see include/wvn_b200.h)."""
+    """Multiscale segment pooling (sparsify_features' pyramid branch).  seg [B,H,W] int64, taps: one to five NHWC bf16
+    maps [B,h_l,w_l,c_l], each dense or the first c_l channels of a dense [B,h_l,w_l,pitch_l] map, centers [B,smax,2]
+    fp32 (col, row) -> feat [B,smax,sum c_l] fp32 (see include/wvn_b200.h, wvn_segment_pool_levels)."""
     B, H, W = seg.shape
-    taps = [t.contiguous() for t in taps]
     D = sum(t.shape[3] for t in taps)
     out = torch.empty(B, smax, D, device=seg.device, dtype=torch.float32)
-    ints = ctypes.c_int * 4
+    pitch = []
+    for t in taps:
+        p = t.stride(2)
+        assert t.is_cuda and t.dtype == torch.bfloat16 and t.stride(3) == 1 and p >= t.shape[3] and \
+            t.stride(1) == t.shape[2] * p and t.stride(0) == t.shape[1] * t.stride(1), "tap must be a dense NHWC map's prefix"
+        pitch.append(p)
+    ints = ctypes.c_int * len(taps)
     th, tw, tc = ints(*[t.shape[1] for t in taps]), ints(*[t.shape[2] for t in taps]), ints(*[t.shape[3] for t in taps])
-    check(lib().wvn_segment_pool_pyramid(ptr(seg.contiguous()), B, H, W, smax, ptr(centers.contiguous()),
-                                         _ptr_array(taps), th, tw, tc, ptr(out), stream()))
+    check(lib().wvn_segment_pool_levels(ptr(seg.contiguous()), B, H, W, smax, ptr(centers.contiguous()), len(taps),
+                                        _ptr_array(taps), th, tw, tc, ints(*pitch), ptr(out), stream()))
     return out
 
 
@@ -1268,3 +1274,108 @@ class FlowTrainer(_TrainerHandle):
                                         ptr(self.cg_mean), ptr(self.cg_std), ptr(self.conf), ptr(self.metrics),
                                         int(phase_mask), stream()))
         return self.conf[:R]
+
+
+# --------------------------------------------------------------------------------------------
+# EfficientNet-B0 backbone handle and its primitives
+# --------------------------------------------------------------------------------------------
+# (channels, stride) of the five taps: features.{2,3,4,6}.0.block.0 (expand convs) and features.8 (the head)
+EFFNET_B0_TAPS = ((96, 2), (144, 4), (240, 8), (672, 16), (1280, 32))
+
+
+def channel_pitch(c):
+    """Channel pitch of the EfficientNet path's NHWC maps: c rounded up to 64, the GEMM's narrowest tile."""
+    return (c + 63) // 64 * 64
+
+
+def depthwise_silu(x, weight, bias, stride, out=None, partial=None):
+    """x [B,H,W,P] bf16 NHWC (P % 8 == 0), weight [k,k,P] fp32, bias [P] fp32 -> (out [B,Ho,Wo,P] bf16 =
+    bf16(SiLU(depthwise conv + bias)), partial [B, nblk, P] fp32 pool sums of the rounded outputs)."""
+    B, H, W, P = x.shape
+    k = weight.shape[0]
+    pad = (k - 1) // 2
+    Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
+    if out is None:
+        out = torch.empty(B, Ho, Wo, P, device=x.device, dtype=torch.bfloat16)
+    if partial is None:
+        partial = torch.empty(B, lib().wvn_depthwise_pool_blocks(Ho, Wo), P, device=x.device, dtype=torch.float32)
+    check(lib().wvn_depthwise_silu_bf16_nhwc(ptr(x.contiguous()), B, H, W, P, k, stride, ptr(weight.contiguous()),
+                                             ptr(bias.contiguous()), ptr(out), ptr(partial), stream()))
+    return out, partial
+
+
+def se_gates(partial, hw, channels, fc1_w, fc1_b, fc2_w, fc2_b):
+    """partial [B, nblk, P] (depthwise_silu's) -> gates [B, P] fp32 = sigmoid(fc2(SiLU(fc1(sum / hw)))), 0 past
+    ``channels``; fc1_w [sq, P], fc2_w [P, sq]."""
+    B, nblk, P = partial.shape
+    gates = torch.empty(B, P, device=partial.device, dtype=torch.float32)
+    check(lib().wvn_se_gates(ptr(partial.contiguous()), B, nblk, hw, channels, P, ptr(fc1_w.contiguous()),
+                             ptr(fc1_b.contiguous()), fc1_w.shape[0], ptr(fc2_w.contiguous()), ptr(fc2_b.contiguous()),
+                             ptr(gates), stream()))
+    return gates
+
+
+def channel_scale(x, gates):
+    """In place: x [B,H,W,P] bf16 *= gates [B,P] per channel, rounded to bf16."""
+    B, H, W, P = x.shape
+    assert x.is_contiguous()
+    check(lib().wvn_channel_scale_bf16_nhwc(ptr(x), B, H * W, P, ptr(gates.contiguous()), stream()))
+    return x
+
+
+def _pad_to(t, shape):
+    out = torch.zeros(shape, dtype=torch.float32)
+    out[tuple(slice(0, n) for n in t.shape)] = t
+    return out
+
+
+class EfficientNetBackbone:
+    """Owns a ``wvn_effnet_t``: a torchvision EfficientNet-B0 trunk with batch norm folded in (GEMM weights bf16,
+    depthwise and squeeze-excitation weights fp32, on device) and workspaces sized for ``max_batch``.  ``folded`` is
+    weights.fold_efficientnet_bn's dict; this class zero-pads each tensor to the handle's channel pitches."""
+
+    def __init__(self, image_size, folded, max_batch=32):
+        _C.require_device()
+        self.image_size, self.max_batch = image_size, max_batch
+        h = c_void_p()
+        check(lib().wvn_effnet_create(byref(EffnetConfig(image_size, max_batch)), byref(h)))
+        self._h = h
+        self.workspace_bytes = lib().wvn_effnet_workspace_bytes(h)
+        # (channels, side, pitch) of each tap
+        self.taps = [(c, image_size // s, channel_pitch(c)) for c, s in EFFNET_B0_TAPS]
+        for name, (w, b) in folded.items():
+            w = w.detach().to(dtype=torch.float32, device="cpu")
+            b = b.detach().to(dtype=torch.float32, device="cpu")
+            if name.endswith(".fc1"):
+                w = _pad_to(w, (w.shape[0], channel_pitch(w.shape[1])))
+            elif name.endswith(".fc2"):
+                w, b = _pad_to(w, (channel_pitch(w.shape[0]), w.shape[1])), _pad_to(b, (channel_pitch(b.shape[0]),))
+            elif w.shape[1] == 1 and w.shape[2] > 1:  # depthwise [c, 1, k, k] -> [k, k, P(c)]
+                w = _pad_to(w[:, 0].permute(1, 2, 0), (w.shape[2], w.shape[3], channel_pitch(w.shape[0])))
+                b = _pad_to(b, (channel_pitch(b.shape[0]),))
+            elif name == "features.0":  # the stem: [out, (ky, kx, in)], rows padded
+                w = _pad_to(w.permute(0, 2, 3, 1).reshape(w.shape[0], -1), (channel_pitch(w.shape[0]), 27))
+                b = _pad_to(b, (channel_pitch(b.shape[0]),))
+            else:  # 1 x 1 conv [out, in, 1, 1] -> [P(out), P(in)]
+                w = _pad_to(w[:, :, 0, 0], (channel_pitch(w.shape[0]), channel_pitch(w.shape[1])))
+                b = _pad_to(b, (channel_pitch(b.shape[0]),))
+            w, b = w.contiguous(), b.contiguous()
+            check(lib().wvn_effnet_set_weight(h, (name + ".weight").encode(), c_void_p(w.data_ptr()), w.numel()))
+            check(lib().wvn_effnet_set_weight(h, (name + ".bias").encode(), c_void_p(b.data_ptr()), b.numel()))
+
+    def forward(self, img: torch.Tensor):
+        """img (B,3,S,S) fp32 CUDA in [0,1] -> the five taps, NHWC bf16 [B, S/s_l, S/s_l, c_l]: views of the first c_l
+        channels of maps at the handle's channel pitch (whose pad channels are zero)."""
+        B = img.shape[0]
+        assert img.dtype == torch.float32 and tuple(img.shape[1:]) == (3, self.image_size, self.image_size)
+        bufs = [torch.empty(B, n, n, p, device=img.device, dtype=torch.bfloat16) for _, n, p in self.taps]
+        check(lib().wvn_effnet_forward(self._h, ptr(img.contiguous()), B, _ptr_array(bufs), stream()))
+        return [t[..., :c] for t, (c, _, _) in zip(bufs, self.taps)]
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().wvn_effnet_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
