@@ -61,7 +61,8 @@ int wvn_check_device(void);
  * each learner's own; wvn_flow_create is renamed wvn_flow_trainer_create and wvn_double_mlp_train_step is removed (its
  * padded form with one group is the same step).  A learner's entry point refuses another learner's handle.
  * Later additions under 108 add symbols only: the dense CRF (wvn_crf_*), the EfficientNet-B0 handle (wvn_effnet_*)
- * with its primitives, GEMM activation 3 (SiLU) and wvn_segment_pool_levels. */
+ * with its primitives, GEMM activation 3 (SiLU), wvn_segment_pool_levels, and the segment-wise inference entries
+ * wvn_segment_maps, wvn_mlp_infer_rows_padded and wvn_flow_infer_rows_padded. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -399,6 +400,13 @@ int wvn_segment_pool_pyramid(const long long* seg, int batch, int h, int w, int 
 int wvn_segment_pool_levels(const long long* seg, int batch, int h, int w, int smax, const float* centers, int levels,
                             void* const* taps, const int* tap_h, const int* tap_w, const int* tap_c, const int* tap_pitch,
                             float* out, void* stream);
+/* Segment-wise maps — replaces the per-pixel lookup of the node's segment-wise mode
+ * (wvn_feature_extractor_node.py:323-338, prediction_per_pixel False): map[b, p] = v[b, seg[b, p]] for every frame at once.
+ * seg: [batch, hw] int64 (seg_is_int64 != 0) or int32; trav / conf: [batch, smax] fp32 per-segment values (conf may be
+ * NULL); n_rows: [batch] int32 on the device.  trav_map / conf_map: [batch, hw] fp32 (conf_map NULL when conf is).  A
+ * pixel whose id is outside [0, min(n_rows[b], smax)) gets NaN; no padding row is read. */
+int wvn_segment_maps(const void* seg, int seg_is_int64, int batch, long long hw, const float* trav, const float* conf,
+                     int smax, const int* n_rows, float* trav_map, float* conf_map, void* stream);
 /* In-place relabel of each frame to 0..S-1; scratch: [batch*num_labels] int32; counts: [batch] int32. */
 int wvn_segment_relabel(long long* seg, int batch, long long pix_per_frame, int num_labels, int* scratch, int* counts,
                         void* stream);
@@ -490,6 +498,14 @@ int wvn_mlp_infer_pixels_vit(wvn_mlp_infer_t* h, wvn_vit_t* vit, int batch, int 
 /* Same arithmetic on explicit rows x: [rows, dim] fp32 (segment-wise prediction mode). */
 int wvn_mlp_infer_rows(wvn_mlp_infer_t* h, const float* x, long long rows, const float* cg_mean,
                        const float* cg_std, float std_factor, float* trav, float* conf, void* stream);
+/* The same on rows padded per frame: x [groups, rows_per_group, dim] fp32, n_rows [groups] int32 on the device (row r of
+ * group g is live when r < n_rows[g]).  trav / conf: [groups, rows_per_group]; padding rows are NaN and their features
+ * are never read (the loader writes zeros in their place).  A live row's values are bit-identical to
+ * wvn_mlp_infer_rows on the compacted rows: the GEMM chain's tiles do not depend on the row count.  No host
+ * synchronisation, no allocation. */
+int wvn_mlp_infer_rows_padded(wvn_mlp_infer_t* h, const float* x, int groups, int rows_per_group, const int* n_rows,
+                              const float* cg_mean, const float* cg_std, float std_factor, float* trav, float* conf,
+                              void* stream);
 /* The same handle for a DoubleMLP(dim, [h1, h2, 1]) (bounds of wvn_double_mlp_trainer_create): set_params takes its
  * flat parameters (networks.0.{0,2,4}.{weight,bias}, then networks.1's) and packs the two nets as one block-structured
  * MLP of widths 2 h1 / 2 h2 — layer 1 [W1_0; W1_1], layer 2 diag(W2_0, W2_1), layer 3 [w3_0 | 0] for traversability and
@@ -717,6 +733,12 @@ int wvn_flow_infer_set_params(wvn_flow_infer_t* h, const float* params, void* st
 int wvn_flow_infer_rows(wvn_flow_infer_t* h, const float* params, const wvn_flow_buffers* buffers, const float* x, int rows,
                         float* z, float* log_det, float* logprob, const float* cg_mean, const float* cg_std,
                         float std_factor, float* trav, void* stream);
+/* The same trav on rows padded per frame: x [groups, rows_per_group, dim] fp32, n_rows [groups] int32 on the device
+ * (groups * rows_per_group <= max_rows).  trav [groups, rows_per_group]: the live rows' values, NaN on padding rows,
+ * which are neither read nor computed.  No host synchronisation, no allocation. */
+int wvn_flow_infer_rows_padded(wvn_flow_infer_t* h, const float* params, const wvn_flow_buffers* buffers, const float* x,
+                               int groups, int rows_per_group, const int* n_rows, const float* cg_mean,
+                               const float* cg_std, float std_factor, float* trav, void* stream);
 /* The per-pixel anomaly map (wvn_feature_extractor_node.py:332-338): tokens [batch, gh * gw, dim] fp32 are upsampled
  * bilinearly (align_corners = True) to out_h x out_w, every net layer runs as a wgmma GEMM (bf16 operands, fp32
  * accumulation), the coupling arithmetic in fp32.  trav [batch, out_h, out_w]: inference_without_update of the NLL;

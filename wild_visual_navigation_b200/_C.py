@@ -119,6 +119,7 @@ SIGNATURES = {
     "wvn_segment_workspace_bytes": (_S, [_I, _I, _I, _I]),
     "wvn_segment_reduce": (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P, _P, _P, _I, _P, _P]),
     "wvn_segment_relabel": (_I, [_P, _I, _L, _I, _P, _P, _P]),
+    "wvn_segment_maps": (_I, [_P, _I, _I, _L, _P, _P, _I, _P, _P, _P, _P]),
     "wvn_supervision_pool": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
     "wvn_slic_tables": (None, [_P, _P, _P]),
     "wvn_slic_geometry": (_I, [_I, _I, _I, _P, _P, _P]),
@@ -134,6 +135,7 @@ SIGNATURES = {
     "wvn_mlp_infer_pixels": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P]),
     "wvn_mlp_infer_pixels_vit": (_I, [_P, _P, _I, _I, _I, _P, _P, _F, _P, _P, _P]),
     "wvn_mlp_infer_rows": (_I, [_P, _P, _L, _P, _P, _F, _P, _P, _P]),
+    "wvn_mlp_infer_rows_padded": (_I, [_P, _P, _I, _I, _P, _P, _P, _F, _P, _P, _P]),
     "wvn_mlp_infer_create_double": (_I, [_I, _I, _I, _I, POINTER(_P)]),
     "wvn_mlp_param_count": (_S, [_I, _I, _I]),
     "wvn_mlp_train_workspace_bytes": (_S, [_I, _I, _I, _I]),
@@ -167,6 +169,7 @@ SIGNATURES = {
     "wvn_flow_infer_destroy": (None, [_P]),
     "wvn_flow_infer_set_params": (_I, [_P, _P, _P]),
     "wvn_flow_infer_rows": (_I, [_P, _P, POINTER(FlowBuffers), _P, _I, _P, _P, _P, _P, _P, _F, _P, _P]),
+    "wvn_flow_infer_rows_padded": (_I, [_P, _P, POINTER(FlowBuffers), _P, _I, _I, _P, _P, _P, _F, _P, _P]),
     "wvn_flow_infer_pixels": (_I, [_P, POINTER(FlowBuffers), _P, _I, _I, _I, _I, _I, _P, _P, _F, _P, _P, _P]),
     "wvn_flow_train_step": (_I, [_P, _P, _P, _P, _P, POINTER(FlowBuffers), _P, _I, _P, _P, _P, _P, _P, _I, _P]),
     "wvn_flow_train_step_padded": (_I, [_P, _P, _P, _P, _P, POINTER(FlowBuffers), _P, _I, _I, _P, _P, _P, _P, _P, _P, _I,

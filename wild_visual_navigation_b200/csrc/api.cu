@@ -617,6 +617,11 @@ int wvn_segment_relabel(long long* seg, int batch, long long pix_per_frame, int 
   return relabel_compact(seg, scratch, counts, batch, pix_per_frame, num_labels, S(stream));
 }
 
+int wvn_segment_maps(const void* seg, int seg_is_int64, int batch, long long hw, const float* trav, const float* conf,
+                     int smax, const int* n_rows, float* trav_map, float* conf_map, void* stream) {
+  return segment_maps(seg, seg_is_int64 != 0, batch, hw, trav, conf, smax, n_rows, trav_map, conf_map, S(stream));
+}
+
 int wvn_supervision_pool(const long long* seg, const float* mask, int batch, int channels, int h, int w, int smax,
                          float* y, unsigned char* y_valid, float* count_ws, void* stream) {
   WVN_REQUIRE(seg && mask && y && y_valid && count_ws, "wvn_supervision_pool: null argument");
@@ -1319,6 +1324,33 @@ int mlp_infer_chunk(wvn_mlp_infer* h, long long rows, long long row0, const floa
   return WVN_OK;
 }
 
+// Rows [r0, r0 + rows) of groups padded to rpg rows each -> bf16 at pitch ld.  A padding row (r >= n_rows[g]) is not
+// read: it is written as zeros, so the GEMM chain sees finite values there.
+__global__ void cast_rows_padded_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long r0,
+                                        long long rows, int rpg, const int* __restrict__ n_rows, int dim, long long ld) {
+  const long long n = rows * dim;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long r = i / dim, pr = r0 + r, g = pr / rpg;
+    const int c = static_cast<int>(i - r * dim);
+    const bool live = pr - g * rpg < n_rows[g];
+    dst[r * ld + c] = __float2bfloat16_rn(live ? src[pr * dim + c] : 0.f);
+  }
+}
+
+// trav / conf of every padding row -> NaN (conf may be null)
+__global__ void nan_padding_rows_kernel(float* __restrict__ trav, float* __restrict__ conf, long long rows, int rpg,
+                                        const int* __restrict__ n_rows) {
+  for (long long r = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; r < rows;
+       r += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long g = r / rpg;
+    if (r - g * rpg >= n_rows[g]) {
+      trav[r] = __int_as_float(0x7fc00000);
+      if (conf) conf[r] = __int_as_float(0x7fc00000);
+    }
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -1550,6 +1582,33 @@ int wvn_mlp_infer_rows(wvn_mlp_infer_t* h, const float* x, long long rows, const
     WVN_CHECK_LAUNCH("cast_rows_kernel");
     WVN_PROPAGATE(mlp_infer_chunk(h, n, r0, cg_mean, cg_std, std_factor, trav, conf, s));
   }
+  return WVN_OK;
+}
+
+// The padded form runs the same chunks over all groups * rows_per_group rows: the GEMMs' tile shapes depend on N and K
+// only (BM is fixed, block_n follows N), so each live row goes through exactly the arithmetic of wvn_mlp_infer_rows.
+int wvn_mlp_infer_rows_padded(wvn_mlp_infer_t* h, const float* x, int groups, int rows_per_group, const int* n_rows,
+                              const float* cg_mean, const float* cg_std, float std_factor, float* trav, float* conf,
+                              void* stream) {
+  WVN_REQUIRE(h && x && n_rows && trav && conf && cg_mean && cg_std, "wvn_mlp_infer_rows_padded: null argument");
+  WVN_REQUIRE(groups >= 0 && rows_per_group >= 0, "wvn_mlp_infer_rows_padded: bad geometry (groups=%d rows=%d)", groups,
+              rows_per_group);
+  if (!h->loaded) return set_error(WVN_ERR_STATE, "wvn_mlp_infer_rows_padded: parameters were never set");
+  cudaStream_t s = S(stream);
+  const long long rows = static_cast<long long>(groups) * rows_per_group;
+  if (rows == 0) return WVN_OK;
+  for (long long r0 = 0; r0 < rows; r0 += h->chunk_rows) {
+    const long long n = std::min<long long>(h->chunk_rows, rows - r0);
+    const long long elems = n * h->dim;
+    int blocks = static_cast<int>(std::min<long long>((elems + 255) / 256, 8192));
+    cast_rows_padded_kernel<<<blocks, 256, 0, s>>>(x, reinterpret_cast<__nv_bfloat16*>(h->x.p), r0, n, rows_per_group,
+                                                   n_rows, h->dim, h->dim_p);
+    WVN_CHECK_LAUNCH("cast_rows_padded_kernel");
+    WVN_PROPAGATE(mlp_infer_chunk(h, n, r0, cg_mean, cg_std, std_factor, trav, conf, s));
+  }
+  const int blocks = static_cast<int>(std::min<long long>((rows + 255) / 256, 4096));
+  nan_padding_rows_kernel<<<blocks, 256, 0, s>>>(trav, conf, rows, rows_per_group, n_rows);
+  WVN_CHECK_LAUNCH("nan_padding_rows_kernel");
   return WVN_OK;
 }
 
@@ -1842,6 +1901,14 @@ int wvn_flow_infer_rows(wvn_flow_infer_t* h, const float* params, const wvn_flow
   WVN_REQUIRE(h && buffers, "wvn_flow_infer_rows: null argument");
   return flow_forward_rows(h->rows, params, buffers_of(buffers), x, rows, z, log_det, logprob, cg_mean, cg_std,
                            std_factor, trav, S(stream));
+}
+
+int wvn_flow_infer_rows_padded(wvn_flow_infer_t* h, const float* params, const wvn_flow_buffers* buffers, const float* x,
+                               int groups, int rows_per_group, const int* n_rows, const float* cg_mean,
+                               const float* cg_std, float std_factor, float* trav, void* stream) {
+  WVN_REQUIRE(h && buffers, "wvn_flow_infer_rows_padded: null argument");
+  return flow_forward_rows_padded(h->rows, params, buffers_of(buffers), x, groups, rows_per_group, n_rows, cg_mean,
+                                  cg_std, std_factor, trav, S(stream));
 }
 
 int wvn_flow_infer_pixels(wvn_flow_infer_t* h, const wvn_flow_buffers* buffers, const float* tokens, int batch, int gh,

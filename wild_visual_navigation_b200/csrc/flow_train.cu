@@ -410,6 +410,47 @@ int flow_forward_rows(Trainer* base, const float* params, const FlowBuffers& b, 
 
 namespace {
 
+__global__ void fill_nan_kernel(float* __restrict__ out, long long n) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    out[i] = __int_as_float(0x7fc00000);
+}
+
+// out[comp[r]] = in[r] for the n_live compacted rows
+__global__ void scatter_live_rows_kernel(const float* __restrict__ in, const int* __restrict__ comp,
+                                         const int* __restrict__ n_live, float* __restrict__ out) {
+  const int n = *n_live;
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) out[comp[r]] = in[r];
+}
+
+}  // namespace
+
+int flow_forward_rows_padded(Trainer* base, const float* params, const FlowBuffers& b, const float* x, int groups,
+                             int rows_per_group, const int* n_rows, const float* cg_mean, const float* cg_std,
+                             float std_factor, float* trav, cudaStream_t stream) {
+  WVN_PROPAGATE(trainer_check(base, TRAINER_FLOW, "flow rows padded"));
+  FlowTrainer* t = static_cast<FlowTrainer*>(base);
+  WVN_REQUIRE(groups >= 0 && rows_per_group >= 0 && static_cast<long long>(groups) * rows_per_group <= t->max_rows,
+              "flow rows padded: %d x %d rows exceed the handle's capacity %d", groups, rows_per_group, t->max_rows);
+  const int rows = groups * rows_per_group;
+  WVN_PROPAGATE(check_args(t, params, b, x, rows));
+  WVN_REQUIRE(n_rows && trav && cg_mean && cg_std, "flow rows padded: null argument");
+  if (rows == 0) return WVN_OK;
+  // The live rows are compacted and run as flow_forward_rows runs them.  Their trav lands in compacted order in u[0],
+  // which nothing reads after the first coupling, and is scattered back to the padded positions.
+  float* trav_c = t->u[0];
+  WVN_PROPAGATE(flow_forward(t, params, b, x, groups, rows_per_group, n_rows, nullptr, nullptr, nullptr, nullptr, trav_c,
+                             cg_mean, cg_std, std_factor, stream));
+  const int blocks = std::min((rows + 255) / 256, 4096);
+  fill_nan_kernel<<<blocks, 256, 0, stream>>>(trav, rows);
+  WVN_CHECK_LAUNCH("fill_nan_kernel");
+  scatter_live_rows_kernel<<<blocks, 256, 0, stream>>>(trav_c, t->comp, t->n_live, trav);
+  WVN_CHECK_LAUNCH("scatter_live_rows_kernel");
+  return WVN_OK;
+}
+
+namespace {
+
 // The stages of a step.  The compacted entry's phase 1 runs kFwd | kGen, the padded entry's phase 2 kGen | kBwd: the
 // statistics exchange sits between kFwd and kGen.
 enum : int { kFwd = 1, kBwd = 2, kAdam = 4, kGen = 8 };

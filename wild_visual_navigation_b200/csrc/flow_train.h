@@ -46,6 +46,12 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
 int flow_forward_rows(Trainer* t, const float* params, const FlowBuffers& b, const float* x, int rows, float* z,
                       float* log_det, float* logprob, const float* cg_mean, const float* cg_std, float std_factor,
                       float* trav, cudaStream_t stream);
+// trav of rows padded per group, x [groups, rows_per_group, dim] with n_rows[g] (device int32) live rows in group g:
+// the live rows are compacted and run as above; trav [groups, rows_per_group] is NaN on padding rows, which are
+// neither read nor computed.
+int flow_forward_rows_padded(Trainer* t, const float* params, const FlowBuffers& b, const float* x, int groups,
+                             int rows_per_group, const int* n_rows, const float* cg_mean, const float* cg_std,
+                             float std_factor, float* trav, cudaStream_t stream);
 
 // One step of TraversabilityEstimator.train in anomaly-detection mode on the rows of x [rows, dim] whose y_valid is set
 // (y_valid NULL: every row).  phase_mask: 1 = forward, NLL statistics, confidence update; 2 = backward (the flat

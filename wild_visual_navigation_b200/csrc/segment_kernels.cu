@@ -6,12 +6,16 @@
 //   SegmentExtractor.centers            (segment_extractor.py:70-92)    per-segment centroid (x=col, y=row)
 //   SegmentExtractor.adjacency_list     (segment_extractor.py:40-67)    4-neighbour segment graph
 //   FeatureExtractor.segment_stego      (feature_extractor.py:245-246)  relabel to 0..S-1
+// and, the other way round, paints per-segment values back into per-pixel maps (segment_maps: the node's segment-wise
+// mode, wvn_feature_extractor_node.py:323-338).
 //
 // The dense (B, D, H, H) feature tensor is never formed: the mean of bilinearly upsampled
 // (align_corners=True) features over a segment is a linear function of the patch tokens,
 //   feat[s] = (sum_p W[s,p] * tok[p]) / count[s],   W[s,p] = sum_{pixels in s} bilinear weight of patch p,
 // so one pass over the pixels accumulates W (plus counts, coordinate sums and adjacency bits)
 // and a small second kernel contracts W with the token grid.
+#include <stdint.h>
+
 #include <algorithm>
 
 #include "common.cuh"
@@ -574,6 +578,92 @@ int supervision_pool(const long long* seg, const float* mask, int batch, int cha
   supervision_finalize_kernel<<<(n + 255) / 256, 256, 0, stream>>>(y, cnt_ws, y_valid, n);
   WVN_CHECK_LAUNCH("supervision_finalize_kernel");
   return WVN_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ segment-wise maps
+namespace {
+
+constexpr int kMapThreads = 256;
+
+// v[id] for a live id, NaN otherwise.  The unsigned compare sends negative ids to NaN as well.
+template <typename Id>
+__device__ __forceinline__ float row_value(const float* __restrict__ v, Id id, unsigned live) {
+  return static_cast<unsigned long long>(static_cast<long long>(id)) < live ? v[id] : __int_as_float(0x7fc00000);
+}
+
+// One (frame, pixel block) per CTA.  VEC: 4 pixels per thread, one 16-byte load of int32 ids or two of int64 ids, and
+// one float4 store per map; needs hw % 4 == 0 and 16-byte aligned pointers.  The per-segment values stay in L1 / L2:
+// a frame reads at most smax of them.
+template <typename Id, bool VEC>
+__global__ void __launch_bounds__(kMapThreads)
+segment_maps_kernel(const Id* __restrict__ seg, long long hw, const float* __restrict__ trav,
+                    const float* __restrict__ conf, int smax, const int* __restrict__ n_rows, float* __restrict__ tmap,
+                    float* __restrict__ cmap) {
+  const int b = blockIdx.y;
+  const unsigned live = static_cast<unsigned>(min(max(n_rows[b], 0), smax));
+  const Id* s = seg + b * hw;
+  const float* tv = trav + static_cast<long long>(b) * smax;
+  const float* cv = conf ? conf + static_cast<long long>(b) * smax : nullptr;
+  float* to = tmap + b * hw;
+  float* co = cmap ? cmap + b * hw : nullptr;
+  const long long stride = static_cast<long long>(gridDim.x) * kMapThreads;
+  if constexpr (VEC) {
+    const long long groups = hw / 4;
+    for (long long g = blockIdx.x * static_cast<long long>(kMapThreads) + threadIdx.x; g < groups; g += stride) {
+      Id id[4];
+      if constexpr (sizeof(Id) == 8) {
+        const longlong2 a = reinterpret_cast<const longlong2*>(s)[2 * g];
+        const longlong2 c = reinterpret_cast<const longlong2*>(s)[2 * g + 1];
+        id[0] = a.x; id[1] = a.y; id[2] = c.x; id[3] = c.y;
+      } else {
+        const int4 a = reinterpret_cast<const int4*>(s)[g];
+        id[0] = a.x; id[1] = a.y; id[2] = a.z; id[3] = a.w;
+      }
+      reinterpret_cast<float4*>(to)[g] = make_float4(row_value(tv, id[0], live), row_value(tv, id[1], live),
+                                                     row_value(tv, id[2], live), row_value(tv, id[3], live));
+      if (co)
+        reinterpret_cast<float4*>(co)[g] = make_float4(row_value(cv, id[0], live), row_value(cv, id[1], live),
+                                                       row_value(cv, id[2], live), row_value(cv, id[3], live));
+    }
+  } else {
+    for (long long p = blockIdx.x * static_cast<long long>(kMapThreads) + threadIdx.x; p < hw; p += stride) {
+      const Id id = s[p];
+      to[p] = row_value(tv, id, live);
+      if (co) co[p] = row_value(cv, id, live);
+    }
+  }
+}
+
+template <typename Id>
+int launch_segment_maps(const Id* seg, int batch, long long hw, const float* trav, const float* conf, int smax,
+                        const int* n_rows, float* tmap, float* cmap, cudaStream_t stream) {
+  auto aligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  const bool vec = hw % 4 == 0 && aligned(seg) && aligned(tmap) && (cmap == nullptr || aligned(cmap));
+  const long long per_thread = vec ? 4 : 1;
+  const long long blocks = std::min<long long>((hw + per_thread * kMapThreads - 1) / (per_thread * kMapThreads), 65535);
+  const dim3 grid(static_cast<unsigned>(blocks), static_cast<unsigned>(batch));
+  if (vec)
+    segment_maps_kernel<Id, true><<<grid, kMapThreads, 0, stream>>>(seg, hw, trav, conf, smax, n_rows, tmap, cmap);
+  else
+    segment_maps_kernel<Id, false><<<grid, kMapThreads, 0, stream>>>(seg, hw, trav, conf, smax, n_rows, tmap, cmap);
+  WVN_CHECK_LAUNCH("segment_maps_kernel");
+  return WVN_OK;
+}
+
+}  // namespace
+
+int segment_maps(const void* seg, bool seg_int64, int batch, long long hw, const float* trav, const float* conf, int smax,
+                 const int* n_rows, float* trav_map, float* conf_map, cudaStream_t stream) {
+  WVN_REQUIRE(seg && trav && n_rows && trav_map, "segment_maps: null argument");
+  WVN_REQUIRE((conf == nullptr) == (conf_map == nullptr), "segment_maps: conf and conf_map go together");
+  WVN_REQUIRE(batch >= 0 && batch <= 65535 && hw >= 0 && smax > 0,
+              "segment_maps: bad geometry (batch=%d hw=%lld smax=%d)", batch, hw, smax);
+  if (batch == 0 || hw == 0) return WVN_OK;
+  if (seg_int64)
+    return launch_segment_maps(static_cast<const long long*>(seg), batch, hw, trav, conf, smax, n_rows, trav_map,
+                               conf_map, stream);
+  return launch_segment_maps(static_cast<const int*>(seg), batch, hw, trav, conf, smax, n_rows, trav_map, conf_map,
+                             stream);
 }
 
 }  // namespace wvn

@@ -34,4 +34,9 @@ int relabel_compact(long long* seg, int* scratch, int* counts, int batch, long l
 int supervision_pool(const long long* seg, const float* mask, int batch, int channels, int h, int w, int smax, float* y,
                      unsigned char* y_valid, float* cnt_ws, cudaStream_t stream);
 
+// Segment-wise maps: map[b, p] = v[b, seg[b, p]] for ids in [0, min(n_rows[b], smax)), NaN otherwise.  seg: [B, hw]
+// int64 or int32; trav / conf: [B, smax] f32 (conf and conf_map may both be null); n_rows: [B] i32 on the device.
+int segment_maps(const void* seg, bool seg_int64, int batch, long long hw, const float* trav, const float* conf, int smax,
+                 const int* n_rows, float* trav_map, float* conf_map, cudaStream_t stream);
+
 }  // namespace wvn

@@ -44,6 +44,8 @@ class FeatureExtractor:
         self._slic_num_components = kwargs.get("slic_num_components", 100)
         self._slic_compactness = kwargs.get("slic_compactness", 10)
         self._slic_iters = kwargs.get("slic_iters", 10)
+        # grid segmentation's cell size when extract / extract_batch are not given one (segment_grid's default, 32)
+        self._cell_size = kwargs.get("cell_size", 32)
         common = dict(backbone_type=kwargs.get("backbone_type", "vit_small"), patch_size=kwargs.get("patch_size", 8),
                       max_batch=kwargs.get("max_batch", 1), chunk=kwargs.get("chunk", 0))
         need_stego = feature_type == "stego" or segmentation_type == "stego"
@@ -110,7 +112,15 @@ class FeatureExtractor:
 
     @property
     def max_segments(self):
-        """Upper bound of segments per frame of the stego segmentation (rows of the padded ``feat`` per frame)."""
+        """Upper bound of segments per frame (rows of the padded ``feat`` per frame) of the stego, slic and grid
+        segmentations at ``input_size`` (grid: at the constructor's ``cell_size``); None for the others."""
+        if self._segmentation_type == "stego":
+            return self._stego.max_segments
+        if self._segmentation_type == "slic":
+            _, nx, ny = ops.slic_geometry(self._input_size, self._input_size, self._slic_num_components)
+            return nx * ny
+        if self._segmentation_type == "grid":
+            return ((self._input_size + self._cell_size - 1) // self._cell_size) ** 2
         return self._stego.max_segments if self._stego is not None else None
 
     def change_device(self, device):
@@ -168,7 +178,7 @@ class FeatureExtractor:
                 tokens = self._stego.backbone_tokens
             # otherwise the features come from their own backbone (DINOv2), run in step 2
         elif self._segmentation_type == "grid":
-            cell = kwargs.get("cell_size", 32)
+            cell = kwargs.get("cell_size", self._cell_size)
             ys = torch.arange(H, device=img.device) // cell
             xs = torch.arange(W, device=img.device) // cell
             ncol = (W + cell - 1) // cell

@@ -25,12 +25,23 @@ through the unfused GEMM chain.
 A ``SimpleGCN`` predicts segment-wise only (``predict_segments`` with the frame's segment adjacency, csrc/gcn_train.cu):
 there is no graph over pixels, so ``predict`` / ``predict_from_tokens`` raise ``ValueError`` (the reference's node
 builds ``Data(x=...)`` without ``edge_index`` and cannot run a GCN either).
+
+Segment-wise mode (``prediction_per_pixel: False``, wvn_feature_extractor_node.py:323-338): the node runs the model on
+``feat[seg.reshape(-1)]``, every pixel carrying its segment's pooled row, so it evaluates each row once per pixel of
+the segment.  ``predict_frames`` evaluates each pooled row once, for a whole batch as ``extract_batch`` leaves it
+(rows padded per frame, device-side counts), and paints the values through ``seg`` (csrc/segment_kernels.cu); it works
+for every learner and never synchronises with the host.  The front end passed in may be a ``DinoInterface``, a
+``StegoInterface`` (its DINO backbone gives the token grid), a ``TorchVisionInterface`` or ``None``.  A feature pyramid
+has no token grid and the reference defines no per-pixel head on it (its per-pixel branch indexes ``dense_feat[0]`` of
+the pyramid dict and crashes), so there ``predict`` / ``predict_from_tokens`` raise ``ValueError``.
 """
 from __future__ import annotations
 
 import torch
 
 from . import ops
+from .feature_extractor.stego_interface import StegoInterface
+from .feature_extractor.torchvision_interface import TorchVisionInterface
 from .model.linear_rnvp import LinearRnvp
 from .model.simple_gcn import SimpleGCN
 from .model.simple_mlp import DoubleMLP, SimpleMLP
@@ -38,12 +49,22 @@ from .utils.confidence_generator import ConfidenceGenerator
 
 
 class TraversabilityInference:
-    def __init__(self, dino, model: SimpleMLP, confidence_generator: ConfidenceGenerator, chunk_rows: int = 0):
+    """``frontend``: the feature front end whose tokens the per-pixel calls read — a ``DinoInterface``, a
+    ``StegoInterface`` (its DINO backbone), a ``TorchVisionInterface`` (segment-wise only) or ``None`` (segment-wise
+    only).  ``max_rows``: padded rows per ``predict_frames`` call (max_batch * smax) the handles are sized for at
+    construction, so that call allocates nothing in the library."""
+
+    def __init__(self, frontend, model: SimpleMLP, confidence_generator: ConfidenceGenerator, chunk_rows: int = 0,
+                 max_rows: int = 1024):
+        self._pyramid = isinstance(frontend, TorchVisionInterface)
+        if isinstance(frontend, StegoInterface):
+            frontend = frontend._dino
+        dino = None if self._pyramid else frontend   # the token grid of the per-pixel calls, if there is one
         self._gcn = isinstance(model, SimpleGCN)
         if self._gcn:
             model.check_supported()
             self._dino, self._model, self._cg = dino, model, confidence_generator
-            self._gcn_infer = ops.GcnInference(model)
+            self._gcn_infer = ops.GcnInference(model, max_rows=max(1024, max_rows))
             self._flow = self._double = False
             return
         self._flow = isinstance(model, LinearRnvp)
@@ -51,7 +72,8 @@ class TraversabilityInference:
             if model.flat_params is None or not model.flat_params.is_cuda:
                 raise ValueError("TraversabilityInference: the LinearRnvp must be on a CUDA device")
             self._dino, self._model, self._cg = dino, model, confidence_generator
-            self._flow_infer = ops.FlowInference(model.input_size, model.hidden, max_rows=1024, chunk_pixels=chunk_rows)
+            self._flow_infer = ops.FlowInference(model.input_size, model.hidden, max_rows=max(1024, max_rows),
+                                                 chunk_pixels=chunk_rows)
             self.refresh_weights()
             return
         self._double = isinstance(model, DoubleMLP)
@@ -65,7 +87,7 @@ class TraversabilityInference:
         # a feature-pyramid backbone (TorchVisionInterface) has no token grid: only the segment-wise mode applies
         grid = getattr(dino, "grid", 0)
         self._mlp = ops.MlpInference(model.input_size, model.hidden[0], model.hidden[1], chunk_rows,
-                                       tokens_per_frame=max(grid * grid, getattr(dino._model, "npad", 0)),
+                                       tokens_per_frame=max(grid * grid, getattr(getattr(dino, "_model", None), "npad", 0)),
                                        double=self._double)
         self.refresh_weights()
 
@@ -94,13 +116,13 @@ class TraversabilityInference:
     @torch.no_grad()
     def predict(self, img: torch.Tensor):
         """img (B,3,H,W) in [0,1] -> (trav (B,H,H), conf (B,H,H)) fp32 on the device."""
-        self._no_pixels_for_gcn()
+        self._check_per_pixel()
         tokens = self._dino.inference_tokens(img)
         return self.predict_from_tokens(tokens, img.shape[2])
 
     @torch.no_grad()
     def predict_from_tokens(self, tokens: torch.Tensor, out_size: int):
-        self._no_pixels_for_gcn()
+        self._check_per_pixel()
         g = self._dino.grid
         if self._flow:   # anomaly mode: (trav, None) — the node publishes no confidence map here
             return self._flow_infer.pixels(self._model, tokens, (g, g), (out_size, out_size), self._cg.mean.data,
@@ -115,23 +137,39 @@ class TraversabilityInference:
         return self._mlp.pixels(tokens, (g, g), (out_size, out_size), self._cg.mean.data, self._cg.std.data,
                                 self._cg.std_factor)
 
-    def _no_pixels_for_gcn(self):
+    def _check_per_pixel(self):
         if self._gcn:
             raise ValueError("SimpleGCN predicts per segment only (there is no graph over pixels): use predict_segments "
                              "with the frame's edges")
+        if self._pyramid:
+            raise ValueError("a feature-pyramid backbone has no per-pixel head (the reference defines none): use "
+                             "predict_frames, or predict_segments for one frame")
+        if self._dino is None:
+            raise ValueError("no token front end was given: per-pixel maps need one; use predict_frames or "
+                             "predict_segments")
+
+    @torch.no_grad()
+    def predict_rows(self, feat, n_rows, edges=None, n_edges=None):
+        """Padded-row inference on a batch as ``extract_batch`` leaves it: feat [B, smax, D] and n_rows [B] int32 on
+        the device -> (trav, conf) [B, smax], NaN on padding rows; conf is None for the LinearRnvp.  A SimpleGCN also
+        needs the frames' edges [B, E, 2] / n_edges [B].  Device ops only (no host synchronisation)."""
+        m, s, f = self._cg.mean.data, self._cg.std.data, self._cg.std_factor
+        if self._gcn:
+            if edges is None or n_edges is None:
+                raise ValueError("predict_frames: a SimpleGCN needs the frames' edges and n_edges")
+            return self._gcn_infer.rows_padded(feat, n_rows, edges, n_edges, m, s, f)
+        if self._flow:
+            return self._flow_infer.trav_padded(self._model, feat, n_rows, m, s, f), None
+        return self._mlp.rows_padded(feat, n_rows, m, s, f)
 
     @torch.no_grad()
     def predict_frames(self, feat, n_rows, edges, n_edges, seg):
-        """SimpleGCN, segment-wise on a batch as ``extract_batch`` leaves it: feat [B, smax, D], n_rows [B], edges
-        [B, E, 2] / n_edges [B] on the device, seg [B, H, W] -> (trav, conf) [B, H, W], each pixel its segment's value.
-        Device ops only (no host synchronisation)."""
-        if not self._gcn:
-            raise ValueError("predict_frames is the SimpleGCN's segment-wise path")
-        trav, conf = self._gcn_infer.rows_padded(feat, n_rows, edges, n_edges, self._cg.mean.data, self._cg.std.data,
-                                                 self._cg.std_factor)
-        B = seg.shape[0]
-        idx = seg.reshape(B, -1).long()
-        return trav.gather(1, idx).view_as(seg), conf.gather(1, idx).view_as(seg)
+        """Segment-wise maps of a batch as ``extract_batch`` leaves it: feat [B, smax, D], n_rows [B] int32, edges
+        [B, E, 2] / n_edges [B] (read by the SimpleGCN only; may be None otherwise), seg [B, H, W] int64 or int32 ->
+        (trav, conf) [B, H, W], each pixel its segment's value (NaN for an id outside [0, n_rows)); conf is None for the
+        LinearRnvp.  Device ops only (no host synchronisation)."""
+        trav, conf = self.predict_rows(feat, n_rows, edges, n_edges)
+        return ops.segment_maps(seg, n_rows, trav, conf)
 
     @torch.no_grad()
     def predict_segments(self, feat: torch.Tensor, seg: torch.Tensor, edges: torch.Tensor = None):

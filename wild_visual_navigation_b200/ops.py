@@ -240,6 +240,27 @@ def relabel(seg, num_labels):
     return counts
 
 
+def segment_maps(seg, n_rows, trav, conf=None):
+    """Paints per-segment values into per-pixel maps: seg [B, H, W] int64 or int32, n_rows [B] int32 and trav / conf
+    [B, smax] fp32 on the device -> (trav_map, conf_map) [B, H, W] fp32 with map[b, p] = v[b, seg[b, p]], NaN where
+    the id is outside [0, n_rows[b]).  conf_map is None when conf is.  One kernel, no host synchronisation."""
+    assert seg.dtype in (torch.int64, torch.int32), "segment_maps: seg must be int64 or int32"
+    assert n_rows.dtype == torch.int32 and trav.dtype == torch.float32 and trav.dim() == 2
+    B, smax = trav.shape
+    assert seg.shape[0] == B and n_rows.shape == (B,), "segment_maps: seg, n_rows and trav disagree on the batch"
+    seg, trav = seg.contiguous(), trav.contiguous()
+    tmap = torch.empty(seg.shape, device=seg.device, dtype=torch.float32)
+    cmap = None
+    if conf is not None:
+        assert conf.shape == trav.shape and conf.dtype == torch.float32
+        conf = conf.contiguous()
+        cmap = torch.empty_like(tmap)
+    hw = seg[0].numel() if B > 0 else 0
+    check(lib().wvn_segment_maps(ptr(seg), int(seg.dtype == torch.int64), B, hw, ptr(trav), ptr(conf), smax,
+                                 ptr(n_rows), ptr(tmap), ptr(cmap), stream()))
+    return tmap, cmap
+
+
 # --------------------------------------------------------------------------------------------
 # ViT backbone handle
 # --------------------------------------------------------------------------------------------
@@ -598,6 +619,16 @@ class MlpInference:
         conf = torch.empty_like(trav)
         check(lib().wvn_mlp_infer_rows(self._h, ptr(x.contiguous()), R, ptr(cg_mean), ptr(cg_std), float(std_factor),
                                        ptr(trav), ptr(conf), stream()))
+        return trav, conf
+
+    def rows_padded(self, feat, n_rows, cg_mean, cg_std, std_factor):
+        """feat [G, S, dim] fp32 with n_rows [G] int32 live rows per group -> (trav [G, S], conf [G, S]); padding rows
+        NaN.  A live row's values are bit-identical to ``rows`` on the compacted rows."""
+        G, S = _check_padded(feat, n_rows, self.dim)
+        trav = torch.empty(G, S, device=feat.device, dtype=torch.float32)
+        conf = torch.empty_like(trav)
+        check(lib().wvn_mlp_infer_rows_padded(self._h, ptr(feat.contiguous()), G, S, ptr(n_rows), ptr(cg_mean),
+                                              ptr(cg_std), float(std_factor), ptr(trav), ptr(conf), stream()))
         return trav, conf
 
     def __del__(self):
@@ -1187,6 +1218,17 @@ class FlowInference:
         out = torch.empty(R, device=x.device)
         check(lib().wvn_flow_infer_rows(self._h, ptr(model.flat_params), byref(flow_buffers(model)), ptr(x), R, None,
                                         None, None, ptr(cg_mean), ptr(cg_std), float(std_factor), ptr(out), stream()))
+        return out
+
+    def trav_padded(self, model, feat, n_rows, cg_mean, cg_std, std_factor):
+        """feat [G, S, D] fp32 with n_rows [G] int32 live rows per group -> trav [G, S] fp32, NaN on padding rows.
+        Allocates nothing in the library once the handle holds G * S rows."""
+        G, S = _check_padded(feat, n_rows, self.dim)
+        self._reserve(G * S)
+        out = torch.empty(G, S, device=feat.device)
+        check(lib().wvn_flow_infer_rows_padded(self._h, ptr(model.flat_params), byref(flow_buffers(model)),
+                                               ptr(feat.contiguous()), G, S, ptr(n_rows), ptr(cg_mean), ptr(cg_std),
+                                               float(std_factor), ptr(out), stream()))
         return out
 
     def pixels(self, model, tokens, grid, out_hw, cg_mean, cg_std, std_factor, want_nll=False):
