@@ -62,7 +62,8 @@ int wvn_check_device(void);
  * padded form with one group is the same step).  A learner's entry point refuses another learner's handle.
  * Later additions under 108 add symbols only: the dense CRF (wvn_crf_*), the EfficientNet-B0 handle (wvn_effnet_*)
  * with its primitives, GEMM activation 3 (SiLU), wvn_segment_pool_levels, and the segment-wise inference entries
- * wvn_segment_maps, wvn_mlp_infer_rows_padded and wvn_flow_infer_rows_padded. */
+ * wvn_segment_maps, wvn_mlp_infer_rows_padded and wvn_flow_infer_rows_padded, and the ViT primitives
+ * wvn_image_to_patches, wvn_init_token_rows, wvn_layernorm_ex and wvn_attention_f32_debug. */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -139,9 +140,40 @@ int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* args, void* stream);
 int wvn_attention_bf16(const void* q, const void* k, const void* vt, void* out, int batch, int heads, int npad,
                        int n_valid, float scale, void* stream);
 
-/* LayerNorm over fp32 rows -> bf16 (and/or fp32) rows; dim in {384, 768}. */
+/* LayerNorm over fp32 rows -> bf16 rows; dim in {384, 768}.  The same as wvn_layernorm_ex without an fp32 output. */
 int wvn_layernorm(const float* x, const float* gamma, const float* beta, void* out_bf16, long long rows, int dim,
                   float eps, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * ViT primitives, exposed for testing: the memory-bound kernels the ViT handle runs around its GEMMs and attention.
+ * ---------------------------------------------------------------------------------------- */
+/* The patch loader: img [src_frames, 3, in_h, in_w] fp32 in [0, 1], or (u8_hwc = 1) [src_frames, in_h, in_w, 3]
+ * uint8 RGB (px = u8 / 255), NEAREST-resized to resized_h x resized_w (torch 'nearest', fp32 scale in / resized),
+ * center-cropped to image_size (offset int(round((resized - image_size) / 2)), half to even), ImageNet-normalised
+ * ((px - mean) * (1 / std) in fp32) and cut into g = image_size / patch patches per side (conv-floor semantics).
+ * out_bf16 [batch * g * g, pitch] bf16, pitch = round_up(3 * patch * patch, 8), row (f, py, px) in (c, ky, kx) order;
+ * columns [3 * patch * patch, pitch) are never written.  Output frame f reads source frame (frame0 + f) % src_frames;
+ * frames with frame0 + f >= flip_from are the horizontal flip of the whole image_size-wide crop.  patch in {8, 14, 16};
+ * the same derivation of crop, scales and frames as wvn_vit_forward / wvn_vit_forward_tta / wvn_vit_forward_u8. */
+int wvn_image_to_patches(const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
+                         int image_size, int patch, int frame0, int src_frames, int flip_from, void* out_bf16,
+                         void* stream);
+/* x [batch, npad, dim] fp32, per frame: row 0 = cls + pos[0, :], rows [1, 1 + registers) = reg (no position
+ * embedding), rows [n_valid, npad) = 0; every other row is left as it is.  cls [dim], pos [>= 1, dim],
+ * reg [registers, dim] (NULL when registers == 0). */
+int wvn_init_token_rows(float* x, const float* cls, const float* pos, const float* reg, int registers, int batch, int npad,
+                        int n_valid, int dim, void* stream);
+/* LayerNorm(dim, eps) of fp32 rows x [rows, dim] (biased variance, eps inside the square root), dim in {384, 768}:
+ * out_bf16 [rows, dim] bf16 (or NULL) and out_f32 (or NULL) fp32, which receives only rows [row0, n_valid) of each
+ * npad-row frame, compacted: frame f's row t lands at f * (n_valid - row0) + t - row0 (rows % npad == 0).
+ * reverse = 1 walks the rows last-to-first; the result does not change. */
+int wvn_layernorm_ex(const float* x, const float* gamma, const float* beta, void* out_bf16, float* out_f32,
+                     long long rows, int dim, float eps, int npad, int n_valid, int row0, int reverse, void* stream);
+/* The parity-debug attention of $WVN_VIT_PRECISE=1: fp32 qkv [batch * npad, 3 * dim] (columns [q | k | v], head h at
+ * columns h * 64 of each) -> out_bf16 [batch * npad, dim] = softmax(q k^T * scale) v over keys [0, n_valid), in fp32
+ * CUDA-core arithmetic; every row of [0, npad) is written.  dim = heads * 64. */
+int wvn_attention_f32_debug(const float* qkv, void* out_bf16, int batch, int heads, int npad, int n_valid, int dim,
+                            float scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * ViT backbone handle — replaces DinoInterface.__init__/inference's backbone
@@ -318,7 +350,9 @@ int wvn_upsample_dense(const float* tokens, float* out, int batch, int dim, int 
                        void* stream);
 /* bilinear (align_corners=False) upsampling of per-patch logits + argmax -> int64 segment ids
  * (STEGO postprocess + stego_interface.py:108-109).  logits: [batch*npad, ld] fp32.  Two logit
- * column ranges (cluster probe -> seg, linear probe -> seg_b; seg_b may be NULL) share one pass. */
+ * column ranges (cluster probe -> seg, linear probe -> seg_b; seg_b may be NULL) share one pass.
+ * Columns are read in float4s: col0, col0_b and ld are multiples of 4 and col0 + round_up(classes, 4) <= ld (likewise
+ * for the second range when it is used). */
 int wvn_logits_argmax(const float* logits, long long ld, int col0, int classes, int col0_b, int classes_b, int batch,
                       int npad, int gh, int gw, int out_h, int out_w, long long* seg, long long* seg_b, void* stream);
 

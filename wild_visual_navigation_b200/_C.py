@@ -77,6 +77,10 @@ SIGNATURES = {
     "wvn_gemm_bf16_ex": (_I, [POINTER(GemmExArgs), _P]),
     "wvn_attention_bf16": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "wvn_layernorm": (_I, [_P, _P, _P, _P, _L, _I, _F, _P]),
+    "wvn_image_to_patches": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "wvn_init_token_rows": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "wvn_layernorm_ex": (_I, [_P, _P, _P, _P, _P, _L, _I, _F, _I, _I, _I, _I, _P]),
+    "wvn_attention_f32_debug": (_I, [_P, _P, _I, _I, _I, _I, _I, _F, _P]),
     "wvn_vit_create": (_I, [POINTER(VitConfig), POINTER(_P)]),
     "wvn_vit_destroy": (None, [_P]),
     "wvn_vit_set_weight": (_I, [_P, c_char_p, _P, _L]),

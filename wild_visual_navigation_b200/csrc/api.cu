@@ -183,9 +183,44 @@ int wvn_attention_bf16(const void* q, const void* k, const void* vt, void* out, 
 
 int wvn_layernorm(const float* x, const float* gamma, const float* beta, void* out_bf16, long long rows, int dim,
                   float eps, void* stream) {
+  return wvn_layernorm_ex(x, gamma, beta, out_bf16, nullptr, rows, dim, eps, 0, 0, 1, 0, stream);
+}
+
+// -------------------------------------------------------------------------------- ViT primitives, exposed for testing
+int wvn_image_to_patches(const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
+                         int image_size, int patch, int frame0, int src_frames, int flip_from, void* out_bf16,
+                         void* stream) {
+  WVN_REQUIRE(img && out_bf16, "wvn_image_to_patches: null argument");
+  ImagePatchArgs a;
+  WVN_PROPAGATE(image_patch_args(batch, in_h, in_w, resized_h, resized_w, image_size, patch, frame0, src_frames, flip_from,
+                                 &a));
+  return image_to_patches(img, u8_hwc != 0, out_bf16, a, S(stream));
+}
+
+int wvn_init_token_rows(float* x, const float* cls, const float* pos, const float* reg, int registers, int batch, int npad,
+                        int n_valid, int dim, void* stream) {
+  WVN_REQUIRE(x && cls && pos, "wvn_init_token_rows: null argument");
+  WVN_REQUIRE(batch > 0 && dim > 0 && n_valid >= 1 + registers && npad >= n_valid,
+              "wvn_init_token_rows: bad geometry (batch %d, npad %d, n_valid %d, registers %d)", batch, npad, n_valid,
+              registers);
+  return init_token_rows(x, cls, pos, reg, registers, batch, npad, n_valid, dim, S(stream));
+}
+
+int wvn_layernorm_ex(const float* x, const float* gamma, const float* beta, void* out_bf16, float* out_f32,
+                     long long rows, int dim, float eps, int npad, int n_valid, int row0, int reverse, void* stream) {
+  WVN_REQUIRE(x && gamma && beta && (out_bf16 || out_f32), "wvn_layernorm_ex: null argument");
+  WVN_REQUIRE(out_f32 == nullptr || (npad > 0 && rows % npad == 0 && 0 <= row0 && row0 <= n_valid && n_valid <= npad),
+              "wvn_layernorm_ex: fp32 output needs rows %% npad == 0 and 0 <= row0 <= n_valid <= npad");
   LayerNormArgs a;
-  a.rows = rows; a.dim = dim; a.eps = eps;
-  return layernorm_rows(x, gamma, beta, out_bf16, nullptr, a, S(stream));
+  a.rows = rows; a.dim = dim; a.eps = eps; a.npad = npad; a.n_valid = n_valid; a.row0 = row0; a.reverse = reverse != 0;
+  return layernorm_rows(x, gamma, beta, out_bf16, out_f32, a, S(stream));
+}
+
+int wvn_attention_f32_debug(const float* qkv, void* out_bf16, int batch, int heads, int npad, int n_valid, int dim,
+                            float scale, void* stream) {
+  WVN_REQUIRE(qkv && out_bf16, "wvn_attention_f32_debug: null argument");
+  WVN_REQUIRE(batch > 0 && heads > 0 && 0 < n_valid && n_valid <= npad, "wvn_attention_f32_debug: bad geometry");
+  return attention_f32_debug(qkv, out_bf16, batch, heads, npad, n_valid, dim, scale, S(stream));
 }
 
 // -------------------------------------------------------------------------------- ViT
@@ -385,20 +420,13 @@ int vit_forward_impl(wvn_vit_t* h, const void* img, bool u8_hwc, int src_batch, 
   const wvn_vit_config& c = h->cfg;
   const int D = c.dim;
 
-  ImagePatchArgs ia;
-  ia.in_h = in_h; ia.in_w = in_w; ia.patch = c.patch_size; ia.grid_h = h->grid; ia.grid_w = h->grid;
-  // torchvision CenterCrop: top = int(round((H - size) / 2.0))
-  ia.crop_top = static_cast<int>(lrintf((resized_h - c.image_size) / 2.0f));
-  ia.crop_left = static_cast<int>(lrintf((resized_w - c.image_size) / 2.0f));
-  ia.scale_y = static_cast<float>(in_h) / static_cast<float>(resized_h);
-  ia.scale_x = static_cast<float>(in_w) / static_cast<float>(resized_w);
-
   for (int b0 = 0; b0 < batch; b0 += h->chunk) {
     const int nb = std::min(h->chunk, batch - b0);
     const int rows = nb * h->npad;
     float* x = reinterpret_cast<float*>(h->x.p);
-    ia.batch = nb;
-    ia.frame0 = b0; ia.src_frames = src_batch; ia.flip_from = flip_tta ? src_batch : (1 << 30);
+    ImagePatchArgs ia;
+    WVN_PROPAGATE(image_patch_args(nb, in_h, in_w, resized_h, resized_w, c.image_size, c.patch_size, b0, src_batch,
+                                   flip_tta ? src_batch : (1 << 30), &ia));
     WVN_PROPAGATE(image_to_patches(img, u8_hwc, h->ape.p, ia, s));
     const float* reg = c.registers > 0 ? h->wp<float>("register_tokens") : nullptr;
     WVN_PROPAGATE(init_token_rows(x, h->wp<float>("cls_token"), h->wp<float>("pos_embed"), reg, c.registers, nb, h->npad,

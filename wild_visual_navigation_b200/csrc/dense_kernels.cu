@@ -199,6 +199,13 @@ int interp_pixel_rows(const float* tokens, void* out_bf16, const DenseArgs& a, l
 int logits_argmax(const float* logits, long long* seg, long long* seg_b, const LogitsArgs& a, cudaStream_t stream) {
   WVN_REQUIRE(a.classes > 0 && a.batch > 0, "logits_argmax: empty problem");
   WVN_REQUIRE(a.col0 % 4 == 0 && a.col0_b % 4 == 0 && a.ld % 4 == 0, "logits_argmax: columns must be float4-aligned");
+  // the kernel reads whole float4s: columns [col0, col0 + round_up(classes, 4)) of each range must lie inside a row
+  const int end = a.col0 + (a.classes + 3) / 4 * 4, end_b = a.col0_b + (a.classes_b + 3) / 4 * 4;
+  WVN_REQUIRE(a.col0 >= 0 && end <= a.ld,
+              "logits_argmax: columns [%d, %d) (classes rounded up to 4) exceed the row length %lld", a.col0, end, a.ld);
+  WVN_REQUIRE(seg_b == nullptr || a.classes_b <= 0 || (a.col0_b >= 0 && end_b <= a.ld),
+              "logits_argmax: second range's columns [%d, %d) (classes rounded up to 4) exceed the row length %lld",
+              a.col0_b, end_b, a.ld);
   const long long total = static_cast<long long>(a.batch) * a.out_h * a.out_w;
   long long blocks = (total + 255) / 256;
   const long long max_blocks = static_cast<long long>(sm_count()) * 16;

@@ -50,14 +50,15 @@ __global__ void image_to_patches_kernel(const void* __restrict__ img_raw, __nv_b
     const int gb = a.frame0 + b;
     const bool flip = gb >= a.flip_from;
     const int sb = gb % a.src_frames;
-    const int crop_w = a.grid_w * ps;
     const float* src_row = img + ((static_cast<long long>(sb) * 3 + c) * a.in_h + sy) * a.in_w;
     const unsigned char* src_row8 = img8 + (static_cast<long long>(sb) * a.in_h + sy) * a.in_w * 3 + c;
     float v[G];
 #pragma unroll
     for (int i = 0; i < G; ++i) {
       const int xo = pw * ps + kx0 + i;
-      const int x = flip ? crop_w - 1 - xo : xo;
+      // the flip mirrors the whole crop: when patch does not divide it, the patches of the flipped image do not cover
+      // its last crop - grid_w * ps columns, which are the first columns of the straight image
+      const int x = flip ? a.crop - 1 - xo : xo;
       const int sx = min(static_cast<int>(floorf((x + a.crop_left) * a.scale_x)), a.in_w - 1);
       // uint8: the same IEEE division torchvision's ToTensor performs, so both sources give identical patches
       const float px = U8_HWC ? static_cast<float>(__ldg(src_row8 + 3 * sx)) / 255.f : __ldg(src_row + sx);
@@ -216,6 +217,30 @@ attention_f32_debug_kernel(const float* __restrict__ qkv, __nv_bfloat16* __restr
 }
 
 }  // namespace
+
+int image_patch_args(int batch, int in_h, int in_w, int resized_h, int resized_w, int image_size, int patch, int frame0,
+                     int src_frames, int flip_from, ImagePatchArgs* a) {
+  WVN_REQUIRE(a != nullptr, "image_patch_args: null argument");
+  WVN_REQUIRE(patch == 8 || patch == 14 || patch == 16, "image_to_patches: patch size %d unsupported", patch);
+  WVN_REQUIRE(batch > 0 && in_h > 0 && in_w > 0 && image_size >= patch, "image_to_patches: empty problem");
+  WVN_REQUIRE(resized_h >= image_size && resized_w >= image_size,
+              "image_to_patches: resized image %dx%d smaller than the crop %d", resized_h, resized_w, image_size);
+  WVN_REQUIRE(frame0 >= 0 && src_frames > 0, "image_to_patches: frame0 %d, src_frames %d", frame0, src_frames);
+  ImagePatchArgs r;
+  r.batch = batch;
+  r.in_h = in_h; r.in_w = in_w; r.patch = patch;
+  r.grid_h = r.grid_w = image_size / patch;
+  r.crop = image_size;
+  // torchvision CenterCrop: top = int(round((H - size) / 2.0)); lrintf rounds half to even, as Python's round does
+  r.crop_top = static_cast<int>(lrintf((resized_h - image_size) / 2.0f));
+  r.crop_left = static_cast<int>(lrintf((resized_w - image_size) / 2.0f));
+  // torch 'nearest' with an output size: scale = (float)in / out
+  r.scale_y = static_cast<float>(in_h) / static_cast<float>(resized_h);
+  r.scale_x = static_cast<float>(in_w) / static_cast<float>(resized_w);
+  r.frame0 = frame0; r.src_frames = src_frames; r.flip_from = flip_from;
+  *a = r;
+  return WVN_OK;
+}
 
 int image_to_patches(const void* img, bool u8_hwc, void* out_bf16, const ImagePatchArgs& a, cudaStream_t stream) {
   WVN_REQUIRE(a.patch == 8 || a.patch == 14 || a.patch == 16, "image_to_patches: patch size %d unsupported", a.patch);

@@ -10,15 +10,24 @@ struct ImagePatchArgs {
   int in_h = 0, in_w = 0;        // source image size
   int patch = 8;
   int grid_h = 0, grid_w = 0;    // patches per column / row of the cropped image
+  int crop = 0;                  // side of the (square) cropped image; grid * patch < crop when patch does not divide it
   int crop_top = 0, crop_left = 0;  // center-crop offsets in the (virtually) resized image
   float scale_y = 1.f, scale_x = 1.f;  // in / resized (torch 'nearest' source index scale)
   // Test-time-augmentation passes: output frame f reads source frame (frame0 + f) % src_frames, and frames with
   // frame0 + f >= flip_from are the horizontal flip of the TRANSFORMED (resized + cropped) image, as Stego.get_code
-  // flips its already-transformed input.  Defaults = identity.
+  // flips its already-transformed input: column x of the flipped image is column crop - 1 - x of the crop (the whole
+  // crop, not just the grid * patch columns the patches cover).  Defaults = identity.
   int frame0 = 0, src_frames = 1 << 30, flip_from = 1 << 30;
   float mean[3] = {0.485f, 0.456f, 0.406f};
   float inv_std[3] = {1.f / 0.229f, 1.f / 0.224f, 1.f / 0.225f};
 };
+
+// The patch loader's arguments for `batch` frames of an in_h x in_w image, NEAREST-resized to resized_h x resized_w and
+// center-cropped to image_size (torchvision CenterCrop: offset int(round((resized - image_size) / 2)), half to even),
+// cut into image_size / patch patches per side (conv-floor semantics), with the TTA fields above.  The ViT forward and
+// the testing entry wvn_image_to_patches both derive their arguments here.
+int image_patch_args(int batch, int in_h, int in_w, int resized_h, int resized_w, int image_size, int patch, int frame0,
+                     int src_frames, int flip_from, ImagePatchArgs* a);
 
 struct LayerNormArgs {
   long long rows = 0;

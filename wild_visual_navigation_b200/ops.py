@@ -44,10 +44,50 @@ def attention(q, k, vt, n_valid, scale=0.125):
     return out
 
 
-def layernorm(x, gamma, beta, eps=1e-6):
+def layernorm(x, gamma, beta, eps=1e-6, *, out=None, out_f32=None, npad=0, n_valid=0, row0=1, reverse=False):
+    """LayerNorm of fp32 rows x [rows, dim] -> bf16 rows (``out``, allocated when None).  ``out_f32`` (optional) receives
+    the fp32 result of rows [row0, n_valid) of each npad-row frame, compacted (see wvn_layernorm_ex)."""
     rows, dim = x.shape
-    out = torch.empty(rows, dim, device=x.device, dtype=torch.bfloat16)
-    check(lib().wvn_layernorm(ptr(x), ptr(gamma), ptr(beta), ptr(out), rows, dim, eps, stream()))
+    if out is None:
+        out = torch.empty(rows, dim, device=x.device, dtype=torch.bfloat16)
+    check(lib().wvn_layernorm_ex(ptr(x), ptr(gamma), ptr(beta), ptr(out), ptr(out_f32), rows, dim, eps, npad, n_valid,
+                                 row0, int(reverse), stream()))
+    return out
+
+
+def image_to_patches(img, image_size, patch, resized_hw=None, batch=None, frame0=0, src_frames=None, flip_from=None,
+                     out=None):
+    """The ViT patch loader on its own: img (S,3,H,W) fp32 or (S,H,W,3) uint8 -> bf16 patch rows
+    [batch * g * g, round_up(3 p^2, 8)] (g = image_size // patch), pad columns left as they are.  Output frame f is
+    source frame (frame0 + f) % src_frames, horizontally flipped when frame0 + f >= flip_from (see
+    wvn_image_to_patches)."""
+    img = img.contiguous()
+    u8 = img.dtype == torch.uint8
+    S, H, W = (img.shape[0], img.shape[1], img.shape[2]) if u8 else (img.shape[0], img.shape[2], img.shape[3])
+    rh, rw = _resized_size(H, W, image_size) if resized_hw is None else resized_hw
+    batch = S if batch is None else batch
+    src_frames = S if src_frames is None else src_frames
+    flip_from = (1 << 30) if flip_from is None else flip_from
+    g = image_size // patch
+    if out is None:
+        out = torch.empty(batch * g * g, (3 * patch * patch + 7) // 8 * 8, device=img.device, dtype=torch.bfloat16)
+    check(lib().wvn_image_to_patches(ptr(img), int(u8), batch, H, W, rh, rw, image_size, patch, frame0, src_frames,
+                                     flip_from, ptr(out), stream()))
+    return out
+
+
+def init_token_rows(x, cls, pos, reg, n_valid):
+    """In place on x [B, npad, D] fp32: CLS row cls + pos[0], register rows reg [R, D] (or None), padding rows 0."""
+    B, npad, D = x.shape
+    R = 0 if reg is None else reg.shape[0]
+    check(lib().wvn_init_token_rows(ptr(x), ptr(cls), ptr(pos), ptr(reg), R, B, npad, n_valid, D, stream()))
+
+
+def attention_f32_debug(qkv, batch, heads, npad, n_valid, scale=0.125, out=None):
+    """fp32 parity-debug attention: qkv [batch * npad, 3 * heads * 64] fp32 -> [batch * npad, heads * 64] bf16."""
+    if out is None:
+        out = torch.empty(batch * npad, heads * 64, device=qkv.device, dtype=torch.bfloat16)
+    check(lib().wvn_attention_f32_debug(ptr(qkv), ptr(out), batch, heads, npad, n_valid, heads * 64, scale, stream()))
     return out
 
 
