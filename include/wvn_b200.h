@@ -140,7 +140,7 @@ int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* args, void* stream);
 int wvn_attention_bf16(const void* q, const void* k, const void* vt, void* out, int batch, int heads, int npad,
                        int n_valid, float scale, void* stream);
 
-/* LayerNorm over fp32 rows -> bf16 rows; dim in {384, 768}.  The same as wvn_layernorm_ex without an fp32 output. */
+/* LayerNorm over fp32 rows -> bf16 rows; dim in {384, 768, 1024}.  The same as wvn_layernorm_ex without an fp32 output. */
 int wvn_layernorm(const float* x, const float* gamma, const float* beta, void* out_bf16, long long rows, int dim,
                   float eps, void* stream);
 
@@ -163,7 +163,7 @@ int wvn_image_to_patches(const void* img, int u8_hwc, int batch, int in_h, int i
  * reg [registers, dim] (NULL when registers == 0). */
 int wvn_init_token_rows(float* x, const float* cls, const float* pos, const float* reg, int registers, int batch, int npad,
                         int n_valid, int dim, void* stream);
-/* LayerNorm(dim, eps) of fp32 rows x [rows, dim] (biased variance, eps inside the square root), dim in {384, 768}:
+/* LayerNorm(dim, eps) of fp32 rows x [rows, dim] (biased variance, eps inside the square root), dim in {384, 768, 1024}:
  * out_bf16 [rows, dim] bf16 (or NULL) and out_f32 (or NULL) fp32, which receives only rows [row0, n_valid) of each
  * npad-row frame, compacted: frame f's row t lands at f * (n_valid - row0) + t - row0 (rows % npad == 0).
  * reverse = 1 walks the rows last-to-first; the result does not change. */
@@ -185,8 +185,8 @@ typedef struct wvn_vit wvn_vit_t;
 typedef struct {
   int image_size;   /* side of the (square) network input after resize + center crop, e.g. 448 */
   int patch_size;   /* 8 or 16 (DINO), 14 (DINOv2) */
-  int dim;          /* 384 (vit_small) or 768 (vit_base) */
-  int depth;        /* 12 */
+  int dim;          /* 384 (vit_small), 768 (vit_base) or 1024 (vit_large) */
+  int depth;        /* 12 (vit_small, vit_base), 24 (vit_large) */
   int heads;        /* dim / 64 */
   int mlp_dim;      /* 4 * dim */
   int max_batch;    /* largest batch a single forward call may carry */

@@ -1,5 +1,5 @@
-"""Backbone forward throughput: DINO ViT-S/8, DINOv2 ViT-S/14 / ViT-B/14 and their register variants (4 register
-tokens), and the torchvision ResNet-18 / ResNet-50 and EfficientNet-B0 feature pyramids, at 448 x 448, B = 32 frames per call,
+"""Backbone forward throughput: DINO ViT-S/8, DINOv2 ViT-S/14 / ViT-B/14 / ViT-L/14 and their register variants (4
+register tokens), and the torchvision ResNet-18 / ResNet-50 and EfficientNet-B0 feature pyramids, at 448 x 448, B = 32 frames per call,
 seeded weights.  `python scripts/bench_backbones.py [--steps 20] [--warmup 3] [--repeats 5] [--batch 32]
 [--backbones NAME ...]`.
 
@@ -33,7 +33,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 RESNETS = [("resnet18", 18), ("resnet50", 50)]
 BACKBONES = [("dino_vit_s8", "dino", "vit_small", 8), ("dinov2_vit_s14", "dinov2", "vit_small", 14),
              ("dinov2_vit_b14", "dinov2", "vit_base", 14), ("dinov2_reg_vit_s14", "dinov2_reg", "vit_small", 14),
-             ("dinov2_reg_vit_b14", "dinov2_reg", "vit_base", 14)]
+             ("dinov2_reg_vit_b14", "dinov2_reg", "vit_base", 14), ("dinov2_vit_l14", "dinov2", "vit_large", 14),
+             ("dinov2_reg_vit_l14", "dinov2_reg", "vit_large", 14)]
 
 
 def gflop_per_frame(dim, depth, mlp_dim, patch, image_size, registers=0):

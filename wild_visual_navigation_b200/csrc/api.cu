@@ -227,7 +227,7 @@ int wvn_attention_f32_debug(const float* qkv, void* out_bf16, int batch, int hea
 int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
   WVN_REQUIRE(cfg && out, "wvn_vit_create: null argument");
   WVN_PROPAGATE(wvn_check_device());
-  WVN_REQUIRE(cfg->dim == 384 || cfg->dim == 768, "vit: dim %d unsupported (384, 768)", cfg->dim);
+  WVN_REQUIRE(cfg->dim == 384 || cfg->dim == 768 || cfg->dim == 1024, "vit: dim %d unsupported (384, 768, 1024)", cfg->dim);
   WVN_REQUIRE(cfg->heads * 64 == cfg->dim, "vit: heads*64 must equal dim");
   WVN_REQUIRE(cfg->patch_size == 8 || cfg->patch_size == 14 || cfg->patch_size == 16, "vit: patch size %d unsupported",
               cfg->patch_size);

@@ -11,7 +11,7 @@ from __future__ import annotations
 import torch
 
 from .. import ops
-from .weights import DINOV2_PATCH, VIT_SHAPES, check_backbone_family, load_dino_state_dict
+from .weights import DINOV2_PATCH, VIT_SHAPES, check_backbone_family, check_backbone_type, load_dino_state_dict
 
 
 class _Cfg(dict):
@@ -25,8 +25,9 @@ class _Cfg(dict):
 
 class DinoInterface:
     """``backbone="dino"``: DINO ViT-S / ViT-B at ``patch_size`` 8 or 16.  ``backbone="dinov2"``: DINOv2 ViT-S/14 /
-    ViT-B/14 (no register tokens).  ``backbone="dinov2_reg"``: DINOv2 ViT-S/14-reg / ViT-B/14-reg (4 register tokens;
-    only the patch tokens are returned).  DINOv2 is released at patch 14 only, so both run at patch 14 whatever
+    ViT-B/14 / ViT-L/14 (no register tokens).  ``backbone="dinov2_reg"``: DINOv2 ViT-S/14-reg / ViT-B/14-reg /
+    ViT-L/14-reg (4 register tokens; only the patch tokens are returned).  ``backbone_type`` is "vit_small", "vit_base"
+    or, for DINOv2 only, "vit_large"; a checkpoint of another width or depth raises ValueError.  DINOv2 is released at patch 14 only, so both run at patch 14 whatever
     ``patch_size`` says (the reference's ROS default passes ``patch_size=8`` with ``dinov2``); ``vit_patch_size`` still
     returns the configured value, as the reference's property does, while ``grid`` is the token grid actually run."""
 
@@ -45,11 +46,12 @@ class DinoInterface:
         if not str(device).startswith("cuda"):
             raise RuntimeError("wild_visual_navigation_b200 runs on CUDA (sm_90a) devices only — no CPU fallback")
         self._device = device
-        shp = VIT_SHAPES[self._cfg.backbone_type]
         backbone = self._cfg.backbone
+        check_backbone_type(backbone, self._cfg.backbone_type)
+        shp = VIT_SHAPES[self._cfg.backbone_type]
         patch = DINOV2_PATCH if backbone in ("dinov2", "dinov2_reg") else self._cfg.patch_size
         if state_dict is not None:
-            sd = check_backbone_family(state_dict, backbone)
+            sd = check_backbone_family(state_dict, backbone, self._cfg.backbone_type)
         else:
             sd = load_dino_state_dict(self._cfg.backbone_type, patch, self._cfg.pretrained_weights, backbone=backbone)
         with torch.cuda.device(torch.device(device)):

@@ -8,7 +8,9 @@
   * adjacency + centroids come from the same pass (no per-segment Python loops / host syncs);
   * when segmentation and features are both "stego"/"dino" on the same backbone, one ViT forward
     serves both (the reference runs two backbones); with "dinov2" / "dinov2_reg" features, STEGO's DINO backbone
-    segments and a second, DINOv2 handle gives the features;
+    segments and a second, DINOv2 handle gives the features.  STEGO's backbone follows ``backbone_type`` unless
+    ``stego_backbone_type`` ("vit_small" / "vit_base") says otherwise; DINO has no ViT-L, so DINOv2 ViT-L/14 features
+    (``backbone_type="vit_large"``) with stego segmentation need it;
   * "torchvision" features (``model_type`` resnet18 / resnet50 / resnet50_dino / efficientnet_b0) are a feature
     pyramid (four levels, five for EfficientNet-B0) pooled per segment level by level (csrc/resnet_kernels.cu), as
     sparsify_features' dict branch does.  Where a segment has no
@@ -28,6 +30,7 @@ from .dino_interface import DinoInterface
 from .segment_extractor import SegmentExtractor
 from .stego_interface import StegoInterface
 from .torchvision_interface import MODEL_TYPES, TorchVisionInterface
+from .weights import DINO_V1_TYPES, VIT_SHAPES, check_backbone_type
 
 
 class FeatureExtractor:
@@ -49,6 +52,12 @@ class FeatureExtractor:
         common = dict(backbone_type=kwargs.get("backbone_type", "vit_small"), patch_size=kwargs.get("patch_size", 8),
                       max_batch=kwargs.get("max_batch", 1), chunk=kwargs.get("chunk", 0))
         need_stego = feature_type == "stego" or segmentation_type == "stego"
+        # the feature backbone, as the reference picks it (feature_extractor.py:61): "dino", "dinov2" or "dinov2_reg"
+        backbone = kwargs.get("backbone", feature_type)
+        # STEGO's own backbone is DINO; it serves the features too unless they come from another backbone
+        share = feature_type == "stego" or backbone == "dino"
+        stego_backbone_type = self._stego_backbone_type(kwargs.get("stego_backbone_type"), common["backbone_type"],
+                                                        need_stego, share)
         if feature_type == "stego":
             self._feature_dim = 90
         elif feature_type == "torchvision":
@@ -58,14 +67,12 @@ class FeatureExtractor:
             if "model_type" not in kwargs:
                 raise ValueError(f"feature_type 'torchvision' needs model_type ({', '.join(MODEL_TYPES)})")
         elif "dino" in feature_type:
-            # the reference hard-codes 384 for every dino variant (feature_extractor.py:56)
-            self._feature_dim = 384 if common["backbone_type"] == "vit_small" else 768
+            # the reference hard-codes 384 for every dino variant (feature_extractor.py:56); here it is the backbone's
+            # width: 384 (vit_small), 768 (vit_base) or 1024 (vit_large, DINOv2 only)
+            check_backbone_type(backbone, common["backbone_type"])
+            self._feature_dim = VIT_SHAPES[common["backbone_type"]]["dim"]
         else:
             raise ValueError(f"Extractor[{feature_type}] is outside the H100 hot path")
-        # the feature backbone, as the reference picks it (feature_extractor.py:61): "dino", "dinov2" or "dinov2_reg"
-        backbone = kwargs.get("backbone", feature_type)
-        # STEGO's own backbone is DINO; it serves the features too unless they come from another backbone
-        share = feature_type == "stego" or backbone == "dino"
         if need_stego:
             self._stego = StegoInterface(device=device, input_size=input_size, run_crf=kwargs.get("run_crf", False),
                                          run_clustering=kwargs.get("run_clustering", True),  # the reference's default (:51)
@@ -73,7 +80,8 @@ class FeatureExtractor:
                                          head_state_dict=kwargs.get("head_state_dict"),
                                          backbone_state_dict=kwargs.get("state_dict" if share else "stego_state_dict"),
                                          flip_tta=kwargs.get("flip_tta", True),
-                                         kmeans_iters=kwargs.get("kmeans_iters", 10), **common)
+                                         kmeans_iters=kwargs.get("kmeans_iters", 10),
+                                         **dict(common, backbone_type=stego_backbone_type))
         else:
             self._stego = None
         self._tv = None
@@ -96,6 +104,23 @@ class FeatureExtractor:
                                        state_dict=kwargs.get("state_dict"),
                                        pretrained_weights=kwargs.get("pretrained_weights"), **common)
             self._extractor = self._dino
+
+    @staticmethod
+    def _stego_backbone_type(stego_backbone_type, backbone_type, need_stego, share):
+        """STEGO segments on its own DINO v1 backbone (ViT-S or ViT-B).  Without ``stego_backbone_type`` it follows
+        ``backbone_type``; when STEGO's backbone also gives the features the two must agree."""
+        if stego_backbone_type is None:
+            if need_stego and not share and backbone_type not in DINO_V1_TYPES:
+                raise ValueError(f"STEGO segments on its own DINO backbone, which has no '{backbone_type}': pass "
+                                 f"stego_backbone_type ({' or '.join(DINO_V1_TYPES)})")
+            return backbone_type
+        if stego_backbone_type not in DINO_V1_TYPES:
+            raise ValueError(f"stego_backbone_type must be {' or '.join(DINO_V1_TYPES)} (STEGO's DINO backbone), got "
+                             f"{stego_backbone_type!r}")
+        if need_stego and share and stego_backbone_type != backbone_type:
+            raise ValueError(f"stego_backbone_type {stego_backbone_type!r} differs from backbone_type {backbone_type!r}, "
+                             f"but STEGO's backbone gives the features here")
+        return stego_backbone_type
 
     # ---- reference properties ---------------------------------------------------------------
     @property

@@ -7,9 +7,10 @@ The reference downloads DINO checkpoints from dl.fbaipublicfiles.com at construc
     (keys cls_token, pos_embed, patch_embed.proj.*, blocks.N.*, norm.*), which is used as is;
   * otherwise seeded DINO-style random weights are generated (SURVEY.md §8d) — results are then
     numerically meaningful only for parity / throughput work, and a warning says so.
-DINOv2 (``backbone="dinov2"``, the ``dinov2_vit{s,b}14_pretrain.pth`` checkpoints) uses the same key names plus the
+DINOv2 (``backbone="dinov2"``, the ``dinov2_vit{s,b,l}14_pretrain.pth`` checkpoints) uses the same key names plus the
 LayerScale gammas ``blocks.N.ls{1,2}.gamma`` and an unused ``mask_token``; DINOv2 with registers
-(``backbone="dinov2_reg"``, ``dinov2_vit{s,b}14_reg4_pretrain.pth``) adds ``register_tokens`` (1, R, D).
+(``backbone="dinov2_reg"``, ``dinov2_vit{s,b,l}14_reg4_pretrain.pth``) adds ``register_tokens`` (1, R, D).  ViT-L/14
+(``backbone_type="vit_large"``) exists for DINOv2 only.
 The torchvision ResNets (``TorchVisionInterface``) take torchvision-layout state dicts (``resnet18`` / ``resnet50``
 ImageNet checkpoints, or DINO's ``dino_resnet50_pretrain.pth`` for ``resnet50_dino``); ``fc.*`` is not needed.
 EfficientNet-B0 (``efficientnet_b0``) takes torchvision-layout ``efficientnet_b0`` state dicts; ``classifier.*`` is not
@@ -26,7 +27,19 @@ import torch
 VIT_SHAPES = {
     "vit_small": dict(dim=384, depth=12, heads=6, mlp_dim=1536),
     "vit_base": dict(dim=768, depth=12, heads=12, mlp_dim=3072),
+    "vit_large": dict(dim=1024, depth=24, heads=16, mlp_dim=4096),
 }
+# DINO v1 is released as ViT-S and ViT-B only; ViT-L exists for DINOv2 (with and without registers)
+DINO_V1_TYPES = ("vit_small", "vit_base")
+
+
+def check_backbone_type(backbone: str, backbone_type: str) -> None:
+    """Raises ValueError for a ``backbone_type`` outside VIT_SHAPES or one that ``backbone`` is not released at."""
+    if backbone_type not in VIT_SHAPES:
+        raise ValueError(f"backbone_type '{backbone_type}' is not supported ({', '.join(VIT_SHAPES)})")
+    if backbone == "dino" and backbone_type not in DINO_V1_TYPES:
+        raise ValueError(f"backbone 'dino' has no '{backbone_type}' (DINO is released as {' and '.join(DINO_V1_TYPES)}); "
+                         f"pass backbone='dinov2' or backbone='dinov2_reg'")
 
 
 def synthetic_dino_state_dict(dim, depth, mlp_dim, patch_size, pretrain_grid, seed=1, attn_std=0.09):
@@ -95,11 +108,24 @@ def synthetic_dinov2_reg_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09, 
     return sd
 
 
-def check_backbone_family(sd: dict, backbone: str) -> dict:
+def _vit_size(dim: int, depth: int) -> str:
+    name = next((k for k, v in VIT_SHAPES.items() if (v["dim"], v["depth"]) == (dim, depth)), None)
+    return f"{name} (D = {dim}, {depth} blocks)" if name else f"D = {dim} with {depth} blocks"
+
+
+def check_backbone_family(sd: dict, backbone: str, backbone_type: str = None) -> dict:
     """Checks that a ViT state dict belongs to ``backbone`` ("dino": DINO v1, "dinov2": DINOv2 without registers,
-    "dinov2_reg": DINOv2 with register tokens) and returns it with the keys the backbone does not use dropped (DINOv2's
-    ``mask_token``).  Raises ValueError on a checkpoint of another family."""
+    "dinov2_reg": DINOv2 with register tokens) and, when ``backbone_type`` is given, has its width and depth; returns it
+    with the keys the backbone does not use dropped (DINOv2's ``mask_token``).  Raises ValueError on a checkpoint of
+    another family or size."""
     sd = {k.replace("module.", "").replace("backbone.", ""): v for k, v in sd.items()}
+    if backbone_type is not None:
+        shp = VIT_SHAPES[backbone_type]
+        dim = int(sd["patch_embed.proj.weight"].shape[0])
+        depth = len({k.split(".")[1] for k in sd if k.startswith("blocks.")})
+        if (dim, depth) != (shp["dim"], shp["depth"]):
+            raise ValueError(f"backbone_type '{backbone_type}' needs a {_vit_size(shp['dim'], shp['depth'])} checkpoint; "
+                             f"got {_vit_size(dim, depth)}")
     has_reg = "register_tokens" in sd
     has_ls = "blocks.0.ls1.gamma" in sd
     patch = int(sd["patch_embed.proj.weight"].shape[-1])
@@ -125,6 +151,7 @@ def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights
     """DINO (``backbone="dino"``), DINOv2 (``"dinov2"``) or DINOv2 with registers (``"dinov2_reg"``; both always patch
     14) weights, from ``pretrained_weights`` / ``$WVN_DINO_WEIGHTS`` or seeded.  A checkpoint is checked against the
     family (check_backbone_family)."""
+    check_backbone_type(backbone, backbone_type)
     shp = VIT_SHAPES[backbone_type]
     path = pretrained_weights or os.environ.get("WVN_DINO_WEIGHTS")
     if path:
@@ -133,7 +160,7 @@ def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights
             sd = sd["state_dict"]
         if "teacher" in sd:
             sd = sd["teacher"]
-        return check_backbone_family(sd, backbone)
+        return check_backbone_family(sd, backbone, backbone_type)
     warnings.warn(f"no {backbone.upper()} checkpoint given (pretrained_weights / $WVN_DINO_WEIGHTS): using seeded random "
                   f"{backbone.upper()}-style weights — fine for parity and throughput work, not for real traversability")
     if backbone == "dinov2":

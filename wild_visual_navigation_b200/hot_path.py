@@ -22,7 +22,10 @@ go to ``FeatureExtractor``); "random" and "none" are refused, because the node's
 unpicked pixels and a pixel-wise graph has one row per pixel.  ``feature_type="torchvision"`` with ``model_type``
 (resnet18, resnet50, resnet50_dino, efficientnet_b0) runs a feature pyramid.  Its weights come from
 ``backbone_state_dict`` or ``pretrained_weights``; ``state_dict`` / ``head_state_dict`` stay STEGO's DINO backbone and
-head, which segment the frames when ``segmentation_type="stego"`` (``FeatureExtractor``'s ``stego_state_dict``).
+head, which segment the frames when ``segmentation_type="stego"`` (``FeatureExtractor``'s ``stego_state_dict``).  ``feature_type="dinov2"`` /
+``"dinov2_reg"`` with ``backbone_type="vit_large"`` runs DINOv2 ViT-L/14 (1024-wide rows); ``state_dict`` is then its
+checkpoint, and with ``segmentation_type="stego"`` STEGO segments on a seeded DINO backbone of
+``stego_backbone_type`` ("vit_small" or "vit_base", whose width ``head_state_dict`` must match).
 
 ``prediction_per_pixel`` is the node's parameter of that name.  With False, or with a SimpleGCN, the maps are
 segment-wise (wvn_feature_extractor_node.py:323-338): each pooled row is evaluated once (padded-row inference with the
@@ -48,7 +51,8 @@ class HotPathStep:
                  run_clustering: bool = True, n_image_clusters: int = 20, process_group=None, feature_type: str = "dino",
                  model: str = "SimpleMLP", anomaly_detection: bool = False, segmentation_type: str = "stego",
                  prediction_per_pixel: bool = True, model_type: str = None, backbone_state_dict=None,
-                 pretrained_weights: str = None, slic_num_components: int = 100, cell_size: int = 32):
+                 pretrained_weights: str = None, slic_num_components: int = 100, cell_size: int = 32,
+                 stego_backbone_type: str = None):
         if segmentation_type not in SEGMENTATION_TYPES:
             raise ValueError(f"HotPathStep: segmentation_type must be one of {SEGMENTATION_TYPES}, got "
                              f"{segmentation_type!r}")
@@ -67,7 +71,8 @@ class HotPathStep:
         self.per_pixel = prediction_per_pixel
         fe_args = dict(head_state_dict=head_state_dict, flip_tta=flip_tta, run_clustering=run_clustering,
                        n_image_clusters=n_image_clusters, max_batch=batch, chunk=chunk, backbone_type=backbone_type,
-                       patch_size=patch_size, slic_num_components=slic_num_components, cell_size=cell_size)
+                       patch_size=patch_size, slic_num_components=slic_num_components, cell_size=cell_size,
+                       stego_backbone_type=stego_backbone_type)
         if pyramid:   # the trunk's own weights; STEGO (when it segments) keeps state_dict
             fe_args.update(model_type=model_type, state_dict=backbone_state_dict, pretrained_weights=pretrained_weights,
                            stego_state_dict=state_dict)
