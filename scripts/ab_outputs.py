@@ -10,8 +10,14 @@ output its SHA-256 plus a strided sample (every 101st element, as float32):
     backbone: QKV (bf16), attention out-projection (fp32 residual add), fc1 (bf16 + GELU), fc2 (fp32 residual add);
   * DinoInterface tokens of ViT-S/8 @448 at B = 32;
   * the fused per-pixel traversability / confidence maps of a seeded SimpleMLP on those tokens;
+  * the fused per-pixel maps of a seeded DoubleMLP(384, [64, 32, 1]) on the first 8 frames of those tokens, from the
+    fp32 tokens (MlpInference.pixels) and from the backbone's own bf16 copy (MlpInference.pixels_from_vit);
   * DinoInterface tokens of ViT-S/16 @448 at B = 8 (the patch-16 loader and patch-embed GEMM);
+  * the taps of seeded ResNet-18, ResNet-50 and EfficientNet-B0 trunks at 448, B = 4;
+  * DinoInterface tokens of DINOv2 ViT-S/14-reg and ViT-L/14 @224 at B = 4;
+  * StegoInterface (ViT-S/8 @224, B = 4, flip TTA): the flip-averaged head output and the linear / cluster segments;
   * ops.mlp_forward_f32 of that SimpleMLP at R = 4096 and 65536 rows;
+  * MlpInference.rows_padded of that SimpleMLP and of the DoubleMLP (6 groups of 700 rows, partly live);
   * FlowInference.rows (z, log_det, logprob) of a seeded LinearRnvp(384, [200]) at R = 4096;
   * after three train steps of each learner (MlpTrainer, DoubleMlpTrainer, GcnTrainer, FlowTrainer) created for
     1024 rows, at R = 1024, 800 and 1500 (the last one replaces the handle by a larger one and copies its generator
@@ -102,6 +108,19 @@ def write(out_dir):
     trav, conf = TraversabilityInference(di, model, cg).predict_from_tokens(tokens, 448)
     _record(out_dir, "pixel_trav", trav, index)
     _record(out_dir, "pixel_conf", conf, index)
+
+    from wild_visual_navigation_b200 import DoubleMLP
+
+    torch.manual_seed(42)
+    double = DoubleMLP(384, [64, 32, 1]).to(dev)
+    dmi = ops.MlpInference(384, 64, 32, double=True)
+    dmi.set_params(double.flat_params)
+    for name, (t, c) in {
+        "pixels": dmi.pixels(tokens[:8].contiguous(), (56, 56), (448, 448), cg.mean, cg.std, 0.5),
+        "pixels_vit": dmi.pixels_from_vit(di._model, 8, (448, 448), cg.mean, cg.std, 0.5),
+    }.items():
+        _record(out_dir, f"double_mlp_{name}_trav", t, index)
+        _record(out_dir, f"double_mlp_{name}_conf", c, index)
     del di, tokens
     torch.cuda.empty_cache()
 
@@ -113,11 +132,60 @@ def write(out_dir):
     del di16
     torch.cuda.empty_cache()
 
+    # ---- the convolutional trunks: ResNet-18 / ResNet-50 and EfficientNet-B0 taps @448, B = 4
+    from wild_visual_navigation_b200.feature_extractor import weights as W
+
+    for depth in (18, 50):
+        rn = ops.ResNetBackbone(448, depth, W.fold_resnet_bn(W.synthetic_resnet_state_dict(depth, seed=1), depth),
+                                max_batch=4)
+        for i, t in enumerate(rn.forward(img[:4])):
+            _record(out_dir, f"resnet{depth}_tap{i + 1}", t, index)
+        del rn
+    en = ops.EfficientNetBackbone(448, W.fold_efficientnet_bn(W.synthetic_efficientnet_b0_state_dict(seed=1)),
+                                  max_batch=4)
+    for i, t in enumerate(en.forward(img[:4])):
+        _record(out_dir, f"effnet_b0_tap{i + 1}", t, index)
+    del en
+    torch.cuda.empty_cache()
+
+    # ---- DINOv2 ViT-S/14-reg and ViT-L/14 tokens @224, B = 4
+    img224 = torch.rand(4, 3, 224, 224, generator=torch.Generator().manual_seed(1)).to(dev)
+    for name, backbone, vit_type in (("dinov2_reg_s14", "dinov2_reg", "vit_small"), ("dinov2_l14", "dinov2", "vit_large")):
+        s = W.VIT_SHAPES[vit_type]
+        make = W.synthetic_dinov2_reg_state_dict if backbone == "dinov2_reg" else W.synthetic_dinov2_state_dict
+        dv = DinoInterface(dev, backbone=backbone, input_size=224, backbone_type=vit_type,
+                           state_dict=make(s["dim"], s["depth"], s["mlp_dim"], seed=5), max_batch=4)
+        _record(out_dir, f"{name}_tokens", dv.inference_tokens(img224), index)
+        del dv
+        torch.cuda.empty_cache()
+
+    # ---- the STEGO head with flip TTA (ViT-S/8 @224, B = 4) and its segments
+    from wild_visual_navigation_b200.feature_extractor import StegoInterface
+
+    si = StegoInterface(dev, input_size=224, backbone_type="vit_small", patch_size=8, flip_tta=True, max_batch=4,
+                        backbone_state_dict=synthetic_state_dict(ViTConfig.from_name("vit_small", 8, 224), seed=6),
+                        head_state_dict=W.synthetic_stego_head(384, 90, 32, 27, seed=3))
+    linear, cluster = si.inference(img224)
+    _record(out_dir, "stego_head_tta", si._head_out, index)
+    _record(out_dir, "stego_linear_segments", linear, index)
+    _record(out_dir, "stego_cluster_segments", cluster, index)
+    del si
+    torch.cuda.empty_cache()
+
     # ---- the fp32 CUDA-core paths: SimpleMLP forward, LinearRnvp row forward and train step
     g = torch.Generator(device=dev).manual_seed(13)
     for R in (4096, 65536):
         x = torch.randn(R, 384, device=dev, generator=g) * 0.5
         _record(out_dir, f"mlp_forward_f32_{R}", ops.mlp_forward_f32(model.flat_params, x, 384, 256, 32), index)
+
+    feat = torch.randn(6, 700, 384, device=dev, generator=g) * 0.5
+    n_rows = torch.tensor([700, 0, 1, 350, 699, 128], device=dev, dtype=torch.int32)
+    for name, (m, mi) in {"mlp": (model, ops.MlpInference(384, 256, 32)),
+                          "double_mlp": (double, ops.MlpInference(384, 64, 32, double=True))}.items():
+        mi.set_params(m.flat_params)
+        t, c = mi.rows_padded(feat, n_rows, cg.mean, cg.std, 0.5)
+        _record(out_dir, f"{name}_rows_padded_trav", t, index)
+        _record(out_dir, f"{name}_rows_padded_conf", c, index)
 
     from wild_visual_navigation_b200 import LinearRnvp
 
@@ -129,7 +197,7 @@ def write(out_dir):
         _record(out_dir, f"flow_rows_{k}", rows[k], index)
 
     # ---- the four learners' train steps, with a regrowth in the last step
-    from wild_visual_navigation_b200 import DoubleMLP, SimpleGCN
+    from wild_visual_navigation_b200 import SimpleGCN
 
     def learner(kind):
         torch.manual_seed(42)

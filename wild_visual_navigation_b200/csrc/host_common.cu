@@ -1,13 +1,33 @@
-// wvn-b200: host-side helpers (error string, tensor-map encoding).
+// wvn-b200: host-side helpers (error string, tensor-map encoding, device buffers, weight stores).
 #include "host_common.h"
 
+#include <cuda_bf16.h>
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <mutex>
 #include <vector>
+
+#include "gemm.h"
+
+namespace {
+
+// fp32 rows [rows, dim] -> bf16 rows [rows, ld] (padding columns left untouched = zero)
+__global__ void cast_rows_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long rows, int dim,
+                                 long long ld) {
+  const long long n = rows * dim;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long r = i / dim;
+    const int c = static_cast<int>(i - r * dim);
+    dst[r * ld + c] = __float2bfloat16_rn(src[i]);
+  }
+}
+
+}  // namespace
 
 namespace wvn {
 
@@ -149,6 +169,87 @@ int prof_collect(float* ms_by_cat, long long* launches_by_cat) {
     g_pool.push_back(r.b);
   }
   g_prof.clear();
+  return WVN_OK;
+}
+
+int cast_rows_to_bf16(const float* src, void* dst, long long rows, int dim, long long ld, int max_blocks,
+                      cudaStream_t s) {
+  const int blocks = static_cast<int>(std::min<long long>((rows * dim + 255) / 256, max_blocks));
+  cast_rows_kernel<<<blocks, 256, 0, s>>>(src, reinterpret_cast<__nv_bfloat16*>(dst), rows, dim, ld);
+  WVN_CHECK_LAUNCH("cast_rows_kernel");
+  return WVN_OK;
+}
+
+int DevBuf::alloc(size_t n) {
+  release();
+  void* q = nullptr;
+  WVN_CHECK_CUDA(cudaMalloc(&q, n ? n : 1));
+  p = q;
+  bytes = n;
+  WVN_CHECK_CUDA(cudaMemset(p, 0, n ? n : 1));
+  return WVN_OK;
+}
+
+void DevBuf::release() {
+  if (p) cudaFree(p);
+  p = nullptr;
+  bytes = 0;
+}
+
+constexpr size_t kStageBytes = 8u << 20;
+
+int WeightStore::add(const std::string& name, long long rows, int cols, bool bf16) {
+  if (!stage.p) WVN_PROPAGATE(stage.alloc(kStageBytes));
+  const long long ld = bf16 ? gemm_w_pitch(cols) : cols;
+  Weight& wt = w[name];
+  WVN_PROPAGATE(wt.buf.alloc(static_cast<size_t>(rows * ld) * (bf16 ? 2 : 4)));
+  wt.numel = rows * cols;
+  wt.bf16 = bf16;
+  wt.cols = cols;
+  wt.ld = static_cast<int>(ld);
+  return WVN_OK;
+}
+
+int WeightStore::set(const char* name, const float* data, long long numel) {
+  auto it = w.find(name);
+  WVN_REQUIRE(it != w.end(), "set_weight: unknown weight '%s'", name);
+  Weight& wt = it->second;
+  WVN_REQUIRE(wt.numel == numel, "set_weight: '%s' expects %lld elements, got %lld", name, wt.numel, numel);
+  cudaPointerAttributes attr;
+  bool on_device = false;
+  if (cudaPointerGetAttributes(&attr, data) == cudaSuccess)
+    on_device = (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+  else
+    cudaGetLastError();
+  // fp32 destination: copy straight in; bf16 destination: stage (if host) + cast on device
+  if (!wt.bf16) {
+    WVN_CHECK_CUDA(
+        cudaMemcpy(wt.buf.p, data, numel * 4, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+  } else {
+    // stage whole rows, cast each into its row of the pitched storage
+    const long long chunk_rows = static_cast<long long>(stage.bytes / 4) / wt.cols;
+    const long long rows = numel / wt.cols;
+    for (long long r0 = 0; r0 < rows; r0 += chunk_rows) {
+      const long long n = std::min(chunk_rows, rows - r0);
+      const float* src = data + r0 * wt.cols;
+      if (!on_device) {
+        WVN_CHECK_CUDA(cudaMemcpy(stage.p, src, n * wt.cols * 4, cudaMemcpyHostToDevice));
+        src = reinterpret_cast<const float*>(stage.p);
+      }
+      WVN_PROPAGATE(cast_rows_to_bf16(src, reinterpret_cast<__nv_bfloat16*>(wt.buf.p) + r0 * wt.ld, n, wt.cols, wt.ld,
+                                      4096, 0));
+      WVN_CHECK_CUDA(cudaStreamSynchronize(0));
+    }
+  }
+  wt.loaded = true;
+  return WVN_OK;
+}
+
+int WeightStore::check_loaded(const char* what, const char* skip_prefix) const {
+  for (auto& kv : w) {
+    if (skip_prefix && kv.first.rfind(skip_prefix, 0) == 0) continue;
+    if (!kv.second.loaded) return set_error(WVN_ERR_STATE, "%s: weight '%s' was never set", what, kv.first.c_str());
+  }
   return WVN_OK;
 }
 

@@ -1,10 +1,14 @@
 // wvn-b200: host-side helpers shared by the translation units of libwvn_b200.so
-// (error reporting, TMA tensor-map encoding through the driver entry point).
+// (error reporting, TMA tensor-map encoding through the driver entry point, device buffers, weight stores).
 #pragma once
 
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
+
+#include <map>
+#include <string>
 
 namespace wvn {
 
@@ -70,5 +74,56 @@ void prof_begin(int cat, cudaStream_t s);
 void prof_end(int cat, cudaStream_t s);
 // Synchronises, sums elapsed ms per category, clears the record list.
 int prof_collect(float* ms_by_cat, long long* launches_by_cat);
+
+inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
+
+// fp32 rows [rows, dim] -> bf16 rows `ld` apart on the device (the pad columns are left untouched), in at most
+// `max_blocks` blocks of 256 threads.
+int cast_rows_to_bf16(const float* src, void* dst, long long rows, int dim, long long ld, int max_blocks,
+                      cudaStream_t s);
+
+// Device memory that frees itself.  alloc() zero-fills (pitched rows rely on their pad columns being zero) and frees
+// what the buffer held before.
+struct DevBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+  ~DevBuf() { release(); }
+  int alloc(size_t n);
+
+ private:
+  void release();
+};
+
+// A handle's named weights: device storage sized at create, filled by set() from fp32 host or device data.
+struct WeightStore {
+  struct Weight {
+    DevBuf buf;            // fp32 dense, or bf16 rows of `cols` elements stored `ld` apart (pad columns zero)
+    long long numel = 0;
+    bool bf16 = false;
+    bool loaded = false;
+    int cols = 0, ld = 0;
+  };
+  std::map<std::string, Weight> w;
+  DevBuf stage;            // host data on its way to a bf16 weight
+
+  // `rows` x `cols` elements; bf16 rows are stored at the GEMM's W pitch gemm_w_pitch(cols)
+  int add(const std::string& name, long long rows, int cols, bool bf16);
+  // Copies fp32 `data` (host or device): fp32 storage as is, bf16 storage cast on the device into its pitched rows,
+  // through `stage` when the source is host memory.
+  int set(const char* name, const float* data, long long numel);
+  // null for a name that was never added
+  template <class T>
+  T* ptr(const std::string& name) const {
+    auto it = w.find(name);
+    return it == w.end() ? nullptr : reinterpret_cast<T*>(it->second.buf.p);
+  }
+  // WVN_ERR_STATE naming the first weight never set; names starting with `skip_prefix` (when given) are not checked
+  int check_loaded(const char* what, const char* skip_prefix = nullptr) const;
+};
 
 }  // namespace wvn

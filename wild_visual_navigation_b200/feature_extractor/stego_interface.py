@@ -2,7 +2,7 @@
 
 ``inference(img) -> (linear_pred, cluster_pred)`` with the ``features`` / ``cluster_segments`` /
 ``linear_segments`` properties.  The STEGO head runs as three wgmma GEMMs on the ViT tokens
-(csrc/api.cu: wvn_vit_stego_head); the cluster / linear probes are folded into the head's output
+(csrc/vit_backbone.cu: vit_stego_head); the cluster / linear probes are folded into the head's output
 columns (weights.fold_stego_head) and evaluated at patch resolution, then one kernel does the
 bilinear(align_corners=False) upsampling + argmax per pixel — algebraically the upstream
 ``postprocess`` (upsample the 90-d code, then probe every pixel) without the 448x448x90 tensor.
