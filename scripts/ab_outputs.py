@@ -12,12 +12,15 @@ output its SHA-256 plus a strided sample (every 101st element, as float32):
   * the fused per-pixel traversability / confidence maps of a seeded SimpleMLP on those tokens;
   * the fused per-pixel maps of a seeded DoubleMLP(384, [64, 32, 1]) on the first 8 frames of those tokens, from the
     fp32 tokens (MlpInference.pixels) and from the backbone's own bf16 copy (MlpInference.pixels_from_vit);
+  * FlowInference.pixels (traversability and NLL) of a seeded LinearRnvp(384, [200]) on those tokens;
   * DinoInterface tokens of ViT-S/16 @448 at B = 8 (the patch-16 loader and patch-embed GEMM);
   * the taps of seeded ResNet-18, ResNet-50 and EfficientNet-B0 trunks at 448, B = 4;
   * DinoInterface tokens of DINOv2 ViT-S/14-reg and ViT-L/14 @224 at B = 4;
   * StegoInterface (ViT-S/8 @224, B = 4, flip TTA): the flip-averaged head output and the linear / cluster segments;
+  * DenseCrf.run on that head output (cluster-probe labels and Q, linear-probe labels) and DenseCrf.workspace_bytes;
   * ops.mlp_forward_f32 of that SimpleMLP at R = 4096 and 65536 rows;
   * MlpInference.rows_padded of that SimpleMLP and of the DoubleMLP (6 groups of 700 rows, partly live);
+  * GcnInference.rows_padded of a seeded SimpleGCN(384, True, [256, 128, 1]) on the same rows with seeded edges;
   * FlowInference.rows (z, log_det, logprob) of a seeded LinearRnvp(384, [200]) at R = 4096;
   * after three train steps of each learner (MlpTrainer, DoubleMlpTrainer, GcnTrainer, FlowTrainer) created for
     1024 rows, at R = 1024, 800 and 1500 (the last one replaces the handle by a larger one and copies its generator
@@ -121,7 +124,17 @@ def write(out_dir):
     }.items():
         _record(out_dir, f"double_mlp_{name}_trav", t, index)
         _record(out_dir, f"double_mlp_{name}_conf", c, index)
-    del di, tokens
+
+    from wild_visual_navigation_b200 import LinearRnvp
+
+    torch.manual_seed(42)
+    flow = LinearRnvp(384, [200], use_permutation=True).to(dev)
+    fi = ops.FlowInference(384, 200)
+    fi.set_params(flow.flat_params)
+    t, nll = fi.pixels(flow, tokens, (56, 56), (448, 448), cg.mean, cg.std, 0.5, want_nll=True)
+    _record(out_dir, "flow_pixels_trav", t, index)
+    _record(out_dir, "flow_pixels_nll", nll, index)
+    del di, tokens, fi
     torch.cuda.empty_cache()
 
     # ---- the patch-16 loader and patch-embed GEMM (K = 768): DINO ViT-S/16 @448, B = 8
@@ -169,7 +182,16 @@ def write(out_dir):
     _record(out_dir, "stego_head_tta", si._head_out, index)
     _record(out_dir, "stego_linear_segments", linear, index)
     _record(out_dir, "stego_cluster_segments", cluster, index)
-    del si
+    _, _, npad, grid, _ = si._geom
+    crf = ops.DenseCrf(224, max(si._n_clusters, si._n_classes), chunk=2)
+    _record(out_dir, "crf_workspace_bytes", torch.tensor([crf.workspace_bytes], dtype=torch.int64), index)
+    labels, q = crf.run(img224, si._head_out, npad, grid, W.HEAD_CLUSTER_COL, si._n_clusters, W.HEAD_CODE_COL,
+                        si._code_dim, 2.0, want_q=True)
+    _record(out_dir, "crf_cluster_labels", labels, index)
+    _record(out_dir, "crf_cluster_q", q, index)
+    _record(out_dir, "crf_linear_labels", crf.run(img224, si._head_out, npad, grid, W.HEAD_LINEAR_COL, si._n_classes),
+            index)
+    del si, crf
     torch.cuda.empty_cache()
 
     # ---- the fp32 CUDA-core paths: SimpleMLP forward, LinearRnvp row forward and train step
@@ -187,18 +209,23 @@ def write(out_dir):
         _record(out_dir, f"{name}_rows_padded_trav", t, index)
         _record(out_dir, f"{name}_rows_padded_conf", c, index)
 
-    from wild_visual_navigation_b200 import LinearRnvp
+    from wild_visual_navigation_b200 import SimpleGCN
 
     torch.manual_seed(42)
-    flow = LinearRnvp(384, [200], use_permutation=True).to(dev)
+    gcn = SimpleGCN(384, True, [256, 128, 1]).to(dev)
+    edges = torch.randint(0, 700, (6, 2100, 2), device=dev, generator=g)
+    n_edges = torch.tensor([2100, 0, 5, 1000, 2100, 300], device=dev, dtype=torch.int32)
+    t, c = ops.GcnInference(gcn, max_rows=6 * 700, max_edges=6 * 2100).rows_padded(feat, n_rows, edges, n_edges, cg.mean,
+                                                                                   cg.std, 0.5)
+    _record(out_dir, "gcn_rows_padded_trav", t, index)
+    _record(out_dir, "gcn_rows_padded_conf", c, index)
+
     x = torch.randn(4096, 384, device=dev, generator=g) * 0.5
     rows = ops.FlowInference(384, 200, max_rows=4096).rows(flow, x)
     for k in ("z", "log_det", "logprob"):
         _record(out_dir, f"flow_rows_{k}", rows[k], index)
 
     # ---- the four learners' train steps, with a regrowth in the last step
-    from wild_visual_navigation_b200 import SimpleGCN
-
     def learner(kind):
         torch.manual_seed(42)
         if kind == "mlp":

@@ -273,26 +273,14 @@ int wvn_slic_geometry(int h, int w, int num_components, int* grid_interval, int*
   return WVN_OK;
 }
 
-struct wvn_crf {
-  DenseCrf* crf = nullptr;
-};
-
 int wvn_crf_create(int size, int max_classes, int chunk, int iterations, wvn_crf_t** out) {
   WVN_REQUIRE(out, "wvn_crf_create: null argument");
   WVN_PROPAGATE(wvn_check_device());
-  DenseCrf* c = nullptr;
-  WVN_PROPAGATE(crf_create(size, max_classes, chunk, iterations, &c));
-  *out = new wvn_crf{c};
-  return WVN_OK;
+  return crf_create(size, max_classes, chunk, iterations, out);
 }
 
-void wvn_crf_destroy(wvn_crf_t* h) {
-  if (!h) return;
-  crf_destroy(h->crf);
-  delete h;
-}
-
-size_t wvn_crf_workspace_bytes(const wvn_crf_t* h) { return h ? crf_workspace_bytes(h->crf) : 0; }
+void wvn_crf_destroy(wvn_crf_t* h) { crf_destroy(h); }
+size_t wvn_crf_workspace_bytes(const wvn_crf_t* h) { return crf_workspace_bytes(h); }
 
 static CrfInput crf_input(const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w) {
   CrfInput in;
@@ -308,24 +296,24 @@ int wvn_crf_run(wvn_crf_t* h, const void* img, int u8_hwc, int batch, int in_h, 
   CrfInput in = crf_input(img, u8_hwc, batch, in_h, in_w, resized_h, resized_w);
   in.head = head; in.ld = ld; in.npad = npad; in.grid = grid; in.col0 = col0; in.classes = classes;
   in.code_col = code_col; in.code_dim = code_dim; in.logit_scale = logit_scale;
-  return crf_run(h->crf, in, labels, q_out, S(stream));
+  return crf_run(h, in, labels, q_out, S(stream));
 }
 
 int wvn_crf_build(wvn_crf_t* h, const void* img, int u8_hwc, int batch, int in_h, int in_w, int resized_h, int resized_w,
                   void* stream) {
   WVN_REQUIRE(h, "wvn_crf_build: null handle");
-  return crf_build(h->crf, crf_input(img, u8_hwc, batch, in_h, in_w, resized_h, resized_w), S(stream));
+  return crf_build(h, crf_input(img, u8_hwc, batch, in_h, in_w, resized_h, resized_w), S(stream));
 }
 
 int wvn_crf_filter(wvn_crf_t* h, int which, const float* values, int v, float* out, void* stream) {
   WVN_REQUIRE(h, "wvn_crf_filter: null handle");
-  return crf_filter(h->crf, which, values, v, out, S(stream));
+  return crf_filter(h, which, values, v, out, S(stream));
 }
 
 int wvn_crf_export(wvn_crf_t* h, int which, unsigned long long* keys, int* counts, int* offsets, float* bary, int* m,
                    void* stream) {
   WVN_REQUIRE(h, "wvn_crf_export: null handle");
-  return crf_export(h->crf, which, keys, counts, offsets, bary, m, S(stream));
+  return crf_export(h, which, keys, counts, offsets, bary, m, S(stream));
 }
 
 size_t wvn_slic_workspace_bytes(int batch, int h, int w, int num_components) {
@@ -698,14 +686,8 @@ int wvn_gcn_infer_rows(wvn_trainer_t* t, const float* params, const float* x, in
 }  // extern "C"
 
 // ============================================================================================
-// LinearRnvp flow: fp32 row forward and online train step (flow_train.cu)
+// LinearRnvp flow: fp32 row forward, online train step and the inference handle (flow_train.cu)
 // ============================================================================================
-// inference only: the fp32 row forward (forward workspaces only) and the per-pixel wgmma path
-struct wvn_flow_infer {
-  Trainer* rows = nullptr;
-  FlowPixels* pix = nullptr;
-};
-
 namespace {
 FlowBuffers buffers_of(const wvn_flow_buffers* b) {
   FlowBuffers f;
@@ -760,51 +742,38 @@ int wvn_flow_infer_create(int dim, int hidden, int max_rows, int chunk_pixels, w
   WVN_PROPAGATE(wvn_check_device());
   FlowShape s;
   s.dim = dim; s.hidden = hidden;
-  wvn_flow_infer* h = new wvn_flow_infer();
-  int rc = flow_trainer_create(s, max_rows, 0.5f, AdamCfg(), nullptr, true, &h->rows);
-  if (rc == WVN_OK) rc = flow_pixels_create(s, chunk_pixels, &h->pix);
-  if (rc != WVN_OK) {
-    wvn_flow_infer_destroy(h);
-    return rc;
-  }
-  *out = h;
-  return WVN_OK;
+  return flow_infer_create(s, max_rows, chunk_pixels, out);
 }
 
-void wvn_flow_infer_destroy(wvn_flow_infer_t* h) {
-  if (!h) return;
-  delete h->rows;
-  flow_pixels_destroy(h->pix);
-  delete h;
-}
+void wvn_flow_infer_destroy(wvn_flow_infer_t* h) { flow_infer_destroy(h); }
 
 int wvn_flow_infer_set_params(wvn_flow_infer_t* h, const float* params, void* stream) {
   WVN_REQUIRE(h, "wvn_flow_infer_set_params: null handle");
-  return flow_pixels_set_params(h->pix, params, S(stream));
+  return flow_infer_set_params(h, params, S(stream));
 }
 
 int wvn_flow_infer_rows(wvn_flow_infer_t* h, const float* params, const wvn_flow_buffers* buffers, const float* x, int rows,
                         float* z, float* log_det, float* logprob, const float* cg_mean, const float* cg_std,
                         float std_factor, float* trav, void* stream) {
   WVN_REQUIRE(h && buffers, "wvn_flow_infer_rows: null argument");
-  return flow_forward_rows(h->rows, params, buffers_of(buffers), x, rows, z, log_det, logprob, cg_mean, cg_std,
-                           std_factor, trav, S(stream));
+  return flow_forward_rows(flow_infer_trainer(h), params, buffers_of(buffers), x, rows, z, log_det, logprob, cg_mean,
+                           cg_std, std_factor, trav, S(stream));
 }
 
 int wvn_flow_infer_rows_padded(wvn_flow_infer_t* h, const float* params, const wvn_flow_buffers* buffers, const float* x,
                                int groups, int rows_per_group, const int* n_rows, const float* cg_mean,
                                const float* cg_std, float std_factor, float* trav, void* stream) {
   WVN_REQUIRE(h && buffers, "wvn_flow_infer_rows_padded: null argument");
-  return flow_forward_rows_padded(h->rows, params, buffers_of(buffers), x, groups, rows_per_group, n_rows, cg_mean,
-                                  cg_std, std_factor, trav, S(stream));
+  return flow_forward_rows_padded(flow_infer_trainer(h), params, buffers_of(buffers), x, groups, rows_per_group, n_rows,
+                                  cg_mean, cg_std, std_factor, trav, S(stream));
 }
 
 int wvn_flow_infer_pixels(wvn_flow_infer_t* h, const wvn_flow_buffers* buffers, const float* tokens, int batch, int gh,
                           int gw, int out_h, int out_w, const float* cg_mean, const float* cg_std, float std_factor,
                           float* trav, float* nll, void* stream) {
   WVN_REQUIRE(h && buffers, "wvn_flow_infer_pixels: null argument");
-  return flow_pixels_run(h->pix, buffers_of(buffers), tokens, batch, gh, gw, out_h, out_w, cg_mean, cg_std, std_factor,
-                         trav, nll, S(stream));
+  return flow_infer_pixels(h, buffers_of(buffers), tokens, batch, gh, gw, out_h, out_w, cg_mean, cg_std, std_factor,
+                           trav, nll, S(stream));
 }
 
 }  // extern "C"

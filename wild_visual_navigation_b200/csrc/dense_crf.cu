@@ -20,6 +20,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <memory>
 
 #include "host_common.h"
 
@@ -42,11 +43,12 @@ struct LatticeBufs {
   float scale[5] = {};
 };
 
-struct DenseCrf {
+}  // namespace wvn
+
+struct wvn_crf {
   int S = 0, N = 0, K = 0, chunk = 0, iters = 0;
-  size_t bytes = 0;
-  void* base = nullptr;
-  LatticeBufs lat[2];
+  wvn::DevBuf arena;
+  wvn::LatticeBufs lat[2];
   unsigned long long *keys_in = nullptr, *keys_out = nullptr;
   int *vals_in = nullptr, *scan = nullptr, *m = nullptr;  // m[2]: vertex counts
   float *va = nullptr, *vb = nullptr;                    // [entries_max * K] vertex values, double-buffered
@@ -56,6 +58,8 @@ struct DenseCrf {
   size_t cub_bytes = 0;
   int frames = 0;                                        // frames of the chunk whose lattices are built
 };
+
+namespace wvn {
 
 namespace {
 
@@ -504,13 +508,13 @@ double key_bound(int d, const float* scale, const double* fmax) {
 
 }  // namespace
 
-int crf_create(int size, int max_classes, int chunk, int iterations, DenseCrf** out) {
+int crf_create(int size, int max_classes, int chunk, int iterations, wvn_crf** out) {
   WVN_REQUIRE(out, "wvn_crf_create: null argument");
   WVN_REQUIRE(size >= 2 && size <= 4096, "wvn_crf_create: size %d outside [2, 4096]", size);
   WVN_REQUIRE(max_classes >= 1 && max_classes <= 64, "wvn_crf_create: classes %d outside [1, 64]", max_classes);
   WVN_REQUIRE(chunk >= 1 && chunk <= 256, "wvn_crf_create: chunk %d outside [1, 256]", chunk);
   WVN_REQUIRE(iterations >= 0, "wvn_crf_create: negative iteration count");
-  DenseCrf* h = new DenseCrf();
+  std::unique_ptr<wvn_crf> h(new wvn_crf());
   h->S = size; h->N = size * size; h->K = max_classes; h->chunk = chunk; h->iters = iterations;
   const long long npix = static_cast<long long>(chunk) * h->N;
   const int dims[2] = {2, 5};
@@ -525,32 +529,14 @@ int crf_create(int size, int max_classes, int chunk, int iterations, DenseCrf** 
     L.weight = l == 0 ? 3.f : 4.f;
     double fmax[5] = {(size - 1) / L.feat_div[0], (size - 1) / L.feat_div[0], 85.0, 85.0, 85.0};
     const int bits = key_bits(L.d);
-    if (key_bound(L.d, L.scale, fmax) >= (1 << (bits - 1)) || (chunk - 1) >= (1ll << (64 - bits * L.d))) {
-      delete h;
+    if (key_bound(L.d, L.scale, fmax) >= (1 << (bits - 1)) || (chunk - 1) >= (1ll << (64 - bits * L.d)))
       return set_error(WVN_ERR_INVALID, "wvn_crf_create: size %d / chunk %d overflow the %d-bit lattice keys", size,
                        chunk, bits);
-    }
   }
   const long long emax = h->lat[1].entries;
-  if (emax >= (1ll << 31)) {
-    delete h;
+  if (emax >= (1ll << 31))
     return set_error(WVN_ERR_INVALID, "wvn_crf_create: chunk %d of %dx%d frames exceeds 2^31 lattice entries", chunk,
                      size, size);
-  }
-  // one allocation, carved below
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~static_cast<size_t>(255); return o; };
-  size_t o_keys_in = take(8 * emax), o_keys_out = take(8 * emax), o_vals = take(4 * emax), o_scan = take(4 * emax);
-  size_t o_m = take(4 * 2);
-  size_t o_va = take(4 * emax * h->K), o_vb = take(4 * emax * h->K);
-  size_t o_U = take(4 * npix * h->K), o_Q = take(4 * npix * h->K), o_acc = take(4 * npix * h->K);
-  size_t o_bgr = take(4 * npix);
-  size_t o_lat[2][7];
-  for (int l = 0; l < 2; ++l) {
-    const long long e = h->lat[l].entries;
-    o_lat[l][0] = take(4 * e); o_lat[l][1] = take(4 * e); o_lat[l][2] = take(4 * e); o_lat[l][3] = take(4 * (e + 1));
-    o_lat[l][4] = take(8 * e); o_lat[l][5] = take(8 * e * (h->lat[l].d + 1)); o_lat[l][6] = take(4 * npix);
-  }
   size_t sort_bytes = 0, scan_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, static_cast<unsigned long long*>(nullptr),
                                   static_cast<unsigned long long*>(nullptr), static_cast<int*>(nullptr),
@@ -558,57 +544,42 @@ int crf_create(int size, int max_classes, int chunk, int iterations, DenseCrf** 
   cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, static_cast<int*>(nullptr), static_cast<int*>(nullptr),
                                 static_cast<int>(emax));
   h->cub_bytes = std::max(sort_bytes, scan_bytes);
-  size_t o_cub = take(h->cub_bytes);
-  h->bytes = off;
-  cudaError_t e = cudaMalloc(&h->base, off);
-  if (e != cudaSuccess) {
-    delete h;
-    return set_error(WVN_ERR_CUDA, "wvn_crf_create: cudaMalloc of %zu bytes failed: %s", off, cudaGetErrorString(e));
-  }
-  e = cudaMemset(h->base, 0, off);
-  if (e != cudaSuccess) {
-    crf_destroy(h);
-    return set_error(WVN_ERR_CUDA, "wvn_crf_create: cudaMemset failed: %s", cudaGetErrorString(e));
-  }
-  char* b = static_cast<char*>(h->base);
-  h->keys_in = reinterpret_cast<unsigned long long*>(b + o_keys_in);
-  h->keys_out = reinterpret_cast<unsigned long long*>(b + o_keys_out);
-  h->vals_in = reinterpret_cast<int*>(b + o_vals);
-  h->scan = reinterpret_cast<int*>(b + o_scan);
-  h->m = reinterpret_cast<int*>(b + o_m);
-  h->va = reinterpret_cast<float*>(b + o_va);
-  h->vb = reinterpret_cast<float*>(b + o_vb);
-  h->U = reinterpret_cast<float*>(b + o_U);
-  h->Q = reinterpret_cast<float*>(b + o_Q);
-  h->acc = reinterpret_cast<float*>(b + o_acc);
-  h->bgr = reinterpret_cast<uchar4*>(b + o_bgr);
-  h->cub_tmp = b + o_cub;
-  for (int l = 0; l < 2; ++l) {
-    LatticeBufs& L = h->lat[l];
-    L.bary = reinterpret_cast<float*>(b + o_lat[l][0]);
-    L.offs = reinterpret_cast<int*>(b + o_lat[l][1]);
-    L.sorted = reinterpret_cast<int*>(b + o_lat[l][2]);
-    L.start = reinterpret_cast<int*>(b + o_lat[l][3]);
-    L.ukeys = reinterpret_cast<unsigned long long*>(b + o_lat[l][4]);
-    L.nbr = reinterpret_cast<int2*>(b + o_lat[l][5]);
-    L.norm = reinterpret_cast<float*>(b + o_lat[l][6]);
-  }
-  *out = h;
+  WVN_PROPAGATE(carve(&h->arena, [&](Carver& a) {
+    h->keys_in = a.take<unsigned long long>(emax);
+    h->keys_out = a.take<unsigned long long>(emax);
+    h->vals_in = a.take<int>(emax);
+    h->scan = a.take<int>(emax);
+    h->m = a.take<int>(2);
+    h->va = a.take<float>(emax * h->K);
+    h->vb = a.take<float>(emax * h->K);
+    h->U = a.take<float>(npix * h->K);
+    h->Q = a.take<float>(npix * h->K);
+    h->acc = a.take<float>(npix * h->K);
+    h->bgr = a.take<uchar4>(npix);
+    for (int l = 0; l < 2; ++l) {
+      LatticeBufs& L = h->lat[l];
+      L.bary = a.take<float>(L.entries);
+      L.offs = a.take<int>(L.entries);
+      L.sorted = a.take<int>(L.entries);
+      L.start = a.take<int>(L.entries + 1);
+      L.ukeys = a.take<unsigned long long>(L.entries);
+      L.nbr = a.take<int2>(L.entries * (L.d + 1));
+      L.norm = a.take<float>(npix);
+    }
+    h->cub_tmp = a.take<char>(h->cub_bytes);
+  }, "wvn_crf_create"));
+  *out = h.release();
   return WVN_OK;
 }
 
-void crf_destroy(DenseCrf* h) {
-  if (!h) return;
-  if (h->base) cudaFree(h->base);
-  delete h;
-}
+void crf_destroy(wvn_crf* h) { delete h; }
 
-size_t crf_workspace_bytes(const DenseCrf* h) { return h ? h->bytes : 0; }
+size_t crf_workspace_bytes(const wvn_crf* h) { return h ? h->arena.bytes : 0; }
 
 namespace {
 
 template <int D>
-int filter_lattice(DenseCrf* h, int l, const float* in, const float* scale, int V, int mode, float* out, cudaStream_t s) {
+int filter_lattice(wvn_crf* h, int l, const float* in, const float* scale, int V, int mode, float* out, cudaStream_t s) {
   LatticeBufs& L = h->lat[l];
   const long long npix = static_cast<long long>(h->frames) * h->N;
   crf_splat_kernel<D><<<grid_for(L.entries, kWarps), kThreads, 0, s>>>(L, h->m + l, in, scale, V, h->va);
@@ -625,12 +596,12 @@ int filter_lattice(DenseCrf* h, int l, const float* in, const float* scale, int 
   return WVN_OK;
 }
 
-int run_filter(DenseCrf* h, int l, const float* in, const float* scale, int V, int mode, float* out, cudaStream_t s) {
+int run_filter(wvn_crf* h, int l, const float* in, const float* scale, int V, int mode, float* out, cudaStream_t s) {
   return l == 0 ? filter_lattice<2>(h, 0, in, scale, V, mode, out, s) : filter_lattice<5>(h, 1, in, scale, V, mode, out, s);
 }
 
 template <int D>
-int build_lattice(DenseCrf* h, int l, cudaStream_t s) {
+int build_lattice(wvn_crf* h, int l, cudaStream_t s) {
   LatticeBufs& L = h->lat[l];
   const long long npix = static_cast<long long>(h->frames) * h->N;
   const long long n = npix * (D + 1);
@@ -657,7 +628,7 @@ int build_lattice(DenseCrf* h, int l, cudaStream_t s) {
   return filter_lattice<D>(h, l, nullptr, nullptr, 1, SLICE_NORM, nullptr, s);
 }
 
-int build_chunk(DenseCrf* h, const CrfInput& in, int frame0, int frames, cudaStream_t s) {
+int build_chunk(wvn_crf* h, const CrfInput& in, int frame0, int frames, cudaStream_t s) {
   WVN_REQUIRE(in.img, "wvn_crf: null image");
   WVN_REQUIRE(in.resized_h >= h->S && in.resized_w >= h->S, "wvn_crf: resized image %dx%d smaller than the crop %d",
               in.resized_h, in.resized_w, h->S);
@@ -676,13 +647,13 @@ int build_chunk(DenseCrf* h, const CrfInput& in, int frame0, int frames, cudaStr
 
 }  // namespace
 
-int crf_build(DenseCrf* h, const CrfInput& in, cudaStream_t s) {
+int crf_build(wvn_crf* h, const CrfInput& in, cudaStream_t s) {
   WVN_REQUIRE(h, "wvn_crf_build: null handle");
   WVN_REQUIRE(in.batch >= 1 && in.batch <= h->chunk, "wvn_crf_build: batch %d outside [1, chunk %d]", in.batch, h->chunk);
   return build_chunk(h, in, 0, in.batch, s);
 }
 
-int crf_filter(DenseCrf* h, int which, const float* values, int v, float* out, cudaStream_t s) {
+int crf_filter(wvn_crf* h, int which, const float* values, int v, float* out, cudaStream_t s) {
   WVN_REQUIRE(h && values && out, "wvn_crf_filter: null argument");
   WVN_REQUIRE(which == 0 || which == 1, "wvn_crf_filter: lattice %d is not 0 (spatial) or 1 (bilateral)", which);
   WVN_REQUIRE(v >= 1 && v <= h->K, "wvn_crf_filter: %d values outside [1, %d]", v, h->K);
@@ -697,7 +668,7 @@ __global__ void crf_counts_kernel(const int* __restrict__ start, const int* __re
 }
 }  // namespace
 
-int crf_export(DenseCrf* h, int which, unsigned long long* keys, int* counts, int* offsets, float* bary, int* m,
+int crf_export(wvn_crf* h, int which, unsigned long long* keys, int* counts, int* offsets, float* bary, int* m,
                cudaStream_t s) {
   WVN_REQUIRE(h && keys && counts && offsets && bary && m, "wvn_crf_export: null argument");
   WVN_REQUIRE(which == 0 || which == 1, "wvn_crf_export: lattice %d is not 0 or 1", which);
@@ -712,7 +683,7 @@ int crf_export(DenseCrf* h, int which, unsigned long long* keys, int* counts, in
   return WVN_OK;
 }
 
-int crf_run(DenseCrf* h, const CrfInput& in, long long* labels, float* q_out, cudaStream_t s) {
+int crf_run(wvn_crf* h, const CrfInput& in, long long* labels, float* q_out, cudaStream_t s) {
   WVN_REQUIRE(h && in.head && labels, "wvn_crf_run: null argument");
   WVN_REQUIRE(in.batch >= 1, "wvn_crf_run: empty batch");
   WVN_REQUIRE(in.classes >= 1 && in.classes <= h->K, "wvn_crf_run: classes %d outside [1, %d]", in.classes, h->K);

@@ -113,35 +113,29 @@ int double_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, 
   t->s = s; t->o = double_mlp_offsets(s); t->loss = loss; t->adam = adam;
   t->max_rows = max_rows;
   const size_t R = max_rows, D = s.dim, h1 = s.h1, h2 = s.h2;
-  // xg [R, D], a1 / d1 [2][R, h1], a2 / d2 [2][R, h2], out / d_out [R, 1 + D], loss_reco / raw / wraw [R], grads
-  const size_t floats = R * D + 2 * (2 * R * h1 + 2 * R * h2 + R * (D + 1)) + 3 * R + (grads_ext ? 0 : t->o.total);
-  const size_t head = 256 + (R * sizeof(int) + 255) / 256 * 256;   // scalars | n_live at 128 | comp at 256
-  const size_t bytes = head + floats * sizeof(float);
-  const int rc = trainer_alloc(t, bytes, "double mlp trainer");
+  // a1 / d1 / a2 / d2 hold both nets, the second R rows after the first
+  const int rc = trainer_alloc(t, [&](Carver& a) {
+    t->sc = a.take<DoubleScalars>(1);
+    t->n_live = a.take<int>(1);
+    t->comp = a.take<int>(R);
+    t->xg = a.take<float>(R * D);
+    t->a1 = a.take<float>(2 * R * h1);
+    t->d1 = a.take<float>(2 * R * h1);
+    t->a2 = a.take<float>(2 * R * h2);
+    t->d2 = a.take<float>(2 * R * h2);
+    t->out = a.take<float>(R * (D + 1));
+    t->d_out = a.take<float>(R * (D + 1));
+    t->loss_reco = a.take<float>(R);
+    t->raw = a.take<float>(R);
+    t->wraw = a.take<float>(R);
+    t->grads = grads_ext ? grads_ext : a.take<float>(t->o.total);
+  }, "double mlp trainer");
   if (rc != WVN_OK) {
     delete t;
     return rc;
   }
-  static_assert(sizeof(DoubleScalars) <= 128, "scalars overlap n_live");
-  char* base = reinterpret_cast<char*>(t->arena);
-  t->sc = reinterpret_cast<DoubleScalars*>(base);
   t->stats = &t->sc->sum_lr;
   t->n_stats = kStatDoubles + 1;
-  t->n_live = reinterpret_cast<int*>(base + 128);
-  t->comp = reinterpret_cast<int*>(base + 256);
-  float* f = reinterpret_cast<float*>(base + head);
-  auto take = [&](size_t n) { float* p = f; f += n; return p; };
-  t->xg = take(R * D);
-  t->a1 = take(2 * R * h1);
-  t->d1 = take(2 * R * h1);
-  t->a2 = take(2 * R * h2);
-  t->d2 = take(2 * R * h2);
-  t->out = take(R * (D + 1));
-  t->d_out = take(R * (D + 1));
-  t->loss_reco = take(R);
-  t->raw = take(R);
-  t->wraw = take(R);
-  t->grads = grads_ext ? grads_ext : take(t->o.total);
   *out = t;
   return WVN_OK;
 }

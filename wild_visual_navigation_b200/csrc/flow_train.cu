@@ -24,6 +24,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
 
 #include "common.cuh"
 #include "flow_train.h"
@@ -286,47 +287,38 @@ int flow_trainer_create(const FlowShape& s, int max_rows, float std_factor, cons
   t->s = s; t->adam = adam; t->loss.std_factor = std_factor; t->forward_only = forward_only;
   t->max_rows = (max_rows + 63) / 64 * 64;   // whole 64-row GEMM tiles
   const size_t R = t->max_rows, D = s.dim, h = s.hidden, np = flow_param_count(s);
-  const size_t floats = R * D * 4 + R * h * 8 + R * D * 4 + R * D + 2 * R       // forward
-                        + (forward_only ? 0 : R * D * 3 + R * h * 4 + R * D * 2 + R * D   // backward
-                                               + (grads_ext ? 0 : np));
-  const size_t head = 256 + ((R + 1) * sizeof(int) + 255) / 256 * 256;
-  const size_t bytes = head + floats * sizeof(float);
-  const int rc = trainer_alloc(t, bytes, "flow trainer");
+  const int rc = trainer_alloc(t, [&](Carver& a) {
+    t->sc = a.take<FlowScalars>(1);
+    t->n_live = a.take<int>(1);
+    t->comp = a.take<int>(R + 1);
+    for (int c = 0; c < 2; ++c) {
+      t->u[c] = a.take<float>(R * D);
+      t->mu[c] = a.take<float>(R * D);
+      for (int k = 0; k < 2; ++k) {
+        t->s1[c][k] = a.take<float>(R * h);
+        t->s2[c][k] = a.take<float>(R * h);
+        t->so[c][k] = a.take<float>(R * D);
+      }
+    }
+    t->z = a.take<float>(R * D);
+    t->ld = a.take<float>(R);
+    t->nll = a.take<float>(R);
+    if (forward_only) return;
+    t->dx = a.take<float>(R * D);
+    t->du = a.take<float>(R * D);
+    for (int k = 0; k < 2; ++k) {
+      t->dso[k] = a.take<float>(R * D);
+      t->d2[k] = a.take<float>(R * h);
+      t->d1[k] = a.take<float>(R * h);
+      t->dmu[k] = a.take<float>(R * D);
+    }
+    t->grads = grads_ext ? grads_ext : a.take<float>(np);
+  }, "flow trainer");
   if (rc != WVN_OK) {
     delete t;
     return rc;
   }
-  char* base = reinterpret_cast<char*>(t->arena);
-  static_assert(sizeof(FlowScalars) <= 128, "scalars overlap n_live");
-  t->sc = reinterpret_cast<FlowScalars*>(base);
   t->stats = &t->sc->s1;
-  t->n_live = reinterpret_cast<int*>(base + 128);
-  t->comp = reinterpret_cast<int*>(base + 256);
-  float* f = reinterpret_cast<float*>(base + head);
-  auto take = [&](size_t n) { float* p = f; f += n; return p; };
-  for (int c = 0; c < 2; ++c) {
-    t->u[c] = take(R * D);
-    t->mu[c] = take(R * D);
-    for (int k = 0; k < 2; ++k) {
-      t->s1[c][k] = take(R * h);
-      t->s2[c][k] = take(R * h);
-      t->so[c][k] = take(R * D);
-    }
-  }
-  t->z = take(R * D);
-  t->ld = take(R);
-  t->nll = take(R);
-  if (!forward_only) {
-    t->dx = take(R * D);
-    t->du = take(R * D);
-    for (int k = 0; k < 2; ++k) {
-      t->dso[k] = take(R * D);
-      t->d2[k] = take(R * h);
-      t->d1[k] = take(R * h);
-      t->dmu[k] = take(R * D);
-    }
-    t->grads = grads_ext ? grads_ext : take(np);
-  }
   *out = t;
   return WVN_OK;
 }
@@ -677,10 +669,11 @@ inline int rup(int v, int m) { return (v + m - 1) / m * m; }
 
 }  // namespace
 
+// The per-pixel path's bf16 operands and chunk workspaces
 struct FlowPixels {
   FlowShape s;
   int dim_p = 0, hid_p = 0, chunk = 0;
-  void* arena = nullptr;
+  DevBuf arena;
   __nv_bfloat16 *w0[2], *w2[2][2], *w4[2][2];   // [coupling][net]; w0 holds s and t stacked (2 hid_p rows)
   float *b0[2], *b2[2][2], *b4[2][2];
   float *u, *so, *to, *ld;
@@ -688,58 +681,57 @@ struct FlowPixels {
   bool loaded = false;
 };
 
-int flow_pixels_create(const FlowShape& s, int chunk, FlowPixels** out) {
-  WVN_REQUIRE(out, "flow pixels: null argument");
-  WVN_REQUIRE(s.dim >= 2 && s.dim <= 4096 && s.hidden >= 8 && s.hidden <= 512 && s.hidden % 8 == 0,
-              "flow pixels: LinearRnvp(%d, [%d]) outside the kernels' range", s.dim, s.hidden);
-  FlowPixels* f = new FlowPixels();
+}  // namespace wvn
+
+// inference only: the fp32 row forward (a forward-only trainer) and the per-pixel wgmma path
+struct wvn_flow_infer {
+  std::unique_ptr<wvn::Trainer> rows;
+  wvn::FlowPixels pix;
+};
+
+namespace wvn {
+
+int flow_infer_create(const FlowShape& s, int max_rows, int chunk, wvn_flow_infer** out) {
+  std::unique_ptr<wvn_flow_infer> h(new wvn_flow_infer());
+  Trainer* rows = nullptr;
+  WVN_PROPAGATE(flow_trainer_create(s, max_rows, 0.5f, AdamCfg(), nullptr, true, &rows));
+  h->rows.reset(rows);
+  FlowPixels* f = &h->pix;
   f->s = s;
   f->dim_p = rup(s.dim, 64);
   f->hid_p = rup(s.hidden, 64);
   f->chunk = chunk > 0 ? rup(chunk, 128) : 8192;
   const size_t Dp = f->dim_p, hp = f->hid_p, C = f->chunk, D = s.dim;
-  // one walk over the layout both sizes the arena (base == nullptr) and assigns the pointers
-  auto layout = [&](char* base) {
-    size_t off = 0;
-    auto take = [&](size_t n) { char* q = base ? base + off : nullptr; off += (n + 255) / 256 * 256; return q; };
+  WVN_PROPAGATE(carve(&f->arena, [&](Carver& a) {
     for (int c = 0; c < 2; ++c) {
-      f->w0[c] = reinterpret_cast<__nv_bfloat16*>(take(2 * 2 * hp * Dp));   // s and t stacked: 2 hp rows of Dp
-      f->b0[c] = reinterpret_cast<float*>(take(4 * 2 * hp));
+      f->w0[c] = a.take<__nv_bfloat16>(2 * hp * Dp);   // s and t stacked: 2 hp rows of Dp
+      f->b0[c] = a.take<float>(2 * hp);
       for (int k = 0; k < 2; ++k) {
-        f->w2[c][k] = reinterpret_cast<__nv_bfloat16*>(take(2 * hp * hp));
-        f->b2[c][k] = reinterpret_cast<float*>(take(4 * hp));
-        f->w4[c][k] = reinterpret_cast<__nv_bfloat16*>(take(2 * Dp * hp));
-        f->b4[c][k] = reinterpret_cast<float*>(take(4 * Dp));
+        f->w2[c][k] = a.take<__nv_bfloat16>(hp * hp);
+        f->b2[c][k] = a.take<float>(hp);
+        f->w4[c][k] = a.take<__nv_bfloat16>(Dp * hp);
+        f->b4[c][k] = a.take<float>(Dp);
       }
     }
-    f->u = reinterpret_cast<float*>(take(4 * C * D));
-    f->so = reinterpret_cast<float*>(take(4 * C * Dp));
-    f->to = reinterpret_cast<float*>(take(4 * C * Dp));
-    f->ld = reinterpret_cast<float*>(take(4 * C));
-    f->mu = reinterpret_cast<__nv_bfloat16*>(take(2 * C * Dp));
-    f->h1 = reinterpret_cast<__nv_bfloat16*>(take(2 * C * 2 * hp));
-    f->h2 = reinterpret_cast<__nv_bfloat16*>(take(2 * C * 2 * hp));
-    return off;
-  };
-  const size_t bytes = layout(nullptr);
-  if (cudaMalloc(&f->arena, bytes) != cudaSuccess) {
-    delete f;
-    return set_error(WVN_ERR_CUDA, "flow pixels: cudaMalloc of %zu bytes failed", bytes);
-  }
-  cudaMemset(f->arena, 0, bytes);
-  layout(reinterpret_cast<char*>(f->arena));
-  *out = f;
+    f->u = a.take<float>(C * D);
+    f->so = a.take<float>(C * Dp);
+    f->to = a.take<float>(C * Dp);
+    f->ld = a.take<float>(C);
+    f->mu = a.take<__nv_bfloat16>(C * Dp);
+    f->h1 = a.take<__nv_bfloat16>(C * 2 * hp);
+    f->h2 = a.take<__nv_bfloat16>(C * 2 * hp);
+  }, "flow pixels"));
+  *out = h.release();
   return WVN_OK;
 }
 
-void flow_pixels_destroy(FlowPixels* f) {
-  if (!f) return;
-  if (f->arena) cudaFree(f->arena);
-  delete f;
-}
+void flow_infer_destroy(wvn_flow_infer* h) { delete h; }
 
-int flow_pixels_set_params(FlowPixels* f, const float* params, cudaStream_t stream) {
-  WVN_REQUIRE(f && params, "flow pixels: null argument");
+Trainer* flow_infer_trainer(wvn_flow_infer* h) { return h->rows.get(); }
+
+int flow_infer_set_params(wvn_flow_infer* fi, const float* params, cudaStream_t stream) {
+  WVN_REQUIRE(params, "flow pixels: null argument");
+  FlowPixels* f = &fi->pix;
   const int D = f->s.dim, h = f->s.hidden, Dp = f->dim_p, hp = f->hid_p;
   for (int c = 0; c < 2; ++c) {
     for (int k = 0; k < 2; ++k) {
@@ -762,10 +754,11 @@ int flow_pixels_set_params(FlowPixels* f, const float* params, cudaStream_t stre
   return WVN_OK;
 }
 
-int flow_pixels_run(FlowPixels* f, const FlowBuffers& b, const float* tokens, int batch, int gh, int gw, int out_h,
-                    int out_w, const float* cg_mean, const float* cg_std, float std_factor, float* trav, float* nll,
-                    cudaStream_t stream) {
-  WVN_REQUIRE(f && tokens && trav && cg_mean && cg_std && b.mask0 && b.mask1 && b.p1 && b.p3, "flow pixels: null argument");
+int flow_infer_pixels(wvn_flow_infer* fi, const FlowBuffers& b, const float* tokens, int batch, int gh, int gw,
+                      int out_h, int out_w, const float* cg_mean, const float* cg_std, float std_factor, float* trav,
+                      float* nll, cudaStream_t stream) {
+  WVN_REQUIRE(tokens && trav && cg_mean && cg_std && b.mask0 && b.mask1 && b.p1 && b.p3, "flow pixels: null argument");
+  FlowPixels* f = &fi->pix;
   if (!f->loaded) return set_error(WVN_ERR_STATE, "flow pixels: parameters were never set");
   WVN_REQUIRE(batch > 0 && gh > 0 && gw > 0 && out_h > 1 && out_w > 1, "flow pixels: bad geometry");
   const int D = f->s.dim, Dp = f->dim_p, hp = f->hid_p;

@@ -1,10 +1,11 @@
 // wvn-b200: internal interface of the LinearRnvp flow kernels (flow_train.cu): the fp32 row forward and the fp32
-// online train step of the anomaly-detection learner.
+// online train step of the anomaly-detection learner, and its inference handle.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <stddef.h>
 
+#include "../../include/wvn_b200.h"
 #include "train_core.h"
 
 namespace wvn {
@@ -70,15 +71,17 @@ int flow_train_step_padded(Trainer* t, float* params, float* exp_avg, float* exp
                            const unsigned char* y_valid, float* cg_mean, float* cg_std, float* conf_out, float* metrics,
                            int phase_mask, cudaStream_t stream);
 
-// Per-pixel anomaly map on wgmma: bf16 operands packed by set_params (re-pack after the parameters change), fp32
-// accumulation; the masks and permutations are read from b on every call.  tokens: [batch, gh * gw, dim] fp32; trav
+// The inference handle (wvn_flow_infer_*): a forward-only trainer of max_rows rows for the two row forwards above, and
+// the per-pixel anomaly map on wgmma in chunks of chunk_pixels (0: 8192).
+int flow_infer_create(const FlowShape& s, int max_rows, int chunk_pixels, wvn_flow_infer** out);
+void flow_infer_destroy(wvn_flow_infer* h);
+Trainer* flow_infer_trainer(wvn_flow_infer* h);
+// Per-pixel anomaly map: bf16 operands packed by set_params (re-pack after the parameters change), fp32 accumulation;
+// the masks and permutations are read from b on every call.  tokens: [batch, gh * gw, dim] fp32; trav
 // [batch, out_h, out_w] = inference_without_update(NLL); nll (may be NULL): the per-pixel NLL.
-struct FlowPixels;
-int flow_pixels_create(const FlowShape& s, int chunk_pixels, FlowPixels** out);
-void flow_pixels_destroy(FlowPixels* f);
-int flow_pixels_set_params(FlowPixels* f, const float* params, cudaStream_t stream);
-int flow_pixels_run(FlowPixels* f, const FlowBuffers& b, const float* tokens, int batch, int gh, int gw, int out_h,
-                    int out_w, const float* cg_mean, const float* cg_std, float std_factor, float* trav, float* nll,
-                    cudaStream_t stream);
+int flow_infer_set_params(wvn_flow_infer* h, const float* params, cudaStream_t stream);
+int flow_infer_pixels(wvn_flow_infer* h, const FlowBuffers& b, const float* tokens, int batch, int gh, int gw,
+                      int out_h, int out_w, const float* cg_mean, const float* cg_std, float std_factor, float* trav,
+                      float* nll, cudaStream_t stream);
 
 }  // namespace wvn

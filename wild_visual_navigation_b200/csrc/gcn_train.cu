@@ -269,39 +269,29 @@ int gcn_trainer_create(const MlpShape& s, int max_rows, int max_edges, const Los
   t->max_rows = max_rows;
   t->max_edges = max_edges;
   const size_t R = max_rows, E = std::max(max_edges, 1), D = s.dim, h1 = s.h1, h2 = s.h2, n3 = D + 1;
-  const size_t ints = R + 4 * R + 2 * E;   // comp, the four row arrays, in_src / out_dst
-  const size_t floats = R + 2 * E + R * D + 3 * R * h1 + 3 * R * h2 + 3 * R * n3 + 3 * R +
-                        (grads_ext ? 0 : t->o.total);
-  const size_t head = 256;   // scalars | n_live at 128 | overflow at 136
-  const size_t ints_bytes = (ints * sizeof(int) + 255) / 256 * 256;
-  const size_t bytes = head + ints_bytes + floats * sizeof(float);
-  const int rc = trainer_alloc(t, bytes, "gcn trainer");
+  const int rc = trainer_alloc(t, [&](Carver& a) {
+    t->sc = a.take<DoubleScalars>(1);
+    t->n_live = a.take<int>(1);
+    t->overflow = a.take<double>(1);
+    t->comp = a.take<int>(R);
+    t->in_start = a.take<int>(R); t->in_cnt = a.take<int>(R);
+    t->out_start = a.take<int>(R); t->out_cnt = a.take<int>(R);
+    t->in_src = a.take<int>(E); t->out_dst = a.take<int>(E);
+    t->dinv = a.take<float>(R);
+    t->in_w = a.take<float>(E); t->out_w = a.take<float>(E);
+    t->xg = a.take<float>(R * D);
+    t->y1 = a.take<float>(R * h1); t->a1 = a.take<float>(R * h1); t->dz1 = a.take<float>(R * h1);
+    t->y2 = a.take<float>(R * h2); t->a2 = a.take<float>(R * h2); t->dz2 = a.take<float>(R * h2);
+    t->y3 = a.take<float>(R * n3); t->out = a.take<float>(R * n3); t->d_out = a.take<float>(R * n3);
+    t->loss_reco = a.take<float>(R); t->raw = a.take<float>(R); t->wraw = a.take<float>(R);
+    t->grads = grads_ext ? grads_ext : a.take<float>(t->o.total);
+  }, "gcn trainer");
   if (rc != WVN_OK) {
     delete t;
     return rc;
   }
-  static_assert(sizeof(DoubleScalars) <= 128, "scalars overlap n_live");
-  char* base = reinterpret_cast<char*>(t->arena);
-  t->sc = reinterpret_cast<DoubleScalars*>(base);
   t->stats = &t->sc->sum_lr;
   t->n_stats = kStatDoubles + 1;
-  t->n_live = reinterpret_cast<int*>(base + 128);
-  t->overflow = reinterpret_cast<double*>(base + 136);
-  int* ip = reinterpret_cast<int*>(base + head);
-  auto take_i = [&](size_t n) { int* p = ip; ip += n; return p; };
-  t->comp = take_i(R);
-  t->in_start = take_i(R); t->in_cnt = take_i(R); t->out_start = take_i(R); t->out_cnt = take_i(R);
-  t->in_src = take_i(E); t->out_dst = take_i(E);
-  float* f = reinterpret_cast<float*>(base + head + ints_bytes);
-  auto take = [&](size_t n) { float* p = f; f += n; return p; };
-  t->dinv = take(R);
-  t->in_w = take(E); t->out_w = take(E);
-  t->xg = take(R * D);
-  t->y1 = take(R * h1); t->a1 = take(R * h1); t->dz1 = take(R * h1);
-  t->y2 = take(R * h2); t->a2 = take(R * h2); t->dz2 = take(R * h2);
-  t->y3 = take(R * n3); t->out = take(R * n3); t->d_out = take(R * n3);
-  t->loss_reco = take(R); t->raw = take(R); t->wraw = take(R);
-  t->grads = grads_ext ? grads_ext : take(t->o.total);
   *out = t;
   return WVN_OK;
 }

@@ -1,4 +1,4 @@
-// wvn-b200: host-side helpers (error string, tensor-map encoding, device buffers, weight stores).
+// wvn-b200: host-side helpers (error string, tensor-map encoding, device buffers and arenas, weight stores).
 #include "host_common.h"
 
 #include <cuda_bf16.h>
@@ -194,6 +194,20 @@ void DevBuf::release() {
   if (p) cudaFree(p);
   p = nullptr;
   bytes = 0;
+}
+
+int carve(DevBuf* buf, const std::function<void(Carver&)>& layout, const char* who) {
+  Carver count;
+  layout(count);
+  const int rc = buf->alloc(count.bytes);
+  if (rc != WVN_OK) {
+    const std::string why = last_error();
+    return set_error(rc, "%s: arena of %zu bytes: %s", who, count.bytes, why.c_str());
+  }
+  Carver pieces;
+  pieces.base = static_cast<char*>(buf->p);
+  layout(pieces);
+  return WVN_OK;
 }
 
 constexpr size_t kStageBytes = 8u << 20;

@@ -1,5 +1,5 @@
 // wvn-b200: host-side helpers shared by the translation units of libwvn_b200.so
-// (error reporting, TMA tensor-map encoding through the driver entry point, device buffers, weight stores).
+// (error reporting, TMA tensor-map encoding through the driver entry point, device buffers and arenas, weight stores).
 #pragma once
 
 #include <cuda.h>
@@ -7,6 +7,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <functional>
 #include <map>
 #include <string>
 
@@ -98,6 +99,22 @@ struct DevBuf {
  private:
   void release();
 };
+
+// One walk over a device arena's layout, run twice: with a null base the carver only counts bytes, with a base it
+// hands out the same pieces in the same order.  Every piece starts on a 256-byte boundary.
+struct Carver {
+  char* base = nullptr;
+  size_t bytes = 0;
+  template <class T>
+  T* take(size_t n) {   // n elements of T
+    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += (n * sizeof(T) + 255) / 256 * 256;
+    return p;
+  }
+};
+// Sizes `buf` by one layout walk, allocates it (zero-filled) and walks again to hand out the pointers.  A failure names
+// `who`.
+int carve(DevBuf* buf, const std::function<void(Carver&)>& layout, const char* who);
 
 // A handle's named weights: device storage sized at create, filled by set() from fp32 host or device data.
 struct WeightStore {

@@ -537,14 +537,22 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
   t->s = s; t->o = mlp_offsets(s); t->loss = loss; t->adam = adam;
   t->max_rows = (max_rows + TR - 1) / TR * TR;
   const size_t R = t->max_rows, n3 = s.dim + 1;
-  const size_t floats = R * s.h1 * 2 + R * s.h2 * 2 + R * n3 * 2 + R * 2 + (t->o.total + 1);
-  const size_t bytes = floats * sizeof(float) + 256;
-  const int rc = trainer_alloc(t, bytes, "trainer");
+  const int rc = trainer_alloc(t, [&](Carver& a) {
+    t->sc = scalars_ext ? reinterpret_cast<FusedScalars*>(scalars_ext) : a.take<FusedScalars>(1);
+    t->h1 = a.take<float>(R * s.h1);
+    t->d_h1 = a.take<float>(R * s.h1);
+    t->h2 = a.take<float>(R * s.h2);
+    t->d_h2 = a.take<float>(R * s.h2);
+    t->out = a.take<float>(R * n3);
+    t->d_out = a.take<float>(R * n3);
+    t->loss_reco = a.take<float>(R);
+    t->raw = a.take<float>(R);
+    t->grads = grads_ext ? grads_ext : a.take<float>(t->o.total + 1);   // + the confidence-weighted traversability sum
+  }, "trainer");
   if (rc != WVN_OK) {
     delete t;
     return rc;
   }
-  t->sc = scalars_ext ? reinterpret_cast<FusedScalars*>(scalars_ext) : reinterpret_cast<FusedScalars*>(t->arena);
   t->stats = &t->sc->sum_lr;
   {
     FusedScalars init;
@@ -552,16 +560,6 @@ int fused_trainer_create(const MlpShape& s, int max_rows, const LossCfg& loss, c
     init.x_min = INFINITY;
     cudaMemcpy(t->sc, &init, sizeof(init), cudaMemcpyHostToDevice);
   }
-  float* f = reinterpret_cast<float*>(reinterpret_cast<char*>(t->arena) + 256);
-  t->h1 = f; f += R * s.h1;
-  t->d_h1 = f; f += R * s.h1;
-  t->h2 = f; f += R * s.h2;
-  t->d_h2 = f; f += R * s.h2;
-  t->out = f; f += R * n3;
-  t->d_out = f; f += R * n3;
-  t->loss_reco = f; f += R;
-  t->raw = f; f += R;
-  t->grads = grads_ext ? grads_ext : f;
   t->smem_fwd = sizeof(float) * (static_cast<size_t>(s.dim) * TR + std::max(KC * (s.h1 + 1), s.h1 * TRP) + s.h1 * TRP +
                                  s.h2 * TR + TR + TR);
   t->smem_bwd = sizeof(float) * (((n3 * TRP + 3) & ~size_t(3)) + s.h2 * TR + TR + 8);

@@ -1,6 +1,6 @@
 // wvn-b200: the fp32 training core shared by the learners' trainers (train_core.h): the private ConfidenceGenerator
 // block, Adam, the batched fp32 CUDA-core GEMM, the compaction of padded rows, the NCCL communicator of data-parallel
-// steps and the trainer base's allocation and release.
+// steps and the trainer base's arena.
 #include <dlfcn.h>
 #include <string.h>
 
@@ -15,22 +15,6 @@ namespace wvn {
 // ------------------------------------------------------------------------------------------------ confidence state
 // Private block (doubles): running_n, running_sum, running_sumsq | var as a float | ring [kConfWindow][3] + count.
 constexpr int kConfBlockDoubles = 32;
-
-int trainer_conf_create(TrainerConf* c) {
-  if (cudaMalloc(&c->priv, sizeof(double) * kConfBlockDoubles) != cudaSuccess) {
-    c->priv = nullptr;
-    return set_error(WVN_ERR_CUDA, "trainer: cudaMalloc of the confidence state failed");
-  }
-  cudaMemset(c->priv, 0, sizeof(double) * kConfBlockDoubles);
-  const float one = 1.f;   // private var = 1 (the reference's initial value) unless the caller binds its own
-  cudaMemcpy(reinterpret_cast<float*>(c->priv + 3), &one, sizeof(float), cudaMemcpyHostToDevice);
-  return trainer_conf_bind(c, CONF_LATEST, nullptr, nullptr, nullptr, nullptr, 0.2f, 1.0f);
-}
-
-void trainer_conf_destroy(TrainerConf* c) {
-  if (c->priv) cudaFree(c->priv);
-  c->priv = nullptr;
-}
 
 int trainer_conf_bind(TrainerConf* c, int method, float* var, double* running_n, double* running_sum,
                       double* running_sumsq, float kf_proc_cov, float kf_meas_cov) {
@@ -366,20 +350,16 @@ int trainer_comm_sum(TrainerComm* c, void* buf, size_t n, bool f64, cudaStream_t
 }
 
 // ------------------------------------------------------------------------------------------------ trainer
-Trainer::~Trainer() {
-  trainer_comm_destroy(&comm);
-  if (arena) cudaFree(arena);
-  trainer_conf_destroy(&conf);
-}
+Trainer::~Trainer() { trainer_comm_destroy(&comm); }
 
-int trainer_alloc(Trainer* t, size_t bytes, const char* who) {
-  if (cudaMalloc(&t->arena, bytes) != cudaSuccess) {
-    t->arena = nullptr;
-    return set_error(WVN_ERR_CUDA, "%s: cudaMalloc of %zu bytes failed", who, bytes);
-  }
-  if (cudaMemset(t->arena, 0, bytes) != cudaSuccess)
-    return set_error(WVN_ERR_CUDA, "%s: cudaMemset of %zu bytes failed", who, bytes);
-  return trainer_conf_create(&t->conf);
+int trainer_alloc(Trainer* t, const std::function<void(Carver&)>& layout, const char* who) {
+  WVN_PROPAGATE(carve(&t->arena, [&](Carver& c) {
+    t->conf.priv = c.take<double>(kConfBlockDoubles);
+    layout(c);
+  }, who));
+  const float one = 1.f;   // private var = 1 (the reference's initial value) unless the caller binds its own
+  WVN_CHECK_CUDA(cudaMemcpy(reinterpret_cast<float*>(t->conf.priv + 3), &one, sizeof(float), cudaMemcpyHostToDevice));
+  return trainer_conf_bind(&t->conf, CONF_LATEST, nullptr, nullptr, nullptr, nullptr, 0.2f, 1.0f);
 }
 
 int trainer_check(const Trainer* t, TrainerKind kind, const char* who) {

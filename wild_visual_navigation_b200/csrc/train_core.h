@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 
+#include "host_common.h"
 #include "mlp_train.h"
 
 namespace wvn {
@@ -33,18 +34,17 @@ struct ConfState {
 
 // A trainer's generator: where its state lives (cs, passed to the kernels) and the device block holding what no caller
 // buffer holds: moving_average's window, and var / the running sums when the caller binds none (var starts at 1, the
-// reference's initial value).
+// reference's initial value).  The block is the first piece of the trainer's arena (trainer_alloc).
 struct TrainerConf {
   ConfState cs;
   double* priv = nullptr;
 };
-int trainer_conf_create(TrainerConf* c);   // allocates the block and binds latest_measurement to it
-void trainer_conf_destroy(TrainerConf* c);
 // method: ConfMethod; pointers may be null for methods that do not use them (the private block then holds that state).
 int trainer_conf_bind(TrainerConf* c, int method, float* var, double* running_n, double* running_sum,
                       double* running_sumsq, float kf_proc_cov, float kf_meas_cov);
 // Copies src's private block into dst's, on `stream`: a caller that replaces a trainer by a larger one keeps the
-// generator where it was.  Ordered after src's last step; destroying src afterwards (cudaFree) waits for the copy.
+// generator where it was.  Ordered after src's last step; destroying src afterwards frees its arena, which waits for
+// the copy.
 int trainer_conf_copy(TrainerConf* dst, const TrainerConf* src, cudaStream_t stream);
 
 // ---- batched fp32 GEMM: 64 x 64 tiles, K step 16, 4 x 4 outputs per thread, CUDA cores
@@ -107,8 +107,7 @@ int trainer_comm_sum(TrainerComm* c, void* buf, size_t n, bool f64, cudaStream_t
 enum TrainerKind : int { TRAINER_MLP = 0, TRAINER_DOUBLE_MLP = 1, TRAINER_GCN = 2, TRAINER_FLOW = 3 };
 
 // The state every learner's trainer (FusedTrainer, DoubleTrainer, GcnTrainer, FlowTrainer) keeps; the C ABI's
-// wvn_trainer_t is a pointer to it.  Deleting a trainer destroys its communicator, frees its arena and destroys its
-// generator block.
+// wvn_trainer_t is a pointer to it.  Deleting a trainer destroys its communicator and frees its arena.
 struct Trainer {
   explicit Trainer(TrainerKind k) : kind(k) {}
   virtual ~Trainer();
@@ -116,16 +115,17 @@ struct Trainer {
   LossCfg loss;
   AdamCfg adam;
   int max_rows = 0;
-  void* arena = nullptr;   // every device workspace of the learner, one allocation
+  DevBuf arena;            // the generator block and every device workspace of the learner, one allocation
   TrainerConf conf;        // ConfidenceGenerator method + where its state lives
   TrainerComm comm;        // the library's communicator of a data-parallel step
   double* stats = nullptr; // the statistics block: kStatDoubles, then the learner's own exchanged doubles
   int n_stats = kStatDoubles;
   float* grads = nullptr;
 };
-// Allocates t's arena of `bytes`, zeroed, and its generator block.  On failure the caller deletes t, which releases
-// whatever was allocated.
-int trainer_alloc(Trainer* t, size_t bytes, const char* who);
+// Allocates t's arena, zeroed: the generator block (bound to latest_measurement, var = 1), then the pieces `layout`
+// takes.  Each piece starts on a 256-byte boundary, so consecutive pieces need not be adjacent: no kernel, memset or
+// copy may span two of them.  On failure the caller deletes t.
+int trainer_alloc(Trainer* t, const std::function<void(Carver&)>& layout, const char* who);
 // WVN_ERR_INVALID unless t is a trainer of `kind`: every entry point of a learner checks its handle on the host,
 // before it enqueues anything.
 int trainer_check(const Trainer* t, TrainerKind kind, const char* who);
