@@ -63,7 +63,9 @@ int wvn_check_device(void);
  * Later additions under 108 add symbols only: the dense CRF (wvn_crf_*), the EfficientNet-B0 handle (wvn_effnet_*)
  * with its primitives, GEMM activation 3 (SiLU), wvn_segment_pool_levels, and the segment-wise inference entries
  * wvn_segment_maps, wvn_mlp_infer_rows_padded and wvn_flow_infer_rows_padded, and the ViT primitives
- * wvn_image_to_patches, wvn_init_token_rows, wvn_layernorm_ex and wvn_attention_f32_debug. */
+ * wvn_image_to_patches, wvn_init_token_rows, wvn_layernorm_ex and wvn_attention_f32_debug; GEMM epilogue 7 (SwiGLU),
+ * wvn_swiglu_packed_rows and wvn_vit_create_ffn (the SwiGLU FFN of DINOv2 ViT-g/14 is selected by an argument of its
+ * own, so wvn_vit_config keeps its layout). */
 int wvn_version(void);
 /* Number of kernel launches this library has issued in this process (bench.py's gpu_launches). */
 long long wvn_launch_count(void);
@@ -96,7 +98,10 @@ int wvn_gemm_bf16(const void* a_bf16, long long lda, const void* w_bf16, const f
  *   4 = QKV: bf16 q_out, k_out [m/npad*heads, npad, 64] and vt_out [m/npad*heads, 64, npad] from the columns of [q | k | v];
  *   5 = MLP head: columns [0, feat) reconstruct x -> loss_reco = mean((out - x)^2) -> conf, column trav_col ->
  *       trav = sigmoid; nothing of [m, n] is stored;
- *   6 = residual: bf16 out[m,ldo] = act(acc + bias + residual[m,ldr]) (residual bf16, ldr even and >= n; act 0 or 1).
+ *   6 = residual: bf16 out[m,ldo] = act(acc + bias + residual[m,ldr]) (residual bf16, ldr even and >= n; act 0 or 1);
+ *   7 = SwiGLU: w [n, k] and bias [n] in the packed row order of wvn_swiglu_packed_rows (n % 256 == 0, block_n 0 or
+ *       256, act 0): bf16 out[m, ldo] (ldo >= n / 2, a multiple of 8), out[:, j] = silu(g_j) * v_j in fp32, rounded
+ *       once, with g_j and v_j = acc + bias of the gate row j and the value row n / 2 + j of the unpacked w12.
  * reverse_m = 1 walks the 64-row blocks last-to-first (the result must not change). */
 typedef struct {
   int m, n, k;
@@ -140,7 +145,8 @@ int wvn_gemm_bf16_ex(const wvn_gemm_ex_args* args, void* stream);
 int wvn_attention_bf16(const void* q, const void* k, const void* vt, void* out, int batch, int heads, int npad,
                        int n_valid, float scale, void* stream);
 
-/* LayerNorm over fp32 rows -> bf16 rows; dim in {384, 768, 1024}.  The same as wvn_layernorm_ex without an fp32 output. */
+/* LayerNorm over fp32 rows -> bf16 rows; dim in {384, 768, 1024, 1536}.  The same as wvn_layernorm_ex without an fp32
+ * output. */
 int wvn_layernorm(const float* x, const float* gamma, const float* beta, void* out_bf16, long long rows, int dim,
                   float eps, void* stream);
 
@@ -163,7 +169,8 @@ int wvn_image_to_patches(const void* img, int u8_hwc, int batch, int in_h, int i
  * reg [registers, dim] (NULL when registers == 0). */
 int wvn_init_token_rows(float* x, const float* cls, const float* pos, const float* reg, int registers, int batch, int npad,
                         int n_valid, int dim, void* stream);
-/* LayerNorm(dim, eps) of fp32 rows x [rows, dim] (biased variance, eps inside the square root), dim in {384, 768, 1024}:
+/* LayerNorm(dim, eps) of fp32 rows x [rows, dim] (biased variance, eps inside the square root), dim in {384, 768, 1024,
+ * 1536}:
  * out_bf16 [rows, dim] bf16 (or NULL) and out_f32 (or NULL) fp32, which receives only rows [row0, n_valid) of each
  * npad-row frame, compacted: frame f's row t lands at f * (n_valid - row0) + t - row0 (rows % npad == 0).
  * reverse = 1 walks the rows last-to-first; the result does not change. */
@@ -185,10 +192,10 @@ typedef struct wvn_vit wvn_vit_t;
 typedef struct {
   int image_size;   /* side of the (square) network input after resize + center crop, e.g. 448 */
   int patch_size;   /* 8 or 16 (DINO), 14 (DINOv2) */
-  int dim;          /* 384 (vit_small), 768 (vit_base) or 1024 (vit_large) */
-  int depth;        /* 12 (vit_small, vit_base), 24 (vit_large) */
+  int dim;          /* 384 (vit_small), 768 (vit_base), 1024 (vit_large) or 1536 (vit_giant) */
+  int depth;        /* 12 (vit_small, vit_base), 24 (vit_large), 40 (vit_giant) */
   int heads;        /* dim / 64 */
-  int mlp_dim;      /* 4 * dim */
+  int mlp_dim;      /* 4 * dim; the SwiGLU FFN's hidden width (4096 for vit_giant), a multiple of 128 */
   int max_batch;    /* largest batch a single forward call may carry */
   int chunk;        /* frames processed together (activations stay L2-resident); 0 = default */
   float ln_eps;     /* 1e-6 */
@@ -199,6 +206,16 @@ typedef struct {
 } wvn_vit_config;
 
 int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out);
+/* The FFN of each block: WVN_VIT_FFN_MLP = fc2(GELU(fc1(x))) (DINO, DINOv2 ViT-S / B / L; what wvn_vit_create
+ * builds), WVN_VIT_FFN_SWIGLU = w3(silu(x1) * x2) with [x1 | x2] = w12(x) (DINOv2 ViT-g/14, SwiGLUFFNFused). */
+#define WVN_VIT_FFN_MLP 0
+#define WVN_VIT_FFN_SWIGLU 1
+int wvn_vit_create_ffn(const wvn_vit_config* cfg, int ffn, wvn_vit_t** out);
+/* The packed row order EPI 7 and the SwiGLU handle store w12 in: src_rows[p] (rows entries) = the checkpoint row of
+ * packed row p.  Each 256-row tile t holds gate rows [128 t, 128 t + 128), then value rows
+ * rows / 2 + [128 t, 128 t + 128).
+ * rows % 256 == 0.  Host only. */
+int wvn_swiglu_packed_rows(long long rows, long long* src_rows);
 void wvn_vit_destroy(wvn_vit_t* h);
 
 /* Weights use the DINO state-dict names (fp32, host or device memory):
@@ -208,7 +225,9 @@ void wvn_vit_destroy(wvn_vit_t* h);
  *   patch_embed.proj.bias [dim],
  *   blocks.{i}.norm1.{weight,bias}, blocks.{i}.attn.qkv.{weight [3dim,dim],bias},
  *   blocks.{i}.attn.proj.{weight,bias}, blocks.{i}.norm2.{weight,bias},
- *   blocks.{i}.mlp.fc1.{weight [mlp,dim],bias}, blocks.{i}.mlp.fc2.{weight [dim,mlp],bias},
+ *   blocks.{i}.mlp.fc1.{weight [mlp,dim],bias}, blocks.{i}.mlp.fc2.{weight [dim,mlp],bias} (WVN_VIT_FFN_MLP), or
+ *   blocks.{i}.mlp.w12.{weight [2 mlp,dim],bias}, blocks.{i}.mlp.w3.{weight [dim,mlp],bias} (WVN_VIT_FFN_SWIGLU; w12 in
+ *   the checkpoint's row order, which the library packs, see wvn_swiglu_packed_rows),
  *   norm.{weight,bias}
  * and for the STEGO head (see wvn_vit_stego_head):
  *   stego.head_a.weight [head_out, dim], stego.head_a.bias [head_out],

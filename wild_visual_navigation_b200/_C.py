@@ -20,6 +20,10 @@ class WvnError(RuntimeError):
     pass
 
 
+# wvn_vit_create_ffn's ffn: the block's FFN (WVN_VIT_FFN_MLP / WVN_VIT_FFN_SWIGLU)
+VIT_FFN_MLP, VIT_FFN_SWIGLU = 0, 1
+
+
 class VitConfig(Structure):
     _fields_ = [
         ("image_size", c_int), ("patch_size", c_int), ("dim", c_int), ("depth", c_int), ("heads", c_int),
@@ -82,6 +86,8 @@ SIGNATURES = {
     "wvn_layernorm_ex": (_I, [_P, _P, _P, _P, _P, _L, _I, _F, _I, _I, _I, _I, _P]),
     "wvn_attention_f32_debug": (_I, [_P, _P, _I, _I, _I, _I, _I, _F, _P]),
     "wvn_vit_create": (_I, [POINTER(VitConfig), POINTER(_P)]),
+    "wvn_vit_create_ffn": (_I, [POINTER(VitConfig), _I, POINTER(_P)]),
+    "wvn_swiglu_packed_rows": (_I, [_L, _P]),
     "wvn_vit_destroy": (None, [_P]),
     "wvn_vit_set_weight": (_I, [_P, c_char_p, _P, _L]),
     "wvn_vit_forward": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),

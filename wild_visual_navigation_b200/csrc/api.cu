@@ -140,10 +140,19 @@ int wvn_attention_f32_debug(const float* qkv, void* out_bf16, int batch, int hea
 }
 
 // -------------------------------------------------------------------------------- ViT (vit_backbone.cu)
-int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) {
+int wvn_vit_create(const wvn_vit_config* cfg, wvn_vit_t** out) { return wvn_vit_create_ffn(cfg, WVN_VIT_FFN_MLP, out); }
+
+int wvn_vit_create_ffn(const wvn_vit_config* cfg, int ffn, wvn_vit_t** out) {
   WVN_REQUIRE(cfg && out, "wvn_vit_create: null argument");
   WVN_PROPAGATE(wvn_check_device());
-  return vit_create(cfg, out);
+  return vit_create(cfg, ffn, out);
+}
+
+int wvn_swiglu_packed_rows(long long rows, long long* src_rows) {
+  WVN_REQUIRE(src_rows, "wvn_swiglu_packed_rows: null argument");
+  WVN_REQUIRE(rows > 0 && rows % 256 == 0, "wvn_swiglu_packed_rows: rows %lld must be a positive multiple of 256", rows);
+  for (long long p = 0; p < rows; ++p) src_rows[p] = swiglu_packed_row(p, rows);
+  return WVN_OK;
 }
 
 void wvn_vit_destroy(wvn_vit_t* h) { vit_destroy(h); }

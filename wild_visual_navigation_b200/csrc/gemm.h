@@ -15,7 +15,18 @@ enum GemmEpilogue : int {
                       //   cols [0,feat) reconstruct x -> loss_reco = mean((out - x)^2) -> confidence,
                       //   col feat = traversability logit -> sigmoid.  Nothing of [M,N] is stored.
   EPI_BF16_RESID = 6, // out(bf16)[row, col]  = act(acc + bias + residual(bf16)[row, col])  (a residual block's last conv)
+  EPI_SWIGLU = 7,     // block_n 256 only, W and bias in swiglu_packed_row order: tile t's columns [0, 128) are gate
+                      //   columns, [128, 256) the matching value columns;
+                      //   out(bf16)[row, 128 t + j] = silu(acc_g + b_g) * (acc_v + b_v), N / 2 columns
 };
+
+// The SwiGLU FFN's w12 = [gate rows (H); value rows (H)] as EPI_SWIGLU reads it: packed row p of the 2H rows holds
+// checkpoint row swiglu_packed_row(p, 2H), so that each 256-row tile is 128 gate rows followed by their 128 value rows.
+// Needs H % 128 == 0.
+inline long long swiglu_packed_row(long long p, long long rows) {
+  const long long t = p / 256, j = p % 256;
+  return j < 128 ? t * 128 + j : rows / 2 + t * 128 + (j - 128);
+}
 
 enum GemmAct : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_SILU = 3 /* EPI_BF16 only */ };
 

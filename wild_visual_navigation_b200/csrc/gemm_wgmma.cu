@@ -62,7 +62,8 @@ struct TileIter {
 };
 
 template <int EPI>
-constexpr bool kStaged = EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_RESID_F32 || EPI == EPI_QKV || EPI == EPI_BF16_RESID;
+constexpr bool kStaged = EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_RESID_F32 || EPI == EPI_QKV ||
+                         EPI == EPI_BF16_RESID || EPI == EPI_SWIGLU;
 
 template <int BN, int EPI>
 struct GemmCfg {
@@ -167,9 +168,15 @@ __device__ __forceinline__ void epilogue_frag(const GemmArgs& args, const float 
 //   fp32        : [64 rows][32 cols], 128-byte rows, 128B swizzle (chunk ^= r & 7)
 //   bf16, Q / K : [64 rows][32 cols], 64-byte rows, 64B swizzle (chunk ^= (r >> 1) & 3)
 //   V^T         : [32 head dims][64 tokens], 128-byte rows, 128B swizzle (chunk ^= dim & 7)
+// EPI_SWIGLU: d is the gate fragment (tile columns [0, 128)) and dv the value fragment (columns [128, 256)).  They are
+// two m64n128 accumulators of the same thread, register i of one and register i of the other holding the same row and
+// the same column within its half, so gate column j meets value column j without a shuffle.  Each slice stores
+// silu(g + b_g) * (v + b_v), computed in fp32 and rounded to bf16 once, at output column col_base / 2 + 32 s (col_base
+// is the tile's first column of W and bias).  Every other epilogue ignores dv.
 template <int EPI, int ACT, int NREG>
 __device__ __forceinline__ void store_frag(const GemmArgs& args, const CUtensorMap* tm0, const CUtensorMap* tm1,
-                                           const CUtensorMap* tm2, const float (&d)[NREG], const int row_tile,
+                                           const CUtensorMap* tm2, const float (&d)[NREG], const float (&dv)[NREG],
+                                           const int row_tile,
                                            const int col_base, const int row_local, const int lane, const bool leader,
                                            const int bar_id, const uint32_t staging, const uint32_t slice_bytes,
                                            const int slice0) {
@@ -195,12 +202,17 @@ __device__ __forceinline__ void store_frag(const GemmArgs& args, const CUtensorM
     for (int js = 0; js < 4; ++js) {
       const int j = 4 * s + js;
       const int c = col + 8 * js + 2 * q;
-      float2 b = make_float2(0.f, 0.f);
+      float2 b = make_float2(0.f, 0.f), bv = make_float2(0.f, 0.f);
       if (args.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(args.bias + c));
+      if (EPI == EPI_SWIGLU && args.bias != nullptr) bv = __ldg(reinterpret_cast<const float2*>(args.bias + c + 128));
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = row_local + 8 * h;
         float a0 = d[4 * j + 2 * h] + b.x, a1 = d[4 * j + 2 * h + 1] + b.y;
+        if (EPI == EPI_SWIGLU) {
+          a0 = activate<ACT_SILU>(a0) * (dv[4 * j + 2 * h] + bv.x);
+          a1 = activate<ACT_SILU>(a1) * (dv[4 * j + 2 * h + 1] + bv.y);
+        }
         if (EPI == EPI_BF16_RESID && row_tile + r < args.M) {
           // the residual is added before the activation: out = act(conv + bias + shortcut)
           const uint32_t rv = __ldg(reinterpret_cast<const uint32_t*>(
@@ -226,6 +238,8 @@ __device__ __forceinline__ void store_frag(const GemmArgs& args, const CUtensorM
     if (leader) {
       if (EPI == EPI_BF16 || EPI == EPI_F32 || EPI == EPI_BF16_RESID) {
         tma_store_2d(tm0, buf, col, row_tile);
+      } else if (EPI == EPI_SWIGLU) {
+        tma_store_2d(tm0, buf, col_base / 2 + kSliceCols * s, row_tile);
       } else if (EPI == EPI_RESID_F32) {
         // x += acc + bias: one fp32 add per element, performed at L2
         tma_reduce_add_2d(tm0, buf, col, row_tile);
@@ -384,18 +398,22 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       const int m_eff = args.reverse_m ? num_m - 1 - it.m_blk : it.m_blk;
       const int row_tile = m_eff * BM;
       const int col0 = it.n_blk * BN;
-      if (kStaged<EPI>) {
+      if constexpr (EPI == EPI_SWIGLU) {
+        static_assert(BN == 256, "EPI_SWIGLU pairs the two n128 halves of a 256-column tile");
+        store_frag<EPI, ACT_NONE>(args, &tmap_c0, &tmap_c1, &tmap_c2, acc128[0], acc128[1], row_tile, col0, row_local,
+                                  lane, leader, 3 + wg, staging, Cfg::kSliceBytes, 0);
+      } else if (kStaged<EPI>) {
         const int bar_id = 3 + wg;
 #pragma unroll
         for (int c = 0; c < Cfg::kN128; ++c)
-          store_frag<EPI, ACT>(args, &tmap_c0, &tmap_c1, &tmap_c2, acc128[c], row_tile, col0 + c * 128, row_local, lane,
-                               leader, bar_id, staging, Cfg::kSliceBytes, 4 * c);
+          store_frag<EPI, ACT>(args, &tmap_c0, &tmap_c1, &tmap_c2, acc128[c], acc128[c], row_tile, col0 + c * 128,
+                               row_local, lane, leader, bar_id, staging, Cfg::kSliceBytes, 4 * c);
         if (Cfg::kN64)
-          store_frag<EPI, ACT>(args, &tmap_c0, &tmap_c1, &tmap_c2, acc64, row_tile, col0 + Cfg::kN128 * 128, row_local,
-                               lane, leader, bar_id, staging, Cfg::kSliceBytes, 4 * Cfg::kN128);
+          store_frag<EPI, ACT>(args, &tmap_c0, &tmap_c1, &tmap_c2, acc64, acc64, row_tile, col0 + Cfg::kN128 * 128,
+                               row_local, lane, leader, bar_id, staging, Cfg::kSliceBytes, 4 * Cfg::kN128);
         if (Cfg::kN32)
-          store_frag<EPI, ACT>(args, &tmap_c0, &tmap_c1, &tmap_c2, acc32, row_tile, col0 + Cfg::kN128 * 128 + Cfg::kN64 * 64,
-                               row_local, lane, leader, bar_id, staging, Cfg::kSliceBytes, 4 * Cfg::kN128 + 2 * Cfg::kN64);
+          store_frag<EPI, ACT>(args, &tmap_c0, &tmap_c1, &tmap_c2, acc32, acc32, row_tile,
+                               col0 + Cfg::kN128 * 128 + Cfg::kN64 * 64, row_local, lane, leader, bar_id, staging, Cfg::kSliceBytes, 4 * Cfg::kN128 + 2 * Cfg::kN64);
       } else {
         const int row0 = row_tile + row_local;
 #pragma unroll
@@ -490,6 +508,11 @@ int dispatch_epi(const GemmArgs& a, const CUtensorMap& ta, const CUtensorMap& tb
         if (a.act == ACT_RELU) return launch_gemm<BN, EPI_BF16_RESID, ACT_RELU>(a, ta, tb, tc, s);
       }
       break;
+    case EPI_SWIGLU:
+      if constexpr (BN == 256) {
+        if (a.act == ACT_NONE) return launch_gemm<BN, EPI_SWIGLU, ACT_NONE>(a, ta, tb, tc, s);
+      }
+      break;
   }
   return set_error(WVN_ERR_INVALID, "gemm: unsupported epilogue/activation combination (%d, %d)", a.epi, a.act);
 }
@@ -509,7 +532,7 @@ int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, in
   WVN_REQUIRE(a.M > 0 && a.N > 0 && a.K > 0, "gemm: empty problem (M=%d N=%d K=%d)", a.M, a.N, a.K);
   WVN_REQUIRE(lda >= a.K, "gemm: lda=%lld is smaller than K=%d", lda, a.K);
   if (block_n == 0) {
-    block_n = pick_block_n(a.N);
+    block_n = a.epi == EPI_SWIGLU ? 256 : pick_block_n(a.N);
     if (a.epi == EPI_BF16_RESID && block_n > kResidMaxBlockN) block_n = a.N % 192 == 0 ? 192 : (a.N % 128 == 0 ? 128 : 64);
   }
   WVN_REQUIRE(a.epi != EPI_BF16_RESID || block_n <= kResidMaxBlockN, "gemm: the residual epilogue takes block_n <= %d",
@@ -532,6 +555,10 @@ int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, in
     WVN_REQUIRE(a.tokens_in > 0 && a.registers >= 0 && 1 + a.registers + a.tokens_in <= a.npad,
                 "gemm: bad patch-embed epilogue geometry (tokens_in=%d registers=%d npad=%d)", a.tokens_in, a.registers,
                 a.npad);
+  if (a.epi == EPI_SWIGLU)
+    WVN_REQUIRE(block_n == 256 && a.act == ACT_NONE && a.ldo % 8 == 0 && a.ldo >= a.N / 2,
+                "gemm: the SwiGLU epilogue takes block_n 256, no activation and a bf16 output pitch ldo >= N / 2, a "
+                "multiple of 8 (block_n=%d act=%d ldo=%lld N=%d)", block_n, a.act, a.ldo, a.N);
   if (a.epi == EPI_F32 || a.epi == EPI_RESID_F32) WVN_REQUIRE(a.ldo % 4 == 0, "gemm: fp32 output pitch must be a multiple of 4");
   if (a.epi == EPI_BF16 || a.epi == EPI_BF16_RESID) WVN_REQUIRE(a.ldo % 8 == 0, "gemm: bf16 output pitch must be a multiple of 8");
   if (a.epi == EPI_BF16_RESID)
@@ -545,6 +572,8 @@ int gemm_bf16(const GemmArgs& a, const void* A, long long lda, const void* W, in
   // output maps for the staged epilogues: 32-column x 64-row boxes (store_frag's layouts); rows past M are clipped
   if (a.epi == EPI_BF16 || a.epi == EPI_BF16_RESID)
     WVN_PROPAGATE(make_tmap_2d(&tc[0], a.out, 2, a.N, a.M, static_cast<uint64_t>(a.ldo) * 2, kSliceCols, BM, 64));
+  if (a.epi == EPI_SWIGLU)
+    WVN_PROPAGATE(make_tmap_2d(&tc[0], a.out, 2, a.N / 2, a.M, static_cast<uint64_t>(a.ldo) * 2, kSliceCols, BM, 64));
   if (a.epi == EPI_F32 || a.epi == EPI_RESID_F32)
     WVN_PROPAGATE(make_tmap_2d(&tc[0], a.out, 4, a.N, a.M, static_cast<uint64_t>(a.ldo) * 4, kSliceCols, BM, 128));
   if (a.epi == EPI_QKV) {

@@ -224,7 +224,8 @@ int WeightStore::add(const std::string& name, long long rows, int cols, bool bf1
   return WVN_OK;
 }
 
-int WeightStore::set(const char* name, const float* data, long long numel) {
+int WeightStore::set(const char* name, const float* data, long long numel,
+                     long long (*src_row)(long long, long long)) {
   auto it = w.find(name);
   WVN_REQUIRE(it != w.end(), "set_weight: unknown weight '%s'", name);
   Weight& wt = it->second;
@@ -235,17 +236,29 @@ int WeightStore::set(const char* name, const float* data, long long numel) {
     on_device = (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
   else
     cudaGetLastError();
+  const long long rows = numel / wt.cols;
+  // the longest run of stored rows from r0 on (at most `limit`) whose source rows are consecutive
+  auto run = [&](long long r0, long long limit) {
+    long long n = std::min(limit, rows - r0);
+    if (src_row != nullptr)
+      for (long long i = 1; i < n; ++i)
+        if (src_row(r0 + i, rows) != src_row(r0, rows) + i) { n = i; break; }
+    return n;
+  };
+  auto src_of = [&](long long r0) { return data + (src_row != nullptr ? src_row(r0, rows) : r0) * wt.cols; };
   // fp32 destination: copy straight in; bf16 destination: stage (if host) + cast on device
   if (!wt.bf16) {
-    WVN_CHECK_CUDA(
-        cudaMemcpy(wt.buf.p, data, numel * 4, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+    for (long long r0 = 0, n = 0; r0 < rows; r0 += n) {
+      n = run(r0, rows);
+      WVN_CHECK_CUDA(cudaMemcpy(reinterpret_cast<float*>(wt.buf.p) + r0 * wt.cols, src_of(r0), n * wt.cols * 4,
+                                on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+    }
   } else {
     // stage whole rows, cast each into its row of the pitched storage
     const long long chunk_rows = static_cast<long long>(stage.bytes / 4) / wt.cols;
-    const long long rows = numel / wt.cols;
-    for (long long r0 = 0; r0 < rows; r0 += chunk_rows) {
-      const long long n = std::min(chunk_rows, rows - r0);
-      const float* src = data + r0 * wt.cols;
+    for (long long r0 = 0, n = 0; r0 < rows; r0 += n) {
+      n = run(r0, chunk_rows);
+      const float* src = src_of(r0);
       if (!on_device) {
         WVN_CHECK_CUDA(cudaMemcpy(stage.p, src, n * wt.cols * 4, cudaMemcpyHostToDevice));
         src = reinterpret_cast<const float*>(stage.p);

@@ -131,8 +131,8 @@ struct WeightStore {
   // `rows` x `cols` elements; bf16 rows are stored at the GEMM's W pitch gemm_w_pitch(cols)
   int add(const std::string& name, long long rows, int cols, bool bf16);
   // Copies fp32 `data` (host or device): fp32 storage as is, bf16 storage cast on the device into its pitched rows,
-  // through `stage` when the source is host memory.
-  int set(const char* name, const float* data, long long numel);
+  // through `stage` when the source is host memory.  With `src_row`, stored row r is row src_row(r, rows) of `data`.
+  int set(const char* name, const float* data, long long numel, long long (*src_row)(long long, long long) = nullptr);
   // null for a name that was never added
   template <class T>
   T* ptr(const std::string& name) const {

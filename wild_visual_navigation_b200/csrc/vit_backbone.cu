@@ -1,9 +1,10 @@
-// wvn-b200: the ViT backbone handle — DINO / DINOv2 ViT-S / B / L token forward and STEGO's segmentation head.
+// wvn-b200: the ViT backbone handle — DINO / DINOv2 ViT-S / B / L / g token forward and STEGO's segmentation head.
 #include "vit_backbone.h"
 
 #include <cuda_bf16.h>
 
 #include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
 #include <string>
@@ -18,7 +19,8 @@ using namespace wvn;
 
 namespace {
 
-// One transformer block's parameters, resolved from the weight store at create (the storage never moves).
+// One transformer block's parameters, resolved from the weight store at create (the storage never moves).  With the
+// SwiGLU FFN, fc1 is w12 (its rows and bias in swiglu_packed_row order) and fc2 is w3.
 struct VitBlock {
   const float *norm1_w, *norm1_b, *qkv_b, *proj_b, *norm2_w, *norm2_b, *fc1_b, *fc2_b;
   const void *qkv_w, *proj_w, *fc1_w, *fc2_w;
@@ -28,6 +30,7 @@ struct VitBlock {
 
 struct wvn_vit {
   wvn_vit_config cfg;
+  int ffn = WVN_VIT_FFN_MLP;
   // t0: first patch row of a frame (1 + register tokens); rows [t0, n_valid) are the P patches
   int grid = 0, P = 0, t0 = 1, n_valid = 0, npad = 0, kpe = 0, kpe_ld = 0, chunk = 0;
   WeightStore weights;
@@ -47,8 +50,14 @@ struct wvn_vit {
 
 namespace wvn {
 
-int vit_create(const wvn_vit_config* cfg, wvn_vit** out) {
-  WVN_REQUIRE(cfg->dim == 384 || cfg->dim == 768 || cfg->dim == 1024, "vit: dim %d unsupported (384, 768, 1024)", cfg->dim);
+int vit_create(const wvn_vit_config* cfg, int ffn, wvn_vit** out) {
+  WVN_REQUIRE(cfg->dim == 384 || cfg->dim == 768 || cfg->dim == 1024 || cfg->dim == 1536,
+              "vit: dim %d unsupported (384, 768, 1024, 1536)", cfg->dim);
+  WVN_REQUIRE(ffn == WVN_VIT_FFN_MLP || ffn == WVN_VIT_FFN_SWIGLU, "vit: ffn %d unsupported (0 = GELU MLP, 1 = SwiGLU)",
+              ffn);
+  // SwiGLU: w12's 2 mlp_dim rows pack into 256-row tiles of 128 gate + 128 value rows (EPI_SWIGLU)
+  WVN_REQUIRE(ffn != WVN_VIT_FFN_SWIGLU || cfg->mlp_dim % 128 == 0,
+              "vit: the SwiGLU FFN needs mlp_dim %% 128 == 0 (got %d)", cfg->mlp_dim);
   WVN_REQUIRE(cfg->heads * 64 == cfg->dim, "vit: heads*64 must equal dim");
   WVN_REQUIRE(cfg->patch_size == 8 || cfg->patch_size == 14 || cfg->patch_size == 16, "vit: patch size %d unsupported",
               cfg->patch_size);
@@ -60,6 +69,7 @@ int vit_create(const wvn_vit_config* cfg, wvn_vit** out) {
   WVN_REQUIRE(cfg->registers == 0 || cfg->head_out == 0, "vit: register tokens and a STEGO head cannot be combined");
   wvn_vit* h = new wvn_vit();
   h->cfg = *cfg;
+  h->ffn = ffn;
   if (h->cfg.ln_eps <= 0.f) h->cfg.ln_eps = 1e-6f;
   h->grid = cfg->image_size / cfg->patch_size;  // conv-floor semantics for non-divisible sizes
   h->P = h->grid * h->grid;
@@ -93,10 +103,18 @@ int vit_create(const wvn_vit_config* cfg, wvn_vit** out) {
     k.proj_b = add(b + "attn.proj.bias", 1, D, false);
     k.norm2_w = add(b + "norm2.weight", 1, D, false);
     k.norm2_b = add(b + "norm2.bias", 1, D, false);
-    k.fc1_w = add(b + "mlp.fc1.weight", cfg->mlp_dim, D, true);
-    k.fc1_b = add(b + "mlp.fc1.bias", 1, cfg->mlp_dim, false);
-    k.fc2_w = add(b + "mlp.fc2.weight", D, cfg->mlp_dim, true);
-    k.fc2_b = add(b + "mlp.fc2.bias", 1, D, false);
+    if (ffn == WVN_VIT_FFN_SWIGLU) {
+      // the bias as 2 mlp_dim rows of one element, so that vit_set_weight packs it row by row as it packs the weight
+      k.fc1_w = add(b + "mlp.w12.weight", 2LL * cfg->mlp_dim, D, true);
+      k.fc1_b = add(b + "mlp.w12.bias", 2LL * cfg->mlp_dim, 1, false);
+      k.fc2_w = add(b + "mlp.w3.weight", D, cfg->mlp_dim, true);
+      k.fc2_b = add(b + "mlp.w3.bias", 1, D, false);
+    } else {
+      k.fc1_w = add(b + "mlp.fc1.weight", cfg->mlp_dim, D, true);
+      k.fc1_b = add(b + "mlp.fc1.bias", 1, cfg->mlp_dim, false);
+      k.fc2_w = add(b + "mlp.fc2.weight", D, cfg->mlp_dim, true);
+      k.fc2_b = add(b + "mlp.fc2.bias", 1, D, false);
+    }
     h->blocks.push_back(k);
   }
   h->norm_w = add("norm.weight", 1, D, false);
@@ -137,7 +155,17 @@ int vit_create(const wvn_vit_config* cfg, wvn_vit** out) {
 
 void vit_destroy(wvn_vit* h) { delete h; }
 
+namespace {
+bool ends_with(const char* s, const char* suffix) {
+  const size_t n = strlen(s), m = strlen(suffix);
+  return n >= m && strcmp(s + n - m, suffix) == 0;
+}
+}  // namespace
+
 int vit_set_weight(wvn_vit* h, const char* name, const float* data, long long numel) {
+  // w12 arrives in the checkpoint's row order [gate; value] and is stored in EPI_SWIGLU's packed order
+  if (h->ffn == WVN_VIT_FFN_SWIGLU && (ends_with(name, ".mlp.w12.weight") || ends_with(name, ".mlp.w12.bias")))
+    return h->weights.set(name, data, numel, swiglu_packed_row);
   return h->weights.set(name, data, numel);
 }
 
@@ -260,6 +288,10 @@ int vit_forward_impl(wvn_vit* h, const void* img, bool u8_hwc, int src_batch, in
           GemmArgs g;
           g.M = srows; g.N = c.mlp_dim; g.K = D; g.epi = EPI_BF16; g.act = ACT_GELU;
           g.bias = b.fc1_b; g.out = h->hid.p; g.ldo = c.mlp_dim;  // hid is reused per sub-chunk
+          if (h->ffn == WVN_VIT_FFN_SWIGLU) {
+            // w12 -> silu(gate) * value, the 2 mlp_dim products never stored
+            g.N = 2 * c.mlp_dim; g.epi = EPI_SWIGLU; g.act = ACT_NONE;
+          }
           g.reverse_m = next_dir();
           WVN_PROPAGATE(gemm_bf16(g, xn + roff * D, D, b.fc1_w, 0, s));
         }

@@ -7,7 +7,8 @@
 
 namespace wvn {
 
-int vit_create(const wvn_vit_config* cfg, wvn_vit** out);
+// ffn: WVN_VIT_FFN_MLP or WVN_VIT_FFN_SWIGLU
+int vit_create(const wvn_vit_config* cfg, int ffn, wvn_vit** out);
 void vit_destroy(wvn_vit* h);
 int vit_set_weight(wvn_vit* h, const char* name, const float* data, long long numel);
 // img: [batch, 3, in_h, in_w] fp32, or (u8_hwc) [batch, in_h, in_w, 3] uint8.  flip_tta: the `batch` source frames are

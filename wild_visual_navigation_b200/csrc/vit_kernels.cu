@@ -96,7 +96,7 @@ __global__ void init_token_rows_kernel(float* __restrict__ x, const float* __res
   }
 }
 
-// One warp per row, D = 128 * VEC_ITERS (384 -> 3, 768 -> 6, 1024 -> 8).  Two-pass statistics in
+// One warp per row, D = 128 * VEC_ITERS (384 -> 3, 768 -> 6, 1024 -> 8, 1536 -> 12).  Two-pass statistics in
 // registers (mean, then centred variance) — the same arithmetic order class as torch's LN.
 template <int ITERS>
 __global__ void __launch_bounds__(256)
@@ -279,7 +279,8 @@ int init_token_rows(float* x, const float* cls, const float* pos, const float* r
 
 int layernorm_rows(const float* x, const float* gamma, const float* beta, void* out_bf16, float* out_f32,
                    const LayerNormArgs& a, cudaStream_t stream) {
-  WVN_REQUIRE(a.dim == 384 || a.dim == 768 || a.dim == 1024, "layernorm: dim %d unsupported (384, 768 or 1024)", a.dim);
+  WVN_REQUIRE(a.dim == 384 || a.dim == 768 || a.dim == 1024 || a.dim == 1536,
+              "layernorm: dim %d unsupported (384, 768, 1024 or 1536)", a.dim);
   const int threads = 256;
   long long blocks = (a.rows * 32 + threads - 1) / threads;
   const long long max_blocks = static_cast<long long>(sm_count()) * 8;
@@ -290,8 +291,11 @@ int layernorm_rows(const float* x, const float* gamma, const float* beta, void* 
   else if (a.dim == 768)
     layernorm_rows_kernel<6><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(
         x, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out_bf16), out_f32, a);
-  else
+  else if (a.dim == 1024)
     layernorm_rows_kernel<8><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(
+        x, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out_bf16), out_f32, a);
+  else
+    layernorm_rows_kernel<12><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(
         x, gamma, beta, reinterpret_cast<__nv_bfloat16*>(out_bf16), out_f32, a);
   WVN_CHECK_LAUNCH("layernorm_rows_kernel");
   return WVN_OK;

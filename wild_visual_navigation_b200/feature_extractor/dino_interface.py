@@ -25,9 +25,12 @@ class _Cfg(dict):
 
 class DinoInterface:
     """``backbone="dino"``: DINO ViT-S / ViT-B at ``patch_size`` 8 or 16.  ``backbone="dinov2"``: DINOv2 ViT-S/14 /
-    ViT-B/14 / ViT-L/14 (no register tokens).  ``backbone="dinov2_reg"``: DINOv2 ViT-S/14-reg / ViT-B/14-reg /
-    ViT-L/14-reg (4 register tokens; only the patch tokens are returned).  ``backbone_type`` is "vit_small", "vit_base"
-    or, for DINOv2 only, "vit_large"; a checkpoint of another width or depth raises ValueError.  DINOv2 is released at patch 14 only, so both run at patch 14 whatever
+    ViT-B/14 / ViT-L/14 / ViT-g/14 (no register tokens).  ``backbone="dinov2_reg"``: DINOv2 ViT-S/14-reg / ViT-B/14-reg /
+    ViT-L/14-reg (4 register tokens; only the patch tokens are returned), and ViT-g/14 / ViT-g/14-reg likewise.
+    ``backbone_type`` is "vit_small", "vit_base" or, for DINOv2 only, "vit_large" or "vit_giant" (ViT-g/14: D = 1536,
+    40 blocks, 24 heads and a SwiGLU FFN; ``vit_giant`` follows the naming of the other sizes, and the name upstream
+    STEGO's ``get_backbone`` gives this model is not pinned); a checkpoint of another width, depth or FFN raises
+    ValueError.  DINOv2 is released at patch 14 only, so both run at patch 14 whatever
     ``patch_size`` says (the reference's ROS default passes ``patch_size=8`` with ``dinov2``); ``vit_patch_size`` still
     returns the configured value, as the reference's property does, while ``grid`` is the token grid actually run."""
 
@@ -53,7 +56,8 @@ class DinoInterface:
         if state_dict is not None:
             sd = check_backbone_family(state_dict, backbone, self._cfg.backbone_type)
         else:
-            sd = load_dino_state_dict(self._cfg.backbone_type, patch, self._cfg.pretrained_weights, backbone=backbone)
+            sd = load_dino_state_dict(self._cfg.backbone_type, patch, self._cfg.pretrained_weights, backbone=backbone,
+                                      device=device)
         with torch.cuda.device(torch.device(device)):
             self._model = ops.ViTBackbone(self._cfg.input_size, patch, shp["dim"], shp["depth"],
                                           shp["heads"], shp["mlp_dim"], sd, max_batch=max_batch, chunk=chunk,

@@ -9,8 +9,8 @@
   * when segmentation and features are both "stego"/"dino" on the same backbone, one ViT forward
     serves both (the reference runs two backbones); with "dinov2" / "dinov2_reg" features, STEGO's DINO backbone
     segments and a second, DINOv2 handle gives the features.  STEGO's backbone follows ``backbone_type`` unless
-    ``stego_backbone_type`` ("vit_small" / "vit_base") says otherwise; DINO has no ViT-L, so DINOv2 ViT-L/14 features
-    (``backbone_type="vit_large"``) with stego segmentation need it;
+    ``stego_backbone_type`` ("vit_small" / "vit_base") says otherwise; DINO has no ViT-L or ViT-g, so DINOv2 ViT-L/14
+    and ViT-g/14 features (``backbone_type="vit_large"`` / ``"vit_giant"``) with stego segmentation need it;
   * "torchvision" features (``model_type`` resnet18 / resnet50 / resnet50_dino / efficientnet_b0) are a feature
     pyramid (four levels, five for EfficientNet-B0) pooled per segment level by level (csrc/resnet_kernels.cu), as
     sparsify_features' dict branch does.  Where a segment has no
@@ -68,7 +68,7 @@ class FeatureExtractor:
                 raise ValueError(f"feature_type 'torchvision' needs model_type ({', '.join(MODEL_TYPES)})")
         elif "dino" in feature_type:
             # the reference hard-codes 384 for every dino variant (feature_extractor.py:56); here it is the backbone's
-            # width: 384 (vit_small), 768 (vit_base) or 1024 (vit_large, DINOv2 only)
+            # width: 384 (vit_small), 768 (vit_base), 1024 (vit_large) or 1536 (vit_giant; both DINOv2 only)
             check_backbone_type(backbone, common["backbone_type"])
             self._feature_dim = VIT_SHAPES[common["backbone_type"]]["dim"]
         else:

@@ -9,8 +9,12 @@ The reference downloads DINO checkpoints from dl.fbaipublicfiles.com at construc
     numerically meaningful only for parity / throughput work, and a warning says so.
 DINOv2 (``backbone="dinov2"``, the ``dinov2_vit{s,b,l}14_pretrain.pth`` checkpoints) uses the same key names plus the
 LayerScale gammas ``blocks.N.ls{1,2}.gamma`` and an unused ``mask_token``; DINOv2 with registers
-(``backbone="dinov2_reg"``, ``dinov2_vit{s,b,l}14_reg4_pretrain.pth``) adds ``register_tokens`` (1, R, D).  ViT-L/14
-(``backbone_type="vit_large"``) exists for DINOv2 only.
+(``backbone="dinov2_reg"``, ``dinov2_vit{s,b,l,g}14_reg4_pretrain.pth``) adds ``register_tokens`` (1, R, D).  ViT-L/14
+(``backbone_type="vit_large"``) and ViT-g/14 (``backbone_type="vit_giant"``, ``dinov2_vitg14{,_reg4}_pretrain.pth``)
+exist for DINOv2 only.  ViT-g/14's FFN is SwiGLU (``SwiGLUFFNFused``): ``blocks.N.mlp.w12`` (2 H rows: the gate half,
+then the value half) and ``blocks.N.mlp.w3`` in place of ``mlp.fc1`` / ``mlp.fc2``, hidden width
+H = (int(4 D 2 / 3) + 7) // 8 * 8 = 4096.  The name ``vit_giant`` follows the ``vit_small`` / ``vit_base`` /
+``vit_large`` pattern; the name upstream STEGO's ``get_backbone`` would give this model is not known here.
 The torchvision ResNets (``TorchVisionInterface``) take torchvision-layout state dicts (``resnet18`` / ``resnet50``
 ImageNet checkpoints, or DINO's ``dino_resnet50_pretrain.pth`` for ``resnet50_dino``); ``fc.*`` is not needed.
 EfficientNet-B0 (``efficientnet_b0``) takes torchvision-layout ``efficientnet_b0`` state dicts; ``classifier.*`` is not
@@ -28,9 +32,16 @@ VIT_SHAPES = {
     "vit_small": dict(dim=384, depth=12, heads=6, mlp_dim=1536),
     "vit_base": dict(dim=768, depth=12, heads=12, mlp_dim=3072),
     "vit_large": dict(dim=1024, depth=24, heads=16, mlp_dim=4096),
+    # SwiGLU FFN: mlp_dim is the hidden width H of w3(silu(x1) * x2), [x1 | x2] = w12(x) (2 H wide)
+    "vit_giant": dict(dim=1536, depth=40, heads=24, mlp_dim=4096, ffn="swiglu"),
 }
-# DINO v1 is released as ViT-S and ViT-B only; ViT-L exists for DINOv2 (with and without registers)
+# DINO v1 is released as ViT-S and ViT-B only; ViT-L and ViT-g exist for DINOv2 (with and without registers)
 DINO_V1_TYPES = ("vit_small", "vit_base")
+
+
+def vit_ffn(backbone_type: str) -> str:
+    """"mlp" (fc2(GELU(fc1(x)))) or "swiglu" (w3(silu(x1) * x2)), the FFN of every block of ``backbone_type``."""
+    return VIT_SHAPES[backbone_type].get("ffn", "mlp")
 
 
 def check_backbone_type(backbone: str, backbone_type: str) -> None:
@@ -77,10 +88,54 @@ def synthetic_dino_state_dict(dim, depth, mlp_dim, patch_size, pretrain_grid, se
 DINOV2_PATCH, DINOV2_PRETRAIN_GRID = 14, 37
 
 
-def synthetic_dinov2_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09):
+def synthetic_swiglu_state_dict(dim, depth, hidden, seed=1, attn_std=0.09, device="cpu"):
+    """Seeded DINOv2 ViT-g-layout weights with a SwiGLU FFN of hidden width ``hidden``: the DINOv2 layout at patch 14 /
+    grid 37 with ``mlp.w12`` (2 hidden x dim) / ``mlp.w3`` (dim x hidden) for ``mlp.fc1`` / ``mlp.fc2``, LayerScale
+    gammas and the (unused) ``mask_token``.  Every tensor is drawn on ``device`` from one generator there, so a full
+    ViT-g/14 (4.5 GB in fp32) never passes through host memory when ``device`` is a GPU."""
+    g = torch.Generator(device=device).manual_seed(seed)
+
+    def n(*shape, std):
+        return torch.randn(*shape, generator=g, device=device) * std
+
+    def u(*shape):
+        return 0.1 + 0.9 * torch.rand(*shape, generator=g, device=device)
+
+    sd = {
+        "cls_token": n(1, 1, dim, std=0.02),
+        "pos_embed": n(1, 1 + DINOV2_PRETRAIN_GRID**2, dim, std=0.02),
+        "patch_embed.proj.weight": n(dim, 3, DINOV2_PATCH, DINOV2_PATCH, std=0.05),
+        "patch_embed.proj.bias": n(dim, std=0.02),
+        "norm.weight": 1.0 + n(dim, std=0.05),
+        "norm.bias": n(dim, std=0.02),
+        "mask_token": torch.zeros(1, dim, device=device),
+    }
+    for i in range(depth):
+        b = f"blocks.{i}."
+        sd[b + "norm1.weight"] = 1.0 + n(dim, std=0.05)
+        sd[b + "norm1.bias"] = n(dim, std=0.02)
+        sd[b + "attn.qkv.weight"] = n(3 * dim, dim, std=attn_std)
+        sd[b + "attn.qkv.bias"] = n(3 * dim, std=0.02)
+        sd[b + "attn.proj.weight"] = n(dim, dim, std=0.02)
+        sd[b + "attn.proj.bias"] = n(dim, std=0.02)
+        sd[b + "ls1.gamma"] = u(dim)
+        sd[b + "norm2.weight"] = 1.0 + n(dim, std=0.05)
+        sd[b + "norm2.bias"] = n(dim, std=0.02)
+        sd[b + "mlp.w12.weight"] = n(2 * hidden, dim, std=0.04)
+        sd[b + "mlp.w12.bias"] = n(2 * hidden, std=0.02)
+        sd[b + "mlp.w3.weight"] = n(dim, hidden, std=0.02)
+        sd[b + "mlp.w3.bias"] = n(dim, std=0.02)
+        sd[b + "ls2.gamma"] = u(dim)
+    return sd
+
+
+def synthetic_dinov2_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09, ffn="mlp", device="cpu"):
     """Seeded DINOv2-layout weights: the DINO layout at patch 14 / grid 37 plus ``blocks.N.ls{1,2}.gamma`` and the
     (unused) ``mask_token``.  The LayerScale gammas vary per channel and are drawn independently for ls1 and ls2, so a
-    missing or swapped LayerScale changes the tokens far beyond the parity tolerance."""
+    missing or swapped LayerScale changes the tokens far beyond the parity tolerance.  ``ffn="swiglu"`` gives ViT-g's
+    layout (synthetic_swiglu_state_dict, drawn on ``device``)."""
+    if ffn == "swiglu":
+        return synthetic_swiglu_state_dict(dim, depth, mlp_dim, seed, attn_std, device)
     sd = synthetic_dino_state_dict(dim, depth, mlp_dim, DINOV2_PATCH, DINOV2_PRETRAIN_GRID, seed, attn_std)
     g = torch.Generator().manual_seed(seed + 1)
     for i in range(depth):
@@ -99,18 +154,25 @@ DINOV2_REGISTERS = 4
 DINOV2_REGISTER_STD = 0.02
 
 
-def synthetic_dinov2_reg_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09, registers=DINOV2_REGISTERS):
+def synthetic_dinov2_reg_state_dict(dim, depth, mlp_dim, seed=1, attn_std=0.09, registers=DINOV2_REGISTERS,
+                                    ffn="mlp", device="cpu"):
     """Seeded DINOv2-with-registers weights: ``synthetic_dinov2_state_dict`` plus ``register_tokens`` (1, R, dim), drawn
     from their own generator (seed + 2) with std DINOV2_REGISTER_STD."""
-    sd = synthetic_dinov2_state_dict(dim, depth, mlp_dim, seed, attn_std)
+    sd = synthetic_dinov2_state_dict(dim, depth, mlp_dim, seed, attn_std, ffn, device)
     g = torch.Generator().manual_seed(seed + 2)
-    sd["register_tokens"] = torch.randn(1, registers, dim, generator=g) * DINOV2_REGISTER_STD
+    sd["register_tokens"] = (torch.randn(1, registers, dim, generator=g) * DINOV2_REGISTER_STD).to(device)
     return sd
 
 
-def _vit_size(dim: int, depth: int) -> str:
-    name = next((k for k, v in VIT_SHAPES.items() if (v["dim"], v["depth"]) == (dim, depth)), None)
-    return f"{name} (D = {dim}, {depth} blocks)" if name else f"D = {dim} with {depth} blocks"
+_FFN_NAME = {"mlp": "GELU MLP", "swiglu": "SwiGLU FFN"}
+
+
+def _vit_size(dim: int, depth: int, ffn: str = None) -> str:
+    """Names a ViT size; with ``ffn``, a size whose FFN differs is named by its shape and FFN."""
+    name = next((k for k, v in VIT_SHAPES.items() if (v["dim"], v["depth"]) == (dim, depth)
+                 and (ffn is None or vit_ffn(k) == ffn)), None)
+    kind = "" if ffn is None else f", {_FFN_NAME[ffn]}"
+    return f"{name} (D = {dim}, {depth} blocks{kind})" if name else f"D = {dim} with {depth} blocks{kind}"
 
 
 def check_backbone_family(sd: dict, backbone: str, backbone_type: str = None) -> dict:
@@ -126,6 +188,11 @@ def check_backbone_family(sd: dict, backbone: str, backbone_type: str = None) ->
         if (dim, depth) != (shp["dim"], shp["depth"]):
             raise ValueError(f"backbone_type '{backbone_type}' needs a {_vit_size(shp['dim'], shp['depth'])} checkpoint; "
                              f"got {_vit_size(dim, depth)}")
+        ffn = "swiglu" if "blocks.0.mlp.w12.weight" in sd else "mlp"
+        if ffn != vit_ffn(backbone_type):
+            want = _vit_size(shp["dim"], shp["depth"], vit_ffn(backbone_type))
+            raise ValueError(f"backbone_type '{backbone_type}' needs a {want} checkpoint; "
+                             f"got {_vit_size(dim, depth, ffn)}")
     has_reg = "register_tokens" in sd
     has_ls = "blocks.0.ls1.gamma" in sd
     patch = int(sd["patch_embed.proj.weight"].shape[-1])
@@ -147,10 +214,10 @@ def check_backbone_family(sd: dict, backbone: str, backbone_type: str = None) ->
 
 
 def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights=None, seed: int = 1,
-                         backbone: str = "dino"):
+                         backbone: str = "dino", device="cpu"):
     """DINO (``backbone="dino"``), DINOv2 (``"dinov2"``) or DINOv2 with registers (``"dinov2_reg"``; both always patch
     14) weights, from ``pretrained_weights`` / ``$WVN_DINO_WEIGHTS`` or seeded.  A checkpoint is checked against the
-    family (check_backbone_family)."""
+    family (check_backbone_family).  Seeded ViT-g weights are drawn on ``device``; the others on the host."""
     check_backbone_type(backbone, backbone_type)
     shp = VIT_SHAPES[backbone_type]
     path = pretrained_weights or os.environ.get("WVN_DINO_WEIGHTS")
@@ -163,10 +230,11 @@ def load_dino_state_dict(backbone_type: str, patch_size: int, pretrained_weights
         return check_backbone_family(sd, backbone, backbone_type)
     warnings.warn(f"no {backbone.upper()} checkpoint given (pretrained_weights / $WVN_DINO_WEIGHTS): using seeded random "
                   f"{backbone.upper()}-style weights — fine for parity and throughput work, not for real traversability")
+    kw = dict(ffn="swiglu", device=device) if vit_ffn(backbone_type) == "swiglu" else {}
     if backbone == "dinov2":
-        return synthetic_dinov2_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], seed)
+        return synthetic_dinov2_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], seed, **kw)
     if backbone == "dinov2_reg":
-        return synthetic_dinov2_reg_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], seed)
+        return synthetic_dinov2_reg_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], seed, **kw)
     return synthetic_dino_state_dict(shp["dim"], shp["depth"], shp["mlp_dim"], patch_size, 224 // patch_size, seed)
 
 

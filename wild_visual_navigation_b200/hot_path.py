@@ -23,9 +23,11 @@ unpicked pixels and a pixel-wise graph has one row per pixel.  ``feature_type="t
 (resnet18, resnet50, resnet50_dino, efficientnet_b0) runs a feature pyramid.  Its weights come from
 ``backbone_state_dict`` or ``pretrained_weights``; ``state_dict`` / ``head_state_dict`` stay STEGO's DINO backbone and
 head, which segment the frames when ``segmentation_type="stego"`` (``FeatureExtractor``'s ``stego_state_dict``).  ``feature_type="dinov2"`` /
-``"dinov2_reg"`` with ``backbone_type="vit_large"`` runs DINOv2 ViT-L/14 (1024-wide rows); ``state_dict`` is then its
-checkpoint, and with ``segmentation_type="stego"`` STEGO segments on a seeded DINO backbone of
-``stego_backbone_type`` ("vit_small" or "vit_base", whose width ``head_state_dict`` must match).
+``"dinov2_reg"`` with ``backbone_type="vit_large"`` runs DINOv2 ViT-L/14 (1024-wide rows), and with
+``backbone_type="vit_giant"`` DINOv2 ViT-g/14 (1536-wide rows, which only the LinearRnvp learner,
+``anomaly_detection=True``, trains on); ``state_dict`` is then its checkpoint, and with ``segmentation_type="stego"``
+STEGO segments on a seeded DINO backbone of ``stego_backbone_type`` ("vit_small" or "vit_base", whose width
+``head_state_dict`` must match).
 
 ``prediction_per_pixel`` is the node's parameter of that name.  With False, or with a SimpleGCN, the maps are
 segment-wise (wvn_feature_extractor_node.py:323-338): each pooled row is evaluated once (padded-row inference with the

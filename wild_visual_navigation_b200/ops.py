@@ -335,14 +335,16 @@ def interpolate_pos_embed_antialias(pos_embed: torch.Tensor, grid: int) -> torch
 
 def fold_layerscale(sd: dict, depth: int) -> dict:
     """DINOv2's LayerScale ``x += gamma * f(x)`` folded into the layer that ends f, in fp32 before any bf16 cast:
-    ``attn.proj`` weight rows and bias times ``ls1.gamma``, ``mlp.fc2`` weight rows and bias times ``ls2.gamma``
-    (at least fp32; a float64 state dict stays float64).  A state dict without gammas (DINO) is returned unchanged."""
+    ``attn.proj`` weight rows and bias times ``ls1.gamma``, ``mlp.fc2`` (``mlp.w3`` of a SwiGLU FFN) weight rows and
+    bias times ``ls2.gamma`` (at least fp32; a float64 state dict stays float64).  A state dict without gammas (DINO) is
+    returned unchanged."""
     if "blocks.0.ls1.gamma" not in sd:
         return sd
     out = {k: v for k, v in sd.items() if ".ls1.gamma" not in k and ".ls2.gamma" not in k}
+    fc2 = "mlp.w3" if "blocks.0.mlp.w3.weight" in sd else "mlp.fc2"
     for i in range(depth):
         b = f"blocks.{i}."
-        for ls, layer in (("ls1", "attn.proj"), ("ls2", "mlp.fc2")):
+        for ls, layer in (("ls1", "attn.proj"), ("ls2", fc2)):
             w, bias, gamma = sd[b + layer + ".weight"], sd[b + layer + ".bias"], sd[b + ls + ".gamma"]
             dt = torch.promote_types(w.dtype, torch.float32)
             gamma = gamma.to(w.device, dt)
@@ -354,7 +356,9 @@ def fold_layerscale(sd: dict, depth: int) -> dict:
 class ViTBackbone:
     """Owns a ``wvn_vit_t``: DINO / DINOv2 ViT weights (bf16 on device) + L2-sized activation workspaces.  A state dict
     with ``register_tokens`` (1, R, D) (DINOv2 *_reg) gives a handle with R register tokens after CLS, whose position
-    embeddings are interpolated by the register models' antialiased form."""
+    embeddings are interpolated by the register models' antialiased form.  A state dict with ``mlp.w12`` / ``mlp.w3``
+    (DINOv2 ViT-g/14's SwiGLU FFN, hidden width ``mlp_dim``) gives a handle with that FFN.  Tensors already on the GPU
+    are loaded from there, without a copy through host memory."""
 
     def __init__(self, image_size, patch_size, dim, depth, heads, mlp_dim, state_dict, max_batch=32, chunk=0,
                  head_weights=None, ln_eps=1e-6):
@@ -366,10 +370,12 @@ class ViTBackbone:
         self.head_out = 0 if head_weights is None else int(head_weights["head_a.weight"].shape[0])
         reg = next((v for k, v in state_dict.items() if k.endswith("register_tokens")), None)
         self.registers = 0 if reg is None else int(reg.shape[-2])
+        swiglu = any(k.endswith("blocks.0.mlp.w12.weight") for k in state_dict)
+        self.ffn = _C.VIT_FFN_SWIGLU if swiglu else _C.VIT_FFN_MLP
         cfg = VitConfig(image_size, patch_size, dim, depth, heads, mlp_dim, max_batch, chunk, ln_eps, self.head_out,
                         self.registers)
         h = c_void_p()
-        check(lib().wvn_vit_create(byref(cfg), byref(h)))
+        check(lib().wvn_vit_create_ffn(byref(cfg), self.ffn, byref(h)))
         self._h = h
         self.npad = lib().wvn_vit_npad(h)
         self._load(state_dict, depth)
@@ -378,7 +384,9 @@ class ViTBackbone:
                 self._set("stego." + k, v)
 
     def _set(self, name, t):
-        t = t.detach().to(dtype=torch.float32, device="cpu").contiguous()
+        t = t.detach().to(dtype=torch.float32, device="cuda" if t.is_cuda else "cpu").contiguous()
+        if t.is_cuda:
+            torch.cuda.current_stream().synchronize()  # the library reads it on its own stream
         check(lib().wvn_vit_set_weight(self._h, name.encode(), c_void_p(t.data_ptr()), t.numel()))
 
     def _load(self, sd, depth):
@@ -391,10 +399,11 @@ class ViTBackbone:
             self._set("register_tokens", sd["register_tokens"].reshape(-1))
         self._set("patch_embed.proj.weight", sd["patch_embed.proj.weight"].reshape(self.dim, -1))
         self._set("patch_embed.proj.bias", sd["patch_embed.proj.bias"])
+        ffn = (("mlp.w12.weight", "mlp.w12.bias", "mlp.w3.weight", "mlp.w3.bias") if self.ffn == _C.VIT_FFN_SWIGLU else
+               ("mlp.fc1.weight", "mlp.fc1.bias", "mlp.fc2.weight", "mlp.fc2.bias"))
         for i in range(depth):
             for leaf in ("norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.qkv.bias", "attn.proj.weight",
-                         "attn.proj.bias", "norm2.weight", "norm2.bias", "mlp.fc1.weight", "mlp.fc1.bias",
-                         "mlp.fc2.weight", "mlp.fc2.bias"):
+                         "attn.proj.bias", "norm2.weight", "norm2.bias") + ffn:
                 self._set(f"blocks.{i}.{leaf}", sd[f"blocks.{i}.{leaf}"])
         self._set("norm.weight", sd["norm.weight"])
         self._set("norm.bias", sd["norm.bias"])
